@@ -1,7 +1,7 @@
 #!/usr/bin/env python3
-"""bench.py — messages/s of the message-scan metric path on N B200s (BASELINE.json metric).
+"""bench.py — messages/s of the message-scan metric path on N H100s (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W [--config C1|C2|C3|C4] [--mode fused|hll|counters|alive]
+  python bench.py --gpus N --steps K --warmup W [--config C1|C2|C3|C4] [--mode fused|hll|counters|alive] [--dump-outputs DIR]
   python bench.py --impl reference --gpus N --steps K ...   the reference's CPU path (oracle port) on host cores
 
 Workloads (BASELINE.json configs; SURVEY.md §8 d) — the default at every N is C1, per-GPU work fixed (weak scaling):
@@ -28,10 +28,12 @@ Modes:
 A "step" is one pass of the hot path over one batch: the fused scan kernel over the rank's shard resident in HBM, added to
 the running topic state.  The K timed steps form one K-batch topic: state reset at the start, and — as the reference reads
 its results once, after the poll loop (src/main.rs:117-170) — ONE merge (N > 1: one NCCL all-reduce) and ONE finalize
-(state to host) at the end, all inside the timed region.  Inputs are >= 3.6 GB per GPU (>> 126 MB L2), so every step
+(state to host) at the end, all inside the timed region.  Inputs are >= 3.6 GB per GPU (>> 50 MB L2), so every step
 streams from HBM.  `value` = all ranks' records / max-over-ranks device time (CUDA events on the scan stream).
 `e2e` = the same metric through the C-ABI host entry point (kta_push_batch_host) with the batch in pinned HOST memory:
 host->device copies every step and the state read-back (finalize) every step are inside the timed region.
+`--dump-outputs DIR` writes the topic state the last timed step finalized (what a caller of the path reads back) as
+DIR/<name>.npy in float64, so that two builds can be compared output for output on the same seeded topic.
 """
 import argparse
 import json
@@ -88,7 +90,10 @@ def parse():
     ap.add_argument("--no-extra", action="store_true")
     ap.add_argument("--no-verify", action="store_true", help="skip the post-run parity check of the (merged) state")
     ap.add_argument("--cpu-sample", type=int, default=0, help="records in the CPU baseline sample (0 = auto)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the state of the last timed step as DIR/<name>.npy")
     a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
     c = CONFIGS[a.config]
     for k_arg, k_cfg in (("n", "n"), ("partitions", "partitions"), ("value_mean", "value_mean"), ("distinct_keys", "distinct_keys"),
                          ("tombstones", "tombstones"), ("null_keys", "nulls"), ("shard_world", "shard_world")):
@@ -135,7 +140,7 @@ def config_dict(a, world):
         "distinct_keys_per_gpu": a.distinct_keys, "shard_world": vw,
         "step": "one scan of the rank's %.0e-record batch into the running topic state; the K timed steps are one K-batch topic "
                 "closed by one merge (N>1) and one finalize inside the timed region" % a.n,
-        "l2": "inputs %.1f GB/GPU, larger than L2 (126 MB): no flush needed" % (a.n * 36 / 1e9),
+        "l2": "inputs %.1f GB/GPU, larger than L2 (50 MB): no flush needed" % (a.n * 36 / 1e9),
         "key_tile_base": "128-record tile offsets column supplied with the batch (feeder-side prefix sum, 0.06 B/record; the "
                          "library derives it with one extra pass when absent)",
     }
@@ -387,6 +392,8 @@ def measure(a, ctx, full):
     barrier()
     clocks = sampler.stop(t_region0, time.perf_counter()) if rank == 0 else None
     ms = e0.elapsed_time(e1)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, eng, P, a.mode)
     kern_ms, kern_n = eng.scan_time_ms()
     eng.set_timing(False)
     kavg = kern_ms / max(1, kern_n)
@@ -422,7 +429,7 @@ def measure(a, ctx, full):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    peak = float(peaks.get("hbm_gbs", 3350.0))
     achieved = alg_bytes / (kern_max_ms / 1e3) / 1e9
     traffic = None
     try:
@@ -438,7 +445,7 @@ def measure(a, ctx, full):
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                      "traffic": traffic, "kernel": KERNEL[a.mode], "kernel_ms": kern_max_ms, "kernel_ms_min_rank": kern_min_ms,
                      "algorithmic_bytes_per_launch": alg_bytes, "mean_key_bytes": topic.key_bytes_len / n,
-                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if "hbm_gbs" in peaks else "fallback 6650"},
+                     "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3350"},
         "logical_topic_gb_s": value * (topic.key_bytes_len / n + a.value_mean) / 1e9,
         "gpu_launches": launches, "clocks": clocks,
     }
@@ -528,6 +535,26 @@ def measure(a, ctx, full):
     return line
 
 
+def dump_outputs(out_dir, eng, P, mode):
+    """The finalized state of the timed topic, as its caller reads it back: per-partition counters [P, 7] (total, tombstones,
+    alive, null keys, non-null keys, key bytes, value bytes), key / value size histograms [P, 32], the global extrema and
+    sums, and per mode the exact alive-key count and the HLL registers and estimate.  float64 holds every count exactly
+    (all < 2^53)."""
+    import numpy as np
+    s = state_of(eng, P, mode)
+    smallest, largest, size, count, latest, (earliest_s, earliest_ns) = s["globals"]
+    arrays = {"counters": s["counters"], "key_size_hist": s["khist"], "value_size_hist": s["vhist"],
+              "globals": [smallest, largest, size, count, latest, earliest_s, earliest_ns]}
+    if "alive_keys" in s:
+        arrays["alive_keys"] = [s["alive_keys"]]
+    if "hll" in s:
+        arrays["hll_registers"] = s["hll"]
+        arrays["hll_estimate"] = [eng.alive_keys_hll()]
+    os.makedirs(out_dir, exist_ok=True)
+    for name, v in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(v, dtype=np.float64))
+
+
 def verify(a, ctx, eng, topic, spec, vw):
     """Parity of the measured path outside the timed region: one pass (reset, scan, merge, finalize) must give
     (i) the closed-form shares of the generator and the counter identities of src/metric.rs, and (ii) at N > 1, on every
@@ -603,6 +630,7 @@ def run_sweep(a, ctx):
     for vm in C4_VALUE_MEANS:
         b = argparse.Namespace(**vars(a))
         b.value_mean = vm
+        b.dump_outputs = a.dump_outputs if vm == a.value_mean else None
         line = measure(b, ctx, full=False)
         points.append({"value_mean": vm, "value": line["value"], "ms_per_step": line["ms_per_step"],
                        "kernel_ms": line["roofline"]["kernel_ms"], "frac": line["roofline"]["frac"],

@@ -1,5 +1,5 @@
 /*
- * kta.h — C ABI of libkta_gpu.so: the B200-native (sm_100a) replacement for the per-message
+ * kta.h — C ABI of libkta_gpu.so: the H100-native (sm_90a) replacement for the per-message
  * metric-aggregation path of xenji/kafka-topic-analyzer.
  *
  * Boundary being replaced (reference, Rust):

@@ -1,4 +1,4 @@
-"""kafka_topic_analyzer_b200 — B200-native (sm_100a) message-scan metric aggregation for
+"""kafka_topic_analyzer_b200 — H100-native (sm_90a) message-scan metric aggregation for
 kafka-topic-analyzer: the per-record path of src/kafka.rs:92-135 → src/metric.rs:206-305 →
 src/fnv32.rs:92-101, rebuilt as hand-written CUDA behind a C ABI (include/kta.h).
 

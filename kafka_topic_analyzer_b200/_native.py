@@ -23,7 +23,7 @@ INT64_MIN = -(1 << 63)
 SEQ_AUTO = (1 << 64) - 1   # include/kta.h KTA_SEQ_AUTO
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "--cudart", "static",
 ]
 
@@ -46,7 +46,7 @@ def build_synth(force: bool = False) -> str:
 
 
 def build(force: bool = False, verbose: bool = False, defines=(), out: str = None) -> str:
-    """Compile libkta_gpu.so for sm_100a with nvcc (cross-compiles without a GPU).
+    """Compile libkta_gpu.so for sm_90a (H100) with nvcc (cross-compiles without a GPU).
     `defines` / `out` build an experimental variant next to it (tuning runs; KTA_LIB selects it)."""
     out = out or LIB_PATH
     if not force and os.path.exists(out):

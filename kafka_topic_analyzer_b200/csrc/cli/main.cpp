@@ -1,4 +1,4 @@
-// kafka-topic-analyzer (B200 build) — the reference's CLI surface (src/main.rs:32-67) over libkta_gpu.so.
+// kafka-topic-analyzer (H100 build) — the reference's CLI surface (src/main.rs:32-67) over libkta_gpu.so.
 //
 //   -t/--topic TOPIC  -b/--bootstrap-server HOSTS  [--librdkafka k=v,...]  [-c/--count-alive-keys]
 //   --synthetic n=...,partitions=...,value_mean=...,run_len=...,distinct_keys=...,key_mode=...,seed=...,

@@ -1,4 +1,4 @@
-// kta_api.cu — host side of libkta_gpu.so: the C ABI of include/kta.h over the sm_100a kernels.
+// kta_api.cu — host side of libkta_gpu.so: the C ABI of include/kta.h over the sm_90a kernels.
 //
 // Mirrors, for this one path, what the reference's host does around the handlers:
 //   MessageMetrics::new / LogCompactionInMemoryMetrics::new      src/metric.rs:30-46, 267-271
@@ -187,7 +187,7 @@ static void scan_shape(const kta_handle *h, bool hash, bool exact, int64_t n, in
     }
     const int P = h->columns;
     // Leave the SM some L1: the header loads stream through it, and with (almost) all 228 KB carved out as shared
-    // memory the loads in flight are throttled (measured at P = 256).  KTA_SCAN_L1_RESERVE (bytes) is a tuning knob.
+    // memory the loads in flight are throttled.  KTA_SCAN_L1_RESERVE (bytes) is a tuning knob.
     static const size_t l1_reserve = [] { const char *e = getenv("KTA_SCAN_L1_RESERVE"); return e ? (size_t)atoll(e) : (size_t)0; }();
     const size_t budget = h->smem_optin > l1_reserve ? h->smem_optin - l1_reserve : h->smem_optin;
     for (threads = MAX_THREADS;; threads -= 128) {
@@ -244,7 +244,7 @@ static int state_reset_device(kta_handle *h) {
     h->launches++;
     CU(cudaGetLastError());
     if (h->d_alive_table) {
-        // the table is a few hundred MB at most for the topics it is meant for: wiping it is a ~20 µs memset
+        // the table is a few hundred MB at most for the topics it is meant for: wiping it is one short memset
         CU(cudaMemsetAsync(h->d_alive_table, 0xff, (size_t)h->alive_pairs * 16, h->stream));
         CU(cudaMemsetAsync(h->d_scalar, 0, 32, h->stream));
         CU(cudaMemsetAsync(h->d_alive_status, 0, 8, h->stream));
@@ -299,7 +299,7 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
     CU(cudaSetDevice(h->device));
     cudaDeviceProp prop;
     CU(cudaGetDeviceProperties(&prop, h->device));
-    if (prop.major < 10) return fail(KTA_ERR_CUDA, "device %s is sm_%d%d; this library is built for sm_100a only",
+    if (prop.major != 9 || prop.minor != 0) return fail(KTA_ERR_CUDA, "device %s is sm_%d%d; this library is built for sm_90a only",
                                      prop.name, prop.major, prop.minor);
     h->sm_count = prop.multiProcessorCount;
     CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
@@ -325,9 +325,8 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
     if (h->nhll) CU(cudaMalloc(&h->d_hll, h->nhll * 4));
     if (cfg->count_alive_keys == 1) {
         // open-addressed last-writer table keyed by the 32-bit hash, sized by the number of DISTINCT hashes and grown
-        // on demand (alive_check): 256 MiB = 2^25 slots holds the 1e7 keys of BASELINE configs[2] at load 0.3 (measured:
-        // at 0.6 every third first-seen key finds its home pair taken and probes on — 10 % of the kernel time; the
-        // table does not fit L2 at either size)
+        // on demand (alive_check): 256 MiB = 2^25 slots holds the 1e7 keys of BASELINE configs[2] at load 0.3 (at 0.6
+        // every third first-seen key finds its home pair taken and probes on; the table does not fit L2 at either size)
         if (cfg->alive_table_kib < 0 || cfg->alive_table_kib > ALIVE_MAX_KIB)
             return fail(KTA_ERR_INVALID, "alive_table_kib %d out of range [0, %d]", cfg->alive_table_kib, ALIVE_MAX_KIB);
         static const int64_t env_kib = [] { const char *e = getenv("KTA_ALIVE_TABLE_KIB"); return e ? atoll(e) : 0ll; }();   // tuning knob
@@ -419,7 +418,7 @@ static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, 
     prm.alive_status = h->d_alive_status;
     prm.alive_cache = nullptr;
     if (exact && prm.n >= ALIVE_CACHE_MIN_RECORDS) {
-        // the seen cache pays for its clearing (32 MiB, ~10 µs) on batches of a million records and more.
+        // the seen cache pays for its clearing (a 32 MiB memset) on batches of a million records and more.
         // Waves cut the batch's seq range [lo, hi] into <= 127 equal slices (any monotone function of seq will do).
         static const bool off = getenv("KTA_ALIVE_NO_CACHE") != nullptr;   // tuning / ablation knob
         uint64_t lo = prm.seq_base, hi = prm.seq_base + (uint64_t)prm.n - 1;

@@ -1,15 +1,15 @@
-// kta_kernels.cuh — sm_100a device code for the message-scan metric path.
+// kta_kernels.cuh — sm_90a (H100) device code for the message-scan metric path.
 //
 // What the kernels compute is exactly what the reference computes once per polled message
 // (src/kafka.rs:107-109) in MessageMetrics::handle_message (src/metric.rs:206-253) and
 // LogCompactionInMemoryMetrics::handle_message (src/metric.rs:288-305, hash src/fnv32.rs:92-101),
-// restructured for a B200: records arrive as SoA columns resident in HBM, one CTA walks 1024-record
+// restructured for an H100: records arrive as SoA columns resident in HBM, one CTA walks 1024-record
 // tiles, per-partition counters live in shared memory (u32 + carry word, native ATOMS), the tile's
 // packed key bytes are staged global→shared with one bulk async copy (cp.async.bulk / UBLKCP, mbarrier
 // completion, double buffered), keys are hashed from shared memory, and the alive-key state is a
 // compact open-addressed table of 64-bit last-writer stamps (hash | seq | alive) sized by the number
-// of distinct key hashes — about the size of the 126 MB L2 for 1e7 keys — so that the one random access every
-// record needs is an L2 hit, not a DRAM sector.
+// of distinct key hashes (8 bytes each: 80 MB of entries for 1e7 keys) rather than by the 2^32 possible hashes, with a
+// 32 MiB seen cache in front of it that fits the 50 MB L2, so that most records need one L2 hit, not a DRAM sector.
 // No tensor cores: there is no dense contraction anywhere on this path.
 #pragma once
 #include <cuda_runtime.h>
@@ -464,8 +464,7 @@ struct Counters {
 // holding the stamp of the LAST record that carried this hash (fmix32 is a bijection: x names the hash exactly, and it
 // is what the table, the seen cache and the HLL sketch all index by, so it is computed once per record).  The reference's BitSet (metric.rs:273-280) is indexed by
 // the hash itself — 2^32 bits, one random DRAM sector per record wherever the state lives; keyed by hash but SIZED by
-// the number of distinct hashes, the same state is about as large as the 126 MB L2 for 1e7 keys, and the one access per
-// record becomes an L2 hit.
+// the number of distinct hashes, the same state is 80 MB of entries for 1e7 keys, and the seen cache below keeps most records in L2.
 //   * A slot is claimed once (CAS from empty) and keeps its hash for ever; linear probing over 16-byte PAIRS of slots
 //     from home = mulhi(x, pairs), so any table size works, not only powers of two.
 //   * On a slot that holds the record's hash, atomicMax makes "last" mean highest seq regardless of execution order
@@ -480,8 +479,8 @@ struct Counters {
 //   * A stamp that finds neither its hash nor an empty slot within ALIVE_MAX_PROBES pairs is counted in status[0] and
 //     dropped; the host then grows the table (rehash) and re-runs the batch stamps-only — stamping is idempotent.
 //
-// The SEEN CACHE in front of it.  Measured (profiles/r02_alive_v0_*): a table of 128 MiB does not stay in the 126 MB L2
-// next to a 3.6 GB stream — 73 % of the probes missed — and 1e8 random DRAM sectors cost 2.4 ms.  But 90–99 % of the
+// The SEEN CACHE in front of it.  A table of 128 MiB or more does not stay in L2 next to a multi-GB record stream, so
+// a table probe per record is a random DRAM sector per record.  But 90–99 % of the
 // records of a compacted topic are superseded by a newer record of the same key, and all they need to learn is that
 // fact.  So each batch keeps a 32 MiB, 2-way set-associative, EXACT cache of (hash → newest wave seen), where a wave is
 // 1/127 of the batch in seq order: set = top 23 bits of fmix32(hash) (a bijection), way = 9-bit tag (the other bits) +
@@ -638,8 +637,8 @@ __device__ __forceinline__ bool alive_cache_newer(uint32_t c, uint32_t x, uint32
 }
 // record the fact "hash x has a record of wave wv" (wv >= 1) in its set; c = the set word as read by the probe.
 // The tag's own way if it has one (and only if that improves on it), else an empty way, else either.  (Picking the way by
-// a bit of the hash instead — nothing to carry from the probe — was measured: two keys that share a set then evict each
-// other for ever, 1.4 GB more table traffic per 1e8 records.)
+// a bit of the hash instead — nothing to carry from the probe — lets two keys that share a set evict each other for
+// ever, and every such eviction is one more table probe.)
 __device__ __forceinline__ void alive_cache_put(uint32_t *cache, uint32_t c, uint32_t x, uint32_t wv, uint32_t pick) {
     const uint32_t tag = x & ((1u << ALIVE_CACHE_TAG_BITS) - 1u);
     const uint32_t mine = (tag << ALIVE_CACHE_WAVE_BITS) | wv;
@@ -773,7 +772,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) scan_kernel(const ScanParams p
     bool try_uni = true;      // probe rows for "one partition" only while that keeps paying off
     // MODE_HLL: the warp's copy of the sketch floor (a lower bound of every register: monotone, so a stale copy only
     // filters less).  Re-read from its global word after the first tiles and then every 16th tile — one global word read by
-    // every warp for EVERY tile made a single L2 line the bottleneck of the whole kernel (measured: +0.46 ms).
+    // every warp for EVERY tile makes a single L2 line the bottleneck of the whole kernel.
     uint32_t floor_reg = MODE == MODE_HLL ? ld_cg_u32(prm.hll_floor) : 0u;
     uint32_t nxt_info = 0;
 
@@ -883,8 +882,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) scan_kernel(const ScanParams p
                             any_uni = true;
                         } else {
                             // a row that straddles a run boundary holds two partitions: left to per-lane adds, its two
-                            // counters would be hit 32 times each, serialised in the shared-memory pipe (measured: +0.09 ms
-                            // at run length 500).  Reduce the two groups separately instead.
+                            // counters would be hit 32 times each, serialised in the shared-memory pipe.  Reduce the two groups separately instead.
                             const int l1 = __ffs(~m0) - 1;                     // first lane of the second group
                             const int p1 = __shfl_sync(full, p[k], l1 & 31);
                             const unsigned m1 = __ballot_sync(full, p[k] == p1);
@@ -1088,8 +1086,6 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) scan_kernel(const ScanParams p
             // latency, not DRAM.  So: exactly ONE random access per record (the seen cache, in flight while the records
             // are counted); the ~12 % that survive it are compacted across the tile into one dense queue (in the key stage
             // the tile has just finished with) and take the exact path through the table, usually in a single pass.
-            // (Measured dead ends, profiles/r02_exact_experiments.md: deferring the table pass by a tile or batching it
-            // over several, with or without L2 prefetch, and giving it to dedicated consumer warps were all slower.)
             uint4 *queue = reinterpret_cast<uint4 *>(wsm + 128 + (size_t)buf * KEYBUF);   // (x, low word, set word, -) x TILE <= stage
             const bool cached = AW.cache != nullptr;
             const uint32_t r32 = (uint32_t)rbase;   // index in the batch (< 2^31: host-checked)
@@ -1174,7 +1170,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) scan_kernel(const ScanParams p
         if (HASH) {
             info = __shfl_sync(full, nxt_info, 0);   // also: every lane is done with stage buf^1 before it is refilled
         }
-        const bool has_next = tile < ntiles - gstride;   // no overflow: gstride <= 148 * 32
+        const bool has_next = tile < ntiles - gstride;   // no overflow: gstride <= SMs * 32
         if (HASH && has_next && lane == 0) nxt_info = issue(phys(tile + gstride), buf ^ 1);
         const int pt = phys(tile);
         if ((int64_t)(pt + 1) * TILE <= prm.n) body(std::true_type{}, pt, buf, info, has_next);
@@ -1183,7 +1179,7 @@ __global__ void __launch_bounds__(MAX_THREADS, 1) scan_kernel(const ScanParams p
         if (SMEM && (it & (FOLD_TILES - 1)) == FOLD_TILES - 1) C.fold_sums(lane, 1u << 30);
         try_uni = try_uni || (it & 15) == 15;   // re-probe for run-structured input now and then
         // HLL floor upkeep: every 4th tile ONE warp of each CTA (the role rotates, so no warp falls behind)
-        // refreshes one slice — the 148 CTAs cover all 64 slices about every two tile-times — and republishes
+        // refreshes one slice — the 132 CTAs of an H100 cover all 64 slices about every two tile-times — and republishes
         // the floor (plus two early refreshes after the first and second tile, so that a cold sketch stops taking every
         // record); every warp picks the published floor up after its first tiles and then every 16th
         if (MODE == MODE_HLL) {

@@ -379,8 +379,8 @@ __global__ void __launch_bounds__(128) log_decompress_kernel(const uint8_t *byte
 // parallel and write the columns coalesced.
 // STAGED: the whole batch (what a producer's batch.size bounds: 16 KiB by default) is first brought global→shared by ONE
 // bulk async copy per batch per warp (cp.async.bulk → UBLKCP, mbarrier completion), so every hop of the chain is a
-// 29-cycle shared-memory read instead of a dependent global access to a new line (measured: the chain of global hops was
-// the decoder's bottleneck).  Batches that do not fit the stage, or whose 16-byte-aligned copy would run past the readable
+// shared-memory read instead of a dependent global access to a new line (the chain of hops is the decoder's
+// critical path).  Batches that do not fit the stage, or whose 16-byte-aligned copy would run past the readable
 // bytes, are read in place.
 // Output: the header columns and, per record, the position of its key bytes in the segment buffer (key_src, only when the
 // keys will be hashed) — the keys themselves are packed afterwards by log_gather_keys_kernel, without a second walk.

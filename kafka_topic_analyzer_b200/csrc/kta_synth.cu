@@ -87,7 +87,7 @@ extern "C" int kta_synth_fill_device(const kta_synth_spec *s, int32_t device, in
         if (key_bytes_len) *key_bytes_len = 0;
         return KTA_OK;
     }
-    int sms = 148;
+    int sms = 132;
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);

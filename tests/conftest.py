@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (sm_90a)")
 
 
 def _has_gpu() -> bool:
@@ -22,7 +22,7 @@ def _has_gpu() -> bool:
 
 
 def pytest_collection_modifyitems(config, items):
-    # On a box without a GPU, gpu-marked tests are skipped (the driver deselects them with -m "not gpu").
+    # On a machine without a GPU, gpu-marked tests are skipped.
     if _has_gpu():
         return
     skip = pytest.mark.skip(reason="no CUDA device")

@@ -67,12 +67,12 @@ def test_product_never_touches_the_oracle():
 
 
 def test_sass_has_bulk_copy_and_no_legacy_paths():
-    """The fused kernel really uses the Blackwell/Hopper bulk async copy (UBLKCP) + mbarrier (SYNCS)."""
+    """The fused kernel really uses the Hopper bulk async copy (UBLKCP) + mbarrier (SYNCS)."""
     r = subprocess.run(["cuobjdump", "-sass", _native.LIB_PATH], capture_output=True, text=True)
     if r.returncode != 0:
         pytest.skip("cuobjdump unavailable")
     assert "UBLKCP" in r.stdout and "SYNCS" in r.stdout and "ATOMS" in r.stdout
-    assert "sm_100a" in r.stdout
+    assert "sm_90a" in r.stdout
 
 
 def test_abi_rejects_bad_arguments_without_cuda():

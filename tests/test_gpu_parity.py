@@ -632,8 +632,9 @@ def test_config2_full_size_alive_exact():
     the distinct hashes; HLL over the resolved set within 4 sigma."""
     import torch
     free, _ = torch.cuda.mem_get_info()
-    if free < 100e9:
-        pytest.skip("needs ~80 GB of HBM")
+    # peak: 40 GB of columns + hashes during the scan, then ~56 GB while sorting 1e9 composite keys (columns freed)
+    if free < 64e9:
+        pytest.skip("needs ~60 GB of HBM")
     P, n = 64, 1_000_000_000
     spec = synth.make_spec(n, P, distinct_keys=10_000_000, null_key_per_10k=0)     # compacted topic: every record keyed, 5 % tombstones
     topic = synth.DeviceTopic(spec)

@@ -13,7 +13,7 @@ for t in memcheck racecheck synccheck initcheck; do grep -E "ok|SUMMARY|Error|ha
 cp $g/${tag}_sanitizer_summary.log $p/r02_sanitizer_summary.log
 for m in hll alive counters; do
   python tools/ncu_summary.py $g/${tag}_prof_$m.ncu-rep $m $p/r02_final_${m}_ncu_summary.txt \
-    "round 2 final, build $head: ncu --set full --clock-control none of kta::scan_kernel, bench.py --mode $m --tombstones 500 --steps 2 --warmup 1 (C1 shape, 1e8 records, one B200)" > /dev/null
+    "round 2 final, build $head: ncu --set full --clock-control none of kta::scan_kernel, bench.py --mode $m --tombstones 500 --steps 2 --warmup 1 (C1 shape, 1e8 records, one GPU)" > /dev/null
 done
 {
   echo "# SASS of the shipped libkta_gpu.so (build $head), cuobjdump -sass, scan_kernel<MODE_HLL, SMEM> = _ZN3kta11scan_kernelILi1ELb1ELb0ELb0EEEvNS_10ScanParamsE"

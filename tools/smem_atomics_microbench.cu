@@ -3,7 +3,7 @@
 // per-lane bucket increments hit few distinct addresses when a tile lies inside one partition run, and many
 // addresses in few banks when P is large.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/smem_atomics tools/smem_atomics_microbench.cu && /tmp/smem_atomics
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o build/smem_atomics tools/smem_atomics_microbench.cu && build/smem_atomics   (after mkdir -p build)
 //
 // Prints, per pattern, cycles per warp-level atomic instruction with 32 resident warps per SM (like the scan kernel)
 // and with 1 warp (latency view).  Patterns: the address each lane uses, in 4-byte words.
