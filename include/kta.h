@@ -63,7 +63,7 @@ typedef struct kta_config {
     int32_t count_alive_keys;  /* 1 = exact alive-key table, i.e. `-c` given once (src/main.rs:77-80) */
     int32_t hll_precision;     /* EXTENSION: 0 = off, else 4..18 HyperLogLog index bits */
     int32_t alive_table_kib;   /* initial size of the alive-key table in KiB (8 bytes per distinct key hash, kept at
-                                  load <= 0.7 and grown on demand); 0 = default (131072 = 128 MiB: 1e7 keys) */
+                                  load <= 0.6 and grown on demand); 0 = default (262144 = 256 MiB: 1e7 keys) */
     int64_t ring_records;      /* records per landing-ring chunk for kta_push / host batches; 0 = default */
     int64_t ring_key_bytes;    /* key bytes per landing-ring chunk; 0 = default */
     int64_t now_s;             /* construction wall clock for earliest_message (Utc::now(), */

@@ -108,7 +108,7 @@ struct kta_handle {
     uint64_t alive_origin = 0;               // seq that a stamp's field value 1 stands for
     bool alive_rebased = false;              // a rebase dropped absolute sequence numbers (exports are refused then)
     uint32_t *d_alive_cache = nullptr;       // seen cache of the batch being scanned (32 MiB, cleared per launch)
-    uint32_t *d_alive_status = nullptr;      // [0] stamps that found no slot, [1] records outside the seq window
+    uint32_t *d_alive_status = nullptr;      // [0] stamps that found no slot, [1] records outside the seq window, [2] wide re-run
     uint32_t *h_alive_status = nullptr;      // pinned copy
     uint64_t alive_window_errors = 0;        // sticky until reset: reported by kta_finalize
     uint64_t alive_grows = 0, alive_reruns = 0;
@@ -259,7 +259,7 @@ static int state_reset_device(kta_handle *h) {
         // the table is a few hundred MB at most for the topics it is meant for: wiping it is one short memset
         CU(cudaMemsetAsync(h->d_alive_table, 0xff, (size_t)h->alive_pairs * 16, h->stream));
         CU(cudaMemsetAsync(h->d_scalar, 0, 32, h->stream));
-        CU(cudaMemsetAsync(h->d_alive_status, 0, 8, h->stream));
+        CU(cudaMemsetAsync(h->d_alive_status, 0, 12, h->stream));
         h->alive_now = h->alive_occupied = 0;
         h->alive_origin = 0;
         h->alive_rebased = false;
@@ -345,7 +345,7 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
         const int64_t kib = cfg->alive_table_kib ? cfg->alive_table_kib : env_kib > 0 ? env_kib : ALIVE_DEFAULT_KIB;
         h->alive_pairs = (uint32_t)std::max<int64_t>(kib * 64, 16);   // 16 bytes per pair
         CU(cudaMalloc(&h->d_alive_table, (size_t)h->alive_pairs * 16));
-        CU(cudaMalloc(&h->d_alive_status, 8));
+        CU(cudaMalloc(&h->d_alive_status, 12));
         CU(cudaMalloc(&h->d_alive_cache, ((size_t)4 << ALIVE_CACHE_SET_BITS)));
         CU(cudaHostAlloc(&h->h_alive_status, 8, cudaHostAllocDefault));
     }
@@ -518,8 +518,12 @@ static int alive_grow(kta_handle *h, uint32_t new_pairs) {
 }
 
 // Confirms every pending MODE_EXACT scan: waits for the stream, reads the status words, and while stamps were dropped
-// for lack of room grows the table and re-runs the pending batches stamps-only (idempotent: atomicMax).  Afterwards
-// nothing is pending.  Also grows ahead of need once the table is more than 70 % full.
+// re-runs the pending batches stamps-only (idempotent: atomicMax).  Afterwards nothing is pending.
+//   * If the table would stay at most 60 % full even were every dropped stamp a new key, the drops are a probe-limit
+//     artefact: keys whose mixed hashes lie close together share a home pair at every table size, and a crafted run of
+//     a few hundred of them would otherwise double the table up to its 32 GiB cap.  The re-run keeps the table and
+//     lets the probe run over all of it; a linear probe in a table at most 60 % full always reaches an empty slot.
+//   * Otherwise the table is grown first.  It is also grown ahead of need once it is more than 60 % full.
 static int alive_check(kta_handle *h) {
     if (!h->d_alive_table) return KTA_OK;
     cudaStream_t s = h->stream;
@@ -541,24 +545,29 @@ static int alive_check(kta_handle *h) {
         const uint64_t slots = (uint64_t)h->alive_pairs * 2;
         const bool crowded = occupied * 10 > slots * 6;
         if (!dropped && !crowded) break;
-        if (h->alive_pairs >= (uint32_t)ALIVE_MAX_KIB * 64u) {
-            if (dropped) return fail(KTA_ERR_NOMEM, "alive-key table is at its maximum (32 GiB) and still too full");
-            break;
-        }
-        // at least double; enough for every known entry plus every dropped stamp at load <= 0.5
-        uint64_t want = slots * 2;
-        while (want < (occupied + dropped) * 2) want *= 2;
-        want = std::min<uint64_t>(want, (uint64_t)ALIVE_MAX_KIB * 128ull);
+        const bool wide = dropped && (occupied + dropped) * 10 <= slots * 6;
         int rc;
-        if ((rc = alive_grow(h, (uint32_t)(want / 2)))) return rc;
-        if (!dropped) break;   // grown ahead of need: every pending stamp had landed
+        if (!wide) {
+            if (h->alive_pairs >= (uint32_t)ALIVE_MAX_KIB * 64u) {
+                if (dropped) return fail(KTA_ERR_NOMEM, "alive-key table is at its maximum (32 GiB) and still too full");
+                break;
+            }
+            // at least double; enough for every known entry plus every dropped stamp at load <= 0.5
+            uint64_t want = slots * 2;
+            while (want < (occupied + dropped) * 2) want *= 2;
+            want = std::min<uint64_t>(want, (uint64_t)ALIVE_MAX_KIB * 128ull);
+            if ((rc = alive_grow(h, (uint32_t)(want / 2)))) return rc;
+            if (!dropped) break;   // grown ahead of need: every pending stamp had landed
+        }
         if (round > 40) return fail(KTA_ERR_INVALID, "alive-key table growth did not converge");
+        if (wide) CU(cudaMemsetAsync(h->d_alive_status + 2, 0xff, 4, s));
         for (const PendingScan &ps : h->pending) {
             ScanParams prm = ps.prm;
             prm.alive_only = 1;
             if ((rc = launch_scan_raw(h, prm, ps.key_readable, ps.key_bytes))) return rc;
             h->alive_reruns++;
         }
+        if (wide) CU(cudaMemsetAsync(h->d_alive_status + 2, 0, 4, s));
     }
     h->pending.clear();
     return KTA_OK;
@@ -1525,20 +1534,26 @@ extern "C" int kta_alive_import_device(kta_handle *h, const uint32_t *dev_hash, 
     if ((rc = set_device(h))) return rc;
     if ((rc = alive_check(h))) return rc;   // nothing pending: a re-run below only concerns the imported stamps
     const int grid = (int)std::min<int64_t>((count + THREADS - 1) / THREADS, (int64_t)h->sm_count * 8);
+    bool wide = false;
     for (int round = 0;; round++) {
         const AliveTable t{h->d_alive_table, h->alive_pairs, h->d_alive_status, 0};
+        if (wide) CU(cudaMemsetAsync(h->d_alive_status + 2, 0xff, 4, h->stream));
         alive_import_kernel<<<grid, THREADS, 0, h->stream>>>(t, h->alive_origin, dev_hash,
                                                              reinterpret_cast<const unsigned long long *>(dev_stamp), count);
         h->launches++;
         CU(cudaGetLastError());
+        if (wide) CU(cudaMemsetAsync(h->d_alive_status + 2, 0, 4, h->stream));
         // the imported list is the caller's and still valid: if the table was too small, alive_check grew it (nothing
         // is pending, so it re-ran nothing) and the import is simply applied again — stamping is idempotent
         CU(cudaMemcpyAsync(h->h_alive_status, h->d_alive_status, 8, cudaMemcpyDeviceToHost, h->stream));
         CU(cudaStreamSynchronize(h->stream));
         const bool dropped = h->h_alive_status[0] != 0;
+        const uint32_t pairs = h->alive_pairs;
         if ((rc = alive_check(h))) return rc;
         if (!dropped) break;
         if (round > 40) return fail(KTA_ERR_INVALID, "alive-key table growth did not converge");
+        // a table that alive_check did not grow had room for every dropped stamp: probe up to the whole of it (see there)
+        wide = h->alive_pairs == pairs;
     }
     h->finalized = false;
     return KTA_OK;

@@ -105,15 +105,16 @@ struct ScanParams {
                                      // table), [1..HLL_SLICES] per-slice minima it is derived from
     unsigned long long *alive_table; // [2 * alive_pairs] stamps: hash(32) | seq - alive_origin + 1 (31) | alive(1); ~0 = empty
     uint32_t alive_pairs;            // table size in 16-byte pairs of slots (any value >= 1, not only powers of two)
-    int32_t alive_only;              // 1: MODE_EXACT re-run after the table grew — stamps only, no counters / extrema
+    int32_t alive_only;              // 1: MODE_EXACT re-run after stamps were dropped — stamps only, no counters / extrema
     uint64_t alive_origin;           // seq that field value 1 stands for (moved forward by a rebase)
     uint64_t alive_fbase;            // seq_base - alive_origin + 1: the field of record 0 when seq is implicit
     unsigned long long *alive_count; // scratch u64 words: [0] alive entries, [1] export cursor, [2] occupied slots (count kernels)
     uint32_t *alive_cache;           // [2^ALIVE_CACHE_SET_BITS] seen cache of this batch (cleared by the host before the launch), or NULL
     int32_t alive_wave_shift;        // wave of a record = 1 + min((field - alive_wave_base) >> alive_wave_shift, 126): a monotone
     uint32_t alive_wave_base;        //   function of seq (field = seq - origin + 1); base = the field of the batch's first record
-    uint32_t *alive_status;          // [0] stamps that found no slot (table too full: host grows it and re-runs the
-                                     //     batch), [1] records whose seq lies outside the 31-bit window of the table
+    uint32_t *alive_status;          // [0] stamps that found no slot (host grows the table or widens the probe and re-runs
+                                     //     the batch), [1] records whose seq lies outside the 31-bit window of the table,
+                                     //     [2] != 0: a wide re-run, probes may cover the whole table (set by the host)
     uint32_t *hash_out;              // per-record hash capture (CAPTURE kernels only; test hook), 0 for null keys
 };
 
@@ -505,7 +506,9 @@ struct Counters {
 //   * 31 bits of seq: when a batch would not fit the window the host REBASES (every entry keeps hash and alive bit, its
 //     seq field drops to 0: older than everything that follows, which is all a later record needs to know).
 //   * A stamp that finds neither its hash nor an empty slot within ALIVE_MAX_PROBES pairs is counted in status[0] and
-//     dropped; the host then grows the table (rehash) and re-runs the batch stamps-only — stamping is idempotent.
+//     dropped; the host then grows the table (rehash) and re-runs the batch stamps-only — stamping is idempotent.  If
+//     the table has room for every dropped stamp, the drops came from keys whose mixed hashes lie close together: they
+//     share a home pair at every table size, so instead of growing, the re-run probes up to the whole table.
 //
 // The SEEN CACHE in front of it.  A table of 128 MiB or more does not stay in L2 next to a multi-GB record stream, so
 // a table probe per record is a random DRAM sector per record.  But 90–99 % of the
@@ -521,7 +524,7 @@ struct Counters {
 // ------------------------------------------------------------------------------------------------
 constexpr unsigned long long ALIVE_EMPTY = ~0ull;
 constexpr uint32_t ALIVE_FIELD_MAX = 0x7ffffffeu;   // largest seq field: a stamp's low word is <= 0xfffffffd, never ~0
-constexpr int ALIVE_MAX_PROBES = 96;                // pairs examined before a stamp gives up
+constexpr int ALIVE_MAX_PROBES = 96;                // pairs examined before a stamp gives up (outside a wide re-run)
 
 #ifndef KTA_L2_HINTS
 #define KTA_L2_HINTS 1
@@ -588,29 +591,45 @@ __device__ __forceinline__ void alive_red_max(unsigned long long *p, unsigned lo
 #endif
 }
 
-// The general stamp: probe from `pair` until the hash or an empty slot is found.  Returns the low word of the newest
+// One pair of a probe: true once the hash or an empty slot is found there, with `newest` = the low word of the newest
 // stamp known for this hash afterwards (the record's own if it won).
-__device__ __noinline__ uint32_t alive_stamp_slow(const AliveTable t, uint32_t pair, uint32_t hash, uint32_t low) {
+__device__ __forceinline__ bool alive_probe_pair(const AliveTable t, uint32_t pair, uint32_t hash, uint32_t low, uint32_t &newest) {
     const unsigned long long stamp = ((unsigned long long)hash << 32) | low;
-    for (int probe = 0; probe < ALIVE_MAX_PROBES; probe++) {
-        unsigned long long *slot = t.slots + 2 * (size_t)pair;
-        const ulonglong2 e = alive_ld_pair(slot, t.pol);
+    unsigned long long *slot = t.slots + 2 * (size_t)pair;
+    const ulonglong2 e = alive_ld_pair(slot, t.pol);
+    newest = low;
 #pragma unroll
-        for (int s = 0; s < 2; s++) {
-            unsigned long long v = s ? e.y : e.x;
-            if (v == ALIVE_EMPTY) {
-                v = atomicCAS(slot + s, ALIVE_EMPTY, stamp);
-                if (v == ALIVE_EMPTY) return low;                   // first record of this hash: mark_key_alive / _dead on a fresh bit
-            }
-            if ((uint32_t)(v >> 32) == hash) {                      // v is a real entry here (never ALIVE_EMPTY)
-                if (v >= stamp) return (uint32_t)v;                 // a later record already spoke for this hash
-                alive_red_max(slot + s, stamp, t.pol);
-                return low;
-            }
+    for (int s = 0; s < 2; s++) {
+        unsigned long long v = s ? e.y : e.x;
+        if (v == ALIVE_EMPTY) {
+            v = atomicCAS(slot + s, ALIVE_EMPTY, stamp);
+            if (v == ALIVE_EMPTY) return true;                      // first record of this hash: mark_key_alive / _dead on a fresh bit
         }
+        if ((uint32_t)(v >> 32) == hash) {                          // v is a real entry here (never ALIVE_EMPTY)
+            if (v >= stamp) newest = (uint32_t)v;                   // a later record already spoke for this hash
+            else alive_red_max(slot + s, stamp, t.pol);
+            return true;
+        }
+    }
+    return false;
+}
+
+// The general stamp: probe from `pair` until the hash or an empty slot is found.  Returns the low word of the newest
+// stamp known for this hash afterwards (the record's own if it won).  A stamp gives up after ALIVE_MAX_PROBES pairs,
+// unless the host has flagged a wide re-run (status[2], see alive_check): then it goes on over the rest of the table.
+__device__ __noinline__ uint32_t alive_stamp_slow(const AliveTable t, uint32_t pair, uint32_t hash, uint32_t low) {
+    uint32_t newest;
+    for (int probe = 0; probe < ALIVE_MAX_PROBES; probe++) {
+        if (alive_probe_pair(t, pair, hash, low, newest)) return newest;
         pair = pair + 1 == t.npairs ? 0 : pair + 1;
     }
-    atomicAdd(t.status, 1u);   // table too full: the host grows it and re-runs this batch's stamps
+    if (__ldcg(t.status + 2)) {
+        for (uint32_t probe = ALIVE_MAX_PROBES; probe < t.npairs; probe++) {
+            if (alive_probe_pair(t, pair, hash, low, newest)) return newest;
+            pair = pair + 1 == t.npairs ? 0 : pair + 1;
+        }
+    }
+    atomicAdd(t.status, 1u);   // table too full, or a long run of nearby hashes: the host re-runs this batch's stamps
     return low;
 }
 

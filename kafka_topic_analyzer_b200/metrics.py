@@ -61,7 +61,7 @@ class KtaEngine:
         cfg.num_partitions = num_partitions
         cfg.count_alive_keys = 1 if count_alive_keys else 0
         cfg.hll_precision = hll_precision
-        cfg.alive_table_kib = alive_table_kib   # initial size of the alive-key table (0 = 128 MiB); it grows on demand
+        cfg.alive_table_kib = alive_table_kib   # initial size of the alive-key table (0 = 256 MiB); it grows on demand
         cfg.ring_records = ring_records
         cfg.ring_key_bytes = ring_key_bytes
         if shard is not None:
