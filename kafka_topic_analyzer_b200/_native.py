@@ -45,16 +45,15 @@ def build_synth(force: bool = False) -> str:
     return SYNTH_LIB_PATH
 
 
-def build(force: bool = False, verbose: bool = False, defines=(), out: str = None) -> str:
-    """Compile libkta_gpu.so for sm_90a (H100) with nvcc (cross-compiles without a GPU).
-    `defines` / `out` build an experimental variant next to it (tuning runs; KTA_LIB selects it)."""
-    out = out or LIB_PATH
+def build(force: bool = False, verbose: bool = False) -> str:
+    """Compile libkta_gpu.so for sm_90a (H100) with nvcc (cross-compiles without a GPU)."""
+    out = LIB_PATH
     if not force and os.path.exists(out):
         newest = max(os.path.getmtime(p) for p in _sources())
         if os.path.getmtime(out) >= newest:
             return out
     nvcc = os.environ.get("NVCC") or "/usr/local/cuda/bin/nvcc"
-    cmd = [nvcc, *NVCC_FLAGS, *["-D" + d for d in defines], "-o", out, os.path.join(CSRC, "kta_lib.cu")]
+    cmd = [nvcc, *NVCC_FLAGS, "-o", out, os.path.join(CSRC, "kta_lib.cu")]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
     res = subprocess.run(cmd, capture_output=True, text=True)

@@ -61,7 +61,7 @@ extern "C" int kta_device_count(void) {
 // handle
 // ------------------------------------------------------------------------------------------------
 static constexpr int NCHUNK = 3;
-static constexpr int32_t ALIVE_DEFAULT_KIB = 256 * 1024;       // initial alive-key table: 256 MiB = 2^25 slots (KTA_ALIVE_TABLE_KIB overrides: tuning)
+static constexpr int32_t ALIVE_DEFAULT_KIB = 256 * 1024;       // initial alive-key table: 256 MiB = 2^25 slots
 static constexpr int32_t ALIVE_MAX_KIB = 32 * 1024 * 1024;     // 32 GiB = one slot per possible 32-bit hash
 static constexpr int64_t ALIVE_CACHE_MIN_RECORDS = 1 << 20;    // smaller batches go straight to the table
 static constexpr int64_t DEFAULT_RING_RECORDS = 1 << 22;  // 4 Mi records per chunk
@@ -209,46 +209,49 @@ static void scan_shape(const kta_handle *h, bool hash, bool hdr_ok, int64_t n, i
         }
         return false;
     };
-    if (hdr_ok && HDR_BYTES > 0 && (fits(true, SCAN_STAGES, 12, 10) || fits(true, 2, 12, 10))) return;
+    if (hdr_ok && (fits(true, SCAN_STAGES, 12, 10) || fits(true, 2, 12, 10))) return;
     if (fits(false, 2, 16, 8)) return;
     keybuf = KEYBUF_MIN;
     fits(false, 2, 16, 1);
 }
 
-// one persistent CTA per SM; every variant may use the whole opt-in shared memory (the shape is chosen per launch).
-// variant index: 0 counters, 1 HLL, 2 exact, 3 HLL+capture, 4 exact+capture, 5..7 = 0..2 for a partition-sharded handle
-template <int MODE, bool SMEM, bool CAPTURE, bool SHARD>
-static int prepare_variant(kta_handle *h) {
-    CU(cudaFuncSetAttribute(scan_kernel<MODE, SMEM, CAPTURE, SHARD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+// Every scan_kernel instance the library launches, [counters in shared memory][partition-sharded][mode][capture].
+// Hash capture is a test hook of unsharded hashing handles; the other slots are empty.  One persistent CTA per SM;
+// every instance may use the whole opt-in shared memory (the shape is chosen per launch).
+using ScanFn = void (*)(ScanParams);
+static const ScanFn SCAN_KERNELS[2][2][3][2] = {
+    {{{scan_kernel<MODE_COUNTERS, false, false, false>, nullptr},
+      {scan_kernel<MODE_HLL, false, false, false>, scan_kernel<MODE_HLL, false, true, false>},
+      {scan_kernel<MODE_EXACT, false, false, false>, scan_kernel<MODE_EXACT, false, true, false>}},
+     {{scan_kernel<MODE_COUNTERS, false, false, true>, nullptr},
+      {scan_kernel<MODE_HLL, false, false, true>, nullptr},
+      {scan_kernel<MODE_EXACT, false, false, true>, nullptr}}},
+    {{{scan_kernel<MODE_COUNTERS, true, false, false>, nullptr},
+      {scan_kernel<MODE_HLL, true, false, false>, scan_kernel<MODE_HLL, true, true, false>},
+      {scan_kernel<MODE_EXACT, true, false, false>, scan_kernel<MODE_EXACT, true, true, false>}},
+     {{scan_kernel<MODE_COUNTERS, true, false, true>, nullptr},
+      {scan_kernel<MODE_HLL, true, false, true>, nullptr},
+      {scan_kernel<MODE_EXACT, true, false, true>, nullptr}}},
+};
+
+template <typename T>
+static int alloc_elems(T *&ptr, int64_t n) {
+    CU(cudaMalloc(&ptr, (size_t)n * sizeof(T)));
     return KTA_OK;
 }
-
-template <bool SMEM>
-static int prepare_all(kta_handle *h) {
-    int rc;
-    if ((rc = prepare_variant<MODE_COUNTERS, SMEM, false, false>(h))) return rc;
-    if ((rc = prepare_variant<MODE_HLL, SMEM, false, false>(h))) return rc;
-    if ((rc = prepare_variant<MODE_EXACT, SMEM, false, false>(h))) return rc;
-    if ((rc = prepare_variant<MODE_HLL, SMEM, true, false>(h))) return rc;
-    if ((rc = prepare_variant<MODE_EXACT, SMEM, true, false>(h))) return rc;
-    if ((rc = prepare_variant<MODE_COUNTERS, SMEM, false, true>(h))) return rc;
-    if ((rc = prepare_variant<MODE_HLL, SMEM, false, true>(h))) return rc;
-    if ((rc = prepare_variant<MODE_EXACT, SMEM, false, true>(h))) return rc;
+// (Re)allocates device buffers that share one capacity, in elements, when `need` exceeds it.
+template <typename... T>
+static int grow(cudaStream_t s, int64_t &cap, int64_t need, T *&...bufs) {
+    if (need <= cap) return KTA_OK;
+    CU(cudaStreamSynchronize(s));   // queued work may still read the old buffers
+    ((cudaFree(bufs), bufs = nullptr), ...);
+    cap = 0;
+    const int64_t n = need + need / 4 + 64;
+    int rc = KTA_OK;
+    ((rc = rc ? rc : alloc_elems(bufs, n)), ...);
+    if (rc) return rc;
+    cap = n;
     return KTA_OK;
-}
-
-template <bool SMEM>
-static void launch_variant(int v, int grid, int threads, size_t sm, cudaStream_t st, const ScanParams &prm) {
-    switch (v) {
-        case 0: scan_kernel<MODE_COUNTERS, SMEM, false><<<grid, threads, sm, st>>>(prm); break;
-        case 1: scan_kernel<MODE_HLL, SMEM, false><<<grid, threads, sm, st>>>(prm); break;
-        case 2: scan_kernel<MODE_EXACT, SMEM, false><<<grid, threads, sm, st>>>(prm); break;
-        case 3: scan_kernel<MODE_HLL, SMEM, true><<<grid, threads, sm, st>>>(prm); break;
-        case 4: scan_kernel<MODE_EXACT, SMEM, true><<<grid, threads, sm, st>>>(prm); break;
-        case 5: scan_kernel<MODE_COUNTERS, SMEM, false, true><<<grid, threads, sm, st>>>(prm); break;
-        case 6: scan_kernel<MODE_HLL, SMEM, false, true><<<grid, threads, sm, st>>>(prm); break;
-        default: scan_kernel<MODE_EXACT, SMEM, false, true><<<grid, threads, sm, st>>>(prm); break;
-    }
 }
 
 static int state_reset_device(kta_handle *h) {
@@ -341,8 +344,7 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
         // every third first-seen key finds its home pair taken and probes on; the table does not fit L2 at either size)
         if (cfg->alive_table_kib < 0 || cfg->alive_table_kib > ALIVE_MAX_KIB)
             return fail(KTA_ERR_INVALID, "alive_table_kib %d out of range [0, %d]", cfg->alive_table_kib, ALIVE_MAX_KIB);
-        static const int64_t env_kib = [] { const char *e = getenv("KTA_ALIVE_TABLE_KIB"); return e ? atoll(e) : 0ll; }();   // tuning knob
-        const int64_t kib = cfg->alive_table_kib ? cfg->alive_table_kib : env_kib > 0 ? env_kib : ALIVE_DEFAULT_KIB;
+        const int64_t kib = cfg->alive_table_kib ? cfg->alive_table_kib : ALIVE_DEFAULT_KIB;
         h->alive_pairs = (uint32_t)std::max<int64_t>(kib * 64, 16);   // 16 bytes per pair
         CU(cudaMalloc(&h->d_alive_table, (size_t)h->alive_pairs * 16));
         CU(cudaMalloc(&h->d_alive_status, 12));
@@ -359,8 +361,11 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
     h->columns = (P - h->shard_rank + h->shard_world - 1) / h->shard_world;   // partitions p < P with p % world == rank
     // counters in shared memory as long as at least 8 warps of 2 smallest key-only stages still fit beside them
     h->smem_counters = smem_counter_bytes(h->columns) + 8 * warp_smem_bytes(true, KEYBUF_MIN, 2, false) <= h->smem_optin;
+    for (const auto &by_mode : SCAN_KERNELS[h->smem_counters])
+        for (const auto &by_capture : by_mode)
+            for (const ScanFn f : by_capture)
+                if (f) CU(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
     int rc;
-    if ((rc = h->smem_counters ? prepare_all<true>(h) : prepare_all<false>(h))) return rc;
     if ((rc = state_reset_device(h))) return rc;
     CU(cudaStreamSynchronize(h->stream));
     return KTA_OK;
@@ -426,16 +431,14 @@ static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, 
     prm.alive_table = h->d_alive_table;
     prm.alive_pairs = h->alive_pairs;
     prm.alive_origin = h->alive_origin;
-    prm.alive_count = h->d_scalar;
     prm.alive_status = h->d_alive_status;
     prm.alive_cache = nullptr;
     if (exact && prm.n >= ALIVE_CACHE_MIN_RECORDS) {
         // the seen cache pays for its clearing (a 32 MiB memset) on batches of a million records and more.
         // Waves cut the batch's seq range [lo, hi] into <= 127 equal slices (any monotone function of seq will do).
-        static const bool off = getenv("KTA_ALIVE_NO_CACHE") != nullptr;   // tuning / ablation knob
         uint64_t lo = prm.seq_base, hi = prm.seq_base + (uint64_t)prm.n - 1;
-        bool ok = !off;
-        if (ok && prm.seq) {
+        bool ok = true;
+        if (prm.seq) {
             // explicit sequence numbers: the range is read off the column's ends (records of a batch are in seq order; a
             // record outside the range just lands in the first or last wave)
             uint64_t ends[2];
@@ -465,7 +468,6 @@ static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, 
         prm.stage_limit = (((uintptr_t)prm.key_bytes & 15u) == 0) ? ((uint64_t)key_readable & ~15ull) : 0;
     }
     if (capture && h->shard_world > 1) return fail(KTA_ERR_INVALID, "hash capture is not available on a partition-sharded handle");
-    const int variant = h->shard_world > 1 ? 5 + mode : mode + (capture ? 2 : 0);
     int threads = 0, keybuf = 0, stages = 0;
     bool hdr = false;
     size_t sm = 0;
@@ -489,8 +491,7 @@ static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, 
         h->ev_used++;
         CU(cudaEventRecord(e0, h->stream));
     }
-    if (h->smem_counters) launch_variant<true>(variant, grid, threads, sm, h->stream, prm);
-    else launch_variant<false>(variant, grid, threads, sm, h->stream, prm);
+    SCAN_KERNELS[h->smem_counters][h->shard_world > 1][mode][capture]<<<grid, threads, sm, h->stream>>>(prm);
     CU(cudaGetLastError());
     h->launches++;
     if (h->timing) CU(cudaEventRecord(e1, h->stream));
@@ -686,15 +687,7 @@ extern "C" int kta_scan_batch_device(kta_handle *h, const kta_batch *b) {
     prm.key_tile_base = b->key_tile_base;
     if ((h->need_hash || h->d_hash_out) && !prm.key_tile_base) {
         const int64_t ntiles = (b->n + TILE - 1) / TILE;
-        if (ntiles + 1 > h->tb_scratch_tiles) {
-            // stream-ordered: earlier scans that still read the old scratch finish first
-            CU(cudaStreamSynchronize(h->stream));
-            cudaFree(h->d_tb_scratch);
-            h->d_tb_scratch = nullptr;
-            h->tb_scratch_tiles = 0;
-            CU(cudaMalloc(&h->d_tb_scratch, (size_t)(ntiles + 1) * 8));
-            h->tb_scratch_tiles = ntiles + 1;
-        }
+        if ((rc = grow(h->stream, h->tb_scratch_tiles, ntiles + 1, h->d_tb_scratch))) return rc;
         if ((rc = derive_tile_base(h, b->key_len, b->n, h->d_tb_scratch))) return rc;
         prm.key_tile_base = h->d_tb_scratch;
     }
@@ -707,19 +700,6 @@ extern "C" int kta_scan_batch_device(kta_handle *h, const kta_batch *b) {
 // Kafka RecordBatch v2 segments → SoA → scan (SURVEY.md §8 f2; kernels in kta_logdecode.cuh)
 // ------------------------------------------------------------------------------------------------
 
-template <typename T>
-static int grow(T *&ptr, int64_t &cap, int64_t need, cudaStream_t s) {
-    if (need <= cap) return KTA_OK;
-    CU(cudaStreamSynchronize(s));   // queued work may still read the old buffer
-    cudaFree(ptr);
-    ptr = nullptr;
-    cap = 0;
-    const int64_t n = need + need / 4 + 64;
-    CU(cudaMalloc(&ptr, (size_t)n * sizeof(T)));
-    cap = n;
-    return KTA_OK;
-}
-
 static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes,
                             int64_t len, int64_t readable /* bytes of dev_bytes that may be READ (>= len when the buffer has slack) */,
                             const uint64_t *dev_batch_off, int64_t nbatches, int64_t *records_out) {
@@ -731,15 +711,7 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     if ((rc = ring_flush(h))) return rc;   // keep seq order with records pushed earlier
     if (!h->pending.empty() && (rc = alive_check(h))) return rc;   // the decode scratch of an earlier call is about to be reused
     cudaStream_t s = h->stream;
-    if (nbatches + 1 > h->log_batch_cap) {
-        CU(cudaStreamSynchronize(s));
-        cudaFree(h->d_log_info); cudaFree(h->d_log_cnt);
-        h->d_log_info = nullptr; h->d_log_cnt = nullptr; h->log_batch_cap = 0;
-        const int64_t n = nbatches + nbatches / 4 + 64;
-        CU(cudaMalloc(&h->d_log_info, (size_t)n * sizeof(LogBatchInfo)));
-        CU(cudaMalloc(&h->d_log_cnt, (size_t)n * 8));
-        h->log_batch_cap = n;
-    }
+    if ((rc = grow(s, h->log_batch_cap, nbatches + 1, h->d_log_info, h->d_log_cnt))) return rc;
     if (!h->d_log_err) CU(cudaMalloc(&h->d_log_err, 8));   // [0] error flags, [1] longest batch
     CU(cudaMemsetAsync(h->d_log_err, 0, 8, s));
     const int grid = (int)std::min<int64_t>((nbatches + 127) / 128, (int64_t)h->sm_count * 16);
@@ -760,7 +732,7 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     if (err[0] & LOGB_CODECS) {
         // compressed batches: size pass, scratch allocation, decompression; afterwards they are ordinary batches that
         // happen to lie in the scratch buffer
-        if ((rc = grow(h->d_unc_slot, h->unc_slot_cap, nbatches + 2, s))) return rc;
+        if ((rc = grow(s, h->unc_slot_cap, nbatches + 2, h->d_unc_slot))) return rc;
         CU(cudaMemsetAsync(h->d_log_err, 0, 4, s));
         log_unc_size_kernel<<<grid, 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_log_err);
         tile_base_scan_kernel<<<1, 1024, 0, s>>>(h->d_unc_slot, nbatches);
@@ -771,7 +743,7 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
         CU(cudaMemcpyAsync(err, h->d_log_err, 4, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         if (err[0]) return fail(KTA_ERR_INVALID, "malformed compressed record batch in partition %d", partition);
-        if ((rc = grow(h->d_unc, h->unc_cap, (int64_t)unc_total + 64, s))) return rc;
+        if ((rc = grow(s, h->unc_cap, (int64_t)unc_total + 64, h->d_unc))) return rc;
         log_decompress_kernel<<<(int)std::min<int64_t>((nbatches + 3) / 4, (int64_t)h->sm_count * 16), 128, 0, s>>>(
             dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_unc, h->d_log_err);
         CU(cudaGetLastError());
@@ -779,18 +751,8 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     }
     if ((int64_t)nrec >= ((int64_t)1 << 31) - 2) return fail(KTA_ERR_INVALID, "%llu records in one call: split the segments", (unsigned long long)nrec);
     const bool hash = h->need_hash || h->d_hash_out;
-    if ((int64_t)nrec > h->dec_rec_cap) {
-        CU(cudaStreamSynchronize(s));
-        cudaFree(h->d_dec_part); cudaFree(h->d_dec_klen); cudaFree(h->d_dec_vlen); cudaFree(h->d_dec_ts); cudaFree(h->d_dec_ksrc);
-        h->d_dec_part = h->d_dec_klen = h->d_dec_vlen = nullptr; h->d_dec_ts = nullptr; h->d_dec_ksrc = nullptr; h->dec_rec_cap = 0;
-        const int64_t n = (int64_t)nrec + (int64_t)nrec / 4 + 1024;
-        CU(cudaMalloc(&h->d_dec_part, (size_t)n * 4));
-        CU(cudaMalloc(&h->d_dec_klen, (size_t)n * 4));
-        CU(cudaMalloc(&h->d_dec_vlen, (size_t)n * 4));
-        CU(cudaMalloc(&h->d_dec_ts, (size_t)n * 8));
-        CU(cudaMalloc(&h->d_dec_ksrc, (size_t)n * 8));
-        h->dec_rec_cap = n;
-    }
+    if ((rc = grow(s, h->dec_rec_cap, (int64_t)nrec, h->d_dec_part, h->d_dec_klen, h->d_dec_vlen, h->d_dec_ts, h->d_dec_ksrc)))
+        return rc;
     // one warp per batch; the batch is staged in shared memory when the longest one fits a stage of <= 48 KiB
     const uint32_t maxlen = err[1];
     const uint32_t stage = (uint32_t)(((size_t)maxlen + 16 + 1023) / 1024 * 1024);
@@ -822,21 +784,14 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     if (hash) {
         // pack the keys in record order: tile bases from the key_len column, then one gather pass (no second walk of the log)
         const int64_t ntiles = ((int64_t)nrec + TILE - 1) / TILE;
-        if (ntiles + 1 > h->tb_scratch_tiles) {
-            CU(cudaStreamSynchronize(s));
-            cudaFree(h->d_tb_scratch);
-            h->d_tb_scratch = nullptr;
-            h->tb_scratch_tiles = 0;
-            CU(cudaMalloc(&h->d_tb_scratch, (size_t)(ntiles + 1) * 8));
-            h->tb_scratch_tiles = ntiles + 1;
-        }
+        if ((rc = grow(s, h->tb_scratch_tiles, ntiles + 1, h->d_tb_scratch))) return rc;
         if ((rc = derive_tile_base(h, h->d_dec_klen, (int64_t)nrec, h->d_tb_scratch))) return rc;
         uint64_t nkey = 0;
         CU(cudaMemcpyAsync(&nkey, h->d_tb_scratch + ntiles, 8, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(err, h->d_log_err, 8, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         if (err[0]) return fail(KTA_ERR_INVALID, "malformed record inside a batch of partition %d", partition);
-        if ((rc = grow(h->d_dec_keys, h->dec_key_cap, (int64_t)nkey + 64, s))) return rc;
+        if ((rc = grow(s, h->dec_key_cap, (int64_t)nkey + 64, h->d_dec_keys))) return rc;
         log_gather_keys_kernel<<<(int)std::min<int64_t>((ntiles + 7) / 8, (int64_t)h->sm_count * 8), 256, 0, s>>>(
             dev_bytes, h->d_dec_ksrc, h->d_dec_klen, (int64_t)nrec, h->d_tb_scratch, h->d_dec_keys);
         CU(cudaGetLastError());
@@ -895,7 +850,7 @@ extern "C" int kta_push_log_segments_host(kta_handle *h, int32_t nsegs, const in
     int rc;
     if ((rc = set_device(h))) return rc;
     cudaStream_t s = h->stream;
-    if ((rc = grow(h->d_log_bytes, h->log_bytes_cap, total + 64, s))) return rc;
+    if ((rc = grow(s, h->log_bytes_cap, total + 64, h->d_log_bytes))) return rc;
     CU(cudaStreamSynchronize(s));
     cudaFree(h->d_log_off);
     h->d_log_off = nullptr;
@@ -966,6 +921,19 @@ static void push_cursor_bind(kta_handle *h) {
     pc.hash = h->need_hash || h->d_hash_out;
 }
 
+// scan the columns staged in ring chunk `cur`, snapshot the alive-table status words right after that scan, and
+// move on to the next chunk
+static int ring_scan_chunk(kta_handle *h, const ScanParams &prm, int64_t key_readable, int64_t key_bytes,
+                           const uint64_t *seq_ends = nullptr) {
+    Chunk &c = h->chunks[h->cur];
+    int rc;
+    if ((rc = launch_scan(h, prm, key_readable, key_bytes, h->cur, seq_ends))) return rc;
+    if (h->d_alive_table) CU(cudaMemcpyAsync(c.h_status, h->d_alive_status, 8, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaEventRecord(c.free_ev, h->stream));
+    h->cur = (h->cur + 1) % NCHUNK;
+    return KTA_OK;
+}
+
 // stage one pinned chunk and scan it
 static int ring_flush(kta_handle *h) {
     if (h->pc.n == 0) return KTA_OK;
@@ -992,11 +960,8 @@ static int ring_flush(kta_handle *h) {
     prm.key_bytes = c.d_keys;
     prm.key_tile_base = c.d_tile_base;
     int rc;
-    if ((rc = launch_scan(h, prm, (kb + 15) & ~(int64_t)15, kb, h->cur))) return rc;
+    if ((rc = ring_scan_chunk(h, prm, (kb + 15) & ~(int64_t)15, kb))) return rc;
     h->next_seq += (uint64_t)n;
-    if (h->d_alive_table) CU(cudaMemcpyAsync(c.h_status, h->d_alive_status, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaEventRecord(c.free_ev, s));
-    h->cur = (h->cur + 1) % NCHUNK;
     push_cursor_bind(h);
     // the next chunk may still be in flight from NCHUNK flushes ago
     CU(cudaEventSynchronize(h->chunks[h->cur].free_ev));
@@ -1138,10 +1103,7 @@ extern "C" int kta_push_batch_host(kta_handle *h, const kta_batch *b) {
         prm.value_len = c.d_vlen;
         prm.seq = use_seq ? c.d_seq : nullptr;
         const uint64_t seq_ends[2] = {use_seq ? b->seq[r0] : 0, use_seq ? b->seq[r0 + cn - 1] : 0};
-        if ((rc = launch_scan(h, prm, (int64_t)((k1 + 15) & ~15ull), (int64_t)(k1 - k0), ci, use_seq ? seq_ends : nullptr))) return rc;
-        if (h->d_alive_table) CU(cudaMemcpyAsync(c.h_status, h->d_alive_status, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaEventRecord(c.free_ev, s));
-        h->cur = (h->cur + 1) % NCHUNK;
+        if ((rc = ring_scan_chunk(h, prm, (int64_t)((k1 + 15) & ~15ull), (int64_t)(k1 - k0), use_seq ? seq_ends : nullptr))) return rc;
         koff = k1;
         r0 += cn;
     }

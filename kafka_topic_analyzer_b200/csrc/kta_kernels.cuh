@@ -21,15 +21,9 @@
 
 namespace kta {
 
-#ifndef KTA_SCAN_THREADS
-#define KTA_SCAN_THREADS 1024
-#endif
-constexpr int MAX_THREADS = KTA_SCAN_THREADS;  // one persistent CTA per SM, up to 32 autonomous warps
+constexpr int MAX_THREADS = 1024;  // one persistent CTA per SM, up to 32 autonomous warps
 // The hashing modes run at most 16 warps per SM (see scan_shape), which leaves each thread 128 registers.
-#ifndef KTA_HASH_THREADS
-#define KTA_HASH_THREADS 512
-#endif
-constexpr int HASH_MAX_THREADS = KTA_HASH_THREADS;
+constexpr int HASH_MAX_THREADS = 512;
 constexpr int TILE = KTA_KEY_TILE;        // records per warp tile (128)
 constexpr int ROWS = TILE / 32;           // records per lane per tile
 constexpr int NB = KTA_HIST_BUCKETS;      // 32 log2 buckets
@@ -42,15 +36,8 @@ constexpr int NB = KTA_HIST_BUCKETS;      // 32 log2 buckets
 constexpr int KEYBUF_MIN = TILE * 18 + 32, KEYBUF_MAX = TILE * 128 + 32, KEYBUF_SLACK = 32;
 // header slices of one tile in a stage: partition (4 B) | ts_ms (8 B) | key_len (4 B) | value_len (4 B) per record
 constexpr int HDR_P = 0, HDR_TS = TILE * 4, HDR_KL = TILE * 12, HDR_VL = TILE * 16;
-#ifndef KTA_EXP_NO_HDR   // ablation knob: stages hold key bytes only, every tile loads its headers from global memory
 constexpr int HDR_BYTES = TILE * 20;
-#else
-constexpr int HDR_BYTES = 0;
-#endif
-#ifndef KTA_SCAN_STAGES
-#define KTA_SCAN_STAGES 3
-#endif
-constexpr int SCAN_STAGES = KTA_SCAN_STAGES;   // stages per warp in the hashing modes (see scan_shape)
+constexpr int SCAN_STAGES = 3;   // stages per warp in the hashing modes (see scan_shape)
 // the descriptors of the tiles in flight are packed one byte per stage into a 32-bit register; the mbarriers sit at
 // +0..31 of the warp's 128 bytes, its scratch at +64
 constexpr int MAX_STAGES = 4;
@@ -108,7 +95,6 @@ struct ScanParams {
     int32_t alive_only;              // 1: MODE_EXACT re-run after stamps were dropped — stamps only, no counters / extrema
     uint64_t alive_origin;           // seq that field value 1 stands for (moved forward by a rebase)
     uint64_t alive_fbase;            // seq_base - alive_origin + 1: the field of record 0 when seq is implicit
-    unsigned long long *alive_count; // scratch u64 words: [0] alive entries, [1] export cursor, [2] occupied slots (count kernels)
     uint32_t *alive_cache;           // [2^ALIVE_CACHE_SET_BITS] seen cache of this batch (cleared by the host before the launch), or NULL
     int32_t alive_wave_shift;        // wave of a record = 1 + min((field - alive_wave_base) >> alive_wave_shift, 126): a monotone
     uint32_t alive_wave_base;        //   function of seq (field = seq - origin + 1); base = the field of the batch's first record
@@ -526,12 +512,6 @@ constexpr unsigned long long ALIVE_EMPTY = ~0ull;
 constexpr uint32_t ALIVE_FIELD_MAX = 0x7ffffffeu;   // largest seq field: a stamp's low word is <= 0xfffffffd, never ~0
 constexpr int ALIVE_MAX_PROBES = 96;                // pairs examined before a stamp gives up (outside a wide re-run)
 
-#ifndef KTA_L2_HINTS
-#define KTA_L2_HINTS 1
-#endif
-#ifndef KTA_EXP_ALIVE_STAGE   // ablation knob: 0 = hashes only, 1 = + seen-cache probe and queue, 2 = everything (the product)
-#define KTA_EXP_ALIVE_STAGE 2
-#endif
 // L2 residency control for MODE_EXACT: the table should stay in L2, the record stream should leave it at once.
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
     uint64_t pol;
@@ -545,26 +525,8 @@ __device__ __forceinline__ uint64_t l2_policy_evict_first() {
 }
 __device__ __forceinline__ ulonglong2 alive_ld_pair(const unsigned long long *p, uint64_t pol) {
     ulonglong2 v;
-#if KTA_L2_HINTS
     asm volatile("ld.global.cg.L2::cache_hint.v2.u64 {%0, %1}, [%2], %3;" : "=l"(v.x), "=l"(v.y) : "l"(p), "l"(pol));
-#else
-    asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(v.x), "=l"(v.y) : "l"(p));
-#endif
     return v;
-}
-__device__ __forceinline__ unsigned long long alive_atom_max(unsigned long long *p, unsigned long long v, uint64_t pol) {
-    unsigned long long old;
-#if KTA_L2_HINTS
-    asm volatile("atom.global.max.L2::cache_hint.u64 %0, [%1], %2, %3;" : "=l"(old) : "l"(p), "l"(v), "l"(pol) : "memory");
-#else
-    old = atomicMax(p, v);
-#endif
-    return old;
-}
-// (atom.cas takes no cache-policy operand in PTX: a claim is a plain compare-and-swap)
-__device__ __forceinline__ unsigned long long alive_atom_cas(unsigned long long *p, unsigned long long cmp, unsigned long long v,
-                                                             uint64_t) {
-    return atomicCAS(p, cmp, v);
 }
 
 __host__ __device__ __forceinline__ uint32_t alive_home(uint32_t x /* mixed hash */, uint32_t npairs) {
@@ -584,11 +546,7 @@ struct AliveTable {
 
 // raise an entry that holds this stamp's hash: no return value, the warp does not wait
 __device__ __forceinline__ void alive_red_max(unsigned long long *p, unsigned long long v, uint64_t pol) {
-#if KTA_L2_HINTS
     asm volatile("red.global.max.L2::cache_hint.u64 [%0], %1, %2;" ::"l"(p), "l"(v), "l"(pol) : "memory");
-#else
-    asm volatile("red.global.max.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-#endif
 }
 
 // One pair of a probe: true once the hash or an empty slot is found there, with `newest` = the low word of the newest
@@ -667,11 +625,7 @@ constexpr uint32_t ALIVE_CACHE_WAVES = (1u << ALIVE_CACHE_WAVE_BITS) - 1;   // w
 static_assert(ALIVE_CACHE_TAG_BITS == 9 && ALIVE_CACHE_WAVE_BITS == 7, "16-bit ways");
 __device__ __forceinline__ uint32_t alive_cache_ld(const uint32_t *p, uint64_t pol) {
     uint32_t v;
-#if KTA_L2_HINTS
     asm volatile("ld.global.cg.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol));
-#else
-    asm volatile("ld.global.cg.u32 %0, [%1];" : "=r"(v) : "l"(p));
-#endif
     return v;
 }
 // is a record of mixed hash x and wave `wv` superseded according to set word c?
@@ -744,6 +698,584 @@ __device__ __forceinline__ uint32_t alive_wave(uint32_t field, const AliveWaves 
 }
 
 // ------------------------------------------------------------------------------------------------
+// the fused scan kernel's stages.  scan_kernel (below) runs them once per tile, each on the data the previous ones hand it.
+// ------------------------------------------------------------------------------------------------
+// what the load pipeline staged for one tile
+struct TileDesc {
+    uint32_t bits;   // bit 0 keys staged, bits 1..4 the first key's offset inside its 16-byte line, bit 5 headers staged
+    __device__ __forceinline__ bool keys_staged() const { return bits & 1u; }
+    __device__ __forceinline__ uint32_t key_lead() const { return (bits >> 1) & 15u; }
+    __device__ __forceinline__ bool hdr_staged() const { return bits & 32u; }
+};
+
+// The hashing modes' load pipeline of one warp: S stages, each on its own mbarrier.  The warp's i-th tile goes into stage
+// i % S, S - 1 tiles ahead of the tile being worked on.  The byte ranges those copies need (key_tile_base) come from a
+// register ring, a round of 32 tiles at a time: lane i of cur_g0/cur_g1 holds key_tile_base[t] and [t + 1] for the i-th
+// tile of the round being issued, nxt_g0/nxt_g1 the same for the next round, loaded a whole round before use.
+template <int MODE>
+struct TilePipe {
+    const ScanParams &prm;
+    unsigned char *wsm;             // the warp's shared memory: S mbarriers at +0, scratch at +64, stages at +128
+    uint32_t mbar, stage0;          // shared-window addresses of mbarrier 0 and of stage 0
+    uint32_t keybuf, stage_bytes;   // key part of a stage; a whole stage (keys [| headers HDR_BYTES])
+    int S, ntiles, tile0, gstride, lane;
+    uint64_t pol;                   // L2 policy of the record stream (MODE_EXACT)
+    uint32_t phase = 0;             // bit b = parity to wait for on mbar[b]
+    int issued = 0;                 // the warp's tiles issued so far (warp-uniform)
+    uint32_t infos = 0;             // lane 0: byte b = descriptor of the tile in flight in stage b
+    uint64_t cur_g0 = 0, cur_g1 = 0, nxt_g0 = 0, nxt_g1 = 0;
+
+    // MODE_EXACT walks the batch from its newest tile to its oldest (see alive_stamp); the other modes ascend
+    __device__ __forceinline__ int phys(int t) const { return MODE == MODE_EXACT ? ntiles - 1 - t : t; }
+    __device__ __forceinline__ uint32_t stage(int b) const { return stage0 + (uint32_t)b * stage_bytes; }
+    __device__ __forceinline__ unsigned char *stage_ptr(int b) const { return wsm + 128 + (size_t)b * stage_bytes; }
+
+    __device__ __forceinline__ void copy(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) const {
+        if (MODE == MODE_EXACT) bulk_g2s(dst, src, bytes, bar, pol);
+        else bulk_g2s(dst, src, bytes, bar);
+    }
+    // lane 0: start the bulk copies of tile `tile` (key bytes [g0, g1)) into stage b; returns the tile's descriptor
+    __device__ __forceinline__ uint32_t issue(int tile, int b, uint64_t g0, uint64_t g1) const {
+        const uint32_t a = (uint32_t)g0 & 15u;
+        // the copy covers [g0 - a, roundup16(g1)).  Staged iff the tile has key bytes, the copy fits the stage
+        // (keybuf and the slack are multiples of 16, so roundup16(g1 - g0 + a) + slack <= keybuf ⇔ g1 - g0 <= cap - a)
+        // and it ends inside the readable bytes (stage_limit is a multiple of 16, so roundup16(g1) <= limit ⇔ g1 <= limit)
+        const bool ok = (g1 - g0) - 1ull < (uint64_t)(keybuf - (uint32_t)KEYBUF_SLACK - a) && g1 <= prm.stage_limit;
+        // the header slices of a full tile: 16-byte aligned when the column bases are (tiles start at multiples of 128 records)
+        const bool hdr = prm.hdr_stage && (int64_t)(tile + 1) * TILE <= prm.n;
+        const uint32_t kbytes = ok ? ((uint32_t)(g1 - g0) + a + 15u) & ~15u : 0u;
+        const uint32_t bar = mbar + 8u * (uint32_t)b, dst = stage0 + (uint32_t)b * stage_bytes;
+        if (ok || hdr) mbar_arrive_expect_tx(bar, kbytes + (hdr ? (uint32_t)HDR_BYTES : 0u));
+        if (ok) copy(dst, prm.key_bytes + (g0 - a), kbytes, bar);
+        if (hdr) {
+            const int64_t r0 = (int64_t)tile * TILE;
+            copy(dst + keybuf + HDR_P, prm.partition + r0, TILE * 4, bar);
+            copy(dst + keybuf + HDR_TS, prm.ts_ms + r0, TILE * 8, bar);
+            copy(dst + keybuf + HDR_KL, prm.key_len + r0, TILE * 4, bar);
+            copy(dst + keybuf + HDR_VL, prm.value_len + r0, TILE * 4, bar);
+        }
+        return (ok ? 1u : 0u) | (a << 1) | (hdr ? 32u : 0u);
+    }
+    __device__ __forceinline__ void ring_load(int round, uint64_t &g0, uint64_t &g1) const {
+        const int64_t t = tile0 + ((int64_t)round * 32 + lane) * gstride;
+        if (t < ntiles) {
+            const int pt = phys((int)t);
+            g0 = __ldg(prm.key_tile_base + pt);
+            g1 = __ldg(prm.key_tile_base + pt + 1);
+        }
+    }
+    // all lanes: issue the warp's next tile into stage b
+    __device__ __forceinline__ void issue_next(int b) {
+        if ((issued & 31) == 0 && issued) {
+            cur_g0 = nxt_g0;
+            cur_g1 = nxt_g1;
+            ring_load((issued >> 5) + 1, nxt_g0, nxt_g1);
+        }
+        const uint64_t g0 = __shfl_sync(0xffffffffu, cur_g0, issued & 31), g1 = __shfl_sync(0xffffffffu, cur_g1, issued & 31);
+        if (lane == 0) {
+            const uint32_t d = issue(phys(tile0 + issued * gstride), b, g0, g1);
+            infos = (infos & ~(0xffu << (8 * b))) | (d << (8 * b));
+        }
+        issued++;
+    }
+    // before the first tile: the first two rounds of the ring, and the first S - 1 tiles
+    __device__ __forceinline__ void start() {
+        ring_load(0, cur_g0, cur_g1);
+        ring_load(1, nxt_g0, nxt_g1);
+        for (int b = 0; b < S - 1 && tile0 + b * gstride < ntiles; b++) issue_next(b);
+    }
+    // the descriptor of the tile in stage `buf`
+    __device__ __forceinline__ TileDesc next(int tile, int buf) {
+        const TileDesc d{(__shfl_sync(0xffffffffu, infos, 0) >> (8 * buf)) & 0xffu};   // also: every lane is done with the previous stage
+        // the tile S - 1 ahead goes into the stage the previous tile has just finished with
+        if (tile < ntiles - (S - 1) * gstride) issue_next(buf == 0 ? S - 1 : buf - 1);   // no overflow: gstride <= SMs * 32
+        return d;
+    }
+    __device__ __forceinline__ void wait(int b) {
+        mbar_wait(mbar + 8u * b, (phase >> b) & 1u);
+        phase ^= 1u << b;
+    }
+};
+
+// the lane's four records of a tile (rows 32 k + lane)
+struct TileRows {
+    int p[ROWS], kl[ROWS], vl[ROWS];   // after partition_check p[k] is the record's counter column
+    long long ts[ROWS];
+    bool valid[ROWS];                  // the record exists
+    bool use[ROWS];                    // it exists and its partition is one this scan counts
+    bool clean;                        // warp-uniform: every record of the tile exists and counts
+};
+
+// a warp's running totals, flushed once after its last tile
+struct WarpTotals {
+    long long tmin = INT64_MAX, tmax = INT64_MIN;   // raw ts_ms extrema (None → 0 applied at read-back)
+    uint32_t smin = 0xffffffffu, smax = 0;          // message size extrema (non-tombstones); sizes < 2^32 - 1
+    uint32_t bad = 0;
+    bool try_uni = true;                            // probe rows for "one partition" only while that keeps paying off
+};
+
+// header columns: 4 rows of 32 consecutive records, from the stage or fully coalesced from global memory
+template <bool FULL, int MODE>
+__device__ __forceinline__ void load_headers(const ScanParams &prm, TilePipe<MODE> &pipe, int buf, TileDesc d, int64_t rbase,
+                                             int lane, TileRows &rec) {
+    if (MODE != MODE_COUNTERS && d.hdr_staged()) {   // staged ⇒ FULL
+        pipe.wait(buf);
+        const uint32_t st = pipe.stage(buf);
+#pragma unroll
+        for (int k = 0; k < ROWS; k++) {
+            const uint32_t r = 32u * k + lane;
+            rec.valid[k] = true;
+            rec.p[k] = (int)lds32(st + pipe.keybuf + HDR_P + 4u * r);
+            rec.ts[k] = lds64(st + pipe.keybuf + HDR_TS + 8u * r);
+            rec.kl[k] = (int)lds32(st + pipe.keybuf + HDR_KL + 4u * r);
+            rec.vl[k] = (int)lds32(st + pipe.keybuf + HDR_VL + 4u * r);
+        }
+    } else {
+#pragma unroll
+        for (int k = 0; k < ROWS; k++) {
+            const int64_t r = rbase + 32 * k;
+            rec.valid[k] = FULL || r < prm.n;
+            if (rec.valid[k]) {
+                if (MODE == MODE_EXACT) {
+                    rec.p[k] = ld_stream_s32(prm.partition + r, pipe.pol);
+                    rec.ts[k] = ld_stream_s64(prm.ts_ms + r, pipe.pol);
+                    rec.kl[k] = ld_stream_s32(prm.key_len + r, pipe.pol);
+                    rec.vl[k] = ld_stream_s32(prm.value_len + r, pipe.pol);
+                } else {
+                    rec.p[k] = ld_stream_s32(prm.partition + r);
+                    rec.ts[k] = ld_stream_s64(prm.ts_ms + r);
+                    rec.kl[k] = ld_stream_s32(prm.key_len + r);
+                    rec.vl[k] = ld_stream_s32(prm.value_len + r);
+                }
+            } else {
+                rec.p[k] = 0; rec.ts[k] = INT64_MAX; rec.kl[k] = -1; rec.vl[k] = -1;
+            }
+        }
+    }
+}
+
+// ---- MessageMetrics::handle_message (metric.rs:206-253) ----
+// A record whose partition lies outside [0, P) is counted in `bad` and takes part in NOTHING else (counters, extrema,
+// alive keys, sketch), so the state stays consistent; its key bytes still occupy their place in the packed keys.
+template <bool FULL, bool SHARD>
+__device__ __forceinline__ void partition_check(const ScanParams &prm, TileRows &rec) {
+    bool inrange = true;
+#pragma unroll
+    for (int k = 0; k < ROWS; k++) {
+        bool ok = (unsigned)rec.p[k] < (unsigned)prm.P;
+        if (SHARD) {
+            // partition → column: c = p / G, and the partition must be one of this shard's (p - c G == rank);
+            // others are left out like out-of-range ones.  From here on p[k] is the column.
+            const int c = (int)__umulhi((uint32_t)rec.p[k], prm.shard_magic);
+            ok = ok && rec.p[k] - c * prm.shard_world == prm.shard_rank;
+            rec.p[k] = ok ? c : 0;
+        }
+        rec.use[k] = rec.valid[k] && ok;
+        inrange = inrange && ok;
+    }
+    rec.clean = FULL && __all_sync(0xffffffffu, inrange);
+}
+
+// the tile's counters, histograms and extrema; count_it = false: a stamps-only re-run.  C is taken by value: taken by
+// reference, ptxas spilled inside the tile loop of the exact scan with counters in shared memory.
+template <bool SMEM>
+__device__ __forceinline__ void count_tile(const Counters<SMEM> C, const TileRows &rec, bool count_it, int lane, WarpTotals &w) {
+    const unsigned full = 0xffffffffu;
+    if (!count_it) {
+        // stamps-only re-run: the counters and extrema of this batch were taken by the first pass
+    } else if (rec.clean) {
+        if (w.try_uni) {
+            // run-structured input (a Kafka fetch delivers long runs of one partition).
+            // A whole tile inside one run (3 of 4 tiles at run length 500): one vote, the lane's four lengths added up
+            // first, two warp reductions and two adds for the tile
+            const int p0t = __shfl_sync(full, rec.p[0], 0);
+            uint32_t kv4 = 0, vv4 = 0, big = 0;
+            bool one = true;
+#pragma unroll
+            for (int k = 0; k < ROWS; k++) {
+                const uint32_t kv = (uint32_t)max(rec.kl[k], 0), vv = (uint32_t)max(rec.vl[k], 0);
+                one = one && rec.p[k] == p0t;
+                kv4 += kv; vv4 += vv; big |= kv | vv;
+            }
+            if (__all_sync(full, one && big < (1u << 24))) {
+#pragma unroll
+                for (int k = 0; k < ROWS; k++) C.buckets(p0t, rec.kl[k], rec.vl[k]);
+                const uint32_t ks = __reduce_add_sync(full, kv4);   // 128 lengths < 2^24: no overflow
+                const uint32_t vs = __reduce_add_sync(full, vv4);
+                if (lane == 0) {
+                    C.sum_add(0, p0t, ks);
+                    C.sum_add(1, p0t, vs);
+                }
+            } else {
+            // otherwise row by row: the byte sums of a row that lies inside one run are reduced in the warp (2 REDUX)
+            // and added once, instead of 32 same-address adds
+            bool any_uni = false;
+#pragma unroll
+            for (int k = 0; k < ROWS; k++) {
+                C.buckets(rec.p[k], rec.kl[k], rec.vl[k]);
+                const int p0 = __shfl_sync(full, rec.p[k], 0);
+                const unsigned m0 = __ballot_sync(full, rec.p[k] == p0);
+                const bool small_row = __all_sync(full, (rec.kl[k] | rec.vl[k]) < (1 << 26));
+                const uint32_t kv = (uint32_t)max(rec.kl[k], 0), vv = (uint32_t)max(rec.vl[k], 0);
+                if (m0 == full && small_row) {
+                    const uint32_t ks = __reduce_add_sync(full, kv);   // each < 2^26: no overflow
+                    const uint32_t vs = __reduce_add_sync(full, vv);
+                    if (lane == 0) {
+                        C.sum_add(0, p0, ks);
+                        C.sum_add(1, p0, vs);
+                    }
+                    any_uni = true;
+                } else {
+                    // a row that straddles a run boundary holds two partitions: left to per-lane adds, its two
+                    // counters would be hit 32 times each, serialised in the shared-memory pipe.  Reduce the two groups separately instead.
+                    const int l1 = __ffs(~m0) - 1;                     // first lane of the second group
+                    const int p1 = __shfl_sync(full, rec.p[k], l1 & 31);
+                    const unsigned m1 = __ballot_sync(full, rec.p[k] == p1);
+                    if (small_row && (m0 | m1) == full) {
+                        const bool in0 = (m0 >> lane) & 1u;
+                        const uint32_t ks0 = __reduce_add_sync(full, in0 ? kv : 0u), vs0 = __reduce_add_sync(full, in0 ? vv : 0u);
+                        const uint32_t ks1 = __reduce_add_sync(full, in0 ? 0u : kv), vs1 = __reduce_add_sync(full, in0 ? 0u : vv);
+                        if (lane == 0) {
+                            C.sum_add(0, p0, ks0);
+                            C.sum_add(1, p0, vs0);
+                        } else if (lane == l1) {
+                            C.sum_add(0, p1, ks1);
+                            C.sum_add(1, p1, vs1);
+                        }
+                        any_uni = true;
+                    } else {
+                        C.sums(rec.p[k], rec.kl[k], rec.vl[k]);
+                    }
+                }
+            }
+            w.try_uni = any_uni;
+            }
+        } else {
+            C.record_rows(rec.p, rec.kl, rec.vl);
+        }
+    } else {
+        // tail tile, or a record with a partition outside [0, P): per-record checks
+#pragma unroll
+        for (int k = 0; k < ROWS; k++) {
+            if (rec.use[k]) C.record(rec.p[k], rec.kl[k], rec.vl[k]);
+            else if (rec.valid[k]) w.bad++;
+        }
+    }
+    // metric.rs:209,247: None → 0 and ms → s are monotone maps, applied once at read-back: the raw
+    // extrema determine the mapped extrema (raw == -1 ⇔ mapped 0, see kta_timestamps).
+    // Timestamps of one topic share their high word for 49 days at a time: when the lane's four and its running
+    // extrema do, the signed 64-bit order is the unsigned order of the low words (2 + 2 three-input min/max).
+    bool ts_fast = false;
+    if (rec.clean && count_it) {
+        const uint32_t hw = hi32(w.tmin);
+        uint32_t x = hi32(w.tmax) ^ hw;
+#pragma unroll
+        for (int k = 0; k < ROWS; k++) x |= hi32(rec.ts[k]) ^ hw;
+        ts_fast = x == 0;
+    }
+    if (ts_fast) {
+        const uint32_t hw = hi32(w.tmin);
+        const uint32_t l0 = (uint32_t)rec.ts[0], l1 = (uint32_t)rec.ts[1], l2 = (uint32_t)rec.ts[2], l3 = (uint32_t)rec.ts[3];
+        const uint32_t lo = min(min(min(l0, l1), l2), min(l3, (uint32_t)w.tmin));
+        const uint32_t hi = max(max(max(l0, l1), l2), max(l3, (uint32_t)w.tmax));
+        w.tmin = pack64(lo, hw);
+        w.tmax = pack64(hi, hw);
+    } else if (count_it) {
+        asm volatile("");   // keep this a real branch: if-converted, the 64-bit chain runs every tile
+#pragma unroll
+        for (int k = 0; k < ROWS; k++) {
+            const bool u = rec.clean || rec.use[k];
+            const long long t0 = u ? rec.ts[k] : INT64_MAX, t1 = u ? rec.ts[k] : INT64_MIN;
+            w.tmin = t0 < w.tmin ? t0 : w.tmin;
+            w.tmax = t1 > w.tmax ? t1 : w.tmax;
+        }
+    }
+    if (count_it) {
+#pragma unroll
+        for (int k = 0; k < ROWS; k++) {
+            // metric.rs:249-251: size extrema, not for tombstones (rows that do not exist carry vl = -1)
+            const uint32_t sz = (uint32_t)max(rec.kl[k], 0) + (uint32_t)rec.vl[k];
+            if (rec.vl[k] >= 0 && (rec.clean || rec.use[k])) {
+                w.smin = min(w.smin, sz);
+                w.smax = max(w.smax, sz);
+            }
+        }
+    }
+}
+
+struct KeyOffsets {
+    uint32_t off[ROWS];   // byte offset of each of the lane's keys inside the tile's packed keys
+    bool fixL;            // every non-null key of the tile has one length L < 2^16
+    bool small;           // the longest key is shorter than 1 MiB
+    bool fix16;           // fixL with L = 16
+};
+
+// byte offset of each key inside the tile: exclusive scan of max(key_len, 0)
+__device__ __forceinline__ KeyOffsets key_offsets(const int (&kl)[ROWS], int lane) {
+    const unsigned full = 0xffffffffu;
+    const unsigned lt_mask = (1u << lane) - 1u;
+    KeyOffsets o;
+    // do all keys of this tile that are not null have ONE length L?  L = the longest; read as unsigned, null (-1)
+    // is the largest value, so the unsigned minimum is the shortest non-null key (or "null" if there is none):
+    // one length ⇔ the two agree.  Two three-input min/max per lane and two warp reductions.
+    const int lmax = max(max(kl[0], kl[1]), max(kl[2], kl[3]));
+    const uint32_t lmin = min(min((uint32_t)kl[0], (uint32_t)kl[1]), min((uint32_t)kl[2], (uint32_t)kl[3]));
+    static_assert(ROWS == 4, "written out for four rows");
+    const int L = __reduce_max_sync(full, lmax);   // -1 when every key is null
+    o.fixL = __reduce_min_sync(full, lmin) == (uint32_t)L && L < (1 << 16);
+    o.small = L < (1 << 20);   // warp-uniform
+    o.fix16 = o.fixL && L == 16;
+    if (o.fixL) {
+        // fixed-width keys (the common case: ids, hashes, UUIDs)
+        const uint32_t Lu = (uint32_t)max(L, 0);
+        if (!__any_sync(full, (kl[0] | kl[1] | kl[2] | kl[3]) < 0)) {
+            // no null key in the tile (every tile of a keyed / compacted topic): record r's key is the r-th
+#pragma unroll
+            for (int k = 0; k < ROWS; k++) o.off[k] = Lu * (uint32_t)(32 * k + lane);
+        } else {
+            // offsets from ballots, no shuffle scan
+            uint32_t before = 0;
+#pragma unroll
+            for (int k = 0; k < ROWS; k++) {
+                const unsigned m = __ballot_sync(full, kl[k] >= 0);
+                o.off[k] = Lu * (before + __popc(m & lt_mask));
+                before += __popc(m);
+            }
+        }
+    } else {
+        static_assert(ROWS == 4, "the packed scan below handles exactly four rows");
+        uint32_t mxl = 0;
+#pragma unroll
+        for (int k = 0; k < ROWS; k++) mxl = max(mxl, (uint32_t)max(kl[k], 0));
+        if (__all_sync(full, mxl < 2048u)) {
+            // short keys (every row sums to < 2^16): scan two rows per 32-bit word, 10 shuffles instead of 20
+            const uint32_t v0 = (uint32_t)max(kl[0], 0), v1 = (uint32_t)max(kl[1], 0);
+            const uint32_t v2 = (uint32_t)max(kl[2], 0), v3 = (uint32_t)max(kl[3], 0);
+            uint32_t a = v0 | (v1 << 16), b = v2 | (v3 << 16);
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t ta = __shfl_up_sync(full, a, d), tb = __shfl_up_sync(full, b, d);
+                if (lane >= d) { a += ta; b += tb; }
+            }
+            const uint32_t ea = __shfl_sync(full, a, 31), eb = __shfl_sync(full, b, 31);
+            const uint32_t t0 = ea & 0xffffu, t1 = ea >> 16, t2 = eb & 0xffffu;
+            o.off[0] = (a & 0xffffu) - v0;
+            o.off[1] = t0 + (a >> 16) - v1;
+            o.off[2] = t0 + t1 + (b & 0xffffu) - v2;
+            o.off[3] = t0 + t1 + t2 + (b >> 16) - v3;
+        } else if (o.small) {
+            uint32_t c32 = 0;
+#pragma unroll
+            for (int k = 0; k < ROWS; k++) {
+                const uint32_t v = (uint32_t)max(kl[k], 0);
+                uint32_t inc = v;
+#pragma unroll
+                for (int d = 1; d < 32; d <<= 1) {
+                    const uint32_t t = __shfl_up_sync(full, inc, d);
+                    if (lane >= d) inc += t;
+                }
+                o.off[k] = c32 + inc - v;
+                c32 += __shfl_sync(full, inc, 31);
+            }
+        }
+    }
+    return o;
+}
+
+// the reference hash of each of the lane's keys (0 for null keys), from the stage when its keys are staged
+template <bool CAPTURE, int MODE>
+__device__ __forceinline__ void hash_tile(const ScanParams &prm, TilePipe<MODE> &pipe, int buf, TileDesc d, int tile, int64_t rbase,
+                                          const TileRows &rec, const KeyOffsets &o, int lane, uint32_t (&h)[ROWS]) {
+    const uint32_t kb = pipe.stage(buf);   // the key part of the stage
+    if (d.keys_staged()) {   // staged ⇒ the tile's keys fit one stage (<= 16 KiB) ⇒ small
+        const uint32_t a0 = d.key_lead();
+        if (!d.hdr_staged()) pipe.wait(buf);   // else done before the headers were read
+        if (o.fix16 && a0 == 0) {
+            // two independent FNV chains at a time per lane, one LDS.128 per key (null keys hash
+            // garbage that is never used); the other warps of the SM sub-partition supply the rest of the ILP
+#pragma unroll
+            for (int k = 0; k < ROWS; k += 2) {
+                const uint4 qa = lds128(kb + o.off[k]);
+                const uint4 qb = lds128(kb + o.off[k + 1]);
+                uint32_t ha = FNV_BASIS, hb = FNV_BASIS;
+                ha = fnv_word(ha, qa.x); hb = fnv_word(hb, qb.x);
+                ha = fnv_word(ha, qa.y); hb = fnv_word(hb, qb.y);
+                ha = fnv_word(ha, qa.z); hb = fnv_word(hb, qb.z);
+                ha = fnv_word(ha, qa.w); hb = fnv_word(hb, qb.w);
+                h[k] = ha;
+                h[k + 1] = hb;
+            }
+        } else {
+#pragma unroll
+            for (int k = 0; k < ROWS; k++) h[k] = rec.kl[k] >= 0 ? fnv_smem(kb, a0 + o.off[k], rec.kl[k]) : 0u;
+        }
+    } else if (o.fixL || o.small) {
+        const uint64_t g0 = prm.key_tile_base[tile];
+#pragma unroll
+        for (int k = 0; k < ROWS; k++)
+            h[k] = (rec.valid[k] && rec.kl[k] >= 0) ? fnv_global(prm.key_bytes + g0 + o.off[k], rec.kl[k]) : 0u;
+    } else {
+        uint32_t *scratch = reinterpret_cast<uint32_t *>(pipe.stage_ptr(buf));  // keys not staged: free
+        wide_tile_hashes(prm.key_len, prm.n, prm.key_bytes + prm.key_tile_base[tile], tile, scratch, lane);
+#pragma unroll
+        for (int k = 0; k < ROWS; k++) h[k] = scratch[32 * k + lane];
+    }
+    if (CAPTURE) {
+#pragma unroll
+        for (int k = 0; k < ROWS; k++)
+            if (rec.valid[k]) prm.hash_out[rbase + 32 * k] = rec.kl[k] >= 0 ? h[k] : 0u;
+    }
+}
+
+// ---- LogCompactionInMemoryMetrics::handle_message, metric.rs:288-305 ----
+// metric.rs:291-302: Some(key) → insert (value) / remove (tombstone); None → nothing.
+// Last-writer-wins per hash in seq order IS the BitSet insert/remove sequence replayed in order
+// (metric.rs:295 mark_key_alive, :298 mark_key_dead).
+// What limits this mode is the L1 pipe — a divergent 32-lane global access costs it ~2 cycles per lane — and
+// latency, not DRAM.  So: exactly ONE random access per record (the seen cache, sent off by exact_probe and in flight
+// while the records are counted); the ~12 % that survive it are compacted across the tile into one dense queue (in the
+// key part of the stage the tile has just finished with) and take the exact path through the table in exact_resolve,
+// usually in a single pass.
+struct ExactProbe {
+    uint32_t x[ROWS];     // mixed hash
+    uint32_t low[ROWS];   // the stamp's low word: seq field << 1 | alive
+    uint32_t cw[ROWS];    // the seen-cache set word (0 when not probed)
+    bool live[ROWS];      // the record takes part: it counts and has a key, and its seq lies in the table's window
+};
+
+__device__ __forceinline__ ExactProbe exact_probe(const ScanParams &prm, const AliveTable &AT, const AliveWaves &AW,
+                                                  const TileRows &rec, const uint32_t (&h)[ROWS], int64_t rbase) {
+    const bool cached = AW.cache != nullptr;
+    const uint32_t r32 = (uint32_t)rbase;   // index in the batch (< 2^31: host-checked)
+    ExactProbe e;
+#pragma unroll
+    for (int k = 0; k < ROWS; k++) {
+        e.live[k] = (rec.clean || rec.use[k]) && rec.kl[k] >= 0;
+        uint32_t field;
+        if (prm.seq) {
+            // explicit global sequence numbers (partition-sharded scans): must fall into the table's window
+            const uint64_t f = e.live[k] ? ld_stream_u64(prm.seq + rbase + 32 * k) - prm.alive_origin + 1ull : 1ull;
+            if (f - 1ull >= (uint64_t)ALIVE_FIELD_MAX) {
+                atomicAdd(prm.alive_status + 1, 1u);
+                e.live[k] = false;
+            }
+            field = (uint32_t)f;
+        } else {
+            field = (uint32_t)prm.alive_fbase + r32 + 32u * k;   // host-checked: seq_base + n fits the window
+        }
+        e.low[k] = (field << 1) | (rec.vl[k] >= 0 ? 1u : 0u);
+        e.x[k] = hll_mix(h[k]);
+        e.cw[k] = 0;
+        if (cached && e.live[k]) e.cw[k] = alive_cache_ld(AW.cache + (e.x[k] >> ALIVE_CACHE_TAG_BITS), AT.pol);
+    }
+    return e;
+}
+
+// the records the seen cache did not settle go through the table; what the table knows afterwards goes back to the cache
+__device__ __forceinline__ void exact_resolve(const AliveTable &AT, const AliveWaves &AW, const ExactProbe &e, unsigned char *stage,
+                                              int lane, unsigned lt_mask) {
+    static_assert(TILE * 16 <= KEYBUF_MIN, "the queue stays inside the key part of the stage");
+    uint4 *queue = reinterpret_cast<uint4 *>(stage);   // (x, low word, set word, -) x TILE
+    const bool cached = AW.cache != nullptr;
+    __syncwarp();      // every lane is done reading its keys from this stage before any lane overwrites it
+    uint32_t qn = 0;   // warp-uniform
+#pragma unroll
+    for (int k = 0; k < ROWS; k++) {
+        const bool go = e.live[k] && !(cached && alive_cache_newer(e.cw[k], e.x[k], alive_wave(e.low[k] >> 1, AW)));
+        const unsigned m = __ballot_sync(0xffffffffu, go);
+        if (go) queue[qn + __popc(m & lt_mask)] = make_uint4(e.x[k], e.low[k], e.cw[k], 0u);
+        qn += __popc(m);
+    }
+    __syncwarp();
+    for (uint32_t q0 = 0; q0 < qn; q0 += 32) {
+        if (q0 + lane < qn) {
+            const uint4 item = queue[q0 + lane];
+            const uint32_t pr = alive_home(item.x, AT.npairs);
+            const ulonglong2 en = alive_ld_pair(AT.slots + 2 * (size_t)pr, AT.pol);
+            const uint32_t newest = alive_stamp(AT, pr, en, item.x, item.y);
+            // tell the cache what the table knows now: the newest stamp of this hash as a wave of THIS batch (0 =
+            // older than the batch: says nothing), or the record's own wave
+            if (cached)
+                alive_cache_put(AW.cache, item.z, item.x, max(alive_wave(item.y >> 1, AW), alive_wave(newest >> 1, AW)), newest >> 1);
+        }
+    }
+    // the queue lives in a key stage that the TMA engine refills next iteration: order these generic-proxy
+    // accesses before that async-proxy write
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncwarp();
+}
+
+// in-stream sketch: every record with a key and a value (invalid rows carry kl = vl = -1)
+__device__ __forceinline__ void sketch_tile(const ScanParams &prm, uint32_t floor_reg, const TileRows &rec, const uint32_t (&h)[ROWS]) {
+    const uint32_t skip_mask = hll_skip_mask(prm.hll_p, floor_reg);
+#pragma unroll
+    for (int k = 0; k < ROWS; k++) {
+        const uint32_t x = hll_mix(h[k]);
+        if (((x & skip_mask) | (uint32_t)((rec.kl[k] | rec.vl[k]) >> 31)) == 0 && (rec.clean || rec.use[k])) hll_raise(prm.hll, prm.hll_p, x);
+    }
+}
+
+// after the last tile (SMEM): bucket rows → global [which][p][bucket]; row 32 → knull; row 65 (tombstones) is derived, not
+// stored; then the split sums.  The adds go through prm.sums, not C.g: the compiler knows that a kernel parameter points to
+// global memory and emits RED, where a pointer held in the Counters struct gets generic atomics.
+template <bool SMEM>
+__device__ __forceinline__ void flush_counters(const ScanParams &prm, const Counters<SMEM> &C, int tid, int warp, int lane) {
+    const int nh = (ROW_V + NB) * C.P;
+    for (int i = tid; i < nh; i += blockDim.x) {
+        const uint32_t v = C.s[i];
+        if (v) {
+            const int row = i / C.P, pp = C.part(i - row * C.P);
+            if (row < NB) atomicAdd(&prm.sums[(size_t)pp * NB + row], (unsigned long long)v);
+            else if (row == NB) atomicAdd(&prm.sums[(size_t)prm.P * (2 * NB + 2) + pp], (unsigned long long)v);
+            else atomicAdd(&prm.sums[(size_t)(prm.P + pp) * NB + (row - ROW_V)], (unsigned long long)v);
+        }
+    }
+    if (warp == 0) C.fold_sums(lane, 1u);
+}
+
+// after the last tile: extrema + bad-partition count, by warp shuffle, then one lane per warp, then one thread per CTA
+// (wsm: this warp's shared memory; warp_bytes: its size)
+__device__ __forceinline__ void flush_totals(const ScanParams &prm, WarpTotals w, unsigned char *wsm, size_t warp_bytes, int tid,
+                                             int lane, int nwarps) {
+    const unsigned full = 0xffffffffu;
+    long long smin64 = w.smin != 0xffffffffu ? (long long)w.smin : INT64_MAX;
+    long long smax64 = w.smin != 0xffffffffu ? (long long)w.smax : -1;
+#pragma unroll
+    for (int d = 16; d; d >>= 1) {
+        const long long a = __shfl_xor_sync(full, w.tmin, d), b = __shfl_xor_sync(full, w.tmax, d);
+        const long long c = __shfl_xor_sync(full, smin64, d), e = __shfl_xor_sync(full, smax64, d);
+        w.tmin = a < w.tmin ? a : w.tmin;
+        w.tmax = b > w.tmax ? b : w.tmax;
+        smin64 = c < smin64 ? c : smin64;
+        smax64 = e > smax64 ? e : smax64;
+        w.bad += __shfl_xor_sync(full, w.bad, d);
+    }
+    long long *red = reinterpret_cast<long long *>(wsm + 64);   // per-warp scratch (4 × i64)
+    if (lane == 0) {
+        red[0] = w.tmin; red[1] = w.tmax; red[2] = smin64; red[3] = smax64;
+        if (w.bad) atomicAdd(&prm.sums[sums_words(prm.P) - 1], (unsigned long long)w.bad);
+    }
+    __syncthreads();
+    if (tid == 0) {
+        for (int i = 1; i < nwarps; i++) {
+            const long long *rw = reinterpret_cast<const long long *>(wsm + (size_t)i * warp_bytes + 64);
+            w.tmin = rw[0] < w.tmin ? rw[0] : w.tmin;
+            w.tmax = rw[1] > w.tmax ? rw[1] : w.tmax;
+            smin64 = rw[2] < smin64 ? rw[2] : smin64;
+            smax64 = rw[3] > smax64 ? rw[3] : smax64;
+        }
+        if (w.tmin != INT64_MAX) {
+            atomicMin(&prm.minmax[0], w.tmin);
+            atomicMax(&prm.minmax[1], w.tmax);
+        }
+        if (smax64 >= 0) {
+            atomicMin(reinterpret_cast<unsigned long long *>(&prm.minmax[2]), (unsigned long long)smin64);
+            atomicMax(reinterpret_cast<unsigned long long *>(&prm.minmax[3]), (unsigned long long)smax64);
+        }
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // the fused scan kernel.
 //   MODE_COUNTERS: counters + histograms + extrema only (20 B/record, no key bytes touched — the reference
 //                  without -c).
@@ -764,7 +1296,6 @@ __global__ void __launch_bounds__(MODE == MODE_COUNTERS ? MAX_THREADS : HASH_MAX
     constexpr bool HASH = MODE != MODE_COUNTERS;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = blockDim.x >> 5;
-    const unsigned full = 0xffffffffu;
     const unsigned lt_mask = (1u << lane) - 1u;
     // SHARD: a partition-sharded scan (SURVEY.md §8 e: gpu = partition mod G) carves counter columns only for the
     // partitions it owns — a rank of BASELINE configs[3] holds 32 columns, not 256
@@ -774,16 +1305,14 @@ __global__ void __launch_bounds__(MODE == MODE_COUNTERS ? MAX_THREADS : HASH_MAX
     const size_t cta_bytes = SMEM ? smem_counter_bytes(P) : CTA_SCRATCH;
     const uint32_t KEYBUF = (uint32_t)prm.keybuf;
     const int S = HASH ? prm.stages : 0;
-    const uint32_t STAGE = KEYBUF + (prm.hdr_stage ? (uint32_t)HDR_BYTES : 0u);
     const size_t warp_bytes = warp_smem_bytes(HASH, prm.keybuf, S, prm.hdr_stage);
     unsigned char *wsm = smem_raw + cta_bytes + (size_t)warp * warp_bytes;
     const uint32_t mbar = smem_u32(wsm);            // S 8-byte mbarriers at +0, +8, ...
-    const uint32_t stage0 = smem_u32(wsm) + 128;    // S STAGE-byte stages
+    const uint32_t stage0 = smem_u32(wsm) + 128;    // S stages
     const Counters<SMEM> C{smem_u32(scnt), scnt, prm.sums, P, prm.P, SHARD ? prm.shard_world : 1, SHARD ? prm.shard_rank : 0};
     // MODE_EXACT: the alive table's lines are asked to stay in L2 (evict_last), the record stream to leave first
-    constexpr bool HINTS = MODE == MODE_EXACT && KTA_L2_HINTS;
-    const uint64_t pol_stream = HINTS ? l2_policy_evict_first() : 0;
-    const AliveTable AT{prm.alive_table, prm.alive_pairs, prm.alive_status, HINTS ? l2_policy_evict_last() : 0};
+    const uint64_t pol_stream = MODE == MODE_EXACT ? l2_policy_evict_first() : 0;
+    const AliveTable AT{prm.alive_table, prm.alive_pairs, prm.alive_status, MODE == MODE_EXACT ? l2_policy_evict_last() : 0};
     const AliveWaves AW{prm.alive_cache, prm.alive_wave_base, prm.alive_wave_shift};
     const bool count_it = !(MODE == MODE_EXACT && prm.alive_only);   // false: a stamps-only re-run after the table grew
 
@@ -797,498 +1326,52 @@ __global__ void __launch_bounds__(MODE == MODE_COUNTERS ? MAX_THREADS : HASH_MAX
     }
     __syncthreads();
 
-    auto copy = [&](uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
-        if (HINTS) bulk_g2s(dst, src, bytes, bar, pol_stream);
-        else bulk_g2s(dst, src, bytes, bar);
-    };
-    // lane 0: start the bulk copies of tile `tile` (key bytes [g0, g1)) into stage b.
-    // Returns the tile's descriptor: bit 0 keys staged, bits 1..4 = first key's offset inside its 16-byte line,
-    // bit 5 headers staged.
-    auto issue = [&](int tile, int b, uint64_t g0, uint64_t g1) -> uint32_t {
-        const uint32_t a = (uint32_t)g0 & 15u;
-        // the copy covers [g0 - a, roundup16(g1)).  Staged iff the tile has key bytes, the copy fits the stage
-        // (KEYBUF and the slack are multiples of 16, so roundup16(g1 - g0 + a) + slack <= KEYBUF ⇔ g1 - g0 <= cap - a)
-        // and it ends inside the readable bytes (stage_limit is a multiple of 16, so roundup16(g1) <= limit ⇔ g1 <= limit)
-        const bool ok = (g1 - g0) - 1ull < (uint64_t)(KEYBUF - (uint32_t)KEYBUF_SLACK - a) && g1 <= prm.stage_limit;
-        // the header slices of a full tile: 16-byte aligned when the column bases are (tiles start at multiples of 128 records)
-        const bool hdr = prm.hdr_stage && (int64_t)(tile + 1) * TILE <= prm.n;
-        const uint32_t kbytes = ok ? ((uint32_t)(g1 - g0) + a + 15u) & ~15u : 0u;
-        const uint32_t bar = mbar + 8u * (uint32_t)b, dst = stage0 + (uint32_t)b * STAGE;
-        if (ok || hdr) mbar_arrive_expect_tx(bar, kbytes + (hdr ? (uint32_t)HDR_BYTES : 0u));
-        if (ok) copy(dst, prm.key_bytes + (g0 - a), kbytes, bar);
-        if (hdr) {
-            const int64_t r0 = (int64_t)tile * TILE;
-            copy(dst + KEYBUF + HDR_P, prm.partition + r0, TILE * 4, bar);
-            copy(dst + KEYBUF + HDR_TS, prm.ts_ms + r0, TILE * 8, bar);
-            copy(dst + KEYBUF + HDR_KL, prm.key_len + r0, TILE * 4, bar);
-            copy(dst + KEYBUF + HDR_VL, prm.value_len + r0, TILE * 4, bar);
-        }
-        return (ok ? 1u : 0u) | (a << 1) | (hdr ? 32u : 0u);
-    };
-
-    long long tmin = INT64_MAX, tmax = INT64_MIN;         // raw ts_ms extrema (None → 0 applied at read-back)
-    uint32_t smin = 0xffffffffu, smax = 0;                // message size extrema (non-tombstones); sizes < 2^32 - 1
-    uint32_t bad = 0;
-    uint32_t phase = 0;       // bit b = parity to wait for on mbar[b]
-    bool try_uni = true;      // probe rows for "one partition" only while that keeps paying off
+    WarpTotals tot;
     // MODE_HLL: the warp's copy of the sketch floor (a lower bound of every register: monotone, so a stale copy only
     // filters less).  Re-read from its global word after the first tiles and then every 16th tile — one global word read by
     // every warp for EVERY tile makes a single L2 line the bottleneck of the whole kernel.
     uint32_t floor_reg = MODE == MODE_HLL ? ld_cg_u32(prm.hll_floor) : 0u;
 
-    // MODE_EXACT walks the batch from its newest tile to its oldest (see alive_stamp); the other modes ascend
     // tile indices fit 32 bits (the host refuses batches of 2^31 tiles = 2.7e11 records): the loop control stays out of
     // 64-bit arithmetic and out of local memory
     const int ntiles = (int)prm.ntiles;
-    auto phys = [&](int t) { return MODE == MODE_EXACT ? ntiles - 1 - t : t; };
     const int gstride = (int)gridDim.x * nwarps;
-    const int tile0 = (int)blockIdx.x * nwarps + warp;
-    int tile = tile0;
+    int tile = (int)blockIdx.x * nwarps + warp;
+    TilePipe<MODE> pipe{prm, wsm, mbar, stage0, KEYBUF, KEYBUF + (prm.hdr_stage ? (uint32_t)HDR_BYTES : 0u), S, ntiles, tile, gstride, lane,
+                        pol_stream};
+    if (HASH) pipe.start();
 
-    // Key byte ranges of the warp's tiles, a round of 32 at a time: lane i of `cur` holds key_tile_base[t] and [t + 1]
-    // for the i-th tile of the round being issued, `nxt` the same for the next round, loaded a whole round before use.
-    uint64_t cur_g0 = 0, cur_g1 = 0, nxt_g0 = 0, nxt_g1 = 0;
-    auto ring_load = [&](int round, uint64_t &g0, uint64_t &g1) {
-        const int64_t t = tile0 + ((int64_t)round * 32 + lane) * gstride;
-        if (t < ntiles) {
-            const int pt = phys((int)t);
-            g0 = __ldg(prm.key_tile_base + pt);
-            g1 = __ldg(prm.key_tile_base + pt + 1);
-        }
-    };
-    int issued = 0;          // the warp's tiles issued so far (warp-uniform)
-    uint32_t infos = 0;      // lane 0: byte b = descriptor of the tile in flight in stage b
-    // all lanes: issue the warp's next tile into stage b
-    auto issue_next = [&](int b) {
-        if ((issued & 31) == 0 && issued) {
-            cur_g0 = nxt_g0;
-            cur_g1 = nxt_g1;
-            ring_load((issued >> 5) + 1, nxt_g0, nxt_g1);
-        }
-        const uint64_t g0 = __shfl_sync(full, cur_g0, issued & 31), g1 = __shfl_sync(full, cur_g1, issued & 31);
-        if (lane == 0) {
-            const uint32_t d = issue(phys(tile0 + issued * gstride), b, g0, g1);
-            infos = (infos & ~(0xffu << (8 * b))) | (d << (8 * b));
-        }
-        issued++;
-    };
-    if (HASH) {
-        ring_load(0, cur_g0, cur_g1);
-        ring_load(1, nxt_g0, nxt_g1);
-        for (int b = 0; b < S - 1 && tile0 + b * gstride < ntiles; b++) issue_next(b);
-    }
-
-    // the body of one tile; FULL = every record of the tile exists (no tail predicates)
-    auto body = [&](auto full_tag, int tile, int buf, uint32_t info) {
+    // one tile; FULL = every record of the tile exists (no tail predicates)
+    auto scan_tile = [&](auto full_tag, int tile, int buf, TileDesc d) {
         constexpr bool FULL = decltype(full_tag)::value;
-        const uint32_t st = stage0 + (uint32_t)buf * STAGE;
-        auto wait_stage = [&]() {
-            mbar_wait(mbar + 8u * buf, (phase >> buf) & 1u);
-            phase ^= 1u << buf;
-        };
-        // ---- header columns: 4 rows of 32 consecutive records, from the stage or fully coalesced from global ----
         const int64_t rbase = (int64_t)tile * TILE + lane;
-        int p[ROWS], kl[ROWS], vl[ROWS];
-        long long ts[ROWS];
-        bool valid[ROWS];
-        if (HASH && (info & 32u)) {   // staged ⇒ FULL
-            wait_stage();
-#pragma unroll
-            for (int k = 0; k < ROWS; k++) {
-                const uint32_t r = 32u * k + lane;
-                valid[k] = true;
-                p[k] = (int)lds32(st + KEYBUF + HDR_P + 4u * r);
-                ts[k] = lds64(st + KEYBUF + HDR_TS + 8u * r);
-                kl[k] = (int)lds32(st + KEYBUF + HDR_KL + 4u * r);
-                vl[k] = (int)lds32(st + KEYBUF + HDR_VL + 4u * r);
-            }
-        } else {
-#pragma unroll
-            for (int k = 0; k < ROWS; k++) {
-                const int64_t r = rbase + 32 * k;
-                valid[k] = FULL || r < prm.n;
-                if (valid[k]) {
-                    if (HINTS) {
-                        p[k] = ld_stream_s32(prm.partition + r, pol_stream);
-                        ts[k] = ld_stream_s64(prm.ts_ms + r, pol_stream);
-                        kl[k] = ld_stream_s32(prm.key_len + r, pol_stream);
-                        vl[k] = ld_stream_s32(prm.value_len + r, pol_stream);
-                    } else {
-                        p[k] = ld_stream_s32(prm.partition + r);
-                        ts[k] = ld_stream_s64(prm.ts_ms + r);
-                        kl[k] = ld_stream_s32(prm.key_len + r);
-                        vl[k] = ld_stream_s32(prm.value_len + r);
-                    }
-                } else {
-                    p[k] = 0; ts[k] = INT64_MAX; kl[k] = -1; vl[k] = -1;
-                }
-            }
-        }
-        // ---- MessageMetrics::handle_message (metric.rs:206-253) ----
-        // A record whose partition lies outside [0, P) is counted in `bad` and takes part in NOTHING else (counters, extrema,
-        // alive keys, sketch), so the state stays consistent; its key bytes still occupy their place in the packed keys.
-        bool use[ROWS];
-        bool inrange = true;
-#pragma unroll
-        for (int k = 0; k < ROWS; k++) {
-            bool ok = (unsigned)p[k] < (unsigned)prm.P;
-            if (SHARD) {
-                // partition → column: c = p / G, and the partition must be one of this shard's (p - c G == rank);
-                // others are left out like out-of-range ones.  From here on p[k] is the column.
-                const int c = (int)__umulhi((uint32_t)p[k], prm.shard_magic);
-                ok = ok && p[k] - c * prm.shard_world == prm.shard_rank;
-                p[k] = ok ? c : 0;
-            }
-            use[k] = valid[k] && ok;
-            inrange = inrange && ok;
-        }
-        const bool clean = FULL && __all_sync(full, inrange);   // warp-uniform: every record of the tile exists and counts
+        TileRows rec;
+        load_headers<FULL>(prm, pipe, buf, d, rbase, lane, rec);
+        partition_check<FULL, SHARD>(prm, rec);
         uint32_t h[ROWS] = {0u, 0u, 0u, 0u};   // the reference hash of each of the lane's four keys (0 for null keys)
         // The two halves of the per-record work are independent of each other: MODE_EXACT runs the hashes FIRST, sends the
         // seen-cache probes off, and counts while they are in flight; the other modes count first (the key bytes arrive later).
-        auto count_records = [&]() {
-            if (!count_it) {
-                // stamps-only re-run: the counters and extrema of this batch were taken by the first pass
-            } else if (clean) {
-                if (try_uni) {
-                    // run-structured input (a Kafka fetch delivers long runs of one partition).
-                    // A whole tile inside one run (3 of 4 tiles at run length 500): one vote, the lane's four lengths added up
-                    // first, two warp reductions and two adds for the tile
-                    const int p0t = __shfl_sync(full, p[0], 0);
-                    uint32_t kv4 = 0, vv4 = 0, big = 0;
-                    bool one = true;
-#pragma unroll
-                    for (int k = 0; k < ROWS; k++) {
-                        const uint32_t kv = (uint32_t)max(kl[k], 0), vv = (uint32_t)max(vl[k], 0);
-                        one = one && p[k] == p0t;
-                        kv4 += kv; vv4 += vv; big |= kv | vv;
-                    }
-                    if (__all_sync(full, one && big < (1u << 24))) {
-#pragma unroll
-                        for (int k = 0; k < ROWS; k++) C.buckets(p0t, kl[k], vl[k]);
-                        const uint32_t ks = __reduce_add_sync(full, kv4);   // 128 lengths < 2^24: no overflow
-                        const uint32_t vs = __reduce_add_sync(full, vv4);
-                        if (lane == 0) {
-                            C.sum_add(0, p0t, ks);
-                            C.sum_add(1, p0t, vs);
-                        }
-                    } else {
-                    // otherwise row by row: the byte sums of a row that lies inside one run are reduced in the warp (2 REDUX)
-                    // and added once, instead of 32 same-address adds
-                    bool any_uni = false;
-#pragma unroll
-                    for (int k = 0; k < ROWS; k++) {
-                        C.buckets(p[k], kl[k], vl[k]);
-                        const int p0 = __shfl_sync(full, p[k], 0);
-                        const unsigned m0 = __ballot_sync(full, p[k] == p0);
-                        const bool small_row = __all_sync(full, (kl[k] | vl[k]) < (1 << 26));
-                        const uint32_t kv = (uint32_t)max(kl[k], 0), vv = (uint32_t)max(vl[k], 0);
-                        if (m0 == full && small_row) {
-                            const uint32_t ks = __reduce_add_sync(full, kv);   // each < 2^26: no overflow
-                            const uint32_t vs = __reduce_add_sync(full, vv);
-                            if (lane == 0) {
-                                C.sum_add(0, p0, ks);
-                                C.sum_add(1, p0, vs);
-                            }
-                            any_uni = true;
-                        } else {
-                            // a row that straddles a run boundary holds two partitions: left to per-lane adds, its two
-                            // counters would be hit 32 times each, serialised in the shared-memory pipe.  Reduce the two groups separately instead.
-                            const int l1 = __ffs(~m0) - 1;                     // first lane of the second group
-                            const int p1 = __shfl_sync(full, p[k], l1 & 31);
-                            const unsigned m1 = __ballot_sync(full, p[k] == p1);
-                            if (small_row && (m0 | m1) == full) {
-                                const bool in0 = (m0 >> lane) & 1u;
-                                const uint32_t ks0 = __reduce_add_sync(full, in0 ? kv : 0u), vs0 = __reduce_add_sync(full, in0 ? vv : 0u);
-                                const uint32_t ks1 = __reduce_add_sync(full, in0 ? 0u : kv), vs1 = __reduce_add_sync(full, in0 ? 0u : vv);
-                                if (lane == 0) {
-                                    C.sum_add(0, p0, ks0);
-                                    C.sum_add(1, p0, vs0);
-                                } else if (lane == l1) {
-                                    C.sum_add(0, p1, ks1);
-                                    C.sum_add(1, p1, vs1);
-                                }
-                                any_uni = true;
-                            } else {
-                                C.sums(p[k], kl[k], vl[k]);
-                            }
-                        }
-                    }
-                    try_uni = any_uni;
-                    }
-                } else {
-                    C.record_rows(p, kl, vl);
-                }
-            } else {
-                // tail tile, or a record with a partition outside [0, P): per-record checks
-#pragma unroll
-                for (int k = 0; k < ROWS; k++) {
-                    if (use[k]) C.record(p[k], kl[k], vl[k]);
-                    else if (valid[k]) bad++;
-                }
-            }
-            // metric.rs:209,247: None → 0 and ms → s are monotone maps, applied once at read-back: the raw
-            // extrema determine the mapped extrema (raw == -1 ⇔ mapped 0, see kta_timestamps).
-            // Timestamps of one topic share their high word for 49 days at a time: when the lane's four and its running
-            // extrema do, the signed 64-bit order is the unsigned order of the low words (2 + 2 three-input min/max).
-            bool ts_fast = false;
-            if (clean && count_it) {
-                const uint32_t hw = hi32(tmin);
-                uint32_t x = hi32(tmax) ^ hw;
-#pragma unroll
-                for (int k = 0; k < ROWS; k++) x |= hi32(ts[k]) ^ hw;
-                ts_fast = x == 0;
-            }
-            if (ts_fast) {
-                const uint32_t hw = hi32(tmin);
-                const uint32_t l0 = (uint32_t)ts[0], l1 = (uint32_t)ts[1], l2 = (uint32_t)ts[2], l3 = (uint32_t)ts[3];
-                const uint32_t lo = min(min(min(l0, l1), l2), min(l3, (uint32_t)tmin));
-                const uint32_t hi = max(max(max(l0, l1), l2), max(l3, (uint32_t)tmax));
-                tmin = pack64(lo, hw);
-                tmax = pack64(hi, hw);
-            } else if (count_it) {
-                asm volatile("");   // keep this a real branch: if-converted, the 64-bit chain runs every tile
-#pragma unroll
-                for (int k = 0; k < ROWS; k++) {
-                    const bool u = clean || use[k];
-                    const long long t0 = u ? ts[k] : INT64_MAX, t1 = u ? ts[k] : INT64_MIN;
-                    tmin = t0 < tmin ? t0 : tmin;
-                    tmax = t1 > tmax ? t1 : tmax;
-                }
-            }
-            if (count_it) {
-#pragma unroll
-                for (int k = 0; k < ROWS; k++) {
-                    // metric.rs:249-251: size extrema, not for tombstones (rows that do not exist carry vl = -1)
-                    const uint32_t sz = (uint32_t)max(kl[k], 0) + (uint32_t)vl[k];
-                    if (vl[k] >= 0 && (clean || use[k])) {
-                        smin = min(smin, sz);
-                        smax = max(smax, sz);
-                    }
-                }
-            }
-
-        };
-        auto hash_keys = [&]() {
-            // ---- byte offset of each key inside the tile: exclusive scan of max(key_len, 0) ----
-            uint32_t off[ROWS];
-            // do all keys of this tile that are not null have ONE length L?  L = the longest; read as unsigned, null (-1)
-            // is the largest value, so the unsigned minimum is the shortest non-null key (or "null" if there is none):
-            // one length ⇔ the two agree.  Two three-input min/max per lane and two warp reductions.
-            const int lmax = max(max(kl[0], kl[1]), max(kl[2], kl[3]));
-            const uint32_t lmin = min(min((uint32_t)kl[0], (uint32_t)kl[1]), min((uint32_t)kl[2], (uint32_t)kl[3]));
-            static_assert(ROWS == 4, "written out for four rows");
-            const int L = __reduce_max_sync(full, lmax);   // -1 when every key is null
-            const bool fixL = __reduce_min_sync(full, lmin) == (uint32_t)L && L < (1 << 16);
-            const bool small = L < (1 << 20);              // warp-uniform
-            const bool fix16 = fixL && L == 16;
-            if (fixL) {
-                // fixed-width keys (the common case: ids, hashes, UUIDs)
-                const uint32_t Lu = (uint32_t)max(L, 0);
-                if (!__any_sync(full, (kl[0] | kl[1] | kl[2] | kl[3]) < 0)) {
-                    // no null key in the tile (every tile of a keyed / compacted topic): record r's key is the r-th
-#pragma unroll
-                    for (int k = 0; k < ROWS; k++) off[k] = Lu * (uint32_t)(32 * k + lane);
-                } else {
-                    // offsets from ballots, no shuffle scan
-                    uint32_t before = 0;
-#pragma unroll
-                    for (int k = 0; k < ROWS; k++) {
-                        const unsigned m = __ballot_sync(full, kl[k] >= 0);
-                        off[k] = Lu * (before + __popc(m & lt_mask));
-                        before += __popc(m);
-                    }
-                }
-            } else {
-                static_assert(ROWS == 4, "the packed scan below handles exactly four rows");
-                uint32_t mxl = 0;
-#pragma unroll
-                for (int k = 0; k < ROWS; k++) mxl = max(mxl, (uint32_t)max(kl[k], 0));
-                if (__all_sync(full, mxl < 2048u)) {
-                    // short keys (every row sums to < 2^16): scan two rows per 32-bit word, 10 shuffles instead of 20
-                    const uint32_t v0 = (uint32_t)max(kl[0], 0), v1 = (uint32_t)max(kl[1], 0);
-                    const uint32_t v2 = (uint32_t)max(kl[2], 0), v3 = (uint32_t)max(kl[3], 0);
-                    uint32_t a = v0 | (v1 << 16), b = v2 | (v3 << 16);
-#pragma unroll
-                    for (int d = 1; d < 32; d <<= 1) {
-                        const uint32_t ta = __shfl_up_sync(full, a, d), tb = __shfl_up_sync(full, b, d);
-                        if (lane >= d) { a += ta; b += tb; }
-                    }
-                    const uint32_t ea = __shfl_sync(full, a, 31), eb = __shfl_sync(full, b, 31);
-                    const uint32_t t0 = ea & 0xffffu, t1 = ea >> 16, t2 = eb & 0xffffu;
-                    off[0] = (a & 0xffffu) - v0;
-                    off[1] = t0 + (a >> 16) - v1;
-                    off[2] = t0 + t1 + (b & 0xffffu) - v2;
-                    off[3] = t0 + t1 + t2 + (b >> 16) - v3;
-                } else if (small) {
-                    uint32_t c32 = 0;
-#pragma unroll
-                    for (int k = 0; k < ROWS; k++) {
-                        const uint32_t v = (uint32_t)max(kl[k], 0);
-                        uint32_t inc = v;
-#pragma unroll
-                        for (int d = 1; d < 32; d <<= 1) {
-                            const uint32_t t = __shfl_up_sync(full, inc, d);
-                            if (lane >= d) inc += t;
-                        }
-                        off[k] = c32 + inc - v;
-                        c32 += __shfl_sync(full, inc, 31);
-                    }
-                }
-            }
-            const uint32_t kb = st;   // the key part of the stage
-            if (info & 1u) {   // staged ⇒ the tile's keys fit one stage (<= 16 KiB) ⇒ small
-                const uint32_t a0 = (info >> 1) & 15u;
-                if (!(info & 32u)) wait_stage();   // else done before the headers were read
-#ifdef KTA_EXP_NO_FNV
-                if (fix16 && a0 == 0) {
-#pragma unroll
-                    for (int k = 0; k < ROWS; k++) h[k] = lds32(kb + off[k]);
-                } else
-#endif
-                if (fix16 && a0 == 0) {
-                    // two independent FNV chains at a time per lane, one LDS.128 per key (null keys hash
-                    // garbage that is never used); the other warps of the SM sub-partition supply the rest of the ILP
-#pragma unroll
-                    for (int k = 0; k < ROWS; k += 2) {
-                        const uint4 qa = lds128(kb + off[k]);
-                        const uint4 qb = lds128(kb + off[k + 1]);
-                        uint32_t ha = FNV_BASIS, hb = FNV_BASIS;
-                        ha = fnv_word(ha, qa.x); hb = fnv_word(hb, qb.x);
-                        ha = fnv_word(ha, qa.y); hb = fnv_word(hb, qb.y);
-                        ha = fnv_word(ha, qa.z); hb = fnv_word(hb, qb.z);
-                        ha = fnv_word(ha, qa.w); hb = fnv_word(hb, qb.w);
-                        h[k] = ha;
-                        h[k + 1] = hb;
-                    }
-                } else {
-#pragma unroll
-                    for (int k = 0; k < ROWS; k++) h[k] = kl[k] >= 0 ? fnv_smem(kb, a0 + off[k], kl[k]) : 0u;
-                }
-            } else if (fixL || small) {
-                const uint64_t g0 = prm.key_tile_base[tile];
-#pragma unroll
-                for (int k = 0; k < ROWS; k++)
-                    h[k] = (valid[k] && kl[k] >= 0) ? fnv_global(prm.key_bytes + g0 + off[k], kl[k]) : 0u;
-            } else {
-                uint32_t *scratch = reinterpret_cast<uint32_t *>(wsm + 128 + (size_t)buf * STAGE);  // keys not staged: free
-                wide_tile_hashes(prm.key_len, prm.n, prm.key_bytes + prm.key_tile_base[tile], tile, scratch, lane);
-#pragma unroll
-                for (int k = 0; k < ROWS; k++) h[k] = scratch[32 * k + lane];
-            }
-
-
-            // ---- LogCompactionInMemoryMetrics::handle_message, metric.rs:288-305 ----
-            if (CAPTURE) {
-#pragma unroll
-                for (int k = 0; k < ROWS; k++)
-                    if (valid[k]) prm.hash_out[rbase + 32 * k] = kl[k] >= 0 ? h[k] : 0u;
-            }
-        };
-        if (MODE != MODE_EXACT) count_records();
-        if (HASH) hash_keys();
+        if (MODE != MODE_EXACT) count_tile(C, rec, count_it, lane, tot);
+        if (HASH) hash_tile<CAPTURE>(prm, pipe, buf, d, tile, rbase, rec, key_offsets(rec.kl, lane), lane, h);
         if (MODE == MODE_EXACT) {
-            // metric.rs:291-302: Some(key) → insert (value) / remove (tombstone); None → nothing.
-            // Last-writer-wins per hash in seq order IS the BitSet insert/remove sequence replayed in order
-            // (metric.rs:295 mark_key_alive, :298 mark_key_dead).
-            // What limits this mode is the L1 pipe — a divergent 32-lane global access costs it ~2 cycles per lane — and
-            // latency, not DRAM.  So: exactly ONE random access per record (the seen cache, in flight while the records
-            // are counted); the ~12 % that survive it are compacted across the tile into one dense queue (in the key part of
-            // the stage the tile has just finished with) and take the exact path through the table, usually in a single pass.
-            static_assert(TILE * 16 <= KEYBUF_MIN, "the queue stays inside the key part of the stage");
-            uint4 *queue = reinterpret_cast<uint4 *>(wsm + 128 + (size_t)buf * STAGE);   // (x, low word, set word, -) x TILE
-            const bool cached = AW.cache != nullptr;
-            const uint32_t r32 = (uint32_t)rbase;   // index in the batch (< 2^31: host-checked)
-            uint32_t x[ROWS], low[ROWS], cw[ROWS];
-            bool live[ROWS];
-#pragma unroll
-            for (int k = 0; k < ROWS; k++) {
-                live[k] = (clean || use[k]) && kl[k] >= 0;
-                uint32_t field;
-                if (prm.seq) {
-                    // explicit global sequence numbers (partition-sharded scans): must fall into the table's window
-                    const uint64_t f = live[k] ? ld_stream_u64(prm.seq + rbase + 32 * k) - prm.alive_origin + 1ull : 1ull;
-                    if (f - 1ull >= (uint64_t)ALIVE_FIELD_MAX) {
-                        atomicAdd(prm.alive_status + 1, 1u);
-                        live[k] = false;
-                    }
-                    field = (uint32_t)f;
-                } else {
-                    field = (uint32_t)prm.alive_fbase + r32 + 32u * k;   // host-checked: seq_base + n fits the window
-                }
-                low[k] = (field << 1) | (vl[k] >= 0 ? 1u : 0u);
-                x[k] = hll_mix(h[k]);
-                cw[k] = 0;
-                if (cached && live[k]) cw[k] = alive_cache_ld(AW.cache + (x[k] >> ALIVE_CACHE_TAG_BITS), AT.pol);
-            }
-            count_records();   // ~250 instructions while the probes are in flight
-#if KTA_EXP_ALIVE_STAGE >= 1
-            __syncwarp();      // every lane is done reading its keys from this stage before any lane overwrites it
-            uint32_t qn = 0;   // warp-uniform
-#pragma unroll
-            for (int k = 0; k < ROWS; k++) {
-                const bool go = live[k] && !(cached && alive_cache_newer(cw[k], x[k], alive_wave(low[k] >> 1, AW)));
-                const unsigned m = __ballot_sync(full, go);
-                if (go) queue[qn + __popc(m & lt_mask)] = make_uint4(x[k], low[k], cw[k], 0u);
-                qn += __popc(m);
-            }
-            __syncwarp();
-#if KTA_EXP_ALIVE_STAGE >= 2
-            for (uint32_t q0 = 0; q0 < qn; q0 += 32) {
-                if (q0 + lane < qn) {
-                    const uint4 item = queue[q0 + lane];
-#if KTA_EXP_ALIVE_STAGE == 3   // ablation: the survivors update the seen cache but never go to the table
-                    const uint32_t newest = item.y;
-#else
-                    const uint32_t pr = alive_home(item.x, AT.npairs);
-                    const ulonglong2 e = alive_ld_pair(AT.slots + 2 * (size_t)pr, AT.pol);
-                    const uint32_t newest = alive_stamp(AT, pr, e, item.x, item.y);
-#endif
-                    // tell the cache what the table knows now: the newest stamp of this hash as a wave of THIS batch (0 =
-                    // older than the batch: says nothing), or the record's own wave
-                    if (cached)
-                        alive_cache_put(AW.cache, item.z, item.x, max(alive_wave(item.y >> 1, AW), alive_wave(newest >> 1, AW)), newest >> 1);
-                }
-            }
-#endif
-            // the queue lives in a key stage that the TMA engine refills next iteration: order these generic-proxy
-            // accesses before that async-proxy write
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            __syncwarp();
-#endif
+            unsigned char *queue = pipe.stage_ptr(buf);   // the resolve queue: the key part of the stage just read
+            const ExactProbe e = exact_probe(prm, AT, AW, rec, h, rbase);
+            count_tile(C, rec, count_it, lane, tot);   // ~250 instructions while the probes are in flight
+            exact_resolve(AT, AW, e, queue, lane, lt_mask);
         }
-#ifndef KTA_EXP_NO_HLL
-        if (MODE == MODE_HLL) {
-            const uint32_t skip_mask = hll_skip_mask(prm.hll_p, floor_reg);
-#pragma unroll
-            for (int k = 0; k < ROWS; k++) {
-                // in-stream sketch: every record with a key and a value (invalid rows carry kl = vl = -1)
-                const uint32_t x = hll_mix(h[k]);
-                if (((x & skip_mask) | (uint32_t)((kl[k] | vl[k]) >> 31)) == 0 && (clean || use[k])) hll_raise(prm.hll, prm.hll_p, x);
-            }
-        }
-#else
-        if (MODE == MODE_HLL) {   // experiment: keep the hashes alive without the sketch
-            if ((h[0] ^ h[1] ^ h[2] ^ h[3]) == 0x12345678u) prm.hll[0] = 1;
-        }
-#endif
+        if (MODE == MODE_HLL) sketch_tile(prm, floor_reg, rec, h);
     };
 
     int buf = 0;   // stage of this tile: it % S
     for (int it = 0; tile < ntiles; tile += gstride, ++it) {
-        uint32_t info = 0;
-        if (HASH) {
-            info = (__shfl_sync(full, infos, 0) >> (8 * buf)) & 0xffu;   // also: every lane is done with the previous stage
-            // the tile S - 1 ahead goes into the stage the previous tile has just finished with
-            if (tile < ntiles - (S - 1) * gstride) issue_next(buf == 0 ? S - 1 : buf - 1);   // no overflow: gstride <= SMs * 32
-        }
-        const int pt = phys(tile);
-        if ((int64_t)(pt + 1) * TILE <= prm.n) body(std::true_type{}, pt, buf, info);
-        else body(std::false_type{}, pt, buf, info);
+        const TileDesc d = HASH ? pipe.next(tile, buf) : TileDesc{0u};
+        const int pt = pipe.phys(tile);
+        if ((int64_t)(pt + 1) * TILE <= prm.n) scan_tile(std::true_type{}, pt, buf, d);
+        else scan_tile(std::false_type{}, pt, buf, d);
         if (HASH) buf = buf + 1 == S ? 0 : buf + 1;
         // every warp examines the CTA's split sums after every 8th tile of its own (bound: see fold_sums)
         if (SMEM && (it & (FOLD_TILES - 1)) == FOLD_TILES - 1) C.fold_sums(lane, 1u << 30);
-        try_uni = try_uni || (it & 15) == 15;   // re-probe for run-structured input now and then
+        tot.try_uni = tot.try_uni || (it & 15) == 15;   // re-probe for run-structured input now and then
         // HLL floor upkeep: every 4th tile ONE warp of each CTA (the role rotates, so no warp falls behind)
         // refreshes one slice — the 132 CTAs of an H100 cover all 64 slices about every two tile-times — and republishes
         // the floor (plus two early refreshes after the first and second tile, so that a cold sketch stops taking every
@@ -1302,56 +1385,8 @@ __global__ void __launch_bounds__(MODE == MODE_COUNTERS ? MAX_THREADS : HASH_MAX
 
     // ---- flush CTA-private state ----
     __syncthreads();
-    if (SMEM) {
-        // bucket rows → global [which][p][bucket]; row 32 → knull; row 65 (tombstones) is derived, not stored
-        const int nh = (ROW_V + NB) * P;
-        for (int i = tid; i < nh; i += blockDim.x) {
-            const uint32_t v = scnt[i];
-            if (v) {
-                const int row = i / P, pp = C.part(i - row * P);
-                if (row < NB) atomicAdd(&prm.sums[(size_t)pp * NB + row], (unsigned long long)v);
-                else if (row == NB) atomicAdd(&prm.sums[(size_t)prm.P * (2 * NB + 2) + pp], (unsigned long long)v);
-                else atomicAdd(&prm.sums[(size_t)(prm.P + pp) * NB + (row - ROW_V)], (unsigned long long)v);
-            }
-        }
-        if (warp == 0) C.fold_sums(lane, 1u);
-    }
-    // extrema + bad-partition count: warp shuffle, then one lane per warp, then one thread per CTA
-    long long smin64 = smin != 0xffffffffu ? (long long)smin : INT64_MAX;
-    long long smax64 = smin != 0xffffffffu ? (long long)smax : -1;
-#pragma unroll
-    for (int d = 16; d; d >>= 1) {
-        const long long a = __shfl_xor_sync(full, tmin, d), b = __shfl_xor_sync(full, tmax, d);
-        const long long c = __shfl_xor_sync(full, smin64, d), e = __shfl_xor_sync(full, smax64, d);
-        tmin = a < tmin ? a : tmin;
-        tmax = b > tmax ? b : tmax;
-        smin64 = c < smin64 ? c : smin64;
-        smax64 = e > smax64 ? e : smax64;
-        bad += __shfl_xor_sync(full, bad, d);
-    }
-    long long *red = reinterpret_cast<long long *>(wsm + 64);   // per-warp scratch (4 × i64)
-    if (lane == 0) {
-        red[0] = tmin; red[1] = tmax; red[2] = smin64; red[3] = smax64;
-        if (bad) atomicAdd(&prm.sums[sums_words(prm.P) - 1], (unsigned long long)bad);
-    }
-    __syncthreads();
-    if (tid == 0) {
-        for (int w = 1; w < nwarps; w++) {
-            const long long *rw = reinterpret_cast<const long long *>(wsm + (size_t)w * warp_bytes + 64);
-            tmin = rw[0] < tmin ? rw[0] : tmin;
-            tmax = rw[1] > tmax ? rw[1] : tmax;
-            smin64 = rw[2] < smin64 ? rw[2] : smin64;
-            smax64 = rw[3] > smax64 ? rw[3] : smax64;
-        }
-        if (tmin != INT64_MAX) {
-            atomicMin(&prm.minmax[0], tmin);
-            atomicMax(&prm.minmax[1], tmax);
-        }
-        if (smax64 >= 0) {
-            atomicMin(reinterpret_cast<unsigned long long *>(&prm.minmax[2]), (unsigned long long)smin64);
-            atomicMax(reinterpret_cast<unsigned long long *>(&prm.minmax[3]), (unsigned long long)smax64);
-        }
-    }
+    if (SMEM) flush_counters(prm, C, tid, warp, lane);
+    flush_totals(prm, tot, wsm, warp_bytes, tid, lane, nwarps);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1450,7 +1485,7 @@ __global__ void __launch_bounds__(THREADS) alive_export_kernel(const unsigned lo
 __global__ void __launch_bounds__(THREADS) alive_import_kernel(const AliveTable t, uint64_t origin, const uint32_t *hash,
                                                                const unsigned long long *stamp, int64_t count) {
     AliveTable tt = t;
-    tt.pol = KTA_L2_HINTS ? l2_policy_evict_last() : 0;
+    tt.pol = l2_policy_evict_last();
     const int64_t stride = (int64_t)gridDim.x * THREADS;
     for (int64_t i = (int64_t)blockIdx.x * THREADS + threadIdx.x; i < count; i += stride) {
         const unsigned long long st = stamp[i];
