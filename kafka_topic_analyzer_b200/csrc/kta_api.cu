@@ -126,7 +126,8 @@ struct kta_handle {
     int32_t *d_dec_part = nullptr, *d_dec_klen = nullptr, *d_dec_vlen = nullptr; int64_t *d_dec_ts = nullptr; int64_t dec_rec_cap = 0;
     uint8_t *d_dec_keys = nullptr; int64_t dec_key_cap = 0;
     uint64_t *d_dec_ksrc = nullptr;          // per decoded record: where its key bytes lie in the segment buffer
-    uint8_t *d_unc = nullptr; int64_t unc_cap = 0;   // uncompressed images of LZ4 / Snappy batches
+    uint8_t *d_unc = nullptr; int64_t unc_cap = 0;   // uncompressed images of compressed batches
+    uint8_t *d_unc_lit = nullptr; int64_t unc_lit_cap = 0;   // zstd: Huffman-decoded literals, at the offsets of d_unc
     uint64_t *d_unc_slot = nullptr; int64_t unc_slot_cap = 0;
     uint32_t *d_log_err = nullptr;
     size_t nsums = 0, nhll = 0;
@@ -290,7 +291,7 @@ extern "C" int kta_destroy(kta_handle *h) {
     cudaFree(h->d_sums); cudaFree(h->d_minmax); cudaFree(h->d_hll); cudaFree(h->d_alive_table);
     cudaFree(h->d_alive_status); cudaFree(h->d_alive_cache); cudaFreeHost(h->h_alive_status); cudaFree(h->d_scalar); cudaFree(h->d_tb_scratch);
     cudaFree(h->d_log_bytes); cudaFree(h->d_log_off); cudaFree(h->d_log_info); cudaFree(h->d_log_cnt);
-    cudaFree(h->d_dec_part); cudaFree(h->d_dec_klen); cudaFree(h->d_dec_vlen); cudaFree(h->d_dec_ts); cudaFree(h->d_dec_keys); cudaFree(h->d_dec_ksrc); cudaFree(h->d_unc); cudaFree(h->d_unc_slot);
+    cudaFree(h->d_dec_part); cudaFree(h->d_dec_klen); cudaFree(h->d_dec_vlen); cudaFree(h->d_dec_ts); cudaFree(h->d_dec_keys); cudaFree(h->d_dec_ksrc); cudaFree(h->d_unc); cudaFree(h->d_unc_lit); cudaFree(h->d_unc_slot);
     cudaFree(h->d_log_err);
     for (auto &e : h->ev_pool) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
     if (h->stream && h->own_stream) cudaStreamDestroy(h->stream);
@@ -726,7 +727,7 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     CU(cudaMemcpyAsync(err, h->d_log_err, 8, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     if (err[0] & LOGB_COMPRESSED)
-        return fail(KTA_ERR_INVALID, "zstd record batches are not supported (gzip, LZ4 and Snappy are decompressed on the GPU)");
+        return fail(KTA_ERR_INVALID, "unknown compression codec (attributes bits 0-2 = 5..7) in partition %d", partition);
     if (err[0] & LOGB_BAD) return fail(KTA_ERR_INVALID, "malformed record batch header in partition %d", partition);
     if (nrec == 0) return KTA_OK;
     if (err[0] & LOGB_CODECS) {
@@ -734,20 +735,32 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
         // happen to lie in the scratch buffer
         if ((rc = grow(s, h->unc_slot_cap, nbatches + 2, h->d_unc_slot))) return rc;
         CU(cudaMemsetAsync(h->d_log_err, 0, 4, s));
+        const uint32_t codecs = err[0] & LOGB_CODECS;   // (err is reused for the size pass's flags below)
+        const bool zstd = (codecs & LOGB_ZSTD) != 0;
+        const int wgrid = (int)std::min<int64_t>((nbatches + 3) / 4, (int64_t)h->sm_count * 16);   // warp per batch
         log_unc_size_kernel<<<grid, 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_log_err);
+        if (zstd) log_zstd_size_kernel<<<wgrid, 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_log_err);
         tile_base_scan_kernel<<<1, 1024, 0, s>>>(h->d_unc_slot, nbatches);
         CU(cudaGetLastError());
-        h->launches += 2;
+        h->launches += zstd ? 3 : 2;
         uint64_t unc_total = 0;
         CU(cudaMemcpyAsync(&unc_total, h->d_unc_slot + nbatches, 8, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(err, h->d_log_err, 4, cudaMemcpyDeviceToHost, s));
         CU(cudaStreamSynchronize(s));
         if (err[0]) return fail(KTA_ERR_INVALID, "malformed compressed record batch in partition %d", partition);
         if ((rc = grow(s, h->unc_cap, (int64_t)unc_total + 64, h->d_unc))) return rc;
-        log_decompress_kernel<<<(int)std::min<int64_t>((nbatches + 3) / 4, (int64_t)h->sm_count * 16), 128, 0, s>>>(
-            dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_unc, h->d_log_err);
+        // zstd's literal buffer has the size of the scratch buffer (a block's literals go at its output's offset); it is
+        // only allocated once zstd batches are seen
+        if (zstd && (rc = grow(s, h->unc_lit_cap, (int64_t)unc_total + 64, h->d_unc_lit))) return rc;
+        if (codecs & ~(uint32_t)LOGB_ZSTD) {
+            log_decompress_kernel<false><<<wgrid, 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_unc, nullptr, h->d_log_err);
+            h->launches++;
+        }
+        if (zstd) {
+            log_decompress_kernel<true><<<wgrid, 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_unc, h->d_unc_lit, h->d_log_err);
+            h->launches++;
+        }
         CU(cudaGetLastError());
-        h->launches++;
     }
     if ((int64_t)nrec >= ((int64_t)1 << 31) - 2) return fail(KTA_ERR_INVALID, "%llu records in one call: split the segments", (unsigned long long)nrec);
     const bool hash = h->need_hash || h->d_hash_out;

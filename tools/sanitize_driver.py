@@ -11,7 +11,7 @@ from kafka_topic_analyzer_b200 import synth
 from parity import assert_parity, oracle_for
 
 NOW = (4102444800, 1)
-which = sys.argv[1:] or ["counters", "hll", "exact", "ragged", "ring", "log", "logz"]
+which = sys.argv[1:] or ["counters", "hll", "exact", "ragged", "ring", "log", "logz", "logzstd"]
 
 
 def compress_segment(seg, b0=0):
@@ -35,13 +35,37 @@ def compress_segment(seg, b0=0):
         b += 1
     return np.frombuffer(bytes(out), dtype=np.uint8)
 
+
+def zstd_segment(seg, b0=0):
+    """every batch of an uncompressed segment re-written as zstd: one-shot (Frame_Content_Size), streaming (none) or left
+    uncompressed, in turn"""
+    import pyarrow as pa
+    raw, out, pos, b = seg.tobytes(), bytearray(), 0, b0
+    while pos + 61 <= len(raw):
+        bl = int.from_bytes(raw[pos + 8:pos + 12], "big", signed=True)
+        hdr, body = bytearray(raw[pos:pos + 61]), raw[pos + 61:pos + 12 + bl]
+        if b % 3 == 0:
+            body = pa.compress(body, codec="zstd", asbytes=True)
+        elif b % 3 == 1:
+            sink = pa.BufferOutputStream()
+            with pa.CompressedOutputStream(sink, "zstd") as z:
+                z.write(body)
+            body = sink.getvalue().to_pybytes()
+        if b % 3 != 2:
+            hdr[8:12] = (49 + len(body)).to_bytes(4, "big")
+            hdr[22] |= 4
+        out += hdr + body
+        pos += 12 + bl
+        b += 1
+    return np.frombuffer(bytes(out), dtype=np.uint8)
+
 P = 8
 n = P * 4096 + 0
 for name in which:
     key_mode = 2 if name in ("ragged", "ring") else 0
     spec = synth.make_spec(n, P, key_mode=key_mode, distinct_keys=3000, tombstone_per_10k=2500, ts_missing_per_10k=20,
                            run_len=64 if name == "counters" else 1)
-    if name in ("log", "logz"):
+    if name in ("log", "logz", "logzstd"):
         host = synth.fill_host(spec)
         o = oracle_for(host, count_alive_keys=True, now=NOW)
         with kta.KtaEngine(P, count_alive_keys=True, hll_precision=10, device=0, now=NOW, alive_table_kib=1) as e:
@@ -49,6 +73,8 @@ for name in which:
             segs = [(p, synth.encode_segment(spec, p, 0, per, batch_records=100)) for p in range(P)]
             if name == "logz":   # gzip / LZ4 / Snappy batches: the decompressors run first
                 segs = [(p, compress_segment(s, p)) for p, s in segs]
+            if name == "logzstd":   # zstd one-shot / streaming batches and uncompressed ones
+                segs = [(p, zstd_segment(s, p)) for p, s in segs]
             e.push_log_segments(segs)
             e.finalize()
             got = (e.message_metrics.overall_count(), e.alive_keys())
