@@ -21,6 +21,7 @@
 
 #include "kta_kernels.cuh"
 #include "kta_logdecode.cuh"
+#include "kta_logdecode_launch.cuh"
 #include "kta_synth.h"
 
 using namespace kta;
@@ -715,8 +716,7 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     if ((rc = grow(s, h->log_batch_cap, nbatches + 1, h->d_log_info, h->d_log_cnt))) return rc;
     if (!h->d_log_err) CU(cudaMalloc(&h->d_log_err, 8));   // [0] error flags, [1] longest batch
     CU(cudaMemsetAsync(h->d_log_err, 0, 8, s));
-    const int grid = (int)std::min<int64_t>((nbatches + 127) / 128, (int64_t)h->sm_count * 16);
-    log_header_kernel<<<grid, 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, h->d_log_info,
+    log_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, h->d_log_info,
                                             h->d_log_cnt, h->d_log_err);
     tile_base_scan_kernel<<<1, 1024, 0, s>>>(h->d_log_cnt, nbatches);   // inclusive scan of [1..nbatches] in place
     CU(cudaGetLastError());
@@ -737,11 +737,7 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
         CU(cudaMemsetAsync(h->d_log_err, 0, 4, s));
         const uint32_t codecs = err[0] & LOGB_CODECS;   // (err is reused for the size pass's flags below)
         const bool zstd = (codecs & LOGB_ZSTD) != 0;
-        const int wgrid = (int)std::min<int64_t>((nbatches + 3) / 4, (int64_t)h->sm_count * 16);   // warp per batch
-        log_unc_size_kernel<<<grid, 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_log_err);
-        if (zstd) log_zstd_size_kernel<<<wgrid, 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_log_err);
-        tile_base_scan_kernel<<<1, 1024, 0, s>>>(h->d_unc_slot, nbatches);
-        CU(cudaGetLastError());
+        CU(log_launch_size_pass(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_log_err, zstd, h->sm_count, s));
         h->launches += zstd ? 3 : 2;
         uint64_t unc_total = 0;
         CU(cudaMemcpyAsync(&unc_total, h->d_unc_slot + nbatches, 8, cudaMemcpyDeviceToHost, s));
@@ -752,15 +748,8 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
         // zstd's literal buffer has the size of the scratch buffer (a block's literals go at its output's offset); it is
         // only allocated once zstd batches are seen
         if (zstd && (rc = grow(s, h->unc_lit_cap, (int64_t)unc_total + 64, h->d_unc_lit))) return rc;
-        if (codecs & ~(uint32_t)LOGB_ZSTD) {
-            log_decompress_kernel<false><<<wgrid, 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_unc, nullptr, h->d_log_err);
-            h->launches++;
-        }
-        if (zstd) {
-            log_decompress_kernel<true><<<wgrid, 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_unc, h->d_unc_lit, h->d_log_err);
-            h->launches++;
-        }
-        CU(cudaGetLastError());
+        CU(log_launch_copy_pass(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_unc, h->d_unc_lit, h->d_log_err, codecs, h->sm_count, s));
+        h->launches += ((codecs & ~(uint32_t)LOGB_ZSTD) ? 1 : 0) + (zstd ? 1 : 0);
     }
     if ((int64_t)nrec >= ((int64_t)1 << 31) - 2) return fail(KTA_ERR_INVALID, "%llu records in one call: split the segments", (unsigned long long)nrec);
     const bool hash = h->need_hash || h->d_hash_out;

@@ -24,15 +24,19 @@ def varint(n: int) -> bytes:
     return uvarint(zigzag(n) & 0xFFFFFFFFFFFFFFFF)
 
 
-def encode_record(offset_delta, ts_delta, key, value_len, headers=()):
-    """value bytes are synthesised (the metric path never reads them); value_len None = tombstone"""
+def encode_record(offset_delta, ts_delta, key, value_len, headers=(), value=None):
+    """value bytes are synthesised (the metric path never reads them) unless `value` gives them; value_len None (and no
+    value) = tombstone"""
     body = bytearray(b"\x00")                      # record attributes
     body += varint(ts_delta) + varint(offset_delta)
     if key is None:
         body += varint(-1)
     else:
         body += varint(len(key)) + key
-    if value_len is None:
+    if value is not None:
+        assert value_len is None or value_len == len(value)
+        body += varint(len(value)) + value
+    elif value_len is None:
         body += varint(-1)
     else:
         body += varint(value_len) + bytes((i * 31 + 7) & 0xFF for i in range(value_len))
@@ -70,7 +74,7 @@ CODEC_BITS = {None: 0, "gzip": 1, "snappy": 2, "snappy-xerial": 2, "lz4": 3, "zs
 
 
 def encode_batch(base_offset, base_ts, records, attributes=0, max_ts=None, compression=None):
-    """records: list of (offset_delta, ts_delta, key|None, value_len|None[, headers])"""
+    """records: list of (offset_delta, ts_delta, key|None, value_len|None[, headers[, value]])"""
     recs = b"".join(encode_record(*r) for r in records)
     if compression:
         recs = compress_records(recs, compression)

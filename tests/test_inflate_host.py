@@ -1,6 +1,8 @@
 """The gzip / DEFLATE decoder of the RecordBatch path (csrc/kta_inflate.cuh) against zlib, on the host: the same
 __host__ __device__ statements log_decompress_kernel runs per warp on the GPU, compiled by nvcc as a plain host program
-(tests/native/inflate_harness.cu).  The GPU tests (test_logdecode.py) then cover the warp-cooperative output side."""
+(tests/native/inflate_harness.cu), one lane with its own output object.  The warp-cooperative output side (InfWarpOut,
+gzip_walk: lane 0's literals, the 32-lane matches) runs only on the GPU: test_logdecomp_gpu.py compares its output with
+zlib's, over these payloads among others."""
 import gzip
 import os
 import shutil

@@ -69,6 +69,16 @@ def test_walks_match_the_compressors(harness):
 def test_damaged_sections_never_leave_their_buffers(harness):
     """Bit flips, truncations and spliced garbage: the harness runs under the address sanitizer with exact-size buffers, so
     any read past the input or write past the size pass's length ends the process with a report."""
+    cases = damaged_sections()
+    res = run_cases(harness, cases)                 # returncode 0 = no sanitizer report, no crash
+    assert len(res) == len(cases)
+    for ok, size_len, out in res:
+        if ok:
+            assert len(out) == size_len
+
+
+def damaged_sections():
+    """(codec, section): 300 damaged sections per codec (test_logdecomp_gpu.py runs the same ones on the GPU)"""
     rng = np.random.default_rng(9)
     data = sections()["records"]
     cases = []
@@ -87,8 +97,4 @@ def test_damaged_sections_never_leave_their_buffers(harness):
             else:
                 b += bytes(rng.integers(0, 256, int(rng.integers(1, 9)), dtype=np.uint8))
             cases.append((CODEC[codec], bytes(b)))
-    res = run_cases(harness, cases)                 # returncode 0 = no sanitizer report, no crash
-    assert len(res) == len(cases)
-    for ok, size_len, out in res:
-        if ok:
-            assert len(out) == size_len
+    return cases

@@ -140,6 +140,126 @@ def rle_literals_block(byte, n, last=1):
     return struct.pack("<I", (len(body) << 3) | (2 << 1) | last)[:3] + body
 
 
+class BackwardBits:
+    """the writing side of a zstd backward bitstream (RFC 8878 4.1): values go in low bits first and are read back last
+    first, from the top; finish() adds the padding marker"""
+
+    def __init__(self):
+        self.v, self.n = 0, 0
+
+    def add(self, value, nbits):
+        assert 0 <= value < (1 << nbits) or (value == 0 and nbits == 0)
+        self.v |= value << self.n
+        self.n += nbits
+
+    def finish(self):
+        return (self.v | (1 << self.n)).to_bytes(self.n // 8 + 1, "little")
+
+
+def huffman_codes(weights):
+    """canonical prefix codes from Huffman weights (RFC 8878 4.2.1.3), the last symbol's weight included: symbols sorted by
+    weight, in symbol order within a weight, codes handed out in sequence from the lowest weight.  {symbol: (code, bits)}"""
+    total = sum(1 << (w - 1) for w in weights if w)
+    log = total.bit_length() - 1
+    assert total == 1 << log
+    codes, at = {}, 0
+    for w in range(1, log + 1):
+        for sym, x in enumerate(weights):
+            if x == w:
+                codes[sym] = (at >> (w - 1), log + 1 - w)
+                at += 1 << (w - 1)
+    return codes
+
+
+def huffman_stream(data, codes):
+    """one Huffman stream: the first literal is read first, so it is written last"""
+    bw = BackwardBits()
+    for b in reversed(data):
+        bw.add(*codes[b])
+    return bw.finish()
+
+
+def block(body, bt, last):
+    return struct.pack("<I", (len(body) << 3) | (bt << 1) | last)[:3] + body
+
+
+def rle_mode_sequences(seqs, ll_code, of_code, ml_code):
+    """a sequences section with RLE mode for all three codes (one symbol each, no state bits): the bitstream holds only the
+    extra bits.  seqs: (ll extra, of extra, ml extra) per sequence → (section, [(literal length, offset value, match length)])"""
+    assert len(seqs) < 128
+    bw = BackwardBits()
+    for lle, ofe, mle in reversed(seqs):                  # read per sequence as OF, ML, LL: written the other way round
+        bw.add(lle, ZSTD_LL_BITS[ll_code])
+        bw.add(mle, ZSTD_ML_BITS[ml_code])
+        bw.add(ofe, of_code)
+    decoded = [(ZSTD_LL_BASE[ll_code] + lle, (1 << of_code) + ofe, ZSTD_ML_BASE[ml_code] + mle) for lle, ofe, mle in seqs]
+    return bytes([len(seqs), 0x54, ll_code, of_code, ml_code]) + bw.finish(), decoded
+
+
+# the few literal-length / match-length codes used below (RFC 8878 3.1.1.3.2.1.1): code → baseline, extra bits
+ZSTD_LL_BASE, ZSTD_LL_BITS = {5: 5, 16: 16, 18: 20}, {5: 0, 16: 1, 18: 1}
+ZSTD_ML_BASE, ZSTD_ML_BITS = {32: 35, 33: 37}, {32: 1, 33: 1}
+
+
+def execute(out, lits, seqs):
+    """RFC 8878 3.1.1.4 for sequences whose offset values are all > 3 (no repeat offsets)"""
+    out, lp = bytearray(out), 0
+    for ll, ov, ml in seqs:
+        assert ov > 3
+        out += lits[lp:lp + ll]
+        lp += ll
+        for _ in range(ml):
+            out.append(out[-(ov - 3)])
+    return bytes(out + lits[lp:])
+
+
+def rle_literals_with_sequences():
+    """a raw block, then a compressed block whose RLE literals are followed by sequences (RLE mode for LL, OF and ML) that
+    reach back into the raw block; single segment, one-byte Frame_Content_Size"""
+    raw = b"0123456789abcdefghijklmnopqrstuvwxyzABCD"
+    seqs = [(1, 5, 0), (0, 13, 1), (1, 0, 1)]
+    section, decoded = rle_mode_sequences(seqs, 16, 4, 32)
+    body = bytes([1 | 4 | ((60 & 15) << 4), 60 >> 4, ord("Z")]) + section   # RLE literals, Size_Format 01: 60 x 'Z'
+    want = execute(raw, b"Z" * 60, decoded)
+    assert len(want) < 256
+    return MAGIC + bytes([0x20, len(want)]) + block(raw, 0, 0) + block(body, 2, 1), want
+
+
+def treeless_one_stream():
+    """a block of Huffman literals in one stream, its table in direct 4-bit weights (header byte >= 128), no sequences; then a
+    block of Treeless literals in one stream that reuses the table, followed by sequences.  No Frame_Content_Size, 4 KiB
+    window."""
+    rng = np.random.default_rng(17)
+    weights = [0] * 103
+    for ch, w in zip(b"abcdef", (5, 4, 3, 2, 1, 1)):      # 16 + 8 + 4 + 2 + 1 + 1 = 32: a complete code, 5-bit table
+        weights[ch] = w
+    codes = huffman_codes(weights)
+    alphabet = np.frombuffer(b"abcdef", dtype=np.uint8)
+    lits_a = rng.choice(alphabet, 200, p=[0.5, 0.25, 0.125, 0.0625, 0.03125, 0.03125]).tobytes()
+    lits_b = rng.choice(alphabet, 150).tobytes()
+    desc = bytes([127 + 102]) + bytes((weights[i] << 4) | weights[i + 1] for i in range(0, 102, 2))   # weights of 0..101; 'f' implied
+    stream_a, stream_b = huffman_stream(lits_a, codes), huffman_stream(lits_b, codes)
+    cs_a = len(desc) + len(stream_a)
+    body_a = struct.pack("<I", 2 | (len(lits_a) << 4) | (cs_a << 14))[:3] + desc + stream_a + b"\x00"
+    section, decoded = rle_mode_sequences([(0, 7, 1), (1, 30, 0)], 16, 5, 33)
+    body_b = struct.pack("<I", 3 | (len(lits_b) << 4) | (len(stream_b) << 14))[:3] + stream_b + section
+    want = execute(execute(b"", lits_a, []), lits_b, decoded)
+    return MAGIC + bytes([0x00, (12 - 10) << 3]) + block(body_a, 2, 0) + block(body_b, 2, 1), want
+
+
+def hand_assembled():
+    return [rle_literals_with_sequences(), treeless_one_stream()]
+
+
+def test_hand_assembled_frames_are_valid_zstd():
+    """the two hand-assembled frames decode with pyarrow's zstd (the reference library) to what they are built to hold, so
+    the walk is measured against the format, not against the encoder above; the code assignment is RFC 8878's example"""
+    import pyarrow as pa
+    assert huffman_codes([4, 3, 2, 0, 1, 1]) == {0: (1, 1), 1: (1, 2), 2: (1, 3), 4: (0, 4), 5: (1, 4)}
+    for f, want in hand_assembled():
+        assert pa.decompress(f, decompressed_size=len(want), codec="zstd", asbytes=True) == want
+
+
 def corpus():
     """(frame, expected output) pairs covering the format's shapes"""
     out = []
@@ -161,6 +281,7 @@ def corpus():
     rle = MAGIC + bytes([0x20, 100]) + rle_literals_block(0x41, 60, last=0) + raw_block(b"xyz", 0) + rle_literals_block(0x7A, 37)
     out.append((rle, b"A" * 60 + b"xyz" + b"z" * 37))                          # RLE literals, one-byte FCS
     out.append((MAGIC + bytes([0x00, 0x00]) + rle_literals_block(0x00, 5), bytes(5)))   # no FCS, 1 KiB window
+    out += hand_assembled()                                                     # modes pyarrow does not write here
     return out
 
 
@@ -172,18 +293,20 @@ def test_walk_matches_pyarrow(harness):
 
 
 def test_corpus_reaches_every_mode():
-    """The corpus above reaches every block type, literals type and stream count, weight encoding and sequence mode except
-    the ones named in NOT_REACHED: pyarrow never writes them for these inputs, and entropy-coded streams are not hand-built."""
+    """The corpus above reaches every block type, literals type and stream count, weight encoding and sequence mode; the
+    hand-assembled frames supply the two that pyarrow never writes for these inputs (one-stream Treeless literals, RLE
+    literals followed by sequences)."""
     seen = collections.Counter()
     for f, _ in corpus():
         inspect(f, seen)
     want = {"fcs", "no_fcs", "skippable", "checksum", "block_raw", "block_rle", "block_compressed",
             "lit_raw", "lit_rle", "lit_huffman_1stream", "lit_huffman_4streams", "lit_treeless_4streams",
-            "weights_direct", "weights_fse", "seq_none", "lit_huffman_1stream+seq_none", "lit_raw+sequences"}
+            "weights_direct", "weights_fse", "seq_none", "lit_huffman_1stream+seq_none", "lit_raw+sequences",
+            "lit_treeless_1stream", "lit_treeless_1stream+sequences", "lit_rle+sequences"}
     want |= {"%s_%s" % (t, m) for t in ("LL", "OF", "ML") for m in ("predefined", "rle", "fse", "repeat")}
     missing = sorted(k for k in want if not seen[k])
     assert not missing, (missing, dict(seen))
-    NOT_REACHED = {"lit_treeless_1stream", "lit_rle+sequences"}
+    NOT_REACHED = set()
     assert not any(seen[k] for k in NOT_REACHED), "now reached: move it into `want`"
 
 
@@ -232,6 +355,17 @@ def test_damaged_frames_never_leave_their_buffers(harness):
     """Bit flips, truncations, spliced garbage and appended bytes, 300 each for one-shot, streaming and level-19 frames: the
     harness runs under the address sanitizer with exact-size buffers, so any read past the input or write past the size
     pass's length ends the process with a report.  A damaged frame that still decodes has the size the size pass gave."""
+    cases = damaged_frames()
+    res = run_cases(harness, cases)                 # returncode 0 = no sanitizer report, no crash
+    assert len(res) == len(cases)
+    for ok, size_len, out in res:
+        if ok:
+            assert len(out) == size_len
+    assert sum(not ok for ok, _, _ in res) > len(cases) // 2
+
+
+def damaged_frames():
+    """900 damaged frames (test_logdecomp_gpu.py runs the same ones on the GPU)"""
     rng = np.random.default_rng(9)
     s = sections()
     data = s["records"] + s["text"][:20_000]
@@ -251,9 +385,4 @@ def test_damaged_frames_never_leave_their_buffers(harness):
             else:
                 b += bytes(rng.integers(0, 256, int(rng.integers(1, 9)), dtype=np.uint8))
             cases.append(bytes(b))
-    res = run_cases(harness, cases)                 # returncode 0 = no sanitizer report, no crash
-    assert len(res) == len(cases)
-    for ok, size_len, out in res:
-        if ok:
-            assert len(out) == size_len
-    assert sum(not ok for ok, _, _ in res) > len(cases) // 2
+    return cases
