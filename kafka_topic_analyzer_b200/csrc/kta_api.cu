@@ -75,7 +75,6 @@ struct Chunk {
     uint8_t *d_keys = nullptr;
     uint64_t *d_tile_base = nullptr;
     cudaEvent_t free_ev = nullptr;  // recorded after the scan that reads this chunk
-    uint32_t *h_status = nullptr;   // pinned [2]: snapshot of the alive-table status words taken right after that scan
     // pinned landing area for kta_push
     int32_t *h_partition = nullptr, *h_klen = nullptr, *h_vlen = nullptr;
     int64_t *h_ts = nullptr;
@@ -83,13 +82,30 @@ struct Chunk {
     uint64_t *h_tile_base = nullptr;
 };
 
-// a MODE_EXACT scan whose stamps have not been confirmed yet (the alive table may turn out too small: then it is
-// grown and these are re-run stamps-only; their input buffers are still valid — caller buffers until kta_sync /
-// kta_finalize by contract, ring chunks until they are reused)
-struct PendingScan {
-    ScanParams prm;
+// Stamps the alive-key table has not confirmed yet (it may turn out too small: then they are applied again, which is
+// idempotent).  Their inputs are still valid: caller buffers until kta_sync / kta_finalize by contract, ring chunks
+// until they are reused, an imported list until kta_alive_import_device returns.
+struct AlivePending {
+    ScanParams prm;   // a MODE_EXACT scan (count == 0) as first launched, seen-cache waves included
     int64_t key_readable, key_bytes;
-    int chunk;   // ring chunk the columns live in, -1 = caller-owned / scratch device buffers
+    int chunk;        // ring chunk the columns live in, -1 = caller-owned / scratch device buffers
+    const uint32_t *hash; const uint64_t *stamp; int64_t count;   // an import (count > 0) of exported pairs
+};
+
+// Host side of the exact alive-key table (-c); only the alive_* functions read the status words or the pending list
+struct AliveKeys {
+    unsigned long long *d_table = nullptr;   // open-addressed last-writer table, 2 * pairs slots
+    uint32_t pairs = 0;
+    uint64_t origin = 0;                     // seq that a stamp's field value 1 stands for
+    bool rebased = false;                    // a rebase dropped absolute sequence numbers (exports are refused then)
+    uint32_t *d_cache = nullptr;             // seen cache of the batch being scanned (32 MiB, cleared per launch)
+    uint32_t *d_status = nullptr;            // [0] stamps that found no slot, [1] records outside the seq window, [2] wide re-run
+    uint32_t *h_status = nullptr;            // pinned: [0..1] read by alive_settle, [2c + 2..] snapshot behind ring chunk c's scan
+    unsigned long long *d_count = nullptr;   // [0] alive entries, [1] export cursor, [2] occupied slots
+    uint64_t window_errors = 0;              // sticky until reset: reported by kta_finalize
+    uint64_t grows = 0, reruns = 0;
+    uint64_t now = 0, occupied = 0;          // counted by the last alive_settle
+    std::vector<AlivePending> pending;
 };
 
 struct kta_handle {
@@ -103,20 +119,8 @@ struct kta_handle {
     unsigned long long *d_sums = nullptr;
     long long *d_minmax = nullptr;
     uint32_t *d_hll = nullptr;
-    uint32_t *d_hll_floor = nullptr;
-    unsigned long long *d_alive_table = nullptr;   // open-addressed last-writer table, 2 * alive_pairs slots
-    uint32_t alive_pairs = 0;
-    uint64_t alive_origin = 0;               // seq that a stamp's field value 1 stands for
-    bool alive_rebased = false;              // a rebase dropped absolute sequence numbers (exports are refused then)
-    uint32_t *d_alive_cache = nullptr;       // seen cache of the batch being scanned (32 MiB, cleared per launch)
-    uint32_t *d_alive_status = nullptr;      // [0] stamps that found no slot, [1] records outside the seq window, [2] wide re-run
-    uint32_t *h_alive_status = nullptr;      // pinned copy
-    uint64_t alive_window_errors = 0;        // sticky until reset: reported by kta_finalize
-    uint64_t alive_grows = 0, alive_reruns = 0;
-    uint64_t alive_now = 0, alive_occupied = 0;   // counted by the last alive_check
-    std::vector<PendingScan> pending;
-    unsigned long long *d_scalar = nullptr;  // [0] alive count, [1] export cursor, [2] occupied slots, [3] spare,
-                                             // [4..] hll floor + slice minima (u32)
+    uint32_t *d_hll_floor = nullptr;         // hll floor + slice minima
+    AliveKeys alive;                         // count_alive_keys only
     uint32_t *d_hash_out = nullptr;          // test hook
     uint64_t *d_tb_scratch = nullptr;        // key_tile_base scratch for device batches
     int64_t tb_scratch_tiles = 0;
@@ -256,26 +260,273 @@ static int grow(cudaStream_t s, int64_t &cap, int64_t need, T *&...bufs) {
     return KTA_OK;
 }
 
-static int state_reset_device(kta_handle *h) {
-    state_init_kernel<<<64, 256, 0, h->stream>>>(h->d_sums, h->nsums, h->d_minmax, h->d_hll, h->nhll, h->d_hll_floor);
+// ------------------------------------------------------------------------------------------------
+// alive-key table (-c): seq window (rebase), confirmation of pending stamps, growth (rehash + re-run), export / import
+// ------------------------------------------------------------------------------------------------
+static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, int64_t key_bytes);
+static int ring_flush(kta_handle *h);
+
+static int alive_create(kta_handle *h) {
+    // open-addressed last-writer table keyed by the 32-bit hash, sized by the number of DISTINCT hashes and grown
+    // on demand (alive_settle): 256 MiB = 2^25 slots holds the 1e7 keys of BASELINE configs[2] at load 0.3 (at 0.6
+    // every third first-seen key finds its home pair taken and probes on; the table does not fit L2 at either size)
+    const int64_t kib = h->cfg.alive_table_kib;
+    if (kib < 0 || kib > ALIVE_MAX_KIB) return fail(KTA_ERR_INVALID, "alive_table_kib %d out of range [0, %d]", (int)kib, ALIVE_MAX_KIB);
+    AliveKeys &a = h->alive;
+    a.pairs = (uint32_t)std::max<int64_t>((kib ? kib : ALIVE_DEFAULT_KIB) * 64, 16);   // 16 bytes per pair
+    CU(cudaMalloc(&a.d_table, (size_t)a.pairs * 16));
+    CU(cudaMalloc(&a.d_status, 12));
+    CU(cudaMalloc(&a.d_count, 24));
+    CU(cudaMalloc(&a.d_cache, ((size_t)4 << ALIVE_CACHE_SET_BITS)));
+    CU(cudaHostAlloc(&a.h_status, 8 * (NCHUNK + 1), cudaHostAllocDefault));
+    return KTA_OK;
+}
+
+static int alive_reset(kta_handle *h) {
+    AliveKeys &a = h->alive;
+    if (!a.d_table) return KTA_OK;
+    // the table is a few hundred MB at most for the topics it is meant for: wiping it is one short memset
+    CU(cudaMemsetAsync(a.d_table, 0xff, (size_t)a.pairs * 16, h->stream));
+    CU(cudaMemsetAsync(a.d_status, 0, 12, h->stream));
+    a.now = a.occupied = a.origin = 0;
+    a.rebased = false;
+    a.window_errors = 0;
+    a.pending.clear();
+    return KTA_OK;
+}
+
+static void alive_destroy(AliveKeys &a) {
+    cudaFree(a.d_table); cudaFree(a.d_status); cudaFree(a.d_count); cudaFree(a.d_cache); cudaFreeHost(a.h_status);
+}
+
+static int alive_grow(kta_handle *h, uint32_t new_pairs) {
+    AliveKeys &a = h->alive;
+    cudaStream_t s = h->stream;
+    unsigned long long *nt = nullptr;
+    CU(cudaMalloc(&nt, (size_t)new_pairs * 16));
+    CU(cudaMemsetAsync(nt, 0xff, (size_t)new_pairs * 16, s));
+    alive_rehash_kernel<<<h->sm_count * 8, THREADS, 0, s>>>(a.d_table, (size_t)a.pairs * 2, nt, new_pairs, a.d_status);
     h->launches++;
     CU(cudaGetLastError());
-    if (h->d_alive_table) {
-        // the table is a few hundred MB at most for the topics it is meant for: wiping it is one short memset
-        CU(cudaMemsetAsync(h->d_alive_table, 0xff, (size_t)h->alive_pairs * 16, h->stream));
-        CU(cudaMemsetAsync(h->d_scalar, 0, 32, h->stream));
-        CU(cudaMemsetAsync(h->d_alive_status, 0, 12, h->stream));
-        h->alive_now = h->alive_occupied = 0;
-        h->alive_origin = 0;
-        h->alive_rebased = false;
-        h->alive_window_errors = 0;
-        h->pending.clear();
+    CU(cudaStreamSynchronize(s));
+    cudaFree(a.d_table);
+    a.d_table = nt;
+    a.pairs = new_pairs;
+    a.grows++;
+    return KTA_OK;
+}
+
+// applies a pending entry's stamps (again) to the table as it is now: an import as it was, a scan stamps-only
+static int alive_apply(kta_handle *h, const AlivePending &p) {
+    AliveKeys &a = h->alive;
+    if (p.count) {
+        const int grid = (int)std::min<int64_t>((p.count + THREADS - 1) / THREADS, (int64_t)h->sm_count * 8);
+        alive_import_kernel<<<grid, THREADS, 0, h->stream>>>(AliveTable{a.d_table, a.pairs, a.d_status, 0}, a.origin, p.hash,
+                                                             reinterpret_cast<const unsigned long long *>(p.stamp), p.count);
+        h->launches++;
+        CU(cudaGetLastError());
+        return KTA_OK;
+    }
+    ScanParams prm = p.prm;
+    prm.alive_only = 1;
+    prm.alive_table = a.d_table;   // the table may have grown since
+    prm.alive_pairs = a.pairs;
+    a.reruns++;                    // re-stamped batches (kta.h): imports are not counted
+    return launch_scan_raw(h, prm, p.key_readable, p.key_bytes);
+}
+
+// Confirms every pending entry: waits for the stream, reads the status words, and while stamps were dropped applies
+// the pending entries again (idempotent: atomicMax).  Afterwards nothing is pending.
+//   * If the table would stay at most 60 % full even were every dropped stamp a new key, the drops are a probe-limit
+//     artefact: keys whose mixed hashes lie close together share a home pair at every table size, and a crafted run of
+//     a few hundred of them would otherwise double the table up to its 32 GiB cap.  The re-run keeps the table and lets
+//     the probe run over all of it (status[2]); a linear probe in a table at most 60 % full always reaches an empty slot.
+//   * Otherwise the table is grown first.  It is also grown ahead of need once it is more than 60 % full.
+static int alive_settle(kta_handle *h) {
+    AliveKeys &a = h->alive;
+    if (!a.d_table) return KTA_OK;
+    cudaStream_t s = h->stream;
+    for (int round = 0;; round++) {
+        unsigned long long counts[3] = {0, 0, 0};   // alive, (export cursor), occupied
+        CU(cudaMemsetAsync(a.d_count, 0, 24, s));
+        alive_count_kernel<<<h->sm_count * 8, THREADS, 0, s>>>(a.d_table, (size_t)a.pairs * 2, a.d_count);
+        h->launches++;
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(a.h_status, a.d_status, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(counts, a.d_count, 24, cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        const unsigned long long occupied = counts[2];
+        a.now = counts[0];
+        a.occupied = occupied;
+        const uint32_t dropped = a.h_status[0];
+        a.window_errors += a.h_status[1];
+        if (dropped || a.h_status[1]) CU(cudaMemsetAsync(a.d_status, 0, 8, s));
+        const uint64_t slots = (uint64_t)a.pairs * 2;
+        const bool crowded = occupied * 10 > slots * 6;
+        if (!dropped && !crowded) break;
+        const bool wide = dropped && (occupied + dropped) * 10 <= slots * 6;
+        int rc;
+        if (!wide) {
+            if (a.pairs >= (uint32_t)ALIVE_MAX_KIB * 64u) {
+                if (dropped) return fail(KTA_ERR_NOMEM, "alive-key table is at its maximum (32 GiB) and still too full");
+                break;
+            }
+            // at least double; enough for every known entry plus every dropped stamp at load <= 0.5
+            uint64_t want = slots * 2;
+            while (want < (occupied + dropped) * 2) want *= 2;
+            want = std::min<uint64_t>(want, (uint64_t)ALIVE_MAX_KIB * 128ull);
+            if ((rc = alive_grow(h, (uint32_t)(want / 2)))) return rc;
+            if (!dropped) break;   // grown ahead of need: every pending stamp had landed
+        }
+        if (round > 40) return fail(KTA_ERR_INVALID, "alive-key table growth did not converge");
+        if (wide) CU(cudaMemsetAsync(a.d_status + 2, 0xff, 4, s));
+        for (const AlivePending &p : a.pending)
+            if ((rc = alive_apply(h, p))) return rc;
+        if (wide) CU(cudaMemsetAsync(a.d_status + 2, 0, 4, s));
+    }
+    a.pending.clear();
+    return KTA_OK;
+}
+
+// settles only when something is pending (no count of the table otherwise)
+static int alive_settle_if_any(kta_handle *h) { return h->alive.pending.empty() ? KTA_OK : alive_settle(h); }
+
+// Fills in the alive-table fields (zero so far) of a MODE_EXACT scan's params; the stamps must fit the table's 31-bit window
+// [origin, origin + ALIVE_FIELD_MAX).  `seq_ends`: host copy of seq[0], seq[n-1] when the seq column came from the host.
+static int alive_prepare(kta_handle *h, ScanParams &prm, const uint64_t *seq_ends) {
+    AliveKeys &a = h->alive;
+    int rc;
+    if ((uint64_t)prm.n > (uint64_t)ALIVE_FIELD_MAX - 1)
+        return fail(KTA_ERR_INVALID, "batch of %lld records with count_alive_keys: split it (< 2^31 per scan)", (long long)prm.n);
+    if (prm.seq_base < a.origin)
+        return fail(KTA_ERR_INVALID, "seq_base %llu lies before the alive-key table's window origin %llu (batches must not "
+                    "go back past a rebase)", (unsigned long long)prm.seq_base, (unsigned long long)a.origin);
+    // explicit seq columns are checked record by record in the kernel; the implicit range is checked here
+    if (!prm.seq && prm.seq_base - a.origin + (uint64_t)prm.n > (uint64_t)ALIVE_FIELD_MAX) {
+        // rebase: everything already in the table is older than this batch; forget by how much.  A re-run launches
+        // the params of its first launch, origin and waves included, so nothing may stay pending across a rebase.
+        if ((rc = alive_settle(h))) return rc;
+        if (!a.pending.empty()) return fail(KTA_ERR_INVALID, "internal: alive-key stamps pending across a rebase");
+        alive_rebase_kernel<<<h->sm_count * 8, THREADS, 0, h->stream>>>(a.d_table, (size_t)a.pairs * 2);
+        h->launches++;
+        CU(cudaGetLastError());
+        a.origin = prm.seq_base;
+        a.rebased = true;
+    }
+    prm.alive_table = a.d_table;
+    prm.alive_pairs = a.pairs;
+    prm.alive_origin = a.origin;
+    prm.alive_fbase = prm.seq_base - a.origin + 1ull;
+    prm.alive_status = a.d_status;
+    if (prm.n >= ALIVE_CACHE_MIN_RECORDS) {
+        // the seen cache pays for its clearing (a 32 MiB memset) on batches of a million records and more.
+        // Waves cut the batch's seq range [lo, hi] into <= 127 equal slices (any monotone function of seq will do).
+        uint64_t lo = prm.seq_base, hi = prm.seq_base + (uint64_t)prm.n - 1;
+        bool ok = true;
+        if (prm.seq) {
+            // explicit sequence numbers: the range is read off the column's ends (records of a batch are in seq order; a
+            // record outside the range just lands in the first or last wave)
+            uint64_t ends[2];
+            if (seq_ends) { ends[0] = seq_ends[0]; ends[1] = seq_ends[1]; }
+            else {
+                CU(cudaMemcpyAsync(&ends[0], prm.seq, 8, cudaMemcpyDeviceToHost, h->stream));
+                CU(cudaMemcpyAsync(&ends[1], prm.seq + (prm.n - 1), 8, cudaMemcpyDeviceToHost, h->stream));
+                CU(cudaStreamSynchronize(h->stream));
+            }
+            lo = std::min(ends[0], ends[1]);
+            hi = std::max(ends[0], ends[1]);
+            ok = lo >= a.origin && hi - a.origin < (uint64_t)ALIVE_FIELD_MAX;
+        }
+        if (ok) {
+            prm.alive_cache = a.d_cache;
+            int sh = 0;
+            while (((hi - lo) >> sh) + 1 > (uint64_t)ALIVE_CACHE_WAVES) sh++;
+            prm.alive_wave_shift = sh;
+            prm.alive_wave_base = (uint32_t)(lo - a.origin + 1ull);   // the stamp field of seq lo
+        }
     }
     return KTA_OK;
 }
 
+// a MODE_EXACT scan was launched: its stamps are pending; a ring chunk's scan is followed by a status snapshot
+static int alive_scanned(kta_handle *h, const ScanParams &prm, int64_t key_readable, int64_t key_bytes, int chunk) {
+    AliveKeys &a = h->alive;
+    if (chunk >= 0) CU(cudaMemcpyAsync(a.h_status + 2 * (chunk + 1), a.d_status, 8, cudaMemcpyDeviceToHost, h->stream));
+    a.pending.push_back(AlivePending{prm, key_readable, key_bytes, chunk, nullptr, nullptr, 0});
+    return KTA_OK;
+}
+
+// a ring chunk is about to be overwritten: its scan must be confirmed first (the chunk's event has been waited for,
+// so its status snapshot is valid)
+static int alive_release_chunk(kta_handle *h, int ci) {
+    AliveKeys &a = h->alive;
+    size_t keep = a.pending.size();   // one past the newest entry of this chunk
+    while (keep > 0 && a.pending[keep - 1].chunk != ci) keep--;
+    if (keep == 0) return KTA_OK;
+    const uint32_t *snap = a.h_status + 2 * (ci + 1);
+    if (snap[0] | snap[1]) return alive_settle(h);   // something was dropped up to this scan: settle everything
+    // nothing dropped up to and including this chunk's scan: it — and every older pending entry — is confirmed
+    a.pending.erase(a.pending.begin(), a.pending.begin() + (long)keep);
+    return KTA_OK;
+}
+
+static int alive_export(kta_handle *h, int mode, uint32_t *dh, uint64_t *ds, int64_t cap, int64_t *count) {
+    if (!h || !count) return fail(KTA_ERR_INVALID, "bad argument");
+    AliveKeys &a = h->alive;
+    if (!a.d_table) return fail(KTA_ERR_NOT_ENABLED, "count_alive_keys was not enabled");
+    int rc;
+    if ((rc = set_device(h))) return rc;
+    if ((rc = ring_flush(h))) return rc;
+    if ((rc = alive_settle(h))) return rc;
+    if (a.rebased)
+        return fail(KTA_ERR_INVALID, "the alive-key table was rebased (more than 2^31 sequence numbers since kta_reset): its "
+                    "entries no longer carry absolute sequence numbers and cannot be merged across GPUs");
+    CU(cudaMemsetAsync(a.d_count + 1, 0, 8, h->stream));
+    alive_export_kernel<<<h->sm_count * 8, THREADS, 0, h->stream>>>(
+        a.d_table, (size_t)a.pairs * 2, a.origin, mode, a.d_count + 1, dh,
+        reinterpret_cast<unsigned long long *>(ds), (unsigned long long)cap);
+    h->launches++;
+    CU(cudaGetLastError());
+    unsigned long long c = 0;
+    CU(cudaMemcpyAsync(&c, a.d_count + 1, 8, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    *count = (int64_t)c;
+    if (mode == 1 && (int64_t)c > cap) return fail(KTA_ERR_INVALID, "export buffer too small: %llu > %lld", c, (long long)cap);
+    return KTA_OK;
+}
+
+extern "C" int kta_alive_export_count(kta_handle *h, int64_t *count) { return alive_export(h, 0, nullptr, nullptr, 0, count); }
+
+extern "C" int kta_alive_export_device(kta_handle *h, uint32_t *dev_hash, uint64_t *dev_stamp, int64_t cap, int64_t *count) {
+    if (!dev_hash || !dev_stamp) return fail(KTA_ERR_INVALID, "bad argument");
+    return alive_export(h, 1, dev_hash, dev_stamp, cap, count);
+}
+
+// an imported list is pending work like a scan: applied, then settled
+extern "C" int kta_alive_import_device(kta_handle *h, const uint32_t *dev_hash, const uint64_t *dev_stamp, int64_t count) {
+    if (!h || count < 0 || (count && (!dev_hash || !dev_stamp))) return fail(KTA_ERR_INVALID, "bad argument");
+    AliveKeys &a = h->alive;
+    if (!a.d_table) return fail(KTA_ERR_NOT_ENABLED, "count_alive_keys was not enabled");
+    if (count == 0) return KTA_OK;
+    int rc;
+    if ((rc = set_device(h))) return rc;
+    if ((rc = alive_settle(h))) return rc;
+    const AlivePending p{ScanParams{}, 0, 0, -1, dev_hash, dev_stamp, count};
+    if ((rc = alive_apply(h, p))) return rc;
+    a.pending.push_back(p);
+    if ((rc = alive_settle(h))) return rc;
+    h->finalized = false;
+    return KTA_OK;
+}
+
+static int state_reset_device(kta_handle *h) {
+    state_init_kernel<<<64, 256, 0, h->stream>>>(h->d_sums, h->nsums, h->d_minmax, h->d_hll, h->nhll, h->d_hll_floor);
+    h->launches++;
+    CU(cudaGetLastError());
+    return alive_reset(h);
+}
+
 static void free_chunk(Chunk &c) {
-    cudaFreeHost(c.h_status);
     cudaFree(c.d_partition); cudaFree(c.d_klen); cudaFree(c.d_vlen); cudaFree(c.d_ts); cudaFree(c.d_seq);
     cudaFree(c.d_keys); cudaFree(c.d_tile_base);
     if (c.free_ev) cudaEventDestroy(c.free_ev);
@@ -289,8 +540,8 @@ extern "C" int kta_destroy(kta_handle *h) {
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
     for (auto &c : h->chunks) free_chunk(c);
-    cudaFree(h->d_sums); cudaFree(h->d_minmax); cudaFree(h->d_hll); cudaFree(h->d_alive_table);
-    cudaFree(h->d_alive_status); cudaFree(h->d_alive_cache); cudaFreeHost(h->h_alive_status); cudaFree(h->d_scalar); cudaFree(h->d_tb_scratch);
+    alive_destroy(h->alive);
+    cudaFree(h->d_sums); cudaFree(h->d_minmax); cudaFree(h->d_hll); cudaFree(h->d_hll_floor); cudaFree(h->d_tb_scratch);
     cudaFree(h->d_log_bytes); cudaFree(h->d_log_off); cudaFree(h->d_log_info); cudaFree(h->d_log_cnt);
     cudaFree(h->d_dec_part); cudaFree(h->d_dec_klen); cudaFree(h->d_dec_vlen); cudaFree(h->d_dec_ts); cudaFree(h->d_dec_keys); cudaFree(h->d_dec_ksrc); cudaFree(h->d_unc); cudaFree(h->d_unc_lit); cudaFree(h->d_unc_slot);
     cudaFree(h->d_log_err);
@@ -337,22 +588,10 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
     h->nhll = cfg->hll_precision ? ((size_t)1 << cfg->hll_precision) : 0;
     CU(cudaMalloc(&h->d_sums, h->nsums * 8));
     CU(cudaMalloc(&h->d_minmax, 4 * 8));
-    CU(cudaMalloc(&h->d_scalar, 4 * 8 + (HLL_SLICES + 1) * 4 + 4));
-    h->d_hll_floor = reinterpret_cast<uint32_t *>(h->d_scalar + 4);
+    CU(cudaMalloc(&h->d_hll_floor, (HLL_SLICES + 1) * 4 + 4));
     if (h->nhll) CU(cudaMalloc(&h->d_hll, h->nhll * 4));
-    if (cfg->count_alive_keys == 1) {
-        // open-addressed last-writer table keyed by the 32-bit hash, sized by the number of DISTINCT hashes and grown
-        // on demand (alive_check): 256 MiB = 2^25 slots holds the 1e7 keys of BASELINE configs[2] at load 0.3 (at 0.6
-        // every third first-seen key finds its home pair taken and probes on; the table does not fit L2 at either size)
-        if (cfg->alive_table_kib < 0 || cfg->alive_table_kib > ALIVE_MAX_KIB)
-            return fail(KTA_ERR_INVALID, "alive_table_kib %d out of range [0, %d]", cfg->alive_table_kib, ALIVE_MAX_KIB);
-        const int64_t kib = cfg->alive_table_kib ? cfg->alive_table_kib : ALIVE_DEFAULT_KIB;
-        h->alive_pairs = (uint32_t)std::max<int64_t>(kib * 64, 16);   // 16 bytes per pair
-        CU(cudaMalloc(&h->d_alive_table, (size_t)h->alive_pairs * 16));
-        CU(cudaMalloc(&h->d_alive_status, 12));
-        CU(cudaMalloc(&h->d_alive_cache, ((size_t)4 << ALIVE_CACHE_SET_BITS)));
-        CU(cudaHostAlloc(&h->h_alive_status, 8, cudaHostAllocDefault));
-    }
+    int rc;
+    if (cfg->count_alive_keys == 1 && (rc = alive_create(h))) return rc;
     h->smem_optin = prop.sharedMemPerBlockOptin;
     if (cfg->shard_world > 1) {
         if (cfg->shard_rank < 0 || cfg->shard_rank >= cfg->shard_world || cfg->shard_world > P)
@@ -367,7 +606,6 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
         for (const auto &by_capture : by_mode)
             for (const ScanFn f : by_capture)
                 if (f) CU(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
-    int rc;
     if ((rc = state_reset_device(h))) return rc;
     CU(cudaStreamSynchronize(h->stream));
     return KTA_OK;
@@ -409,7 +647,7 @@ extern "C" int kta_set_stream(kta_handle *h, void *stream) {
 // scan launch
 // ------------------------------------------------------------------------------------------------
 // one launch of the fused scan; prm is complete apart from the state pointers filled in here
-static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, int64_t key_bytes, const uint64_t *seq_ends = nullptr) {
+static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, int64_t key_bytes) {
     const int P = h->cfg.num_partitions;
     const bool exact = h->cfg.count_alive_keys == 1;
     const bool capture = h->d_hash_out != nullptr && !prm.alive_only;
@@ -430,39 +668,6 @@ static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, 
     prm.minmax = h->d_minmax;
     prm.hll = h->d_hll;
     prm.hll_floor = h->d_hll_floor;
-    prm.alive_table = h->d_alive_table;
-    prm.alive_pairs = h->alive_pairs;
-    prm.alive_origin = h->alive_origin;
-    prm.alive_status = h->d_alive_status;
-    prm.alive_cache = nullptr;
-    if (exact && prm.n >= ALIVE_CACHE_MIN_RECORDS) {
-        // the seen cache pays for its clearing (a 32 MiB memset) on batches of a million records and more.
-        // Waves cut the batch's seq range [lo, hi] into <= 127 equal slices (any monotone function of seq will do).
-        uint64_t lo = prm.seq_base, hi = prm.seq_base + (uint64_t)prm.n - 1;
-        bool ok = true;
-        if (prm.seq) {
-            // explicit sequence numbers: the range is read off the column's ends (records of a batch are in seq order; a
-            // record outside the range just lands in the first or last wave)
-            uint64_t ends[2];
-            if (seq_ends) { ends[0] = seq_ends[0]; ends[1] = seq_ends[1]; }
-            else {
-                CU(cudaMemcpyAsync(&ends[0], prm.seq, 8, cudaMemcpyDeviceToHost, h->stream));
-                CU(cudaMemcpyAsync(&ends[1], prm.seq + (prm.n - 1), 8, cudaMemcpyDeviceToHost, h->stream));
-                CU(cudaStreamSynchronize(h->stream));
-            }
-            lo = std::min(ends[0], ends[1]);
-            hi = std::max(ends[0], ends[1]);
-            ok = lo >= h->alive_origin && hi - h->alive_origin < (uint64_t)ALIVE_FIELD_MAX;
-        }
-        if (ok) {
-            CU(cudaMemsetAsync(h->d_alive_cache, 0, (size_t)4 << ALIVE_CACHE_SET_BITS, h->stream));
-            prm.alive_cache = h->d_alive_cache;
-            int sh = 0;
-            while (((hi - lo) >> sh) + 1 > (uint64_t)ALIVE_CACHE_WAVES) sh++;
-            prm.alive_wave_shift = sh;
-            prm.alive_wave_base = (uint32_t)(lo - h->alive_origin + 1ull);   // the stamp field of seq lo
-        }
-    }
     prm.hash_out = capture ? h->d_hash_out : nullptr;
     if (mode != MODE_COUNTERS) {
         if (!prm.key_tile_base) return fail(KTA_ERR_INVALID, "internal: key_tile_base missing");
@@ -480,6 +685,7 @@ static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, 
     prm.keybuf = keybuf;
     prm.stages = stages;
     const int grid = (int)std::min<int64_t>((prm.ntiles + threads / 32 - 1) / (threads / 32), h->sm_count);
+    if (prm.alive_cache) CU(cudaMemsetAsync(prm.alive_cache, 0, (size_t)4 << ALIVE_CACHE_SET_BITS, h->stream));
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     if (h->timing) {
         if (h->ev_used == h->ev_pool.size()) {
@@ -500,129 +706,17 @@ static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, 
     return KTA_OK;
 }
 
-// ------------------------------------------------------------------------------------------------
-// alive-key table upkeep: seq window (rebase), confirmation of pending stamps, growth (rehash + re-run)
-// ------------------------------------------------------------------------------------------------
-static int alive_grow(kta_handle *h, uint32_t new_pairs) {
-    cudaStream_t s = h->stream;
-    unsigned long long *nt = nullptr;
-    CU(cudaMalloc(&nt, (size_t)new_pairs * 16));
-    CU(cudaMemsetAsync(nt, 0xff, (size_t)new_pairs * 16, s));
-    const size_t old_slots = (size_t)h->alive_pairs * 2;
-    alive_rehash_kernel<<<h->sm_count * 8, THREADS, 0, s>>>(h->d_alive_table, old_slots, nt, new_pairs, h->d_alive_status);
-    h->launches++;
-    CU(cudaGetLastError());
-    CU(cudaStreamSynchronize(s));
-    cudaFree(h->d_alive_table);
-    h->d_alive_table = nt;
-    h->alive_pairs = new_pairs;
-    h->alive_grows++;
-    return KTA_OK;
-}
-
-// Confirms every pending MODE_EXACT scan: waits for the stream, reads the status words, and while stamps were dropped
-// re-runs the pending batches stamps-only (idempotent: atomicMax).  Afterwards nothing is pending.
-//   * If the table would stay at most 60 % full even were every dropped stamp a new key, the drops are a probe-limit
-//     artefact: keys whose mixed hashes lie close together share a home pair at every table size, and a crafted run of
-//     a few hundred of them would otherwise double the table up to its 32 GiB cap.  The re-run keeps the table and
-//     lets the probe run over all of it; a linear probe in a table at most 60 % full always reaches an empty slot.
-//   * Otherwise the table is grown first.  It is also grown ahead of need once it is more than 60 % full.
-static int alive_check(kta_handle *h) {
-    if (!h->d_alive_table) return KTA_OK;
-    cudaStream_t s = h->stream;
-    for (int round = 0;; round++) {
-        unsigned long long counts[3] = {0, 0, 0};   // alive, (export cursor), occupied
-        CU(cudaMemsetAsync(h->d_scalar, 0, 24, s));
-        alive_count_kernel<<<h->sm_count * 8, THREADS, 0, s>>>(h->d_alive_table, (size_t)h->alive_pairs * 2, h->d_scalar);
-        h->launches++;
-        CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(h->h_alive_status, h->d_alive_status, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaMemcpyAsync(counts, h->d_scalar, 24, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
-        const unsigned long long occupied = counts[2];
-        h->alive_now = counts[0];
-        h->alive_occupied = occupied;
-        const uint32_t dropped = h->h_alive_status[0];
-        h->alive_window_errors += h->h_alive_status[1];
-        if (dropped || h->h_alive_status[1]) CU(cudaMemsetAsync(h->d_alive_status, 0, 8, s));
-        const uint64_t slots = (uint64_t)h->alive_pairs * 2;
-        const bool crowded = occupied * 10 > slots * 6;
-        if (!dropped && !crowded) break;
-        const bool wide = dropped && (occupied + dropped) * 10 <= slots * 6;
-        int rc;
-        if (!wide) {
-            if (h->alive_pairs >= (uint32_t)ALIVE_MAX_KIB * 64u) {
-                if (dropped) return fail(KTA_ERR_NOMEM, "alive-key table is at its maximum (32 GiB) and still too full");
-                break;
-            }
-            // at least double; enough for every known entry plus every dropped stamp at load <= 0.5
-            uint64_t want = slots * 2;
-            while (want < (occupied + dropped) * 2) want *= 2;
-            want = std::min<uint64_t>(want, (uint64_t)ALIVE_MAX_KIB * 128ull);
-            if ((rc = alive_grow(h, (uint32_t)(want / 2)))) return rc;
-            if (!dropped) break;   // grown ahead of need: every pending stamp had landed
-        }
-        if (round > 40) return fail(KTA_ERR_INVALID, "alive-key table growth did not converge");
-        if (wide) CU(cudaMemsetAsync(h->d_alive_status + 2, 0xff, 4, s));
-        for (const PendingScan &ps : h->pending) {
-            ScanParams prm = ps.prm;
-            prm.alive_only = 1;
-            if ((rc = launch_scan_raw(h, prm, ps.key_readable, ps.key_bytes))) return rc;
-            h->alive_reruns++;
-        }
-        if (wide) CU(cudaMemsetAsync(h->d_alive_status + 2, 0, 4, s));
-    }
-    h->pending.clear();
-    return KTA_OK;
-}
-
+// one scan of a batch whose columns lie in ring chunk `chunk` (-1: elsewhere); `seq_ends`: see alive_prepare
 static int launch_scan(kta_handle *h, ScanParams prm, int64_t key_readable, int64_t key_bytes, int chunk = -1,
-                       const uint64_t *seq_ends = nullptr /* host copy of seq[0], seq[n-1] when the column came from the host */) {
+                       const uint64_t *seq_ends = nullptr) {
     if (prm.n <= 0) return KTA_OK;
+    const bool exact = h->alive.d_table != nullptr;
     int rc;
-    if (h->cfg.count_alive_keys == 1) {
-        // the stamps of this batch must fit the table's 31-bit window [origin, origin + ALIVE_FIELD_MAX)
-        if ((uint64_t)prm.n > (uint64_t)ALIVE_FIELD_MAX - 1)
-            return fail(KTA_ERR_INVALID, "batch of %lld records with count_alive_keys: split it (< 2^31 per scan)", (long long)prm.n);
-        if (prm.seq_base < h->alive_origin)
-            return fail(KTA_ERR_INVALID, "seq_base %llu lies before the alive-key table's window origin %llu (batches must not "
-                        "go back past a rebase)", (unsigned long long)prm.seq_base, (unsigned long long)h->alive_origin);
-        // explicit seq columns are checked record by record in the kernel; the implicit range is checked here
-        if (!prm.seq && prm.seq_base - h->alive_origin + (uint64_t)prm.n > (uint64_t)ALIVE_FIELD_MAX) {
-            // rebase: everything already in the table is older than this batch; forget by how much
-            if ((rc = alive_check(h))) return rc;
-            alive_rebase_kernel<<<h->sm_count * 8, THREADS, 0, h->stream>>>(h->d_alive_table, (size_t)h->alive_pairs * 2);
-            h->launches++;
-            CU(cudaGetLastError());
-            h->alive_origin = prm.seq_base;
-            h->alive_rebased = true;
-        }
-        prm.alive_fbase = prm.seq_base - h->alive_origin + 1ull;
-        prm.alive_only = 0;
-    }
-    if ((rc = launch_scan_raw(h, prm, key_readable, key_bytes, seq_ends))) return rc;
-    if (h->cfg.count_alive_keys == 1) h->pending.push_back(PendingScan{prm, key_readable, key_bytes, chunk});
+    if (exact && (rc = alive_prepare(h, prm, seq_ends))) return rc;
+    if ((rc = launch_scan_raw(h, prm, key_readable, key_bytes))) return rc;
+    if (exact && (rc = alive_scanned(h, prm, key_readable, key_bytes, chunk))) return rc;
     h->records += (uint64_t)prm.n;
     h->finalized = false;
-    return KTA_OK;
-}
-
-// a ring chunk is about to be overwritten: its scan must be confirmed first (the chunk's event has been waited for,
-// so its status snapshot is valid)
-static int alive_release_chunk(kta_handle *h, int ci) {
-    if (!h->d_alive_table || h->pending.empty()) return KTA_OK;
-    bool mine = false;
-    for (const PendingScan &ps : h->pending) mine = mine || ps.chunk == ci;
-    if (!mine) return KTA_OK;
-    const Chunk &c = h->chunks[ci];
-    if (c.h_status[0] | c.h_status[1]) return alive_check(h);   // something was dropped up to this scan: settle everything
-    // nothing dropped up to and including this chunk's scan: it — and every older pending scan — is confirmed
-    size_t keep = 0;
-    bool seen = false;
-    for (size_t i = h->pending.size(); i-- > 0;) {   // find the newest entry of this chunk; drop it and everything older
-        if (h->pending[i].chunk == ci) { keep = i + 1; seen = true; break; }
-    }
-    if (seen) h->pending.erase(h->pending.begin(), h->pending.begin() + (long)keep);
     return KTA_OK;
 }
 
@@ -647,8 +741,6 @@ static int derive_tile_base(kta_handle *h, const int32_t *d_klen, int64_t n, uin
     h->launches += 2;
     return KTA_OK;
 }
-
-static int ring_flush(kta_handle *h);
 
 // seq of a batch's record 0.  KTA_SEQ_AUTO continues the handle's running count (what kta_push and the log-segment
 // entry points do).  With -c and no explicit seq column, last-writer-wins is decided by seq_base + i alone, so a batch
@@ -711,7 +803,7 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     int rc;
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;   // keep seq order with records pushed earlier
-    if (!h->pending.empty() && (rc = alive_check(h))) return rc;   // the decode scratch of an earlier call is about to be reused
+    if ((rc = alive_settle_if_any(h))) return rc;   // the decode scratch of an earlier call is about to be reused
     cudaStream_t s = h->stream;
     if ((rc = grow(s, h->log_batch_cap, nbatches + 1, h->d_log_info, h->d_log_cnt))) return rc;
     if (!h->d_log_err) CU(cudaMalloc(&h->d_log_err, 8));   // [0] error flags, [1] longest batch
@@ -889,8 +981,6 @@ static int ring_dev_init(kta_handle *h) {
         CU(cudaMalloc(&c.d_keys, KB + 64));
         CU(cudaMalloc(&c.d_tile_base, (R / TILE + 2) * 8));
         CU(cudaEventCreateWithFlags(&c.free_ev, cudaEventDisableTiming));
-        CU(cudaHostAlloc(&c.h_status, 8, cudaHostAllocDefault));
-        c.h_status[0] = c.h_status[1] = 0;
     }
     h->ring_dev_ready = true;
     return KTA_OK;
@@ -923,17 +1013,20 @@ static void push_cursor_bind(kta_handle *h) {
     pc.hash = h->need_hash || h->d_hash_out;
 }
 
-// scan the columns staged in ring chunk `cur`, snapshot the alive-table status words right after that scan, and
-// move on to the next chunk
+// scan the columns staged in ring chunk `cur` and move on to the next chunk
 static int ring_scan_chunk(kta_handle *h, const ScanParams &prm, int64_t key_readable, int64_t key_bytes,
                            const uint64_t *seq_ends = nullptr) {
-    Chunk &c = h->chunks[h->cur];
     int rc;
     if ((rc = launch_scan(h, prm, key_readable, key_bytes, h->cur, seq_ends))) return rc;
-    if (h->d_alive_table) CU(cudaMemcpyAsync(c.h_status, h->d_alive_status, 8, cudaMemcpyDeviceToHost, h->stream));
-    CU(cudaEventRecord(c.free_ev, h->stream));
+    CU(cudaEventRecord(h->chunks[h->cur].free_ev, h->stream));
     h->cur = (h->cur + 1) % NCHUNK;
     return KTA_OK;
+}
+
+// ring chunk ci is about to be overwritten: wait for the scan that read it and confirm that scan's stamps
+static int ring_reuse_chunk(kta_handle *h, int ci) {
+    CU(cudaEventSynchronize(h->chunks[ci].free_ev));
+    return alive_release_chunk(h, ci);
 }
 
 // stage one pinned chunk and scan it
@@ -966,8 +1059,7 @@ static int ring_flush(kta_handle *h) {
     h->next_seq += (uint64_t)n;
     push_cursor_bind(h);
     // the next chunk may still be in flight from NCHUNK flushes ago
-    CU(cudaEventSynchronize(h->chunks[h->cur].free_ev));
-    return alive_release_chunk(h, h->cur);
+    return ring_reuse_chunk(h, h->cur);
 }
 
 // kta_push off the fast path: first call (ring not yet allocated), chunk full, or an oversized key
@@ -1078,9 +1170,7 @@ extern "C" int kta_push_batch_host(kta_handle *h, const kta_batch *b) {
                             (long long)r0);
             cn = std::min<int64_t>(cn, tiles * TILE);
         }
-        // chunk ci's buffers are about to be overwritten: wait for the scan that read them and confirm its stamps
-        CU(cudaEventSynchronize(c.free_ev));
-        if ((rc = alive_release_chunk(h, ci))) return rc;
+        if ((rc = ring_reuse_chunk(h, ci))) return rc;
         const int64_t ntiles = (cn + TILE - 1) / TILE;
         CU(cudaMemcpyAsync(c.d_partition, b->partition + r0, cn * 4, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(c.d_ts, b->ts_ms + r0, cn * 8, cudaMemcpyHostToDevice, s));
@@ -1123,7 +1213,7 @@ extern "C" int kta_sync(kta_handle *h) {
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;
     CU(cudaStreamSynchronize(h->stream));
-    if ((rc = alive_check(h))) return rc;
+    if ((rc = alive_settle(h))) return rc;
     return collect_timing(h);
 }
 
@@ -1146,11 +1236,11 @@ extern "C" int kta_finalize(kta_handle *h) {
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;
     cudaStream_t s = h->stream;
-    if ((rc = alive_check(h))) return rc;   // every stamp has landed (grows the table and re-runs batches if it was too small)
-    if (h->d_alive_table && h->nhll) {
+    if ((rc = alive_settle(h))) return rc;   // every stamp has landed (grows the table and re-runs batches if it was too small)
+    if (h->alive.d_table && h->nhll) {
         // EXTENSION: with -c the sketch describes the resolved alive set, so it is rebuilt from the table
         CU(cudaMemsetAsync(h->d_hll, 0, h->nhll * 4, s));
-        alive_hll_kernel<<<h->sm_count * 8, THREADS, 0, s>>>(h->d_alive_table, (size_t)h->alive_pairs * 2, h->d_hll,
+        alive_hll_kernel<<<h->sm_count * 8, THREADS, 0, s>>>(h->alive.d_table, (size_t)h->alive.pairs * 2, h->d_hll,
                                                              h->cfg.hll_precision);
         CU(cudaGetLastError());
         h->launches++;
@@ -1162,12 +1252,12 @@ extern "C" int kta_finalize(kta_handle *h) {
     if (h->nhll) CU(cudaMemcpyAsync(h->h_hll.data(), h->d_hll, h->nhll * 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     if ((rc = collect_timing(h))) return rc;
-    h->h_alive = h->alive_now;   // counted over the table by alive_check above (sum_all_alive, src/metric.rs:282-284)
+    h->h_alive = h->alive.now;   // counted over the table by alive_settle above (sum_all_alive, src/metric.rs:282-284)
     h->finalized = true;
-    if (h->alive_window_errors)
+    if (h->alive.window_errors)
         return fail(KTA_ERR_INVALID, "%llu record(s) carried a sequence number outside the alive-key table's window "
                     "[origin, origin + 2^31 - 2): with an explicit seq column the span between kta_reset calls is limited",
-                    (unsigned long long)h->alive_window_errors);
+                    (unsigned long long)h->alive.window_errors);
     // Records with a partition outside [0, P) took part in nothing (no counter, no extremum, no alive key): the getters
     // are valid and describe the in-range records; the status tells the caller that some were left out.
     const uint64_t bad = h->h_sums[h->nsums - 1];
@@ -1431,7 +1521,7 @@ extern "C" int kta_merge_export_device(kta_handle *h, int32_t rank, int32_t worl
     int rc;
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;
-    if (!h->pending.empty() && (rc = alive_check(h))) return rc;
+    if ((rc = alive_settle_if_any(h))) return rc;
     merge_export_kernel<<<h->sm_count, 256, 0, h->stream>>>(h->d_sums, h->nsums, h->d_minmax, h->d_hll, h->nhll, rank,
                                                            world, reinterpret_cast<unsigned long long *>(dev_buf));
     h->launches++;
@@ -1459,70 +1549,6 @@ extern "C" int kta_merge_import_device(kta_handle *h, int32_t world, const uint6
     return KTA_OK;
 }
 
-static int alive_export(kta_handle *h, int mode, uint32_t *dh, uint64_t *ds, int64_t cap, int64_t *count) {
-    if (!h || !count) return fail(KTA_ERR_INVALID, "bad argument");
-    if (!h->d_alive_table) return fail(KTA_ERR_NOT_ENABLED, "count_alive_keys was not enabled");
-    int rc;
-    if ((rc = set_device(h))) return rc;
-    if ((rc = ring_flush(h))) return rc;
-    if ((rc = alive_check(h))) return rc;
-    if (h->alive_rebased)
-        return fail(KTA_ERR_INVALID, "the alive-key table was rebased (more than 2^31 sequence numbers since kta_reset): its "
-                    "entries no longer carry absolute sequence numbers and cannot be merged across GPUs");
-    CU(cudaMemsetAsync(h->d_scalar + 1, 0, 8, h->stream));
-    alive_export_kernel<<<h->sm_count * 8, THREADS, 0, h->stream>>>(
-        h->d_alive_table, (size_t)h->alive_pairs * 2, h->alive_origin, mode, h->d_scalar + 1, dh,
-        reinterpret_cast<unsigned long long *>(ds), (unsigned long long)cap);
-    h->launches++;
-    CU(cudaGetLastError());
-    unsigned long long c = 0;
-    CU(cudaMemcpyAsync(&c, h->d_scalar + 1, 8, cudaMemcpyDeviceToHost, h->stream));
-    CU(cudaStreamSynchronize(h->stream));
-    *count = (int64_t)c;
-    if (mode == 1 && (int64_t)c > cap) return fail(KTA_ERR_INVALID, "export buffer too small: %llu > %lld", c, (long long)cap);
-    return KTA_OK;
-}
-
-extern "C" int kta_alive_export_count(kta_handle *h, int64_t *count) { return alive_export(h, 0, nullptr, nullptr, 0, count); }
-
-extern "C" int kta_alive_export_device(kta_handle *h, uint32_t *dev_hash, uint64_t *dev_stamp, int64_t cap, int64_t *count) {
-    if (!dev_hash || !dev_stamp) return fail(KTA_ERR_INVALID, "bad argument");
-    return alive_export(h, 1, dev_hash, dev_stamp, cap, count);
-}
-
-extern "C" int kta_alive_import_device(kta_handle *h, const uint32_t *dev_hash, const uint64_t *dev_stamp, int64_t count) {
-    if (!h || count < 0 || (count && (!dev_hash || !dev_stamp))) return fail(KTA_ERR_INVALID, "bad argument");
-    if (!h->d_alive_table) return fail(KTA_ERR_NOT_ENABLED, "count_alive_keys was not enabled");
-    if (count == 0) return KTA_OK;
-    int rc;
-    if ((rc = set_device(h))) return rc;
-    if ((rc = alive_check(h))) return rc;   // nothing pending: a re-run below only concerns the imported stamps
-    const int grid = (int)std::min<int64_t>((count + THREADS - 1) / THREADS, (int64_t)h->sm_count * 8);
-    bool wide = false;
-    for (int round = 0;; round++) {
-        const AliveTable t{h->d_alive_table, h->alive_pairs, h->d_alive_status, 0};
-        if (wide) CU(cudaMemsetAsync(h->d_alive_status + 2, 0xff, 4, h->stream));
-        alive_import_kernel<<<grid, THREADS, 0, h->stream>>>(t, h->alive_origin, dev_hash,
-                                                             reinterpret_cast<const unsigned long long *>(dev_stamp), count);
-        h->launches++;
-        CU(cudaGetLastError());
-        if (wide) CU(cudaMemsetAsync(h->d_alive_status + 2, 0, 4, h->stream));
-        // the imported list is the caller's and still valid: if the table was too small, alive_check grew it (nothing
-        // is pending, so it re-ran nothing) and the import is simply applied again — stamping is idempotent
-        CU(cudaMemcpyAsync(h->h_alive_status, h->d_alive_status, 8, cudaMemcpyDeviceToHost, h->stream));
-        CU(cudaStreamSynchronize(h->stream));
-        const bool dropped = h->h_alive_status[0] != 0;
-        const uint32_t pairs = h->alive_pairs;
-        if ((rc = alive_check(h))) return rc;
-        if (!dropped) break;
-        if (round > 40) return fail(KTA_ERR_INVALID, "alive-key table growth did not converge");
-        // a table that alive_check did not grow had room for every dropped stamp: probe up to the whole of it (see there)
-        wide = h->alive_pairs == pairs;
-    }
-    h->finalized = false;
-    return KTA_OK;
-}
-
 // ------------------------------------------------------------------------------------------------
 // introspection
 // ------------------------------------------------------------------------------------------------
@@ -1535,15 +1561,15 @@ extern "C" int kta_stats(const kta_handle *h, uint64_t *kernel_launches, uint64_
 
 extern "C" int kta_alive_table_stats(kta_handle *h, uint64_t *slots, uint64_t *occupied, uint64_t *grows, uint64_t *reruns) {
     if (!h) return fail(KTA_ERR_INVALID, "null handle");
-    if (!h->d_alive_table) return fail(KTA_ERR_NOT_ENABLED, "count_alive_keys was not enabled");
+    if (!h->alive.d_table) return fail(KTA_ERR_NOT_ENABLED, "count_alive_keys was not enabled");
     int rc;
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;
-    if ((rc = alive_check(h))) return rc;   // settles pending stamps and counts the table
-    if (slots) *slots = (uint64_t)h->alive_pairs * 2;
-    if (occupied) *occupied = h->alive_occupied;
-    if (grows) *grows = h->alive_grows;
-    if (reruns) *reruns = h->alive_reruns;
+    if ((rc = alive_settle(h))) return rc;   // confirms every stamp and counts the table
+    if (slots) *slots = (uint64_t)h->alive.pairs * 2;
+    if (occupied) *occupied = h->alive.occupied;
+    if (grows) *grows = h->alive.grows;
+    if (reruns) *reruns = h->alive.reruns;
     return KTA_OK;
 }
 

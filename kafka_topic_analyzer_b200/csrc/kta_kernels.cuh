@@ -574,7 +574,7 @@ __device__ __forceinline__ bool alive_probe_pair(const AliveTable t, uint32_t pa
 
 // The general stamp: probe from `pair` until the hash or an empty slot is found.  Returns the low word of the newest
 // stamp known for this hash afterwards (the record's own if it won).  A stamp gives up after ALIVE_MAX_PROBES pairs,
-// unless the host has flagged a wide re-run (status[2], see alive_check): then it goes on over the rest of the table.
+// unless the host has flagged a wide re-run (status[2], see alive_settle): then it goes on over the rest of the table.
 __device__ __noinline__ uint32_t alive_stamp_slow(const AliveTable t, uint32_t pair, uint32_t hash, uint32_t low) {
     uint32_t newest;
     for (int probe = 0; probe < ALIVE_MAX_PROBES; probe++) {
