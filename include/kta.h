@@ -56,6 +56,10 @@ enum {
 
 typedef struct kta_handle kta_handle;
 
+/* kta_config.isolation_level (librdkafka's isolation.level) */
+#define KTA_READ_UNCOMMITTED 0
+#define KTA_READ_COMMITTED 1
+
 typedef struct kta_config {
     int32_t struct_size;       /* = sizeof(kta_config) */
     int32_t device;            /* CUDA device ordinal, -1 = current device */
@@ -68,7 +72,8 @@ typedef struct kta_config {
     int64_t ring_key_bytes;    /* key bytes per landing-ring chunk; 0 = default */
     int64_t now_s;             /* construction wall clock for earliest_message (Utc::now(), */
     int32_t now_ns;            /*   src/metric.rs:39); now_s == INT64_MIN → library reads the clock */
-    int32_t reserved1;
+    int32_t isolation_level;   /* log entry points: KTA_READ_UNCOMMITTED (0, every data batch is delivered) or
+                                  KTA_READ_COMMITTED (records of aborted transactions are left out, see below) */
     int32_t shard_world;       /* partition-sharded job (one handle per GPU, gpu = partition mod G, SURVEY.md §8 e): this */
     int32_t shard_rank;        /*   handle scans only partitions p with p % shard_world == shard_rank; records of other
                                     partitions are left out like out-of-range ones.  0 or 1 = not sharded.  The handle
@@ -210,8 +215,19 @@ int kta_alive_import_device(kta_handle *h, const uint32_t *dev_hash, const uint6
  * xerial-framed) and zstd batches are decompressed on the GPU; the checksums inside a compressed section (gzip's
  * CRC32, zstd's Content_Checksum) are skipped, not verified, like the batch CRC.  zstd frames with a Dictionary_ID and
  * the unassigned codecs 5-7 are rejected (KTA_ERR_INVALID).
- * Differences from a librdkafka consumer: records of aborted transactions ARE delivered (read_committed filtering
- * needs the transaction index, which is not read), legacy magic 0/1 message sets are reported as malformed. */
+ * Isolation (cfg.isolation_level).  KTA_READ_UNCOMMITTED delivers every data batch.  KTA_READ_COMMITTED (librdkafka's
+ * default) leaves out the records of aborted transactions.  A transactional batch (attributes bit 4) of partition p and
+ * producerId q is aborted when the first control batch of the same (p, q) that follows it in the same call is an ABORT
+ * marker, or when its baseOffset lies in an aborted range of (p, q) registered with kta_log_add_txn_index_host.  Matching
+ * ignores producerEpoch.  Non-transactional batches, committed transactions and producerId -1 are delivered as with
+ * read_uncommitted; control batches never are.  Aborted batches are not decompressed or decoded, so damage inside them is
+ * no error.  A control batch whose marker cannot be read (compressed, no record, key length != 4, version != 0) and a call
+ * in which the batches of one (p, q) do not have increasing baseOffsets are KTA_ERR_INVALID.
+ * Differences from a librdkafka consumer: under read_committed, a transactional batch that has no following marker in its
+ * call and no registered range (a transaction still open at the end of what was read, or closed in a later call) is
+ * delivered and counted as undecided (kta_log_txn_stats); a consumer would stop at the last stable offset and wait.
+ * Legacy magic 0/1 message sets are reported as malformed.
+ * records_out of every log entry point counts the records delivered. */
 /* raw bytes already in device memory; batch_off[nbatches] = byte offset of every batch header (device memory) */
 int kta_scan_log_segment_device(kta_handle *h, int32_t partition, const uint8_t *dev_bytes, int64_t len,
                                 const uint64_t *dev_batch_off, int64_t nbatches, int64_t *records_out);
@@ -224,6 +240,16 @@ int kta_push_log_segment_host(kta_handle *h, int32_t partition, const uint8_t *b
 /* several segments (any partitions) in one go: one staging copy per segment, ONE decode and ONE scan for all of them */
 int kta_push_log_segments_host(kta_handle *h, int32_t nsegs, const int32_t *partitions, const uint8_t *const *bytes,
                                const int64_t *lens, int64_t *records_out);
+/* read_committed only: parse one .txnindex image of `partition` (34-byte big-endian entries version i16 = 0 |
+ * producerId i64 | firstOffset i64 | lastOffset i64 | lastStableOffset i64) and register its aborted ranges
+ * [firstOffset, lastOffset] for every later log call on this handle (until kta_reset).  KTA_ERR_INVALID on a
+ * read_uncommitted handle and on a malformed image (length not a multiple of 34, version != 0, firstOffset > lastOffset);
+ * nothing of a malformed image is registered.  An empty image is fine (the broker writes the file lazily). */
+int kta_log_add_txn_index_host(kta_handle *h, int32_t partition, const uint8_t *bytes, int64_t len);
+/* read_committed only (KTA_ERR_NOT_ENABLED otherwise): totals over the successful log calls since create / reset of
+ * the batches and records left out as aborted, and the records of undecided transactional batches that were delivered
+ * (any pointer may be NULL) */
+int kta_log_txn_stats(kta_handle *h, uint64_t *aborted_batches, uint64_t *aborted_records, uint64_t *undecided_records);
 
 /* ---- introspection for benchmarks ---- */
 /* kernels launched by this handle since create/reset, and device time of the scan kernels (ms,

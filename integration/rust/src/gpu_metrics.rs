@@ -16,7 +16,7 @@ use std::os::raw::{c_char, c_int};
 #[repr(C)]
 pub struct KtaConfig {
     struct_size: i32, device: i32, num_partitions: i32, count_alive_keys: i32, hll_precision: i32, alive_table_kib: i32,
-    ring_records: i64, ring_key_bytes: i64, now_s: i64, now_ns: i32, reserved1: i32, shard_world: i32, shard_rank: i32,
+    ring_records: i64, ring_key_bytes: i64, now_s: i64, now_ns: i32, isolation_level: i32, shard_world: i32, shard_rank: i32,
 }
 #[repr(C)]
 pub struct KtaHandle { _private: [u8; 0] }
@@ -49,7 +49,7 @@ impl GpuMetrics {
             struct_size: std::mem::size_of::<KtaConfig>() as i32, device: -1, num_partitions,
             count_alive_keys: count_alive_keys as i32, hll_precision: 0, alive_table_kib: 0, ring_records: 0, ring_key_bytes: 0,
             now_s: i64::MIN, // the library reads the clock itself: earliest_message starts at Utc::now() (metric.rs:39)
-            now_ns: 0, reserved1: 0, shard_world: 0, shard_rank: 0,
+            now_ns: 0, isolation_level: 0, shard_world: 0, shard_rank: 0,
         };
         let mut h = std::ptr::null_mut();
         if unsafe { kta_create(&cfg, &mut h) } != 0 { panic!("kta_create failed: {}", last_error()); }

@@ -21,6 +21,7 @@ KTA_KEY_TILE = 128
 KTA_HIST_BUCKETS = 32
 INT64_MIN = -(1 << 63)
 SEQ_AUTO = (1 << 64) - 1   # include/kta.h KTA_SEQ_AUTO
+READ_UNCOMMITTED, READ_COMMITTED = 0, 1   # include/kta.h KTA_READ_UNCOMMITTED / KTA_READ_COMMITTED
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -78,7 +79,7 @@ class Config(C.Structure):
         ("struct_size", C.c_int32), ("device", C.c_int32), ("num_partitions", C.c_int32),
         ("count_alive_keys", C.c_int32), ("hll_precision", C.c_int32), ("alive_table_kib", C.c_int32),
         ("ring_records", C.c_int64), ("ring_key_bytes", C.c_int64), ("now_s", C.c_int64),
-        ("now_ns", C.c_int32), ("reserved1", C.c_int32), ("shard_world", C.c_int32), ("shard_rank", C.c_int32),
+        ("now_ns", C.c_int32), ("isolation_level", C.c_int32), ("shard_world", C.c_int32), ("shard_rank", C.c_int32),
     ]
 
 
@@ -136,6 +137,8 @@ SYMBOLS = {
     "kta_scan_log_batches_device": (C.c_int, [_P, _P, C.c_int64, _P, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "kta_push_log_segment_host": (C.c_int, [_P, C.c_int32, _P, C.c_int64, C.POINTER(C.c_int64)]),
     "kta_push_log_segments_host": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.POINTER(C.c_int64)]),
+    "kta_log_add_txn_index_host": (C.c_int, [_P, C.c_int32, _P, C.c_int64]),
+    "kta_log_txn_stats": (C.c_int, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "kta_stats": (C.c_int, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "kta_set_timing": (C.c_int, [_P, C.c_int]),
     "kta_scan_time_ms": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),

@@ -6,10 +6,14 @@
 //                                                                (the in-memory topic of BASELINE.json configs)
 //   --log-dir DIR              read Kafka log segments from DIR/<topic>-<partition>/*.log (a broker's data directory)
 //                              and decode them on the GPU (RecordBatch v2, magic 2; uncompressed, gzip, LZ4, Snappy or
-//                              zstd batches; compressed sections' checksums are not verified).  Differences from a librdkafka
-//                              consumer: records of ABORTED transactions are counted (a consumer with the default
-//                              isolation.level=read_committed filters them; the .txnindex files are not read here),
-//                              and legacy magic 0/1 message sets are reported as malformed.
+//                              zstd batches; compressed sections' checksums are not verified).  Isolation follows
+//                              --librdkafka isolation.level=read_committed|read_uncommitted; the default here is
+//                              read_uncommitted (every record counted), the reference's librdkafka default is read_committed.
+//                              Under read_committed the *.txnindex files of every partition directory are read first and the
+//                              records of aborted transactions are left out (include/kta.h).  Differences from a librdkafka
+//                              consumer: records of transactions still open at the end of the files are counted (with a
+//                              warning) instead of waiting at the last stable offset, and legacy magic 0/1 message sets are
+//                              reported as malformed.
 //   --feed push|batch|device   how records reach the handlers: kta_push per record (the reference's call shape),
 //                              kta_push_batch_host, or generated and scanned in HBM
 //
@@ -63,11 +67,11 @@ static bool read_file(const std::string &path, std::vector<uint8_t> &out) {
 static int print_report(kta_handle *h, const std::string &topic, const std::vector<int> &partitions, const std::vector<int64_t> &start_offsets,
                         const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs);
 
-static int analyze_log_dir(const std::string &topic, const std::string &dir, bool alive, int hll,
+static int analyze_log_dir(const std::string &topic, const std::string &dir, bool alive, int hll, bool read_committed,
                            std::chrono::steady_clock::time_point start_time) {
     // get_topic_offsets (src/kafka.rs:60-72) from the files: partitions = <topic>-<n> directories, low watermark =
     // first batch's baseOffset, high watermark = last batch's baseOffset + lastOffsetDelta + 1
-    std::map<int, std::vector<std::string>> segs;
+    std::map<int, std::vector<std::string>> segs, txn_indexes;
     DIR *d = opendir(dir.c_str());
     if (!d) { fprintf(stderr, "Error fetching metadata: cannot open %s\n", dir.c_str()); return 101; }
     while (dirent *e = readdir(d)) {
@@ -82,6 +86,7 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
         while (dirent *fe = readdir(pd)) {
             const std::string fn = fe->d_name;
             if (fn.size() > 4 && fn.substr(fn.size() - 4) == ".log") files.push_back(dir + "/" + name + "/" + fn);
+            if (fn.size() > 9 && fn.substr(fn.size() - 9) == ".txnindex") txn_indexes[p].push_back(dir + "/" + name + "/" + fn);
         }
         closedir(pd);
         std::sort(files.begin(), files.end());
@@ -98,8 +103,22 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
     cfg.count_alive_keys = alive ? 1 : 0;
     cfg.hll_precision = hll;
     cfg.now_s = INT64_MIN;
+    cfg.isolation_level = read_committed ? KTA_READ_COMMITTED : KTA_READ_UNCOMMITTED;
     kta_handle *h = nullptr;
     KTA(kta_create(&cfg, &h));
+    // read_committed: every partition's aborted transactions are known before any segment is decoded, so a transaction
+    // whose marker lies in a later group of segments is decided exactly
+    if (read_committed)
+        for (auto &kv : txn_indexes)
+            if (segs.count(kv.first))
+                for (const auto &path : kv.second) {
+                    std::vector<uint8_t> buf;
+                    if (!read_file(path, buf)) { fprintf(stderr, "cannot read %s\n", path.c_str()); return 1; }
+                    if (kta_log_add_txn_index_host(h, kv.first, buf.data(), (int64_t)buf.size()) != KTA_OK) {
+                        fprintf(stderr, "error: %s: %s\n", path.c_str(), kta_last_error());
+                        return 1;
+                    }
+                }
     printf("Subscribing to %s\n", topic.c_str());
     printf("Starting message consumption...\n");
     auto be64 = [](const uint8_t *p) { uint64_t v = 0; for (int i = 0; i < 8; i++) v = (v << 8) | p[i]; return (int64_t)v; };
@@ -142,6 +161,13 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
         return 254;
     }
     finalize_or_warn(h);
+    if (read_committed) {
+        uint64_t undecided = 0;
+        KTA(kta_log_txn_stats(h, nullptr, nullptr, &undecided));
+        if (undecided)
+            fprintf(stderr, "warning: %llu record(s) of transactions without a commit or abort marker in the files were counted "
+                    "(a read_committed consumer would wait for them to be decided)\n", (unsigned long long)undecided);
+    }
     const uint64_t secs = (uint64_t)std::chrono::duration_cast<std::chrono::seconds>(std::chrono::steady_clock::now() - start_time).count();
     // the report has one row per partition of the topic's metadata (main.rs:103-106): the <topic>-<n> directories found
     std::vector<int> present;
@@ -172,6 +198,11 @@ int main(int argc, char **argv) {
                  "FLAGS:\n    -c, --count-alive-keys    Counts the effective number of alive keys in a log compacted topic\n\n"
                  "OPTIONS:\n    -b, --bootstrap-server <BOOTSTRAP_SERVER>    Bootstrap server(s) to work with, comma separated\n"
                  "        --librdkafka <LIBRDKAFKA>                Options to pass into the underlying librdkafka\n"
+                 "                                                 (this build reads isolation.level=read_committed|read_uncommitted\n"
+                 "                                                 for --log-dir; its default is read_uncommitted, librdkafka's is\n"
+                 "                                                 read_committed: pass isolation.level=read_committed to match it)\n"
+                 "        --log-dir <DIR>                          read <DIR>/<TOPIC>-<partition>/*.log (and, read_committed,\n"
+                 "                                                 *.txnindex) instead of a broker\n"
                  "    -t, --topic <TOPIC>                          The topic to analyze\n"
                  "        --synthetic <k=v,...>                    in-memory synthetic topic (this build has no Kafka client)\n"
                  "        --feed <push|batch|device>               how records are handed to the metric handlers");
@@ -186,8 +217,26 @@ int main(int argc, char **argv) {
         fprintf(stderr, "Error fetching metadata: this build has no librdkafka client (no broker access); pass --log-dir DIR or --synthetic n=...,partitions=...\n");
         return 101;  // the reference panics here (src/kafka.rs:61)
     }
+    // --librdkafka k=v,k=v (src/main.rs:84-93).  Without a client only isolation.level has a meaning here.
+    bool read_committed = false;
+    for (size_t p = 0; !librdkafka.empty() && p <= librdkafka.size();) {
+        size_t e = librdkafka.find(',', p);
+        if (e == std::string::npos) e = librdkafka.size();
+        const std::string item = librdkafka.substr(p, e - p);
+        const size_t q = item.find('=');
+        if (q == std::string::npos) { fprintf(stderr, "error: --librdkafka: '%s' is not key=value\n", item.c_str()); return 2; }
+        if (item.substr(0, q) == "isolation.level") {
+            const std::string v = item.substr(q + 1);
+            if (v != "read_committed" && v != "read_uncommitted") {
+                fprintf(stderr, "error: --librdkafka: isolation.level must be read_committed or read_uncommitted, not '%s'\n", v.c_str());
+                return 2;
+            }
+            read_committed = v == "read_committed";
+        }
+        p = e + 1;
+    }
     const auto start_time = std::chrono::steady_clock::now();  // main.rs:69
-    if (!log_dir.empty()) return analyze_log_dir(topic, log_dir, count_alive_occurrences == 1, hll, start_time);
+    if (!log_dir.empty()) return analyze_log_dir(topic, log_dir, count_alive_occurrences == 1, hll, read_committed, start_time);
 
     std::map<std::string, std::string> kv;
     for (size_t p = 0; p < synthetic.size();) {

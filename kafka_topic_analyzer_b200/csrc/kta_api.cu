@@ -19,9 +19,12 @@
 #include <new>
 #include <vector>
 
+#include <cub/device/device_radix_sort.cuh>
+
 #include "kta_kernels.cuh"
 #include "kta_logdecode.cuh"
 #include "kta_logdecode_launch.cuh"
+#include "kta_logtxn.cuh"
 #include "kta_synth.h"
 
 using namespace kta;
@@ -108,6 +111,21 @@ struct AliveKeys {
     std::vector<AlivePending> pending;
 };
 
+// read_committed isolation of the log entry points (kta_logtxn.cuh); allocated only on a read_committed handle
+struct TxnState {
+    TxnKey *d_keys = nullptr, *d_sorted = nullptr;   // classify's keys / sorted by (partition, producerId, batch)
+    uint8_t *d_kind = nullptr;                       // per batch: TxnKind of transactional data batches and markers
+    uint8_t *d_res = nullptr;                        // per sorted key: next marker within its resolve tile
+    int64_t cap = 0;
+    uint8_t *d_tile = nullptr; int64_t tile_cap = 0; // tile heads, then the carries behind each tile
+    void *d_sort_tmp = nullptr; size_t sort_tmp_bytes = 0;
+    uint32_t *d_word = nullptr;                      // [0] keys classified, [1] TxnErr bits
+    unsigned long long *d_stats = nullptr;           // this call: aborted batches, aborted records, undecided records
+    std::vector<TxnRange> ranges;                    // registered aborted ranges, sorted and merged; mirrored in d_ranges
+    TxnRange *d_ranges = nullptr; int64_t ranges_cap = 0;
+    uint64_t totals[3] = {0, 0, 0};                  // the stats of every successful call since create / reset
+};
+
 struct kta_handle {
     kta_config cfg{};
     int device = 0;
@@ -135,6 +153,8 @@ struct kta_handle {
     uint8_t *d_unc_lit = nullptr; int64_t unc_lit_cap = 0;   // zstd: Huffman-decoded literals, at the offsets of d_unc
     uint64_t *d_unc_slot = nullptr; int64_t unc_slot_cap = 0;
     uint32_t *d_log_err = nullptr;
+    bool read_committed = false;
+    TxnState txn;
     size_t nsums = 0, nhll = 0;
     // landing ring
     Chunk chunks[NCHUNK];
@@ -545,6 +565,9 @@ extern "C" int kta_destroy(kta_handle *h) {
     cudaFree(h->d_log_bytes); cudaFree(h->d_log_off); cudaFree(h->d_log_info); cudaFree(h->d_log_cnt);
     cudaFree(h->d_dec_part); cudaFree(h->d_dec_klen); cudaFree(h->d_dec_vlen); cudaFree(h->d_dec_ts); cudaFree(h->d_dec_keys); cudaFree(h->d_dec_ksrc); cudaFree(h->d_unc); cudaFree(h->d_unc_lit); cudaFree(h->d_unc_slot);
     cudaFree(h->d_log_err);
+    TxnState &t = h->txn;
+    cudaFree(t.d_keys); cudaFree(t.d_sorted); cudaFree(t.d_kind); cudaFree(t.d_res); cudaFree(t.d_tile); cudaFree(t.d_sort_tmp);
+    cudaFree(t.d_word); cudaFree(t.d_stats); cudaFree(t.d_ranges);
     for (auto &e : h->ev_pool) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
     if (h->stream && h->own_stream) cudaStreamDestroy(h->stream);
     cudaGetLastError();
@@ -558,6 +581,9 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
         return fail(KTA_ERR_INVALID, "num_partitions %d out of range [1, 2^20]", cfg->num_partitions);
     if (cfg->hll_precision != 0 && (cfg->hll_precision < 4 || cfg->hll_precision > 18))
         return fail(KTA_ERR_INVALID, "hll_precision %d not 0 or 4..18", cfg->hll_precision);
+    if (cfg->isolation_level != KTA_READ_UNCOMMITTED && cfg->isolation_level != KTA_READ_COMMITTED)
+        return fail(KTA_ERR_INVALID, "isolation_level %d is neither KTA_READ_UNCOMMITTED (0) nor KTA_READ_COMMITTED (1)", cfg->isolation_level);
+    h->read_committed = cfg->isolation_level == KTA_READ_COMMITTED;
     int ndev = 0;
     CU(cudaGetDeviceCount(&ndev));
     if (ndev < 1) return fail(KTA_ERR_CUDA, "no CUDA device (this library has no CPU fallback)");
@@ -592,6 +618,10 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
     if (h->nhll) CU(cudaMalloc(&h->d_hll, h->nhll * 4));
     int rc;
     if (cfg->count_alive_keys == 1 && (rc = alive_create(h))) return rc;
+    if (h->read_committed) {
+        CU(cudaMalloc(&h->txn.d_word, 8));
+        CU(cudaMalloc(&h->txn.d_stats, 24));
+    }
     h->smem_optin = prop.sharedMemPerBlockOptin;
     if (cfg->shard_world > 1) {
         if (cfg->shard_rank < 0 || cfg->shard_rank >= cfg->shard_world || cfg->shard_world > P)
@@ -794,6 +824,56 @@ extern "C" int kta_scan_batch_device(kta_handle *h, const kta_batch *b) {
 // Kafka RecordBatch v2 segments → SoA → scan (SURVEY.md §8 f2; kernels in kta_logdecode.cuh)
 // ------------------------------------------------------------------------------------------------
 
+// read_committed: the passes of kta_logtxn.cuh over the batches log_header_kernel has read, before the record count is
+// scanned.  Classify always; sort, resolve, carry and apply only when the call has transactional batches.  One host round
+// trip (the classify count).  *ran: the apply pass was launched, so its error word and counters are to be read back.
+static int txn_passes(kta_handle *h, int32_t partition, const uint8_t *dev_bytes, int64_t nbatches, bool *ran) {
+    TxnState &t = h->txn;
+    cudaStream_t s = h->stream;
+    *ran = false;
+    if (nbatches > (int64_t)UINT32_MAX) return fail(KTA_ERR_INVALID, "%lld batches in one read_committed call: split them", (long long)nbatches);
+    int rc;
+    if ((rc = grow(s, t.cap, nbatches, t.d_keys, t.d_sorted, t.d_kind, t.d_res))) return rc;
+    CU(cudaMemsetAsync(t.d_word, 0, 8, s));
+    txn_classify_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, t.d_keys, t.d_kind, t.d_word);
+    CU(cudaGetLastError());
+    h->launches++;
+    uint32_t w[3] = {0, 0, 0};   // keys, TxnErr bits, header flags
+    CU(cudaMemcpyAsync(w, t.d_word, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(w + 2, h->d_log_err, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (w[2] & (LOGB_BAD | LOGB_COMPRESSED)) return KTA_OK;   // the call is refused for its headers (scan_log_batches says so)
+    if (w[1] & TXN_ERR_MARKER)
+        return fail(KTA_ERR_INVALID, "unreadable transaction marker in partition %d (control batch compressed, without a record, "
+                    "truncated, or with a key that is not version 0 | type)", partition);
+    const int64_t m = w[0];
+    if (m == 0) return KTA_OK;
+    size_t tmp = 0;
+    CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp, t.d_keys, t.d_sorted, m, TxnKeyDecomposer{}, s));
+    if (tmp > t.sort_tmp_bytes) {
+        CU(cudaStreamSynchronize(s));
+        cudaFree(t.d_sort_tmp);
+        t.d_sort_tmp = nullptr;
+        t.sort_tmp_bytes = 0;
+        CU(cudaMalloc(&t.d_sort_tmp, tmp));
+        t.sort_tmp_bytes = tmp;
+    }
+    tmp = t.sort_tmp_bytes;
+    CU(cub::DeviceRadixSort::SortKeys(t.d_sort_tmp, tmp, t.d_keys, t.d_sorted, m, TxnKeyDecomposer{}, s));
+    const int64_t tiles = (m + TXN_TILE - 1) / TXN_TILE;
+    if ((rc = grow(s, t.tile_cap, 2 * tiles, t.d_tile))) return rc;
+    CU(cudaMemsetAsync(t.d_stats, 0, 24, s));
+    txn_resolve_kernel<<<(unsigned)tiles, TXN_TILE, 0, s>>>(t.d_sorted, m, t.d_kind, h->d_log_info, t.d_res, t.d_tile, t.d_word);
+    txn_carry_kernel<<<1, 1024, 0, s>>>(t.d_tile, tiles, t.d_tile + tiles);
+    txn_apply_kernel<<<(int)std::min<int64_t>((m + 255) / 256, (int64_t)h->sm_count * 16), 256, 0, s>>>(
+        t.d_sorted, m, t.d_kind, t.d_res, t.d_tile + tiles, t.d_ranges, (int64_t)t.ranges.size(), h->d_log_info, h->d_log_cnt, t.d_word,
+        t.d_stats);
+    CU(cudaGetLastError());
+    h->launches += 4;   // (the sort counted as one)
+    *ran = true;
+    return KTA_OK;
+}
+
 static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes,
                             int64_t len, int64_t readable /* bytes of dev_bytes that may be READ (>= len when the buffer has slack) */,
                             const uint64_t *dev_batch_off, int64_t nbatches, int64_t *records_out) {
@@ -810,18 +890,35 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     CU(cudaMemsetAsync(h->d_log_err, 0, 8, s));
     log_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, h->d_log_info,
                                             h->d_log_cnt, h->d_log_err);
+    CU(cudaGetLastError());
+    bool txn = false;   // read_committed and the call has transactional batches
+    if (h->read_committed && (rc = txn_passes(h, partition, dev_bytes, nbatches, &txn))) return rc;
     tile_base_scan_kernel<<<1, 1024, 0, s>>>(h->d_log_cnt, nbatches);   // inclusive scan of [1..nbatches] in place
     CU(cudaGetLastError());
     h->launches += 2;
     uint64_t nrec = 0;
     uint32_t err[2] = {0, 0};
+    uint32_t txn_word[2] = {0, 0};
+    unsigned long long txn_stats[3] = {0, 0, 0};
     CU(cudaMemcpyAsync(&nrec, h->d_log_cnt + nbatches, 8, cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(err, h->d_log_err, 8, cudaMemcpyDeviceToHost, s));
+    if (txn) {
+        CU(cudaMemcpyAsync(txn_word, h->txn.d_word, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(txn_stats, h->txn.d_stats, 24, cudaMemcpyDeviceToHost, s));
+    }
     CU(cudaStreamSynchronize(s));
     if (err[0] & LOGB_COMPRESSED)
         return fail(KTA_ERR_INVALID, "unknown compression codec (attributes bits 0-2 = 5..7) in partition %d", partition);
     if (err[0] & LOGB_BAD) return fail(KTA_ERR_INVALID, "malformed record batch header in partition %d", partition);
-    if (nrec == 0) return KTA_OK;
+    if (txn_word[1] & TXN_ERR_ORDER)
+        return fail(KTA_ERR_INVALID, "the batches of one producer in partition %d are not in increasing baseOffset order", partition);
+    auto count_txn = [&]() {   // the call succeeded: its transaction counters join the handle's totals
+        for (int i = 0; i < 3; i++) h->txn.totals[i] += txn_stats[i];
+    };
+    if (nrec == 0) {
+        count_txn();
+        return KTA_OK;
+    }
     if (err[0] & LOGB_CODECS) {
         // compressed batches: size pass, scratch allocation, decompression; afterwards they are ordinary batches that
         // happen to lie in the scratch buffer
@@ -899,6 +996,7 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
         if (err[0]) return fail(KTA_ERR_INVALID, "malformed record inside a batch of partition %d", partition);
     }
     if ((rc = kta_scan_batch_device(h, &b))) return rc;
+    count_txn();
     if (records_out) *records_out = (int64_t)nrec;
     return KTA_OK;
 }
@@ -964,6 +1062,59 @@ extern "C" int kta_push_log_segments_host(kta_handle *h, int32_t nsegs, const in
 extern "C" int kta_push_log_segment_host(kta_handle *h, int32_t partition, const uint8_t *bytes, int64_t len,
                                          int64_t *records_out) {
     return kta_push_log_segments_host(h, 1, &partition, &bytes, &len, records_out);
+}
+
+// A .txnindex image: 34-byte big-endian entries version i16 (= 0) | producerId i64 | firstOffset i64 | lastOffset i64 |
+// lastStableOffset i64.  All of it is checked before any range is added.
+extern "C" int kta_log_add_txn_index_host(kta_handle *h, int32_t partition, const uint8_t *bytes, int64_t len) {
+    if (!h || len < 0 || (len && !bytes)) return fail(KTA_ERR_INVALID, "bad argument");
+    if (!h->read_committed) return fail(KTA_ERR_INVALID, "transaction index on a read_uncommitted handle");
+    if (partition < 0 || partition >= h->cfg.num_partitions)
+        return fail(KTA_ERR_INVALID, "partition %d outside [0, %d)", partition, h->cfg.num_partitions);
+    constexpr int64_t ENTRY = 34;
+    if (len % ENTRY) return fail(KTA_ERR_INVALID, "transaction index of %lld bytes: not a multiple of %lld", (long long)len, (long long)ENTRY);
+    auto be = [](const uint8_t *p, int n) { uint64_t v = 0; for (int i = 0; i < n; i++) v = (v << 8) | p[i]; return v; };
+    std::vector<TxnRange> add;
+    for (int64_t at = 0; at < len; at += ENTRY) {
+        const uint8_t *e = bytes + at;
+        const TxnRange r{partition, 0u, be(e + 2, 8), (int64_t)be(e + 10, 8), (int64_t)be(e + 18, 8)};
+        if (be(e, 2) != 0) return fail(KTA_ERR_INVALID, "transaction index entry %lld: version %d", (long long)(at / ENTRY), (int)be(e, 2));
+        if (r.first > r.last)
+            return fail(KTA_ERR_INVALID, "transaction index entry %lld: firstOffset %lld > lastOffset %lld", (long long)(at / ENTRY),
+                        (long long)r.first, (long long)r.last);
+        add.push_back(r);
+    }
+    if (add.empty()) return KTA_OK;
+    // sorted by (partition, producerId, firstOffset), overlapping ranges of one producer merged: the apply pass's binary
+    // search then has one candidate per offset
+    std::vector<TxnRange> &v = h->txn.ranges;
+    v.insert(v.end(), add.begin(), add.end());
+    std::sort(v.begin(), v.end(), [](const TxnRange &a, const TxnRange &b) {
+        return a.part != b.part ? a.part < b.part : a.pid != b.pid ? a.pid < b.pid : a.first < b.first;
+    });
+    size_t out = 0;
+    for (size_t i = 0; i < v.size(); i++) {
+        if (out && v[out - 1].part == v[i].part && v[out - 1].pid == v[i].pid && v[i].first <= v[out - 1].last)
+            v[out - 1].last = std::max(v[out - 1].last, v[i].last);
+        else v[out++] = v[i];
+    }
+    v.resize(out);
+    int rc;
+    if ((rc = set_device(h))) return rc;
+    if ((rc = grow(h->stream, h->txn.ranges_cap, (int64_t)v.size(), h->txn.d_ranges))) return rc;
+    CU(cudaStreamSynchronize(h->stream));   // no queued pass reads the ranges while they are replaced
+    CU(cudaMemcpyAsync(h->txn.d_ranges, v.data(), v.size() * sizeof(TxnRange), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    return KTA_OK;
+}
+
+extern "C" int kta_log_txn_stats(kta_handle *h, uint64_t *aborted_batches, uint64_t *aborted_records, uint64_t *undecided_records) {
+    if (!h) return fail(KTA_ERR_INVALID, "null handle");
+    if (!h->read_committed) return fail(KTA_ERR_NOT_ENABLED, "the handle is read_uncommitted");
+    if (aborted_batches) *aborted_batches = h->txn.totals[0];
+    if (aborted_records) *aborted_records = h->txn.totals[1];
+    if (undecided_records) *undecided_records = h->txn.totals[2];
+    return KTA_OK;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1227,6 +1378,8 @@ extern "C" int kta_reset(kta_handle *h) {
     h->finalized = false;
     h->launches = 0;
     h->records = 0;
+    h->txn.ranges.clear();
+    for (uint64_t &v : h->txn.totals) v = 0;
     return state_reset_device(h);
 }
 

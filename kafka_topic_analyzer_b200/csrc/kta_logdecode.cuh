@@ -17,8 +17,9 @@
 // format), Snappy (raw or xerial-framed) and zstd (kta_zstd.cuh) batches are decompressed on the GPU into a scratch buffer and
 // then decoded like the others; the unassigned codes 5-7 are rejected.  Checksums inside the compressed sections (gzip's
 // CRC32, zstd's Content_Checksum) are skipped, not verified, like the batch CRC.
-// Not handled: records of aborted transactions are delivered (a read_committed consumer would filter them through the
-// .txnindex / abort markers), legacy magic 0/1 message sets are flagged as malformed.
+// Isolation: on a read_committed handle the passes of kta_logtxn.cuh mark the batches of aborted transactions
+// LOGB_SKIP_ABORTED before anything here decompresses or decodes them; on a read_uncommitted handle (the default) every
+// data batch is delivered, as before.  Not handled: legacy magic 0/1 message sets are flagged as malformed.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -32,9 +33,10 @@ namespace kta {
 constexpr int LOG_HEADER_BYTES = 61;
 // LOGB_COMPRESSED: an unknown compression codec (the unassigned codes 5-7).  LOGB_LZ4 / LOGB_SNAPPY / LOGB_GZIP / LOGB_ZSTD: the
 // records section must be decompressed first (log_unc_size_kernel, log_zstd_size_kernel for zstd, and log_decompress_kernel
-// turn such a batch into LOGB_OK).
+// turn such a batch into LOGB_OK).  LOGB_SKIP_ABORTED: a batch of an aborted transaction (read_committed only,
+// kta_logtxn.cuh); it replaces any codec flag, so no later pass touches the batch.
 enum LogBatchFlags { LOGB_OK = 0, LOGB_SKIP_CONTROL = 1, LOGB_BAD = 2, LOGB_COMPRESSED = 4, LOGB_LZ4 = 8, LOGB_SNAPPY = 16, LOGB_GZIP = 32,
-                     LOGB_ZSTD = 64 };
+                     LOGB_ZSTD = 64, LOGB_SKIP_ABORTED = 128 };
 constexpr uint32_t LOGB_CODECS = LOGB_LZ4 | LOGB_SNAPPY | LOGB_GZIP | LOGB_ZSTD;   // batches log_decompress_kernel turns into LOGB_OK
 
 __device__ __forceinline__ uint64_t be_u64(const uint8_t *p) {

@@ -53,9 +53,16 @@ class KtaEngine:
 
     def __init__(self, num_partitions: int, count_alive_keys: bool = False, hll_precision: int = 0,
                  device: int = -1, ring_records: int = 0, ring_key_bytes: int = 0,
-                 now: Optional[tuple] = None, alive_table_kib: int = 0, shard: Optional[tuple] = None):
-        """shard = (rank, world): this engine scans only partitions p with p % world == rank (a partition-sharded job)."""
+                 now: Optional[tuple] = None, alive_table_kib: int = 0, shard: Optional[tuple] = None,
+                 isolation_level: str = "read_uncommitted"):
+        """shard = (rank, world): this engine scans only partitions p with p % world == rank (a partition-sharded job).
+        isolation_level: "read_uncommitted" (every data batch of a log segment is delivered) or "read_committed" (records
+        of aborted transactions are left out, include/kta.h)."""
+        levels = {"read_uncommitted": N.READ_UNCOMMITTED, "read_committed": N.READ_COMMITTED}
+        if isolation_level not in levels:
+            raise ValueError("isolation_level must be 'read_uncommitted' or 'read_committed', not %r" % (isolation_level,))
         cfg = Config()
+        cfg.isolation_level = levels[isolation_level]
         cfg.struct_size = C.sizeof(Config)
         cfg.device = device
         cfg.num_partitions = num_partitions
@@ -173,6 +180,18 @@ class KtaEngine:
         n = C.c_int64()
         check(lib().kta_push_log_segments_host(self._h, k, parts, ptrs, lens, C.byref(n)))
         return n.value
+
+    def push_txn_index(self, partition: int, data) -> None:
+        """Register the aborted transactions of one .txnindex image of `partition` for every later log call
+        (read_committed engines only)."""
+        buf = np.frombuffer(data, dtype=np.uint8) if not isinstance(data, np.ndarray) else data
+        check(lib().kta_log_add_txn_index_host(self._h, partition, buf.ctypes.data if buf.size else None, buf.size))
+
+    def log_txn_stats(self):
+        """(aborted batches, aborted records, undecided records) since create / reset (read_committed engines only)."""
+        v = [C.c_uint64() for _ in range(3)]
+        check(lib().kta_log_txn_stats(self._h, *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
 
     def sync(self) -> None:
         check(lib().kta_sync(self._h))

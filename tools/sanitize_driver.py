@@ -1,6 +1,6 @@
 """Small end-to-end runs of every scan-kernel mode for compute-sanitizer (tools/sanitize.sh): counters, in-stream HLL,
 exact alive keys (table starting far too small, so growth + stamps-only re-runs happen too), ragged keys, a tail tile,
-the host ring path and the log-segment decoder.  Each run is checked against the oracle so a 'clean' sanitizer log is the
+the host ring path, the log-segment decoder and its read_committed passes.  Each run is checked against the oracle so a 'clean' sanitizer log is the
 log of a run that also computed the right answer."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -11,7 +11,7 @@ from kafka_topic_analyzer_b200 import synth
 from parity import assert_parity, oracle_for
 
 NOW = (4102444800, 1)
-which = sys.argv[1:] or ["counters", "hll", "exact", "ragged", "ring", "log", "logz", "logzstd"]
+which = sys.argv[1:] or ["counters", "hll", "exact", "ragged", "ring", "log", "logz", "logzstd", "logtxn"]
 
 
 def compress_segment(seg, b0=0):
@@ -62,6 +62,21 @@ def zstd_segment(seg, b0=0):
 P = 8
 n = P * 4096 + 0
 for name in which:
+    if name == "logtxn":   # read_committed: markers, aborted compressed batches, registered ranges, two calls
+        import test_log_txn as lt
+        t = lt.gen_topic(3, P=P, steps=200)
+        cut = {p: len(t.batches[p]) // 2 for p in range(P)}
+        calls = [[b for p in range(P) for b in t.batches[p][:cut[p]]], [b for p in range(P) for b in t.batches[p][cut[p]:]]]
+        want, stats = lt.rule_model(calls, t.aborted)
+        with kta.KtaEngine(P, count_alive_keys=True, device=0, now=NOW, alive_table_kib=1, isolation_level="read_committed") as e:
+            for p in range(P):
+                e.push_txn_index(p, lt.txn_index(t.aborted[p]))
+            e.push_log_segments([(p, t.segment(p, 0, cut[p])) for p in range(P)])
+            e.push_log_segments([(p, t.segment(p, cut[p])) for p in range(P)])
+            e.finalize()
+            assert e.log_txn_stats() == stats and e.message_metrics.overall_count() == len(want)
+        print(name, "ok", stats)
+        continue
     key_mode = 2 if name in ("ragged", "ring") else 0
     spec = synth.make_spec(n, P, key_mode=key_mode, distinct_keys=3000, tombstone_per_10k=2500, ts_missing_per_10k=20,
                            run_len=64 if name == "counters" else 1)
