@@ -70,19 +70,57 @@ static constexpr int32_t ALIVE_MAX_KIB = 32 * 1024 * 1024;     // 32 GiB = one s
 static constexpr int64_t ALIVE_CACHE_MIN_RECORDS = 1 << 20;    // smaller batches go straight to the table
 static constexpr int64_t DEFAULT_RING_RECORDS = 1 << 22;  // 4 Mi records per chunk
 
+// Owner of `cap` elements of device (DevBuf) or pinned host (PinnedBuf) memory: move-only, freed by its destructor.
+template <typename T, bool PINNED>
+class Buf {
+    T *p_ = nullptr;
+    void release() {
+        if (p_) PINNED ? cudaFreeHost(p_) : cudaFree(p_);
+        p_ = nullptr;
+        cap = 0;
+    }
+
+  public:
+    int64_t cap = 0;
+    Buf() = default;
+    Buf(Buf &&o) noexcept : p_(o.p_), cap(o.cap) { o.p_ = nullptr; o.cap = 0; }
+    Buf &operator=(Buf &&o) noexcept { std::swap(p_, o.p_); std::swap(cap, o.cap); return *this; }   // o frees the old memory
+    ~Buf() { release(); }
+    T *get() const { return p_; }
+    operator T *() const { return p_; }
+    // n elements, for a buffer of fixed size
+    int alloc(int64_t n) {
+        release();
+        void *p = nullptr;
+        const size_t bytes = (size_t)n * sizeof(T);
+        CU(PINNED ? cudaHostAlloc(&p, bytes, cudaHostAllocDefault) : cudaMalloc(&p, bytes));
+        p_ = static_cast<T *>(p);
+        cap = n;
+        return KTA_OK;
+    }
+    // at least `need` elements (contents not kept): null with cap 0 if the allocation fails
+    int grow(cudaStream_t s, int64_t need) {
+        if (need <= cap) return KTA_OK;
+        CU(cudaStreamSynchronize(s));   // queued work may still read the old buffer
+        return alloc(need + need / 4 + 64);
+    }
+};
+template <typename T> using DevBuf = Buf<T, false>;
+template <typename T> using PinnedBuf = Buf<T, true>;
+
 struct Chunk {
     // device staging (shared by kta_push and kta_push_batch_host)
-    int32_t *d_partition = nullptr, *d_klen = nullptr, *d_vlen = nullptr;
-    int64_t *d_ts = nullptr;
-    uint64_t *d_seq = nullptr;
-    uint8_t *d_keys = nullptr;
-    uint64_t *d_tile_base = nullptr;
+    DevBuf<int32_t> d_partition, d_klen, d_vlen;
+    DevBuf<int64_t> d_ts;
+    DevBuf<uint64_t> d_seq;
+    DevBuf<uint8_t> d_keys;
+    DevBuf<uint64_t> d_tile_base;
     cudaEvent_t free_ev = nullptr;  // recorded after the scan that reads this chunk
     // pinned landing area for kta_push
-    int32_t *h_partition = nullptr, *h_klen = nullptr, *h_vlen = nullptr;
-    int64_t *h_ts = nullptr;
-    uint8_t *h_keys = nullptr;
-    uint64_t *h_tile_base = nullptr;
+    PinnedBuf<int32_t> h_partition, h_klen, h_vlen;
+    PinnedBuf<int64_t> h_ts;
+    PinnedBuf<uint8_t> h_keys;
+    PinnedBuf<uint64_t> h_tile_base;
 };
 
 // Stamps the alive-key table has not confirmed yet (it may turn out too small: then they are applied again, which is
@@ -97,14 +135,14 @@ struct AlivePending {
 
 // Host side of the exact alive-key table (-c); only the alive_* functions read the status words or the pending list
 struct AliveKeys {
-    unsigned long long *d_table = nullptr;   // open-addressed last-writer table, 2 * pairs slots
+    DevBuf<unsigned long long> d_table;      // open-addressed last-writer table, 2 * pairs slots
     uint32_t pairs = 0;
     uint64_t origin = 0;                     // seq that a stamp's field value 1 stands for
     bool rebased = false;                    // a rebase dropped absolute sequence numbers (exports are refused then)
-    uint32_t *d_cache = nullptr;             // seen cache of the batch being scanned (32 MiB, cleared per launch)
-    uint32_t *d_status = nullptr;            // [0] stamps that found no slot, [1] records outside the seq window, [2] wide re-run
-    uint32_t *h_status = nullptr;            // pinned: [0..1] read by alive_settle, [2c + 2..] snapshot behind ring chunk c's scan
-    unsigned long long *d_count = nullptr;   // [0] alive entries, [1] export cursor, [2] occupied slots
+    DevBuf<uint32_t> d_cache;                // seen cache of the batch being scanned (32 MiB, cleared per launch)
+    DevBuf<uint32_t> d_status;               // [0] stamps that found no slot, [1] records outside the seq window, [2] wide re-run
+    PinnedBuf<uint32_t> h_status;            // [0..1] read by alive_settle, [2c + 2..] snapshot behind ring chunk c's scan
+    DevBuf<unsigned long long> d_count;      // [0] alive entries, [1] export cursor, [2] occupied slots
     uint64_t window_errors = 0;              // sticky until reset: reported by kta_finalize
     uint64_t grows = 0, reruns = 0;
     uint64_t now = 0, occupied = 0;          // counted by the last alive_settle
@@ -113,17 +151,35 @@ struct AliveKeys {
 
 // read_committed isolation of the log entry points (kta_logtxn.cuh); allocated only on a read_committed handle
 struct TxnState {
-    TxnKey *d_keys = nullptr, *d_sorted = nullptr;   // classify's keys / sorted by (partition, producerId, batch)
-    uint8_t *d_kind = nullptr;                       // per batch: TxnKind of transactional data batches and markers
-    uint8_t *d_res = nullptr;                        // per sorted key: next marker within its resolve tile
-    int64_t cap = 0;
-    uint8_t *d_tile = nullptr; int64_t tile_cap = 0; // tile heads, then the carries behind each tile
-    void *d_sort_tmp = nullptr; size_t sort_tmp_bytes = 0;
-    uint32_t *d_word = nullptr;                      // [0] keys classified, [1] TxnErr bits
-    unsigned long long *d_stats = nullptr;           // this call: aborted batches, aborted records, undecided records
+    DevBuf<TxnKey> d_keys, d_sorted;                 // classify's keys / sorted by (partition, producerId, batch)
+    DevBuf<uint8_t> d_kind;                          // per batch: TxnKind of transactional data batches and markers
+    DevBuf<uint8_t> d_res;                           // per sorted key: next marker within its resolve tile
+    DevBuf<uint8_t> d_tile;                          // tile heads, then the carries behind each tile
+    DevBuf<uint8_t> d_sort_tmp;
+    DevBuf<uint32_t> d_word;                         // [0] keys classified, [1] TxnErr bits
+    DevBuf<unsigned long long> d_stats;              // this call: aborted batches, aborted records, undecided records
     std::vector<TxnRange> ranges;                    // registered aborted ranges, sorted and merged; mirrored in d_ranges
-    TxnRange *d_ranges = nullptr; int64_t ranges_cap = 0;
+    DevBuf<TxnRange> d_ranges;
     uint64_t totals[3] = {0, 0, 0};                  // the stats of every successful call since create / reset
+};
+
+// State of the log entry points (Kafka RecordBatch v2 segments → SoA → scan), reused from call to call
+struct LogScan {
+    DevBuf<uint8_t> bytes;                   // segments staged from the host (kta_push_log_segments_host)
+    DevBuf<uint64_t> off;                    // their batch offsets
+    DevBuf<int32_t> part;                    // and each batch's partition
+    DevBuf<LogBatchInfo> info;               // per batch, from the header pass
+    DevBuf<uint64_t> cnt;                    // records per batch, then their inclusive scan
+    DevBuf<uint32_t> err;                    // [0] error flags, [1] longest batch
+    DevBuf<int32_t> dec_part, dec_klen, dec_vlen;   // the decoded columns
+    DevBuf<int64_t> dec_ts;
+    DevBuf<uint64_t> dec_ksrc;               // per decoded record: where its key bytes lie in the segment buffer
+    DevBuf<uint8_t> dec_keys;                // the keys gathered in record order
+    DevBuf<uint8_t> unc;                     // uncompressed images of compressed batches
+    DevBuf<uint8_t> unc_lit;                 // zstd: Huffman-decoded literals, at the offsets of unc
+    DevBuf<uint64_t> unc_slot;               // per compressed batch: offset of its image in unc
+    bool read_committed = false;
+    TxnState txn;
 };
 
 struct kta_handle {
@@ -134,27 +190,14 @@ struct kta_handle {
     bool own_stream = true;
     bool need_hash = false;
     // device state
-    unsigned long long *d_sums = nullptr;
-    long long *d_minmax = nullptr;
-    uint32_t *d_hll = nullptr;
-    uint32_t *d_hll_floor = nullptr;         // hll floor + slice minima
+    DevBuf<unsigned long long> d_sums;
+    DevBuf<long long> d_minmax;
+    DevBuf<uint32_t> d_hll;
+    DevBuf<uint32_t> d_hll_floor;            // hll floor + slice minima
     AliveKeys alive;                         // count_alive_keys only
-    uint32_t *d_hash_out = nullptr;          // test hook
-    uint64_t *d_tb_scratch = nullptr;        // key_tile_base scratch for device batches
-    int64_t tb_scratch_tiles = 0;
-    // RecordBatch decoder scratch (kta_scan_log_segment_device / kta_push_log_segment_host)
-    uint8_t *d_log_bytes = nullptr; int64_t log_bytes_cap = 0;       // raw segment staged from the host
-    uint64_t *d_log_off = nullptr;                                    // batch offsets staged from the host
-    LogBatchInfo *d_log_info = nullptr; uint64_t *d_log_cnt = nullptr; int64_t log_batch_cap = 0;
-    int32_t *d_dec_part = nullptr, *d_dec_klen = nullptr, *d_dec_vlen = nullptr; int64_t *d_dec_ts = nullptr; int64_t dec_rec_cap = 0;
-    uint8_t *d_dec_keys = nullptr; int64_t dec_key_cap = 0;
-    uint64_t *d_dec_ksrc = nullptr;          // per decoded record: where its key bytes lie in the segment buffer
-    uint8_t *d_unc = nullptr; int64_t unc_cap = 0;   // uncompressed images of compressed batches
-    uint8_t *d_unc_lit = nullptr; int64_t unc_lit_cap = 0;   // zstd: Huffman-decoded literals, at the offsets of d_unc
-    uint64_t *d_unc_slot = nullptr; int64_t unc_slot_cap = 0;
-    uint32_t *d_log_err = nullptr;
-    bool read_committed = false;
-    TxnState txn;
+    uint32_t *d_hash_out = nullptr;          // test hook (the caller's buffer)
+    DevBuf<uint64_t> d_tb_scratch;           // key_tile_base scratch for device batches and decoded segments
+    LogScan log;
     size_t nsums = 0, nhll = 0;
     // landing ring
     Chunk chunks[NCHUNK];
@@ -196,6 +239,9 @@ static int set_device(const kta_handle *h) {
     CU(cudaSetDevice(h->device));
     return KTA_OK;
 }
+
+// key bytes travel to the device only when they are hashed (kta_push reads the copy in pc.hash)
+static bool keys_travel(const kta_handle *h) { return h->need_hash || h->d_hash_out; }
 
 static size_t scan_smem_bytes(bool hash, bool smem, int P, int threads, int keybuf, int stages, bool hdr) {
     return (smem ? smem_counter_bytes(P) : CTA_SCRATCH) + (size_t)(threads / 32) * warp_smem_bytes(hash, keybuf, stages, hdr);
@@ -260,26 +306,6 @@ static const ScanFn SCAN_KERNELS[2][2][3][2] = {
       {scan_kernel<MODE_EXACT, true, false, true>, nullptr}}},
 };
 
-template <typename T>
-static int alloc_elems(T *&ptr, int64_t n) {
-    CU(cudaMalloc(&ptr, (size_t)n * sizeof(T)));
-    return KTA_OK;
-}
-// (Re)allocates device buffers that share one capacity, in elements, when `need` exceeds it.
-template <typename... T>
-static int grow(cudaStream_t s, int64_t &cap, int64_t need, T *&...bufs) {
-    if (need <= cap) return KTA_OK;
-    CU(cudaStreamSynchronize(s));   // queued work may still read the old buffers
-    ((cudaFree(bufs), bufs = nullptr), ...);
-    cap = 0;
-    const int64_t n = need + need / 4 + 64;
-    int rc = KTA_OK;
-    ((rc = rc ? rc : alloc_elems(bufs, n)), ...);
-    if (rc) return rc;
-    cap = n;
-    return KTA_OK;
-}
-
 // ------------------------------------------------------------------------------------------------
 // alive-key table (-c): seq window (rebase), confirmation of pending stamps, growth (rehash + re-run), export / import
 // ------------------------------------------------------------------------------------------------
@@ -294,11 +320,10 @@ static int alive_create(kta_handle *h) {
     if (kib < 0 || kib > ALIVE_MAX_KIB) return fail(KTA_ERR_INVALID, "alive_table_kib %d out of range [0, %d]", (int)kib, ALIVE_MAX_KIB);
     AliveKeys &a = h->alive;
     a.pairs = (uint32_t)std::max<int64_t>((kib ? kib : ALIVE_DEFAULT_KIB) * 64, 16);   // 16 bytes per pair
-    CU(cudaMalloc(&a.d_table, (size_t)a.pairs * 16));
-    CU(cudaMalloc(&a.d_status, 12));
-    CU(cudaMalloc(&a.d_count, 24));
-    CU(cudaMalloc(&a.d_cache, ((size_t)4 << ALIVE_CACHE_SET_BITS)));
-    CU(cudaHostAlloc(&a.h_status, 8 * (NCHUNK + 1), cudaHostAllocDefault));
+    int rc;
+    if ((rc = a.d_table.alloc((int64_t)a.pairs * 2)) || (rc = a.d_status.alloc(3)) || (rc = a.d_count.alloc(3)) ||
+        (rc = a.d_cache.alloc((int64_t)1 << ALIVE_CACHE_SET_BITS)) || (rc = a.h_status.alloc(2 * (NCHUNK + 1))))
+        return rc;
     return KTA_OK;
 }
 
@@ -315,22 +340,18 @@ static int alive_reset(kta_handle *h) {
     return KTA_OK;
 }
 
-static void alive_destroy(AliveKeys &a) {
-    cudaFree(a.d_table); cudaFree(a.d_status); cudaFree(a.d_count); cudaFree(a.d_cache); cudaFreeHost(a.h_status);
-}
-
 static int alive_grow(kta_handle *h, uint32_t new_pairs) {
     AliveKeys &a = h->alive;
     cudaStream_t s = h->stream;
-    unsigned long long *nt = nullptr;
-    CU(cudaMalloc(&nt, (size_t)new_pairs * 16));
+    DevBuf<unsigned long long> nt;
+    int rc;
+    if ((rc = nt.alloc((int64_t)new_pairs * 2))) return rc;
     CU(cudaMemsetAsync(nt, 0xff, (size_t)new_pairs * 16, s));
     alive_rehash_kernel<<<h->sm_count * 8, THREADS, 0, s>>>(a.d_table, (size_t)a.pairs * 2, nt, new_pairs, a.d_status);
     h->launches++;
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(s));
-    cudaFree(a.d_table);
-    a.d_table = nt;
+    a.d_table = std::move(nt);   // nt frees the old table
     a.pairs = new_pairs;
     a.grows++;
     return KTA_OK;
@@ -546,32 +567,18 @@ static int state_reset_device(kta_handle *h) {
     return alive_reset(h);
 }
 
-static void free_chunk(Chunk &c) {
-    cudaFree(c.d_partition); cudaFree(c.d_klen); cudaFree(c.d_vlen); cudaFree(c.d_ts); cudaFree(c.d_seq);
-    cudaFree(c.d_keys); cudaFree(c.d_tile_base);
-    if (c.free_ev) cudaEventDestroy(c.free_ev);
-    cudaFreeHost(c.h_partition); cudaFreeHost(c.h_klen); cudaFreeHost(c.h_vlen); cudaFreeHost(c.h_ts);
-    cudaFreeHost(c.h_keys); cudaFreeHost(c.h_tile_base);
-    c = Chunk{};
-}
-
+// the handle's buffers free themselves; its streams and events are released here
 extern "C" int kta_destroy(kta_handle *h) {
     if (!h) return KTA_OK;
     cudaSetDevice(h->device);
     if (h->stream) cudaStreamSynchronize(h->stream);
-    for (auto &c : h->chunks) free_chunk(c);
-    alive_destroy(h->alive);
-    cudaFree(h->d_sums); cudaFree(h->d_minmax); cudaFree(h->d_hll); cudaFree(h->d_hll_floor); cudaFree(h->d_tb_scratch);
-    cudaFree(h->d_log_bytes); cudaFree(h->d_log_off); cudaFree(h->d_log_info); cudaFree(h->d_log_cnt);
-    cudaFree(h->d_dec_part); cudaFree(h->d_dec_klen); cudaFree(h->d_dec_vlen); cudaFree(h->d_dec_ts); cudaFree(h->d_dec_keys); cudaFree(h->d_dec_ksrc); cudaFree(h->d_unc); cudaFree(h->d_unc_lit); cudaFree(h->d_unc_slot);
-    cudaFree(h->d_log_err);
-    TxnState &t = h->txn;
-    cudaFree(t.d_keys); cudaFree(t.d_sorted); cudaFree(t.d_kind); cudaFree(t.d_res); cudaFree(t.d_tile); cudaFree(t.d_sort_tmp);
-    cudaFree(t.d_word); cudaFree(t.d_stats); cudaFree(t.d_ranges);
+    for (auto &c : h->chunks)
+        if (c.free_ev) cudaEventDestroy(c.free_ev);
     for (auto &e : h->ev_pool) { cudaEventDestroy(e.first); cudaEventDestroy(e.second); }
-    if (h->stream && h->own_stream) cudaStreamDestroy(h->stream);
-    cudaGetLastError();
+    cudaStream_t own = h->own_stream ? h->stream : nullptr;
     delete h;
+    if (own) cudaStreamDestroy(own);
+    cudaGetLastError();
     return KTA_OK;
 }
 
@@ -583,7 +590,7 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
         return fail(KTA_ERR_INVALID, "hll_precision %d not 0 or 4..18", cfg->hll_precision);
     if (cfg->isolation_level != KTA_READ_UNCOMMITTED && cfg->isolation_level != KTA_READ_COMMITTED)
         return fail(KTA_ERR_INVALID, "isolation_level %d is neither KTA_READ_UNCOMMITTED (0) nor KTA_READ_COMMITTED (1)", cfg->isolation_level);
-    h->read_committed = cfg->isolation_level == KTA_READ_COMMITTED;
+    h->log.read_committed = cfg->isolation_level == KTA_READ_COMMITTED;
     int ndev = 0;
     CU(cudaGetDeviceCount(&ndev));
     if (ndev < 1) return fail(KTA_ERR_CUDA, "no CUDA device (this library has no CPU fallback)");
@@ -598,7 +605,7 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
     h->sm_count = prop.multiProcessorCount;
     CU(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     h->need_hash = cfg->count_alive_keys == 1 || cfg->hll_precision != 0;
-    h->pc.hash = h->need_hash;   // kta_push reads it before its first (slow-path) call has bound the ring
+    h->pc.hash = keys_travel(h);   // kta_push reads it before its first (slow-path) call has bound the ring
     if (cfg->now_s == INT64_MIN) {
         const auto now = std::chrono::system_clock::now().time_since_epoch();
         const int64_t ns = std::chrono::duration_cast<std::chrono::nanoseconds>(now).count();
@@ -612,16 +619,12 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
     const int P = cfg->num_partitions;
     h->nsums = sums_words(P);
     h->nhll = cfg->hll_precision ? ((size_t)1 << cfg->hll_precision) : 0;
-    CU(cudaMalloc(&h->d_sums, h->nsums * 8));
-    CU(cudaMalloc(&h->d_minmax, 4 * 8));
-    CU(cudaMalloc(&h->d_hll_floor, (HLL_SLICES + 1) * 4 + 4));
-    if (h->nhll) CU(cudaMalloc(&h->d_hll, h->nhll * 4));
     int rc;
+    if ((rc = h->d_sums.alloc((int64_t)h->nsums)) || (rc = h->d_minmax.alloc(4)) || (rc = h->d_hll_floor.alloc(HLL_SLICES + 2)))
+        return rc;
+    if (h->nhll && (rc = h->d_hll.alloc((int64_t)h->nhll))) return rc;
     if (cfg->count_alive_keys == 1 && (rc = alive_create(h))) return rc;
-    if (h->read_committed) {
-        CU(cudaMalloc(&h->txn.d_word, 8));
-        CU(cudaMalloc(&h->txn.d_stats, 24));
-    }
+    if (h->log.read_committed && ((rc = h->log.txn.d_word.alloc(2)) || (rc = h->log.txn.d_stats.alloc(3)))) return rc;
     h->smem_optin = prop.sharedMemPerBlockOptin;
     if (cfg->shard_world > 1) {
         if (cfg->shard_rank < 0 || cfg->shard_rank >= cfg->shard_world || cfg->shard_world > P)
@@ -636,6 +639,8 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
         for (const auto &by_capture : by_mode)
             for (const ScanFn f : by_capture)
                 if (f) CU(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+    // the record decoder stages a batch of up to 48 KiB per warp (log_decode); attributes belong to the device
+    CU(cudaFuncSetAttribute(log_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
     if ((rc = state_reset_device(h))) return rc;
     CU(cudaStreamSynchronize(h->stream));
     return KTA_OK;
@@ -761,14 +766,32 @@ static int collect_timing(kta_handle *h) {
     return KTA_OK;
 }
 
-static int derive_tile_base(kta_handle *h, const int32_t *d_klen, int64_t n, uint64_t *d_tile_base) {
+// the key_tile_base column of n records' key lengths, into h->d_tb_scratch ([ntiles] = the key bytes in all)
+static int derive_tile_base(kta_handle *h, const int32_t *d_klen, int64_t n) {
     const int64_t ntiles = (n + TILE - 1) / TILE;
+    int rc;
+    if ((rc = h->d_tb_scratch.grow(h->stream, ntiles + 1))) return rc;
     const int grid = (int)std::min<int64_t>((ntiles + 7) / 8, (int64_t)h->sm_count * 8);
-    tile_key_bytes_kernel<<<grid, 256, 0, h->stream>>>(d_klen, n, ntiles, d_tile_base);
+    tile_key_bytes_kernel<<<grid, 256, 0, h->stream>>>(d_klen, n, ntiles, h->d_tb_scratch);
     CU(cudaGetLastError());
-    tile_base_scan_kernel<<<1, 1024, 0, h->stream>>>(d_tile_base, ntiles);
+    tile_base_scan_kernel<<<1, 1024, 0, h->stream>>>(h->d_tb_scratch, ntiles);
     CU(cudaGetLastError());
     h->launches += 2;
+    return KTA_OK;
+}
+
+// a scan's params over the columns of n records from seq_base on (ScanParams' leading fields, in their order; the rest zero)
+static ScanParams scan_params(int64_t n, uint64_t seq_base, const int32_t *partition, const int64_t *ts_ms, const int32_t *key_len,
+                              const int32_t *value_len, const uint8_t *key_bytes, const uint64_t *key_tile_base, const uint64_t *seq) {
+    return ScanParams{n, seq_base, partition, ts_ms, key_len, value_len, key_bytes, key_tile_base, seq};
+}
+
+// the checks a batch passes at both batch entry points (an empty batch passes: there is nothing to scan)
+static int check_batch(const kta_handle *h, const kta_batch *b) {
+    if (!h || !b) return fail(KTA_ERR_INVALID, "null argument");
+    if (b->n < 0) return fail(KTA_ERR_INVALID, "negative n");
+    if (b->n > 0 && (!b->partition || !b->ts_ms || !b->key_len || !b->value_len))
+        return fail(KTA_ERR_INVALID, "partition/ts_ms/key_len/value_len columns are required");
     return KTA_OK;
 }
 
@@ -788,36 +811,27 @@ static int resolve_seq_base(kta_handle *h, const kta_batch *b, uint64_t *out) {
     return KTA_OK;
 }
 
-extern "C" int kta_scan_batch_device(kta_handle *h, const kta_batch *b) {
-    if (!h || !b) return fail(KTA_ERR_INVALID, "null argument");
-    if (b->n < 0) return fail(KTA_ERR_INVALID, "negative n");
-    if (b->n == 0) return KTA_OK;
-    if (!b->partition || !b->ts_ms || !b->key_len || !b->value_len)
-        return fail(KTA_ERR_INVALID, "partition/ts_ms/key_len/value_len columns are required");
-    int rc;
-    if ((rc = set_device(h))) return rc;
-    if ((rc = ring_flush(h))) return rc;   // records pushed earlier come first in seq order
+// scans a checked, non-empty batch of device columns behind the records the handle has already scanned
+static int scan_device_batch(kta_handle *h, const kta_batch *b) {
     uint64_t seq_base = 0;
+    int rc;
     if ((rc = resolve_seq_base(h, b, &seq_base))) return rc;
-    ScanParams prm{};
-    prm.n = b->n;
-    prm.seq_base = seq_base;
-    prm.partition = b->partition;
-    prm.ts_ms = b->ts_ms;
-    prm.key_len = b->key_len;
-    prm.value_len = b->value_len;
-    prm.key_bytes = b->key_bytes;
-    prm.seq = b->seq;
-    prm.key_tile_base = b->key_tile_base;
-    if ((h->need_hash || h->d_hash_out) && !prm.key_tile_base) {
-        const int64_t ntiles = (b->n + TILE - 1) / TILE;
-        if ((rc = grow(h->stream, h->tb_scratch_tiles, ntiles + 1, h->d_tb_scratch))) return rc;
-        if ((rc = derive_tile_base(h, b->key_len, b->n, h->d_tb_scratch))) return rc;
+    ScanParams prm = scan_params(b->n, seq_base, b->partition, b->ts_ms, b->key_len, b->value_len, b->key_bytes, b->key_tile_base, b->seq);
+    if (keys_travel(h) && !prm.key_tile_base) {
+        if ((rc = derive_tile_base(h, b->key_len, b->n))) return rc;
         prm.key_tile_base = h->d_tb_scratch;
     }
     if ((rc = launch_scan(h, prm, b->key_bytes_len, b->key_bytes_len))) return rc;
     h->next_seq = std::max<uint64_t>(h->next_seq, seq_base + (uint64_t)b->n);
     return KTA_OK;
+}
+
+extern "C" int kta_scan_batch_device(kta_handle *h, const kta_batch *b) {
+    int rc;
+    if ((rc = check_batch(h, b)) || b->n == 0) return rc;
+    if ((rc = set_device(h))) return rc;
+    if ((rc = ring_flush(h))) return rc;   // records pushed earlier come first in seq order
+    return scan_device_batch(h, b);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -828,49 +842,171 @@ extern "C" int kta_scan_batch_device(kta_handle *h, const kta_batch *b) {
 // scanned.  Classify always; sort, resolve, carry and apply only when the call has transactional batches.  One host round
 // trip (the classify count).  *ran: the apply pass was launched, so its error word and counters are to be read back.
 static int txn_passes(kta_handle *h, int32_t partition, const uint8_t *dev_bytes, int64_t nbatches, bool *ran) {
-    TxnState &t = h->txn;
+    LogScan &L = h->log;
+    TxnState &t = L.txn;
     cudaStream_t s = h->stream;
     *ran = false;
     if (nbatches > (int64_t)UINT32_MAX) return fail(KTA_ERR_INVALID, "%lld batches in one read_committed call: split them", (long long)nbatches);
     int rc;
-    if ((rc = grow(s, t.cap, nbatches, t.d_keys, t.d_sorted, t.d_kind, t.d_res))) return rc;
+    if ((rc = t.d_keys.grow(s, nbatches)) || (rc = t.d_sorted.grow(s, nbatches)) || (rc = t.d_kind.grow(s, nbatches)) ||
+        (rc = t.d_res.grow(s, nbatches)))
+        return rc;
     CU(cudaMemsetAsync(t.d_word, 0, 8, s));
-    txn_classify_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, h->d_log_info, nbatches, t.d_keys, t.d_kind, t.d_word);
+    txn_classify_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, L.info, nbatches, t.d_keys, t.d_kind, t.d_word);
     CU(cudaGetLastError());
     h->launches++;
     uint32_t w[3] = {0, 0, 0};   // keys, TxnErr bits, header flags
     CU(cudaMemcpyAsync(w, t.d_word, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(w + 2, h->d_log_err, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(w + 2, L.err, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
-    if (w[2] & (LOGB_BAD | LOGB_COMPRESSED)) return KTA_OK;   // the call is refused for its headers (scan_log_batches says so)
+    if (w[2] & (LOGB_BAD | LOGB_COMPRESSED)) return KTA_OK;   // the call is refused for its headers (log_headers says so)
     if (w[1] & TXN_ERR_MARKER)
         return fail(KTA_ERR_INVALID, "unreadable transaction marker in partition %d (control batch compressed, without a record, "
                     "truncated, or with a key that is not version 0 | type)", partition);
     const int64_t m = w[0];
     if (m == 0) return KTA_OK;
     size_t tmp = 0;
-    CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp, t.d_keys, t.d_sorted, m, TxnKeyDecomposer{}, s));
-    if (tmp > t.sort_tmp_bytes) {
-        CU(cudaStreamSynchronize(s));
-        cudaFree(t.d_sort_tmp);
-        t.d_sort_tmp = nullptr;
-        t.sort_tmp_bytes = 0;
-        CU(cudaMalloc(&t.d_sort_tmp, tmp));
-        t.sort_tmp_bytes = tmp;
-    }
-    tmp = t.sort_tmp_bytes;
-    CU(cub::DeviceRadixSort::SortKeys(t.d_sort_tmp, tmp, t.d_keys, t.d_sorted, m, TxnKeyDecomposer{}, s));
+    CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp, t.d_keys.get(), t.d_sorted.get(), m, TxnKeyDecomposer{}, s));
+    if ((rc = t.d_sort_tmp.grow(s, (int64_t)tmp))) return rc;
+    tmp = (size_t)t.d_sort_tmp.cap;
+    CU(cub::DeviceRadixSort::SortKeys(t.d_sort_tmp.get(), tmp, t.d_keys.get(), t.d_sorted.get(), m, TxnKeyDecomposer{}, s));
     const int64_t tiles = (m + TXN_TILE - 1) / TXN_TILE;
-    if ((rc = grow(s, t.tile_cap, 2 * tiles, t.d_tile))) return rc;
+    if ((rc = t.d_tile.grow(s, 2 * tiles))) return rc;
     CU(cudaMemsetAsync(t.d_stats, 0, 24, s));
-    txn_resolve_kernel<<<(unsigned)tiles, TXN_TILE, 0, s>>>(t.d_sorted, m, t.d_kind, h->d_log_info, t.d_res, t.d_tile, t.d_word);
+    txn_resolve_kernel<<<(unsigned)tiles, TXN_TILE, 0, s>>>(t.d_sorted, m, t.d_kind, L.info, t.d_res, t.d_tile, t.d_word);
     txn_carry_kernel<<<1, 1024, 0, s>>>(t.d_tile, tiles, t.d_tile + tiles);
     txn_apply_kernel<<<(int)std::min<int64_t>((m + 255) / 256, (int64_t)h->sm_count * 16), 256, 0, s>>>(
-        t.d_sorted, m, t.d_kind, t.d_res, t.d_tile + tiles, t.d_ranges, (int64_t)t.ranges.size(), h->d_log_info, h->d_log_cnt, t.d_word,
+        t.d_sorted, m, t.d_kind, t.d_res, t.d_tile + tiles, t.d_ranges, (int64_t)t.ranges.size(), L.info, L.cnt, t.d_word,
         t.d_stats);
     CU(cudaGetLastError());
     h->launches += 4;   // (the sort counted as one)
     *ran = true;
+    return KTA_OK;
+}
+
+// What the header pass (and read_committed's passes) found in one call's batches
+struct LogHeaders {
+    uint64_t nrec = 0;                               // records in all
+    uint32_t err[2] = {0, 0};                        // the header pass's error word: [0] LOGB_* flags, [1] longest batch
+    unsigned long long txn_stats[3] = {0, 0, 0};     // this call's aborted batches, aborted records, undecided records
+};
+
+// The header pass, read_committed's passes and the scan of the record counts.  One host round trip (two under
+// read_committed); refuses the call for its headers and for the order of a producer's batches.
+static int log_headers(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes, int64_t len,
+                       const uint64_t *dev_batch_off, int64_t nbatches, LogHeaders &out) {
+    LogScan &L = h->log;
+    cudaStream_t s = h->stream;
+    int rc;
+    if ((rc = L.info.grow(s, nbatches + 1)) || (rc = L.cnt.grow(s, nbatches + 1))) return rc;
+    if (!L.err && (rc = L.err.alloc(2))) return rc;
+    CU(cudaMemsetAsync(L.err, 0, 8, s));
+    log_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, partition,
+                                                                            dev_batch_partition, L.info, L.cnt, L.err);
+    CU(cudaGetLastError());
+    bool txn = false;   // read_committed and the call has transactional batches
+    if (L.read_committed && (rc = txn_passes(h, partition, dev_bytes, nbatches, &txn))) return rc;
+    tile_base_scan_kernel<<<1, 1024, 0, s>>>(L.cnt, nbatches);   // inclusive scan of [1..nbatches] in place
+    CU(cudaGetLastError());
+    h->launches += 2;
+    uint32_t txn_word[2] = {0, 0};
+    CU(cudaMemcpyAsync(&out.nrec, L.cnt + nbatches, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(out.err, L.err, 8, cudaMemcpyDeviceToHost, s));
+    if (txn) {
+        CU(cudaMemcpyAsync(txn_word, L.txn.d_word, 8, cudaMemcpyDeviceToHost, s));
+        CU(cudaMemcpyAsync(out.txn_stats, L.txn.d_stats, 24, cudaMemcpyDeviceToHost, s));
+    }
+    CU(cudaStreamSynchronize(s));
+    if (out.err[0] & LOGB_COMPRESSED)
+        return fail(KTA_ERR_INVALID, "unknown compression codec (attributes bits 0-2 = 5..7) in partition %d", partition);
+    if (out.err[0] & LOGB_BAD) return fail(KTA_ERR_INVALID, "malformed record batch header in partition %d", partition);
+    if (txn_word[1] & TXN_ERR_ORDER)
+        return fail(KTA_ERR_INVALID, "the batches of one producer in partition %d are not in increasing baseOffset order", partition);
+    return KTA_OK;
+}
+
+// Compressed batches (codecs: the LOGB_CODECS bits the header pass saw): size pass, scratch allocation, decompression.
+// Afterwards they are ordinary batches that happen to lie in the scratch buffer.  One host round trip.
+static int log_decompress(kta_handle *h, int32_t partition, const uint8_t *dev_bytes, int64_t nbatches, uint32_t codecs) {
+    LogScan &L = h->log;
+    cudaStream_t s = h->stream;
+    int rc;
+    if ((rc = L.unc_slot.grow(s, nbatches + 2))) return rc;
+    CU(cudaMemsetAsync(L.err, 0, 4, s));
+    const bool zstd = (codecs & LOGB_ZSTD) != 0;
+    CU(log_launch_size_pass(dev_bytes, L.info, nbatches, L.unc_slot, L.err, zstd, h->sm_count, s));
+    h->launches += zstd ? 3 : 2;
+    uint64_t unc_total = 0;
+    uint32_t bad = 0;
+    CU(cudaMemcpyAsync(&unc_total, L.unc_slot + nbatches, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&bad, L.err, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (bad) return fail(KTA_ERR_INVALID, "malformed compressed record batch in partition %d", partition);
+    if ((rc = L.unc.grow(s, (int64_t)unc_total + 64))) return rc;
+    // zstd's literal buffer has the size of the scratch buffer (a block's literals go at its output's offset); it is
+    // only allocated once zstd batches are seen
+    if (zstd && (rc = L.unc_lit.grow(s, (int64_t)unc_total + 64))) return rc;
+    CU(log_launch_copy_pass(dev_bytes, L.info, nbatches, L.unc_slot, L.unc, L.unc_lit, L.err, codecs, h->sm_count, s));
+    h->launches += ((codecs & ~(uint32_t)LOGB_ZSTD) ? 1 : 0) + (zstd ? 1 : 0);
+    return KTA_OK;
+}
+
+// The records of every batch into the decoded columns, which b then names; with keys, where each record's key bytes lie.
+// One warp per batch; the batch is staged in shared memory when the longest one fits a stage of <= 48 KiB.
+static int log_decode(kta_handle *h, const uint8_t *dev_bytes, int64_t readable, int64_t nbatches, uint64_t nrec,
+                      uint32_t longest, bool keys, kta_batch &b) {
+    LogScan &L = h->log;
+    cudaStream_t s = h->stream;
+    if ((int64_t)nrec >= ((int64_t)1 << 31) - 2) return fail(KTA_ERR_INVALID, "%llu records in one call: split the segments", (unsigned long long)nrec);
+    int rc;
+    if ((rc = L.dec_part.grow(s, (int64_t)nrec)) || (rc = L.dec_klen.grow(s, (int64_t)nrec)) || (rc = L.dec_vlen.grow(s, (int64_t)nrec)) ||
+        (rc = L.dec_ts.grow(s, (int64_t)nrec)) || (rc = L.dec_ksrc.grow(s, (int64_t)nrec)))
+        return rc;
+    const uint32_t stage = (uint32_t)(((size_t)longest + 16 + 1023) / 1024 * 1024);
+    const bool staged = stage <= 48u * 1024u;
+    const size_t dsm = (size_t)(LOG_DECODE_THREADS / 32) * (LOG_WARP_HEADER + (staged ? stage : 0u));
+    const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(16, h->smem_optin / std::max<size_t>(dsm, 1)));
+    const int dgrid = (int)std::min<int64_t>((nbatches + 3) / 4, (int64_t)h->sm_count * per_sm);
+    const auto decode = staged ? log_decode_kernel<true> : log_decode_kernel<false>;
+    decode<<<dgrid, LOG_DECODE_THREADS, dsm, s>>>(dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, nullptr, L.dec_ts,
+                                                  L.dec_klen, L.dec_vlen, keys ? L.dec_ksrc.get() : nullptr, staged ? stage : 0u, L.err);
+    CU(cudaGetLastError());
+    h->launches++;
+    b = kta_batch{};
+    b.n = (int64_t)nrec;
+    b.seq_base = KTA_SEQ_AUTO;
+    b.partition = L.dec_part;
+    b.ts_ms = L.dec_ts;
+    b.key_len = L.dec_klen;
+    b.value_len = L.dec_vlen;
+    return KTA_OK;
+}
+
+// Reads the decode's error word back (one host round trip).  With keys, first packs them in record order into b's key
+// columns: tile bases from the key_len column, then one gather pass (no second walk of the log).
+static int log_gather_keys(kta_handle *h, int32_t partition, const uint8_t *dev_bytes, bool keys, kta_batch &b) {
+    LogScan &L = h->log;
+    cudaStream_t s = h->stream;
+    int rc;
+    uint32_t err[2] = {0, 0};
+    uint64_t nkey = 0;
+    const int64_t ntiles = (b.n + TILE - 1) / TILE;
+    if (keys) {
+        if ((rc = derive_tile_base(h, b.key_len, b.n))) return rc;
+        CU(cudaMemcpyAsync(&nkey, h->d_tb_scratch + ntiles, 8, cudaMemcpyDeviceToHost, s));
+    }
+    CU(cudaMemcpyAsync(err, L.err, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (err[0]) return fail(KTA_ERR_INVALID, "malformed record inside a batch of partition %d", partition);
+    if (!keys) return KTA_OK;
+    if ((rc = L.dec_keys.grow(s, (int64_t)nkey + 64))) return rc;
+    log_gather_keys_kernel<<<(int)std::min<int64_t>((ntiles + 7) / 8, (int64_t)h->sm_count * 8), 256, 0, s>>>(
+        dev_bytes, L.dec_ksrc, L.dec_klen, b.n, h->d_tb_scratch, L.dec_keys);
+    CU(cudaGetLastError());
+    h->launches++;
+    b.key_bytes = L.dec_keys;
+    b.key_bytes_len = (int64_t)nkey;
+    b.key_tile_base = h->d_tb_scratch;
     return KTA_OK;
 }
 
@@ -884,120 +1020,20 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;   // keep seq order with records pushed earlier
     if ((rc = alive_settle_if_any(h))) return rc;   // the decode scratch of an earlier call is about to be reused
-    cudaStream_t s = h->stream;
-    if ((rc = grow(s, h->log_batch_cap, nbatches + 1, h->d_log_info, h->d_log_cnt))) return rc;
-    if (!h->d_log_err) CU(cudaMalloc(&h->d_log_err, 8));   // [0] error flags, [1] longest batch
-    CU(cudaMemsetAsync(h->d_log_err, 0, 8, s));
-    log_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, h->d_log_info,
-                                            h->d_log_cnt, h->d_log_err);
-    CU(cudaGetLastError());
-    bool txn = false;   // read_committed and the call has transactional batches
-    if (h->read_committed && (rc = txn_passes(h, partition, dev_bytes, nbatches, &txn))) return rc;
-    tile_base_scan_kernel<<<1, 1024, 0, s>>>(h->d_log_cnt, nbatches);   // inclusive scan of [1..nbatches] in place
-    CU(cudaGetLastError());
-    h->launches += 2;
-    uint64_t nrec = 0;
-    uint32_t err[2] = {0, 0};
-    uint32_t txn_word[2] = {0, 0};
-    unsigned long long txn_stats[3] = {0, 0, 0};
-    CU(cudaMemcpyAsync(&nrec, h->d_log_cnt + nbatches, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(err, h->d_log_err, 8, cudaMemcpyDeviceToHost, s));
-    if (txn) {
-        CU(cudaMemcpyAsync(txn_word, h->txn.d_word, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaMemcpyAsync(txn_stats, h->txn.d_stats, 24, cudaMemcpyDeviceToHost, s));
+    LogHeaders hd;
+    if ((rc = log_headers(h, partition, dev_batch_partition, dev_bytes, len, dev_batch_off, nbatches, hd))) return rc;
+    if (hd.nrec > 0) {
+        const uint32_t codecs = hd.err[0] & LOGB_CODECS;
+        if (codecs && (rc = log_decompress(h, partition, dev_bytes, nbatches, codecs))) return rc;
+        const bool keys = keys_travel(h);
+        kta_batch b;
+        if ((rc = log_decode(h, dev_bytes, readable, nbatches, hd.nrec, hd.err[1], keys, b))) return rc;
+        if ((rc = log_gather_keys(h, partition, dev_bytes, keys, b))) return rc;
+        if ((rc = scan_device_batch(h, &b))) return rc;
     }
-    CU(cudaStreamSynchronize(s));
-    if (err[0] & LOGB_COMPRESSED)
-        return fail(KTA_ERR_INVALID, "unknown compression codec (attributes bits 0-2 = 5..7) in partition %d", partition);
-    if (err[0] & LOGB_BAD) return fail(KTA_ERR_INVALID, "malformed record batch header in partition %d", partition);
-    if (txn_word[1] & TXN_ERR_ORDER)
-        return fail(KTA_ERR_INVALID, "the batches of one producer in partition %d are not in increasing baseOffset order", partition);
-    auto count_txn = [&]() {   // the call succeeded: its transaction counters join the handle's totals
-        for (int i = 0; i < 3; i++) h->txn.totals[i] += txn_stats[i];
-    };
-    if (nrec == 0) {
-        count_txn();
-        return KTA_OK;
-    }
-    if (err[0] & LOGB_CODECS) {
-        // compressed batches: size pass, scratch allocation, decompression; afterwards they are ordinary batches that
-        // happen to lie in the scratch buffer
-        if ((rc = grow(s, h->unc_slot_cap, nbatches + 2, h->d_unc_slot))) return rc;
-        CU(cudaMemsetAsync(h->d_log_err, 0, 4, s));
-        const uint32_t codecs = err[0] & LOGB_CODECS;   // (err is reused for the size pass's flags below)
-        const bool zstd = (codecs & LOGB_ZSTD) != 0;
-        CU(log_launch_size_pass(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_log_err, zstd, h->sm_count, s));
-        h->launches += zstd ? 3 : 2;
-        uint64_t unc_total = 0;
-        CU(cudaMemcpyAsync(&unc_total, h->d_unc_slot + nbatches, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaMemcpyAsync(err, h->d_log_err, 4, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
-        if (err[0]) return fail(KTA_ERR_INVALID, "malformed compressed record batch in partition %d", partition);
-        if ((rc = grow(s, h->unc_cap, (int64_t)unc_total + 64, h->d_unc))) return rc;
-        // zstd's literal buffer has the size of the scratch buffer (a block's literals go at its output's offset); it is
-        // only allocated once zstd batches are seen
-        if (zstd && (rc = grow(s, h->unc_lit_cap, (int64_t)unc_total + 64, h->d_unc_lit))) return rc;
-        CU(log_launch_copy_pass(dev_bytes, h->d_log_info, nbatches, h->d_unc_slot, h->d_unc, h->d_unc_lit, h->d_log_err, codecs, h->sm_count, s));
-        h->launches += ((codecs & ~(uint32_t)LOGB_ZSTD) ? 1 : 0) + (zstd ? 1 : 0);
-    }
-    if ((int64_t)nrec >= ((int64_t)1 << 31) - 2) return fail(KTA_ERR_INVALID, "%llu records in one call: split the segments", (unsigned long long)nrec);
-    const bool hash = h->need_hash || h->d_hash_out;
-    if ((rc = grow(s, h->dec_rec_cap, (int64_t)nrec, h->d_dec_part, h->d_dec_klen, h->d_dec_vlen, h->d_dec_ts, h->d_dec_ksrc)))
-        return rc;
-    // one warp per batch; the batch is staged in shared memory when the longest one fits a stage of <= 48 KiB
-    const uint32_t maxlen = err[1];
-    const uint32_t stage = (uint32_t)(((size_t)maxlen + 16 + 1023) / 1024 * 1024);
-    const bool staged = stage <= 48u * 1024u;
-    const size_t dsm = (size_t)(LOG_DECODE_THREADS / 32) * (LOG_WARP_HEADER + (staged ? stage : 0u));
-    static bool attr_set = false;
-    if (!attr_set) {
-        CU(cudaFuncSetAttribute(log_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
-        attr_set = true;
-    }
-    const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(16, h->smem_optin / std::max<size_t>(dsm, 1)));
-    const int dgrid = (int)std::min<int64_t>((nbatches + 3) / 4, (int64_t)h->sm_count * per_sm);
-    uint64_t *ksrc = hash ? h->d_dec_ksrc : nullptr;
-    if (staged)
-        log_decode_kernel<true><<<dgrid, LOG_DECODE_THREADS, dsm, s>>>(dev_bytes, (uint64_t)readable, h->d_log_info, nbatches, h->d_log_cnt, h->d_dec_part,
-                                                                       nullptr, h->d_dec_ts, h->d_dec_klen, h->d_dec_vlen, ksrc, stage, h->d_log_err);
-    else
-        log_decode_kernel<false><<<dgrid, LOG_DECODE_THREADS, dsm, s>>>(dev_bytes, (uint64_t)readable, h->d_log_info, nbatches, h->d_log_cnt, h->d_dec_part,
-                                                                        nullptr, h->d_dec_ts, h->d_dec_klen, h->d_dec_vlen, ksrc, 0u, h->d_log_err);
-    CU(cudaGetLastError());
-    h->launches++;
-    kta_batch b{};
-    b.n = (int64_t)nrec;
-    b.seq_base = KTA_SEQ_AUTO;
-    b.partition = h->d_dec_part;
-    b.ts_ms = h->d_dec_ts;
-    b.key_len = h->d_dec_klen;
-    b.value_len = h->d_dec_vlen;
-    if (hash) {
-        // pack the keys in record order: tile bases from the key_len column, then one gather pass (no second walk of the log)
-        const int64_t ntiles = ((int64_t)nrec + TILE - 1) / TILE;
-        if ((rc = grow(s, h->tb_scratch_tiles, ntiles + 1, h->d_tb_scratch))) return rc;
-        if ((rc = derive_tile_base(h, h->d_dec_klen, (int64_t)nrec, h->d_tb_scratch))) return rc;
-        uint64_t nkey = 0;
-        CU(cudaMemcpyAsync(&nkey, h->d_tb_scratch + ntiles, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaMemcpyAsync(err, h->d_log_err, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
-        if (err[0]) return fail(KTA_ERR_INVALID, "malformed record inside a batch of partition %d", partition);
-        if ((rc = grow(s, h->dec_key_cap, (int64_t)nkey + 64, h->d_dec_keys))) return rc;
-        log_gather_keys_kernel<<<(int)std::min<int64_t>((ntiles + 7) / 8, (int64_t)h->sm_count * 8), 256, 0, s>>>(
-            dev_bytes, h->d_dec_ksrc, h->d_dec_klen, (int64_t)nrec, h->d_tb_scratch, h->d_dec_keys);
-        CU(cudaGetLastError());
-        h->launches++;
-        b.key_bytes = h->d_dec_keys;
-        b.key_bytes_len = (int64_t)nkey;
-        b.key_tile_base = h->d_tb_scratch;
-    } else {
-        CU(cudaMemcpyAsync(err, h->d_log_err, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
-        if (err[0]) return fail(KTA_ERR_INVALID, "malformed record inside a batch of partition %d", partition);
-    }
-    if ((rc = kta_scan_batch_device(h, &b))) return rc;
-    count_txn();
-    if (records_out) *records_out = (int64_t)nrec;
+    // the call succeeded: its transaction counters join the handle's totals
+    for (int i = 0; i < 3; i++) h->log.txn.totals[i] += hd.txn_stats[i];
+    if (records_out) *records_out = (int64_t)hd.nrec;
     return KTA_OK;
 }
 
@@ -1042,19 +1078,16 @@ extern "C" int kta_push_log_segments_host(kta_handle *h, int32_t nsegs, const in
     int rc;
     if ((rc = set_device(h))) return rc;
     cudaStream_t s = h->stream;
-    if ((rc = grow(s, h->log_bytes_cap, total + 64, h->d_log_bytes))) return rc;
-    CU(cudaStreamSynchronize(s));
-    cudaFree(h->d_log_off);
-    h->d_log_off = nullptr;
-    CU(cudaMalloc(&h->d_log_off, offs.size() * 12));
-    int32_t *d_parts = reinterpret_cast<int32_t *>(h->d_log_off + offs.size());
+    LogScan &L = h->log;
+    const int64_t nb = (int64_t)offs.size();
+    if ((rc = L.bytes.grow(s, total + 64)) || (rc = L.off.grow(s, nb)) || (rc = L.part.grow(s, nb))) return rc;
     for (int32_t sgi = 0; sgi < nsegs; sgi++)
         if (used[(size_t)sgi])
-            CU(cudaMemcpyAsync(h->d_log_bytes + base[(size_t)sgi], bytes[sgi], (size_t)used[(size_t)sgi], cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(h->d_log_off, offs.data(), offs.size() * 8, cudaMemcpyHostToDevice, s));
-    CU(cudaMemcpyAsync(d_parts, parts.data(), parts.size() * 4, cudaMemcpyHostToDevice, s));
+            CU(cudaMemcpyAsync(L.bytes + base[(size_t)sgi], bytes[sgi], (size_t)used[(size_t)sgi], cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(L.off, offs.data(), offs.size() * 8, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(L.part, parts.data(), parts.size() * 4, cudaMemcpyHostToDevice, s));
     // the staging buffer has 64 bytes of slack behind `total`: 16-byte-granular bulk copies may run into it
-    if ((rc = scan_log_batches(h, 0, d_parts, h->d_log_bytes, total, total + 48, h->d_log_off, (int64_t)offs.size(), records_out))) return rc;
+    if ((rc = scan_log_batches(h, 0, L.part, L.bytes, total, total + 48, L.off, nb, records_out))) return rc;
     CU(cudaStreamSynchronize(s));   // the caller may reuse its buffers, and the scratch may be reused by the next call
     return collect_timing(h);
 }
@@ -1068,7 +1101,7 @@ extern "C" int kta_push_log_segment_host(kta_handle *h, int32_t partition, const
 // lastStableOffset i64.  All of it is checked before any range is added.
 extern "C" int kta_log_add_txn_index_host(kta_handle *h, int32_t partition, const uint8_t *bytes, int64_t len) {
     if (!h || len < 0 || (len && !bytes)) return fail(KTA_ERR_INVALID, "bad argument");
-    if (!h->read_committed) return fail(KTA_ERR_INVALID, "transaction index on a read_uncommitted handle");
+    if (!h->log.read_committed) return fail(KTA_ERR_INVALID, "transaction index on a read_uncommitted handle");
     if (partition < 0 || partition >= h->cfg.num_partitions)
         return fail(KTA_ERR_INVALID, "partition %d outside [0, %d)", partition, h->cfg.num_partitions);
     constexpr int64_t ENTRY = 34;
@@ -1087,7 +1120,8 @@ extern "C" int kta_log_add_txn_index_host(kta_handle *h, int32_t partition, cons
     if (add.empty()) return KTA_OK;
     // sorted by (partition, producerId, firstOffset), overlapping ranges of one producer merged: the apply pass's binary
     // search then has one candidate per offset
-    std::vector<TxnRange> &v = h->txn.ranges;
+    TxnState &t = h->log.txn;
+    std::vector<TxnRange> &v = t.ranges;
     v.insert(v.end(), add.begin(), add.end());
     std::sort(v.begin(), v.end(), [](const TxnRange &a, const TxnRange &b) {
         return a.part != b.part ? a.part < b.part : a.pid != b.pid ? a.pid < b.pid : a.first < b.first;
@@ -1101,19 +1135,19 @@ extern "C" int kta_log_add_txn_index_host(kta_handle *h, int32_t partition, cons
     v.resize(out);
     int rc;
     if ((rc = set_device(h))) return rc;
-    if ((rc = grow(h->stream, h->txn.ranges_cap, (int64_t)v.size(), h->txn.d_ranges))) return rc;
+    if ((rc = t.d_ranges.grow(h->stream, (int64_t)v.size()))) return rc;
     CU(cudaStreamSynchronize(h->stream));   // no queued pass reads the ranges while they are replaced
-    CU(cudaMemcpyAsync(h->txn.d_ranges, v.data(), v.size() * sizeof(TxnRange), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(t.d_ranges, v.data(), v.size() * sizeof(TxnRange), cudaMemcpyHostToDevice, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     return KTA_OK;
 }
 
 extern "C" int kta_log_txn_stats(kta_handle *h, uint64_t *aborted_batches, uint64_t *aborted_records, uint64_t *undecided_records) {
     if (!h) return fail(KTA_ERR_INVALID, "null handle");
-    if (!h->read_committed) return fail(KTA_ERR_NOT_ENABLED, "the handle is read_uncommitted");
-    if (aborted_batches) *aborted_batches = h->txn.totals[0];
-    if (aborted_records) *aborted_records = h->txn.totals[1];
-    if (undecided_records) *undecided_records = h->txn.totals[2];
+    if (!h->log.read_committed) return fail(KTA_ERR_NOT_ENABLED, "the handle is read_uncommitted");
+    if (aborted_batches) *aborted_batches = h->log.txn.totals[0];
+    if (aborted_records) *aborted_records = h->log.txn.totals[1];
+    if (undecided_records) *undecided_records = h->log.txn.totals[2];
     return KTA_OK;
 }
 
@@ -1123,15 +1157,12 @@ extern "C" int kta_log_txn_stats(kta_handle *h, uint64_t *aborted_batches, uint6
 static int ring_dev_init(kta_handle *h) {
     if (h->ring_dev_ready) return KTA_OK;
     const int64_t R = h->ring_records, KB = h->ring_key_bytes;
+    int rc;
     for (auto &c : h->chunks) {
-        CU(cudaMalloc(&c.d_partition, R * 4));
-        CU(cudaMalloc(&c.d_klen, R * 4));
-        CU(cudaMalloc(&c.d_vlen, R * 4));
-        CU(cudaMalloc(&c.d_ts, R * 8));
-        CU(cudaMalloc(&c.d_seq, R * 8));
-        CU(cudaMalloc(&c.d_keys, KB + 64));
-        CU(cudaMalloc(&c.d_tile_base, (R / TILE + 2) * 8));
-        CU(cudaEventCreateWithFlags(&c.free_ev, cudaEventDisableTiming));
+        if ((rc = c.d_partition.alloc(R)) || (rc = c.d_klen.alloc(R)) || (rc = c.d_vlen.alloc(R)) || (rc = c.d_ts.alloc(R)) ||
+            (rc = c.d_seq.alloc(R)) || (rc = c.d_keys.alloc(KB + 64)) || (rc = c.d_tile_base.alloc(R / TILE + 2)))
+            return rc;
+        if (!c.free_ev) CU(cudaEventCreateWithFlags(&c.free_ev, cudaEventDisableTiming));
     }
     h->ring_dev_ready = true;
     return KTA_OK;
@@ -1142,14 +1173,10 @@ static int ring_host_init(kta_handle *h) {
     int rc;
     if ((rc = ring_dev_init(h))) return rc;
     const int64_t R = h->ring_records, KB = h->ring_key_bytes;
-    for (auto &c : h->chunks) {
-        CU(cudaHostAlloc(&c.h_partition, R * 4, cudaHostAllocDefault));
-        CU(cudaHostAlloc(&c.h_klen, R * 4, cudaHostAllocDefault));
-        CU(cudaHostAlloc(&c.h_vlen, R * 4, cudaHostAllocDefault));
-        CU(cudaHostAlloc(&c.h_ts, R * 8, cudaHostAllocDefault));
-        CU(cudaHostAlloc(&c.h_keys, KB + 64, cudaHostAllocDefault));
-        CU(cudaHostAlloc(&c.h_tile_base, (R / TILE + 2) * 8, cudaHostAllocDefault));
-    }
+    for (auto &c : h->chunks)
+        if ((rc = c.h_partition.alloc(R)) || (rc = c.h_klen.alloc(R)) || (rc = c.h_vlen.alloc(R)) || (rc = c.h_ts.alloc(R)) ||
+            (rc = c.h_keys.alloc(KB + 64)) || (rc = c.h_tile_base.alloc(R / TILE + 2)))
+            return rc;
     h->ring_host_ready = true;
     return KTA_OK;
 }
@@ -1161,7 +1188,7 @@ static void push_cursor_bind(kta_handle *h) {
     pc.n = 0; pc.kb = 0;
     pc.cap = h->ring_host_ready ? h->ring_records : 0;
     pc.kcap = h->ring_key_bytes;
-    pc.hash = h->need_hash || h->d_hash_out;
+    pc.hash = keys_travel(h);
 }
 
 // scan the columns staged in ring chunk `cur` and move on to the next chunk
@@ -1192,19 +1219,11 @@ static int ring_flush(kta_handle *h) {
     CU(cudaMemcpyAsync(c.d_ts, c.h_ts, n * 8, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(c.d_klen, c.h_klen, n * 4, cudaMemcpyHostToDevice, s));
     CU(cudaMemcpyAsync(c.d_vlen, c.h_vlen, n * 4, cudaMemcpyHostToDevice, s));
-    if (h->need_hash || h->d_hash_out) {
+    if (keys_travel(h)) {
         if (kb) CU(cudaMemcpyAsync(c.d_keys, c.h_keys, kb, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(c.d_tile_base, c.h_tile_base, (ntiles + 1) * 8, cudaMemcpyHostToDevice, s));
     }
-    ScanParams prm{};
-    prm.n = n;
-    prm.seq_base = h->next_seq;
-    prm.partition = c.d_partition;
-    prm.ts_ms = c.d_ts;
-    prm.key_len = c.d_klen;
-    prm.value_len = c.d_vlen;
-    prm.key_bytes = c.d_keys;
-    prm.key_tile_base = c.d_tile_base;
+    const ScanParams prm = scan_params(n, h->next_seq, c.d_partition, c.d_ts, c.d_klen, c.d_vlen, c.d_keys, c.d_tile_base, nullptr);
     int rc;
     if ((rc = ring_scan_chunk(h, prm, (kb + 15) & ~(int64_t)15, kb))) return rc;
     h->next_seq += (uint64_t)n;
@@ -1262,14 +1281,10 @@ extern "C" int kta_push(kta_handle *h, int32_t partition, int64_t offset, int64_
 }
 
 extern "C" int kta_push_batch_host(kta_handle *h, const kta_batch *b) {
-    if (!h || !b) return fail(KTA_ERR_INVALID, "null argument");
-    if (b->n < 0) return fail(KTA_ERR_INVALID, "negative n");
-    if (b->n == 0) return KTA_OK;
-    if (!b->partition || !b->ts_ms || !b->key_len || !b->value_len)
-        return fail(KTA_ERR_INVALID, "partition/ts_ms/key_len/value_len columns are required");
-    const bool hash = h->need_hash || h->d_hash_out;
-    if (hash && !b->key_bytes && b->key_bytes_len > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL");
     int rc;
+    if ((rc = check_batch(h, b)) || b->n == 0) return rc;
+    const bool hash = keys_travel(h);
+    if (hash && !b->key_bytes && b->key_bytes_len > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL");
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;  // keep seq order with earlier kta_push records
     if ((rc = ring_dev_init(h))) return rc;
@@ -1328,23 +1343,16 @@ extern "C" int kta_push_batch_host(kta_handle *h, const kta_batch *b) {
         CU(cudaMemcpyAsync(c.d_klen, b->key_len + r0, cn * 4, cudaMemcpyHostToDevice, s));
         CU(cudaMemcpyAsync(c.d_vlen, b->value_len + r0, cn * 4, cudaMemcpyHostToDevice, s));
         if (use_seq) CU(cudaMemcpyAsync(c.d_seq, b->seq + r0, cn * 8, cudaMemcpyHostToDevice, s));
-        ScanParams prm{};
+        // keep absolute offsets: place the keys so that (virtual base + k0) is where they land and the
+        // virtual base stays 16-byte aligned
+        const uint64_t shift = k0 & 15ull;
         if (hash) {
-            // keep absolute offsets: place the keys so that (virtual base + k0) is where they land and the
-            // virtual base stays 16-byte aligned
-            const uint64_t shift = k0 & 15ull;
             if (k1 > k0) CU(cudaMemcpyAsync(c.d_keys + shift, b->key_bytes + k0, k1 - k0, cudaMemcpyHostToDevice, s));
             CU(cudaMemcpyAsync(c.d_tile_base, tb_src, (ntiles + 1) * 8, cudaMemcpyHostToDevice, s));
-            prm.key_bytes = c.d_keys + shift - k0;
-            prm.key_tile_base = c.d_tile_base;
         }
-        prm.n = cn;
-        prm.seq_base = seq_base + (uint64_t)r0;
-        prm.partition = c.d_partition;
-        prm.ts_ms = c.d_ts;
-        prm.key_len = c.d_klen;
-        prm.value_len = c.d_vlen;
-        prm.seq = use_seq ? c.d_seq : nullptr;
+        const ScanParams prm = scan_params(cn, seq_base + (uint64_t)r0, c.d_partition, c.d_ts, c.d_klen, c.d_vlen,
+                                           hash ? c.d_keys + shift - k0 : nullptr, hash ? c.d_tile_base.get() : nullptr,
+                                           use_seq ? c.d_seq.get() : nullptr);
         const uint64_t seq_ends[2] = {use_seq ? b->seq[r0] : 0, use_seq ? b->seq[r0 + cn - 1] : 0};
         if ((rc = ring_scan_chunk(h, prm, (int64_t)((k1 + 15) & ~15ull), (int64_t)(k1 - k0), use_seq ? seq_ends : nullptr))) return rc;
         koff = k1;
@@ -1352,8 +1360,7 @@ extern "C" int kta_push_batch_host(kta_handle *h, const kta_batch *b) {
     }
     // the caller may reuse its buffers when we return: all host→device copies must have been consumed
     CU(cudaStreamSynchronize(s));
-    int rc2;
-    if ((rc2 = collect_timing(h))) return rc2;
+    if ((rc = collect_timing(h))) return rc;
     h->next_seq = std::max<uint64_t>(h->next_seq, seq_base + (uint64_t)b->n);
     return KTA_OK;
 }
@@ -1378,8 +1385,8 @@ extern "C" int kta_reset(kta_handle *h) {
     h->finalized = false;
     h->launches = 0;
     h->records = 0;
-    h->txn.ranges.clear();
-    for (uint64_t &v : h->txn.totals) v = 0;
+    h->log.txn.ranges.clear();
+    for (uint64_t &v : h->log.txn.totals) v = 0;
     return state_reset_device(h);
 }
 
@@ -1625,28 +1632,20 @@ extern "C" int kta_fnv32_host(kta_handle *h, int64_t n, const int32_t *key_len, 
     }
     if ((int64_t)acc > key_bytes_len) return fail(KTA_ERR_INVALID, "key_bytes_len %lld < sum of key_len %llu",
                                                   (long long)key_bytes_len, (unsigned long long)acc);
-    int32_t *d_len = nullptr;
-    uint64_t *d_off = nullptr;
-    uint8_t *d_keys = nullptr;
-    uint32_t *d_out = nullptr;
+    DevBuf<int32_t> d_len;
+    DevBuf<uint64_t> d_off;
+    DevBuf<uint8_t> d_keys;
+    DevBuf<uint32_t> d_out;
     cudaStream_t s = h->stream;
-    cudaError_t e = cudaSuccess;
-    do {
-        if ((e = cudaMalloc(&d_len, n * 4))) break;
-        if ((e = cudaMalloc(&d_off, n * 8))) break;
-        if ((e = cudaMalloc(&d_keys, acc + 16))) break;
-        if ((e = cudaMalloc(&d_out, n * 4))) break;
-        if ((e = cudaMemcpyAsync(d_len, key_len, n * 4, cudaMemcpyHostToDevice, s))) break;
-        if ((e = cudaMemcpyAsync(d_off, off.data(), n * 8, cudaMemcpyHostToDevice, s))) break;
-        if (acc && (e = cudaMemcpyAsync(d_keys, key_bytes, acc, cudaMemcpyHostToDevice, s))) break;
-        fnv32_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 1024), 256, 0, s>>>(n, d_len, d_off, d_keys, d_out);
-        h->launches++;
-        if ((e = cudaGetLastError())) break;
-        if ((e = cudaMemcpyAsync(out, d_out, n * 4, cudaMemcpyDeviceToHost, s))) break;
-        e = cudaStreamSynchronize(s);
-    } while (0);
-    cudaFree(d_len); cudaFree(d_off); cudaFree(d_keys); cudaFree(d_out);
-    if (e != cudaSuccess) return fail(KTA_ERR_CUDA, "kta_fnv32_host: %s", cudaGetErrorString(e));
+    if ((rc = d_len.alloc(n)) || (rc = d_off.alloc(n)) || (rc = d_keys.alloc((int64_t)acc + 16)) || (rc = d_out.alloc(n))) return rc;
+    CU(cudaMemcpyAsync(d_len, key_len, n * 4, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(d_off, off.data(), n * 8, cudaMemcpyHostToDevice, s));
+    if (acc) CU(cudaMemcpyAsync(d_keys, key_bytes, acc, cudaMemcpyHostToDevice, s));
+    fnv32_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 1024), 256, 0, s>>>(n, d_len, d_off, d_keys, d_out);
+    h->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(out, d_out, n * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
     return KTA_OK;
 }
 
@@ -1657,7 +1656,7 @@ extern "C" int kta_set_hash_capture(kta_handle *h, uint32_t *dev_out) {
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;   // records already landed were taken with the old setting
     h->d_hash_out = dev_out;
-    h->pc.hash = h->need_hash || h->d_hash_out;
+    h->pc.hash = keys_travel(h);
     return KTA_OK;
 }
 
