@@ -1,23 +1,19 @@
 // kta_inflate.cuh — DEFLATE (RFC 1951) inside a gzip member (RFC 1952): the records section of a Kafka record batch whose
 // attributes name codec 1 (gzip), which librdkafka inflates inside poll before the handlers see a message
-// (src/kafka.rs:93).  Used by log_decompress_kernel (kta_logdecode.cuh), one warp per batch.
+// (src/kafka.rs:93).  Used by log_unc_size_kernel (gzip_size) and log_decompress_kernel (gzip_walk) in kta_logdecode.cuh,
+// one warp per batch for the copy.
 //
 // Shape: every lane of the warp walks the same bit stream (lane-uniform control flow, shared-memory tables read as
 // broadcasts); lane 0 alone writes tables and literals, all 32 lanes copy the bytes of a match.  Huffman codes are decoded
 // canonically, one bit at a time against the per-length code counts (the tables are 16 counts + the symbols in code order:
 // no lookup tables to build per block) — a batch is a few thousand symbols, and thousands of batches decode side by side.
-// The code is __host__ __device__ so that the host-side unit test (tests/test_inflate_host.py, compiled by nvcc as a plain
-// host program) can run the same statements against zlib's output; the product only ever calls it on the device.
+// The code is __host__ __device__ so that tests/test_inflate_host.py and tests/test_lzwalk_host.py (through
+// tests/native/codec_harness.cu, compiled by nvcc as a plain host program, one lane) run the same statements against zlib's
+// output; the product only ever calls it on the device.
 #pragma once
 #include <stdint.h>
 
-#ifdef __CUDA_ARCH__
-#define KTA_INF_SYNC() __syncwarp()
-#define KTA_INF_LANES 32        // table fills are spread over the warp
-#else
-#define KTA_INF_SYNC() ((void)0)
-#define KTA_INF_LANES 1
-#endif
+#include "kta_codec.cuh"
 
 namespace kta {
 
@@ -105,10 +101,10 @@ __host__ __device__ inline int inf_construct(InfHuff &h, const uint16_t *length,
         for (int l = 0; l <= 15; l++) h.count[l] = 0;
         for (int i = 0; i < n; i++) h.count[length[i]]++;
     }
-    KTA_INF_SYNC();
+    KTA_LANE_SYNC();
     if (h.fast) {   // no entry of an earlier block's code may survive
-        for (int i = lane; i < (1 << INF_FAST_BITS); i += KTA_INF_LANES) h.fast[i] = 0;
-        KTA_INF_SYNC();
+        for (int i = lane; i < (1 << INF_FAST_BITS); i += KTA_LANES) h.fast[i] = 0;
+        KTA_LANE_SYNC();
     }
     if (h.count[0] == n) return 0;   // no codes at all: complete, but decoding anything will fail
     int left = 1;
@@ -123,14 +119,14 @@ __host__ __device__ inline int inf_construct(InfHuff &h, const uint16_t *length,
         for (int i = 0; i < n; i++)
             if (length[i] != 0) h.symbol[offs[length[i]]++] = (uint16_t)i;
     }
-    KTA_INF_SYNC();
+    KTA_LANE_SYNC();
     if (h.fast) {
         // the lookup table: the code of the j-th symbol of length l is first_l + j (canonical order), sent MSB first, so
         // it occupies the LOW l bits of the look-ahead in reversed order; every setting of the bits above it maps to it
         int first = 0, index = 0;
         for (int l = 1; l <= INF_FAST_BITS; l++) {
             const int count = h.count[l];
-            for (int j = lane; j < count; j += KTA_INF_LANES) {
+            for (int j = lane; j < count; j += KTA_LANES) {
                 uint32_t code = (uint32_t)(first + j), rev = 0;
                 for (int b = 0; b < l; b++) {
                     rev = (rev << 1) | (code & 1u);
@@ -142,13 +138,13 @@ __host__ __device__ inline int inf_construct(InfHuff &h, const uint16_t *length,
             index += count;
             first = (first + count) << 1;
         }
-        KTA_INF_SYNC();
+        KTA_LANE_SYNC();
     }
     return left;
 }
 
-// Output policy Out:  bool lit(uint8_t)  |  bool match(uint32_t dist, uint32_t len)  |  bool stored(const uint8_t *, uint32_t)
-// each returning false when the output would overflow or a distance reaches before the start.
+// Output policy Out (InfOut below):  bool lit(uint8_t)  |  bool match(uint32_t dist, uint32_t len)  |  bool stored(const uint8_t *,
+// uint32_t), each returning false when the output would overflow or a distance reaches before the start.
 
 // length / distance symbols, RFC 1951 3.2.5, in closed form (no tables in local memory): a length symbol s = 0..28 (code
 // 257 + s) carries e = (s - 4) / 4 extra bits from s = 8 on and starts at 3 + ((4 + s % 4) << e); a distance symbol s = 0..29
@@ -204,7 +200,7 @@ __host__ __device__ inline bool inf_stream(InfBits &s, Out &out, InfWork &w, int
             if (!out.stored(s.p + s.pos, len)) return false;
             s.pos += len;
         } else if (type == 1 || type == 2) {
-            KTA_INF_SYNC();   // every lane is done with the previous block's tables
+            KTA_LANE_SYNC();   // every lane is done with the previous block's tables
             if (type == 1) {
                 // fixed codes (RFC 1951 3.2.6)
                 if (lane == 0) {
@@ -213,12 +209,12 @@ __host__ __device__ inline bool inf_stream(InfBits &s, Out &out, InfWork &w, int
                     for (int i = 256; i < 280; i++) w.lengths[i] = 7;
                     for (int i = 280; i < 288; i++) w.lengths[i] = 8;
                 }
-                KTA_INF_SYNC();
+                KTA_LANE_SYNC();
                 inf_construct(lencode, w.lengths, 288, w.offs, lane);
-                KTA_INF_SYNC();
+                KTA_LANE_SYNC();
                 if (lane == 0)
                     for (int i = 0; i < 30; i++) w.lengths[i] = 5;
-                KTA_INF_SYNC();
+                KTA_LANE_SYNC();
                 inf_construct(distcode, w.lengths, 30, w.offs, lane);
             } else {
                 // dynamic codes (RFC 1951 3.2.7): the code lengths are themselves Huffman coded
@@ -233,9 +229,9 @@ __host__ __device__ inline bool inf_stream(InfBits &s, Out &out, InfWork &w, int
                     if (lane == 0)
                         for (int i = 0; i < 19; i++) w.lengths[i] = cl[i];
                 }
-                KTA_INF_SYNC();
+                KTA_LANE_SYNC();
                 if (inf_construct(clcode, w.lengths, 19, w.offs, lane) != 0) return false;   // the code-length code must be complete
-                KTA_INF_SYNC();
+                KTA_LANE_SYNC();
                 // the nlen + ndist lengths; they go to a second array (the code-length code's own lengths are still in use
                 // through lencode's tables only, so w.lengths may be overwritten now)
                 int index = 0;
@@ -262,16 +258,16 @@ __host__ __device__ inline bool inf_stream(InfBits &s, Out &out, InfWork &w, int
                     index += rep;
                     prev = val;
                 }
-                KTA_INF_SYNC();
+                KTA_LANE_SYNC();
                 if (w.lengths[256] == 0) return false;   // no end-of-block code
                 // an incomplete code is allowed only when it is a single code of length 1 (RFC 1951 as zlib reads it)
                 int err = inf_construct(lencode, w.lengths, nlen, w.offs, lane);
                 if (err < 0 || (err > 0 && nlen != lencode.count[0] + lencode.count[1])) return false;
-                KTA_INF_SYNC();
+                KTA_LANE_SYNC();
                 err = inf_construct(distcode, w.lengths + nlen, ndist, w.offs, lane);
                 if (err < 0 || (err > 0 && ndist != distcode.count[0] + distcode.count[1])) return false;
             }
-            KTA_INF_SYNC();
+            KTA_LANE_SYNC();
             if (!inf_codes(s, out, lencode, distcode)) return false;
         } else {
             return false;
@@ -301,6 +297,53 @@ __host__ __device__ inline uint32_t gzip_header_len(const uint8_t *in, uint32_t 
 // ISIZE: the uncompressed length mod 2^32, the last four bytes of the member
 __host__ __device__ inline uint32_t gzip_isize(const uint8_t *in, uint32_t n) {
     return (uint32_t)in[n - 4] | ((uint32_t)in[n - 3] << 8) | ((uint32_t)in[n - 2] << 16) | ((uint32_t)in[n - 1] << 24);
+}
+
+// gzip: one member (what producers write: the records section is one gzip stream).  The size pass trusts ISIZE, but not
+// beyond what DEFLATE can expand n bytes to (a forged trailer must not size the scratch buffer); the copy pass is bounded by
+// it and must produce exactly that many bytes.  The CRC32 of the trailer is not verified (like the batch CRC: check.crcs=false).
+__host__ __device__ inline LzWalk gzip_size(const uint8_t *in, uint32_t n) {
+    if (gzip_header_len(in, n) && (uint64_t)gzip_isize(in, n) <= (uint64_t)n * 1032u + 64u) return LzWalk{gzip_isize(in, n), true};
+    return LzWalk{0, false};
+}
+
+// The output policy of the copy: lane 0 writes the literals, all lanes copy matches and stored blocks (on the host, lane 0 is
+// the only lane).
+struct InfOut {
+    uint8_t *out;
+    uint64_t op, cap;
+    int lane;
+    __host__ __device__ bool lit(uint8_t b) {
+        if (op >= cap) return false;
+        if (lane == 0) out[op] = b;
+        op++;
+        return true;
+    }
+    __host__ __device__ bool match(uint32_t dist, uint32_t len) {
+        if (dist > op || op + len > cap) return false;
+        lz_emit_match<true>(out, op, dist, len, lane);   // syncs the warp first: lane 0's literals are visible
+        op += len;
+        return true;
+    }
+    __host__ __device__ bool stored(const uint8_t *src, uint32_t len) {
+        if (op + len > cap) return false;
+        lz_emit_literals<true>(out, op, src, len, lane);
+        op += len;
+        return true;
+    }
+};
+
+// The copy of the member at in[0, n) into out[0, out_cap), the whole warp (out_cap: what gzip_size gave)
+__host__ __device__ inline LzWalk gzip_walk(const uint8_t *in, uint32_t n, uint8_t *out, uint64_t out_cap, InfWork &work, int lane) {
+    LzWalk w{0, false};
+    const uint32_t hl = gzip_header_len(in, n);
+    if (!hl) return w;
+    InfBits s{in + hl, n - hl - 8u, 0u, 0ull, 0, false};
+    InfOut o{out, 0, out_cap, lane};
+    const bool ok = inf_stream(s, o, work, lane);
+    w.out_len = o.op;
+    w.ok = ok && o.op == (uint64_t)gzip_isize(in, n);
+    return w;
 }
 
 }  // namespace kta

@@ -14,9 +14,9 @@
 // timestampDelta as the consumer computes it, and only a RESULT of -1 means "not available"; key/value length -1 means
 // null.  CRCs are not verified (librdkafka's default check.crcs=false).
 // Compression (attributes bits 0-2, librdkafka decompresses inside poll, src/kafka.rs:93): gzip (kta_inflate.cuh), LZ4 (frame
-// format), Snappy (raw or xerial-framed) and zstd (kta_zstd.cuh) batches are decompressed on the GPU into a scratch buffer and
-// then decoded like the others; the unassigned codes 5-7 are rejected.  Checksums inside the compressed sections (gzip's
-// CRC32, zstd's Content_Checksum) are skipped, not verified, like the batch CRC.
+// format), Snappy (raw or xerial-framed; both kta_lz4_snappy.cuh) and zstd (kta_zstd.cuh) batches are decompressed on the GPU
+// into a scratch buffer and then decoded like the others; the unassigned codes 5-7 are rejected.  Checksums inside the
+// compressed sections (gzip's CRC32, zstd's Content_Checksum) are skipped, not verified, like the batch CRC.
 // Isolation: on a read_committed handle the passes of kta_logtxn.cuh mark the batches of aborted transactions
 // LOGB_SKIP_ABORTED before anything here decompresses or decodes them; on a read_uncommitted handle (the default) every
 // data batch is delivered, as before.  Not handled: legacy magic 0/1 message sets are flagged as malformed.
@@ -26,7 +26,10 @@
 
 #include <type_traits>
 
+#include "kta_codec.cuh"
 #include "kta_inflate.cuh"
+#include "kta_lz4_snappy.cuh"
+#include "kta_zstd.cuh"
 
 namespace kta {
 
@@ -38,6 +41,11 @@ constexpr int LOG_HEADER_BYTES = 61;
 enum LogBatchFlags { LOGB_OK = 0, LOGB_SKIP_CONTROL = 1, LOGB_BAD = 2, LOGB_COMPRESSED = 4, LOGB_LZ4 = 8, LOGB_SNAPPY = 16, LOGB_GZIP = 32,
                      LOGB_ZSTD = 64, LOGB_SKIP_ABORTED = 128 };
 constexpr uint32_t LOGB_CODECS = LOGB_LZ4 | LOGB_SNAPPY | LOGB_GZIP | LOGB_ZSTD;   // batches log_decompress_kernel turns into LOGB_OK
+
+// the flag of Kafka's compression codec id 0-4 (attributes & 7: none, gzip, Snappy, LZ4, zstd)
+__host__ __device__ __forceinline__ uint32_t log_codec_flag(uint32_t codec) {
+    return codec == 0 ? LOGB_OK : codec == 1 ? LOGB_GZIP : codec == 2 ? LOGB_SNAPPY : codec == 3 ? LOGB_LZ4 : LOGB_ZSTD;
+}
 
 __device__ __forceinline__ uint64_t be_u64(const uint8_t *p) {
     uint64_t v = 0;
@@ -91,7 +99,7 @@ __global__ void log_header_kernel(const uint8_t *bytes, int64_t nbytes, const ui
                 bi.log_append_time = (attrs >> 3) & 1u;
                 if (attrs & 0x20u) bi.flags = LOGB_SKIP_CONTROL;
                 else if (codec <= 4) {
-                    bi.flags = codec == 0 ? LOGB_OK : codec == 1 ? LOGB_GZIP : codec == 2 ? LOGB_SNAPPY : codec == 3 ? LOGB_LZ4 : LOGB_ZSTD;
+                    bi.flags = log_codec_flag(codec);
                     bi.records = count;
                 } else bi.flags = LOGB_COMPRESSED;   // unassigned codes
             }
@@ -104,228 +112,21 @@ __global__ void log_header_kernel(const uint8_t *bytes, int64_t nbytes, const ui
     if (blockIdx.x == 0 && threadIdx.x == 0) rec_count[0] = 0;
 }
 
-// unsigned LEB128 at p (bounded by end); returns bytes consumed, 0 on malformed input.  Generic byte loads: the batch may
-// sit in shared memory or in global memory.
-__host__ __device__ __forceinline__ int uvarint_g(const uint8_t *p, const uint8_t *end, uint64_t &out) {
-    uint64_t v = 0;
-    int shift = 0, n = 0;
-    while (p + n < end && n < 10) {
-        const uint8_t b = p[n];
-        n++;
-        v |= (uint64_t)(b & 0x7f) << shift;
-        if (!(b & 0x80)) {
-            out = v;
-            return n;
-        }
-        shift += 7;
-    }
-    return 0;
+// The records section in[0, n) of a gzip, LZ4 or Snappy batch (flags: its LOGB_GZIP / LOGB_LZ4 / LOGB_SNAPPY): its uncompressed
+// size (thread per batch), then its copy to out + at, out_cap bytes (the whole warp; work: the warp's inflate tables).  The
+// copy kernel passes its image and the header's length as `at`: with the offset added in each branch it compiles to the same
+// code as with the walks called in place.  zstd batches have a size kernel and a copy instance of their own (zstd_walk).
+__host__ __device__ __forceinline__ LzWalk section_size(uint32_t flags, const uint8_t *in, uint32_t n) {
+    return flags == LOGB_GZIP  ? gzip_size(in, n)
+           : flags == LOGB_LZ4 ? lz4_frame_walk<false>(in, n, nullptr, 0, 0)
+                               : snappy_walk<false>(in, n, nullptr, 0, 0);
 }
-
-// ------------------------------------------------------------------------------------------------
-// Decompression of the records section (everything behind the 61-byte header) of LZ4 and Snappy batches.
-//   LZ4: the frame format (magic 0x184D2204 | FLG | BD | [content size] | [dict id] | HC | blocks… | EndMark | [checksum]);
-//        a block is a u32 LE size (top bit = stored uncompressed) + data [+ block checksum]; block data = sequences of
-//        token | literal length… | literals | offset u16 | match length… ; matches may reach back into earlier blocks.
-//   Snappy: raw (uvarint uncompressed length, then elements: literal / copy with 1-, 2-, 4-byte offset) or the xerial
-//        framing Java clients write ("\x82SNAPPY\0", two version words, then chunks of u32 BE length + raw snappy).
-// A "walk" goes through the elements once; with out == nullptr it only adds up the output size.  One lane parses, all 32
-// lanes of the warp copy (a match that overlaps itself repeats with period `offset`, so every byte's source is known up
-// front: out[op + i] = out[op - offset + i % offset]).
-// ------------------------------------------------------------------------------------------------
-struct LzWalk {
-    uint64_t out_len;   // bytes produced
-    bool ok;
-};
-
-// (the walks are __host__ __device__ like kta_inflate.cuh: tests/test_lzwalk_host.py runs them on the host, where the
-// "warp" is one lane; the product calls them on the device only)
-template <bool COPY>
-__host__ __device__ __forceinline__ void lz_emit_literals(uint8_t *out, uint64_t op, const uint8_t *in, uint32_t n, int lane) {
-    if (COPY) for (uint32_t i = lane; i < n; i += KTA_INF_LANES) out[op + i] = in[i];
+__host__ __device__ __forceinline__ LzWalk section_copy(uint32_t flags, const uint8_t *in, uint32_t n, uint8_t *out, uint32_t at,
+                                                        uint64_t out_cap, InfWork &work, int lane) {
+    return flags == LOGB_LZ4    ? lz4_frame_walk<true>(in, n, out + at, out_cap, lane)
+           : flags == LOGB_GZIP ? gzip_walk(in, n, out + at, out_cap, work, lane)
+                                : snappy_walk<true>(in, n, out + at, out_cap, lane);
 }
-template <bool COPY>
-__host__ __device__ __forceinline__ void lz_emit_match(uint8_t *out, uint64_t op, uint32_t offset, uint32_t n, int lane) {
-    if (COPY) {
-        KTA_INF_SYNC();   // the bytes the match refers to have been written
-        for (uint32_t i = lane; i < n; i += KTA_INF_LANES) out[op + i] = out[op - offset + (i % offset)];
-        KTA_INF_SYNC();
-    }
-}
-
-// LZ4 frame at in[0, n).  COPY: the whole warp calls this (lane-uniform control flow: every lane parses the same bytes).
-template <bool COPY>
-__host__ __device__ LzWalk lz4_frame_walk(const uint8_t *in, uint32_t n, uint8_t *out, uint64_t out_cap, int lane) {
-    LzWalk w{0, false};
-    if (n < 7 || in[0] != 0x04 || in[1] != 0x22 || in[2] != 0x4D || in[3] != 0x18) return w;
-    const uint32_t flg = in[4];
-    if ((flg >> 6) != 1) return w;
-    uint32_t ip = 6 + ((flg & 0x08) ? 8u : 0u) + ((flg & 0x01) ? 4u : 0u) + 1u;   // FLG, BD, [content size], [dict id], HC
-    const bool block_checksum = (flg & 0x10) != 0;
-    for (;;) {
-        if (ip + 4 > n) return w;
-        const uint32_t bs = (uint32_t)in[ip] | ((uint32_t)in[ip + 1] << 8) | ((uint32_t)in[ip + 2] << 16) | ((uint32_t)in[ip + 3] << 24);
-        ip += 4;
-        if (bs == 0) break;                                  // EndMark
-        const uint32_t blen = bs & 0x7fffffffu;
-        if (blen > n - ip) return w;
-        if (bs & 0x80000000u) {                              // stored block
-            if (COPY && w.out_len + blen > out_cap) return w;
-            lz_emit_literals<COPY>(out, w.out_len, in + ip, blen, lane);
-            w.out_len += blen;
-        } else {
-            uint32_t p = ip;
-            const uint32_t bend = ip + blen;
-            while (p < bend) {
-                const uint32_t token = in[p++];
-                uint32_t lit = token >> 4;
-                if (lit == 15) {
-                    uint32_t b;
-                    do { if (p >= bend) return w; b = in[p++]; lit += b; } while (b == 255);
-                }
-                if (lit > bend - p) return w;
-                if (COPY && w.out_len + lit > out_cap) return w;
-                lz_emit_literals<COPY>(out, w.out_len, in + p, lit, lane);
-                w.out_len += lit;
-                p += lit;
-                if (p >= bend) break;                        // the last sequence of a block has no match
-                if (p + 2 > bend) return w;
-                const uint32_t offset = (uint32_t)in[p] | ((uint32_t)in[p + 1] << 8);
-                p += 2;
-                uint32_t ml = (token & 15u) + 4u;
-                if ((token & 15u) == 15u) {
-                    uint32_t b;
-                    do { if (p >= bend) return w; b = in[p++]; ml += b; } while (b == 255);
-                }
-                if (offset == 0 || offset > w.out_len) return w;
-                if (COPY && w.out_len + ml > out_cap) return w;
-                lz_emit_match<COPY>(out, w.out_len, offset, ml, lane);
-                w.out_len += ml;
-            }
-        }
-        ip += blen + (block_checksum ? 4u : 0u);
-    }
-    w.ok = true;
-    return w;
-}
-
-// one raw Snappy block at in[0, n)
-template <bool COPY>
-__host__ __device__ bool snappy_raw_walk(const uint8_t *in, uint32_t n, uint8_t *out, uint64_t out_cap, uint64_t &op, int lane) {
-    uint64_t want;
-    const int hn = uvarint_g(in, in + n, want);
-    if (hn <= 0) return false;
-    const uint64_t start = op;
-    uint32_t p = (uint32_t)hn;
-    while (p < n) {
-        const uint32_t tag = in[p++];
-        if ((tag & 3u) == 0) {                               // literal
-            uint32_t len = (tag >> 2) + 1u;
-            if (len > 60) {
-                const uint32_t nb = len - 60;                // 1..4 length bytes follow
-                if (p + nb > n) return false;
-                len = 0;
-                for (uint32_t i = 0; i < nb; i++) len |= (uint32_t)in[p + i] << (8 * i);
-                len += 1u;
-                p += nb;
-            }
-            if (len > n - p) return false;
-            if (COPY && op + len > out_cap) return false;
-            lz_emit_literals<COPY>(out, op, in + p, len, lane);
-            op += len;
-            p += len;
-        } else {
-            uint32_t len, offset;
-            if ((tag & 3u) == 1) {
-                if (p + 1 > n) return false;
-                len = ((tag >> 2) & 7u) + 4u;
-                offset = ((tag >> 5) << 8) | in[p];
-                p += 1;
-            } else if ((tag & 3u) == 2) {
-                if (p + 2 > n) return false;
-                len = (tag >> 2) + 1u;
-                offset = (uint32_t)in[p] | ((uint32_t)in[p + 1] << 8);
-                p += 2;
-            } else {
-                if (p + 4 > n) return false;
-                len = (tag >> 2) + 1u;
-                offset = (uint32_t)in[p] | ((uint32_t)in[p + 1] << 8) | ((uint32_t)in[p + 2] << 16) | ((uint32_t)in[p + 3] << 24);
-                p += 4;
-            }
-            if (offset == 0 || offset > op - start) return false;
-            if (COPY && op + len > out_cap) return false;
-            lz_emit_match<COPY>(out, op, offset, len, lane);
-            op += len;
-        }
-    }
-    return op - start == want;
-}
-
-template <bool COPY>
-__host__ __device__ LzWalk snappy_walk(const uint8_t *in, uint32_t n, uint8_t *out, uint64_t out_cap, int lane) {
-    LzWalk w{0, false};
-    const bool xerial = n >= 16 && in[0] == 0x82 && in[1] == 'S' && in[2] == 'N' && in[3] == 'A' && in[4] == 'P' && in[5] == 'P' &&
-                        in[6] == 'Y' && in[7] == 0;
-    if (!xerial) {
-        w.ok = snappy_raw_walk<COPY>(in, n, out, out_cap, w.out_len, lane);
-        return w;
-    }
-    uint32_t p = 16;                                         // magic (8) + version (4) + compatible version (4)
-    while (p < n) {
-        if (p + 4 > n) return w;
-        const uint32_t cl = ((uint32_t)in[p] << 24) | ((uint32_t)in[p + 1] << 16) | ((uint32_t)in[p + 2] << 8) | in[p + 3];
-        p += 4;
-        if (cl > n - p) return w;
-        if (!snappy_raw_walk<COPY>(in + p, cl, out, out_cap, w.out_len, lane)) return w;
-        p += cl;
-    }
-    w.ok = true;
-    return w;
-}
-
-// gzip: one member (what producers write: the records section is one gzip stream).  The size pass trusts ISIZE; the copy
-// pass is bounded by it and must produce exactly that many bytes.  The CRC32 of the trailer is not verified (like the batch
-// CRC: check.crcs=false).
-struct InfWarpOut {
-    uint8_t *out;
-    uint64_t op, cap;
-    int lane;
-    __device__ bool lit(uint8_t b) {
-        if (op >= cap) return false;
-        if (lane == 0) out[op] = b;
-        op++;
-        return true;
-    }
-    __device__ bool match(uint32_t dist, uint32_t len) {
-        if (dist > op || op + len > cap) return false;
-        lz_emit_match<true>(out, op, dist, len, lane);   // syncs the warp first: lane 0's literals are visible
-        op += len;
-        return true;
-    }
-    __device__ bool stored(const uint8_t *src, uint32_t len) {
-        if (op + len > cap) return false;
-        lz_emit_literals<true>(out, op, src, len, lane);
-        op += len;
-        return true;
-    }
-};
-__device__ inline LzWalk gzip_walk(const uint8_t *in, uint32_t n, uint8_t *out, uint64_t out_cap, InfWork &work, int lane) {
-    LzWalk w{0, false};
-    const uint32_t hl = gzip_header_len(in, n);
-    if (!hl) return w;
-    InfBits s{in + hl, n - hl - 8u, 0u, 0ull, 0, false};
-    InfWarpOut o{out, 0, out_cap, lane};
-    const bool ok = inf_stream(s, o, work, lane);
-    w.out_len = o.op;
-    w.ok = ok && o.op == (uint64_t)gzip_isize(in, n);
-    return w;
-}
-
-}  // namespace kta
-
-#include "kta_zstd.cuh"   // (uses LzWalk and the lz_emit_* copies above)
-
-namespace kta {
 
 // the scratch bytes a batch's uncompressed image (header + records, rounded up to 16) needs, or 0 (and LOGB_BAD) when the walk
 // failed or recordsCount is implausible for the uncompressed size (it sizes the output columns: 7 bytes per record at least)
@@ -343,17 +144,8 @@ __global__ void log_unc_size_kernel(const uint8_t *bytes, const LogBatchInfo *in
     for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nbatches; b += (int64_t)gridDim.x * blockDim.x) {
         const LogBatchInfo bi = info[b];
         uint64_t need = 0;
-        if ((bi.flags & LOGB_CODECS) && bi.flags != LOGB_ZSTD) {
-            const uint8_t *in = bytes + bi.off + LOG_HEADER_BYTES;
-            const uint32_t n = bi.len - LOG_HEADER_BYTES;
-            LzWalk w{0, false};
-            if (bi.flags == LOGB_GZIP) {
-                // ISIZE is taken on trust here (the copy pass must then produce exactly that much), but not beyond what
-                // DEFLATE can expand to (1032 : 1): a forged trailer must not size the scratch buffer
-                if (gzip_header_len(in, n) && (uint64_t)gzip_isize(in, n) <= (uint64_t)n * 1032u + 64u) w = LzWalk{gzip_isize(in, n), true};
-            } else w = bi.flags == LOGB_LZ4 ? lz4_frame_walk<false>(in, n, nullptr, 0, 0) : snappy_walk<false>(in, n, nullptr, 0, 0);
-            need = unc_need(bi, w, error_flags);
-        }
+        if ((bi.flags & LOGB_CODECS) && bi.flags != LOGB_ZSTD)
+            need = unc_need(bi, section_size(bi.flags, bytes + bi.off + LOG_HEADER_BYTES, bi.len - LOG_HEADER_BYTES), error_flags);
         slot[b + 1] = need;
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) slot[0] = 0;
@@ -404,10 +196,7 @@ __global__ void __launch_bounds__(128) log_decompress_kernel(const uint8_t *byte
         const uint32_t n = bi.len - LOG_HEADER_BYTES;
         LzWalk w;
         if constexpr (ZSTD) w = zstd_walk<true>(in, n, dst + LOG_HEADER_BYTES, lit_scratch + slot[b] + LOG_HEADER_BYTES, cap, work[threadIdx.x >> 5], lane);
-        else
-            w = bi.flags == LOGB_LZ4    ? lz4_frame_walk<true>(in, n, dst + LOG_HEADER_BYTES, cap, lane)
-                : bi.flags == LOGB_GZIP ? gzip_walk(in, n, dst + LOG_HEADER_BYTES, cap, work[threadIdx.x >> 5], lane)
-                                        : snappy_walk<true>(in, n, dst + LOG_HEADER_BYTES, cap, lane);
+        else w = section_copy(bi.flags, in, n, dst, LOG_HEADER_BYTES, cap, work[threadIdx.x >> 5], lane);
         for (int i = lane; i < LOG_HEADER_BYTES; i += 32) dst[i] = src[i];
         __syncwarp();
         if (lane == 0) {

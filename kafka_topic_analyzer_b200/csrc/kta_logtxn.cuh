@@ -23,6 +23,7 @@
 
 #include <cuda/std/tuple>
 
+#include "kta_codec.cuh"
 #include "kta_logdecode.cuh"
 
 namespace kta {

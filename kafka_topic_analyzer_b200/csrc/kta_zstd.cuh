@@ -1,6 +1,6 @@
 // kta_zstd.cuh — Zstandard frames (RFC 8878): the records section of a Kafka record batch whose attributes name codec 4
 // (zstd), which librdkafka decompresses inside poll before the handlers see a message (src/kafka.rs:93).  Used by
-// log_zstd_size_kernel and log_decompress_kernel (kta_logdecode.cuh, which includes this file), one warp per batch.
+// log_zstd_size_kernel and log_decompress_kernel<true> (kta_logdecode.cuh), one warp per batch.
 //
 // Accepted: any number of frames, with or without Frame_Content_Size (one-shot compressors write it, streaming ones such as
 // the Java client's do not), skippable frames among them, Raw / RLE / Compressed blocks, every literals and sequences mode.
@@ -13,10 +13,13 @@
 // the block's output offset (a block's literals are at most its output, so they always fit); all lanes copy literals and
 // matches.  The tables live in a per-warp ZstdWork that persists over the blocks of a frame (Repeat mode, Treeless
 // literals) and is reset at each frame.
-// The code is __host__ __device__ so that tests/test_zstd_host.py (compiled by nvcc as a plain host program, one "lane")
-// runs the same statements against pyarrow's zstd; the product only ever calls it on the device.
+// The code is __host__ __device__ so that tests/test_zstd_host.py (through tests/native/codec_harness.cu, compiled by nvcc as
+// a plain host program, one "lane") runs the same statements against pyarrow's zstd; the product only ever calls it on the
+// device.
 #pragma once
 #include <stdint.h>
+
+#include "kta_codec.cuh"
 
 namespace kta {
 
@@ -29,7 +32,7 @@ struct ZstdWork {            // per warp, in shared memory on the device
     int16_t norm[3][64];                  // normalized counts of the tables being built
     uint16_t next[3][64];                 // per-symbol state counters while building
     uint8_t hw[256];                      // Huffman weights
-    uint16_t rank[12][KTA_INF_LANES];     // per lane: next Huffman table cell of each weight
+    uint16_t rank[12][KTA_LANES];         // per lane: next Huffman table cell of each weight
 };
 
 __host__ __device__ __forceinline__ int zstd_hibit(uint32_t v) {   // v > 0
@@ -37,14 +40,6 @@ __host__ __device__ __forceinline__ int zstd_hibit(uint32_t v) {   // v > 0
     return 31 - __clz(v);
 #else
     return 31 - __builtin_clz(v);
-#endif
-}
-
-__host__ __device__ __forceinline__ bool zstd_all(bool v) {   // the warp agrees (on the host the "warp" is one lane)
-#ifdef __CUDA_ARCH__
-    return __all_sync(0xffffffffu, v);
-#else
-    return v;
 #endif
 }
 
@@ -204,7 +199,7 @@ __host__ __device__ inline bool zstd_huf_table(const uint8_t *b, uint32_t cs, ui
     if (cs < 1) return false;
     const uint32_t hb = b[0];
     uint32_t nw = 0;
-    KTA_INF_SYNC();   // every lane is done with the previous table and weights
+    KTA_LANE_SYNC();   // every lane is done with the previous table and weights
     if (hb >= 128) {  // direct: 4 bits per weight
         nw = hb - 127u;
         const uint32_t nb = (nw + 1u) >> 1;
@@ -217,9 +212,9 @@ __host__ __device__ inline bool zstd_huf_table(const uint8_t *b, uint32_t cs, ui
         int al, nsym;
         uint32_t used;
         if (!zstd_fse_norm(b + 1, hb, 6, 12, w.norm[0], al, nsym, used, lane)) return false;
-        KTA_INF_SYNC();
+        KTA_LANE_SYNC();
         if (lane == 0) zstd_fse_build(w.hwt, w.norm[0], nsym, al, w.next[0]);
-        KTA_INF_SYNC();
+        KTA_LANE_SYNC();
         ZstdBits s;
         if (used > hb || !zstd_bits_init(s, b + 1 + used, hb - used)) return false;
         uint32_t s1 = zstd_bits_read(s, al), s2 = zstd_bits_read(s, al);
@@ -251,7 +246,7 @@ __host__ __device__ inline bool zstd_huf_table(const uint8_t *b, uint32_t cs, ui
         }
         q = 1u + hb;
     }
-    KTA_INF_SYNC();
+    KTA_LANE_SYNC();
     // the last weight is implied: the weights' powers of two must add up to the next power of two
     uint32_t total = 0;
     for (uint32_t i = 0; i < nw; i++) {
@@ -265,27 +260,27 @@ __host__ __device__ inline bool zstd_huf_table(const uint8_t *b, uint32_t cs, ui
     const uint32_t rest = (1u << bits) - total;
     if (rest & (rest - 1u)) return false;
     if (lane == 0) w.hw[nw] = (uint8_t)(zstd_hibit(rest) + 1);
-    KTA_INF_SYNC();
+    KTA_LANE_SYNC();
     // table: the symbols of weight x fill 2^(x-1) cells each, weight 1 first, symbols in order within a weight
-    uint16_t *start = &w.rank[0][lane];   // start[x * KTA_INF_LANES]: this lane's copy, no bank conflicts
-    for (int x = 0; x < 12; x++) start[x * KTA_INF_LANES] = 0;
-    for (uint32_t i = 0; i <= nw; i++) start[w.hw[i] * KTA_INF_LANES]++;
+    uint16_t *start = &w.rank[0][lane];   // start[x * KTA_LANES]: this lane's copy, no bank conflicts
+    for (int x = 0; x < 12; x++) start[x * KTA_LANES] = 0;
+    for (uint32_t i = 0; i <= nw; i++) start[w.hw[i] * KTA_LANES]++;
     uint32_t at = 0;
     for (int x = 1; x <= bits; x++) {
-        const uint32_t c = (uint32_t)start[x * KTA_INF_LANES] << (x - 1);
-        start[x * KTA_INF_LANES] = (uint16_t)at;
+        const uint32_t c = (uint32_t)start[x * KTA_LANES] << (x - 1);
+        start[x * KTA_LANES] = (uint16_t)at;
         at += c;
     }
     for (uint32_t i = 0; i <= nw; i++) {
         const uint32_t x = w.hw[i];
         if (!x) continue;
-        const uint32_t a = start[x * KTA_INF_LANES], len = 1u << (x - 1u);
-        start[x * KTA_INF_LANES] = (uint16_t)(a + len);
+        const uint32_t a = start[x * KTA_LANES], len = 1u << (x - 1u);
+        start[x * KTA_LANES] = (uint16_t)(a + len);
         const uint16_t e = (uint16_t)(i | ((uint32_t)(bits + 1 - (int)x) << 8));
-        for (uint32_t j = a + (((uint32_t)lane - a) & (KTA_INF_LANES - 1u)); j < a + len; j += KTA_INF_LANES) w.huf[j] = e;
+        for (uint32_t j = a + (((uint32_t)lane - a) & (KTA_LANES - 1u)); j < a + len; j += KTA_LANES) w.huf[j] = e;
     }
     f.huf_bits = bits;
-    KTA_INF_SYNC();
+    KTA_LANE_SYNC();
     return true;
 }
 
@@ -334,7 +329,7 @@ __host__ __device__ inline bool zstd_block(const uint8_t *b, uint32_t bs, uint8_
     } else if (lt == 1) {
         if (q >= bs) return false;
         if (COPY)
-            for (uint32_t i = lane; i < rs; i += KTA_INF_LANES) lit[f.op + i] = b[q];
+            for (uint32_t i = lane; i < rs; i += KTA_LANES) lit[f.op + i] = b[q];
         q += 1;
     } else {
         if (cs > bs - q) return false;
@@ -357,18 +352,18 @@ __host__ __device__ inline bool zstd_block(const uint8_t *b, uint32_t bs, uint8_
                 ok = true;
 #pragma unroll
                 for (int k = 0; k < 4; k++) {
-                    if (KTA_INF_LANES > 1 && lane != k) continue;
+                    if (KTA_LANES > 1 && lane != k) continue;
                     const uint32_t off = 6u + (k > 0 ? l0 : 0u) + (k > 1 ? l1 : 0u) + (k > 2 ? l2 : 0u);
                     const uint32_t len = k == 0 ? l0 : k == 1 ? l1 : k == 2 ? l2 : l3;
                     ok = zstd_huf_stream(src + off, len, lit + f.op + (uint64_t)k * seg, k < 3 ? seg : rs - 3u * seg, w.huf, f.huf_bits) && ok;
                 }
             }
-            if (!zstd_all(ok)) return false;
+            if (!lanes_all(ok)) return false;
         } else if (lt == 2) f.huf_bits = 1;     // (the size pass only notes that a table exists)
         else if (f.huf_bits == 0) return false;
         q += cs;
     }
-    KTA_INF_SYNC();   // the literals are in the buffer
+    KTA_LANE_SYNC();   // the literals are in the buffer
     // --- sequences section
     if (q >= bs) return false;
     uint32_t nseq = b[q++];
@@ -388,7 +383,7 @@ __host__ __device__ inline bool zstd_block(const uint8_t *b, uint32_t bs, uint8_
         if (q >= bs) return false;
         const uint32_t modes = b[q++];
         if (modes & 3u) return false;
-        KTA_INF_SYNC();   // every lane is done with the previous block's tables
+        KTA_LANE_SYNC();   // every lane is done with the previous block's tables
         uint32_t build = 0;
         int nsym[3] = {0, 0, 0};
 #pragma unroll
@@ -421,15 +416,15 @@ __host__ __device__ inline bool zstd_block(const uint8_t *b, uint32_t bs, uint8_
                 build |= 1u << t;
             } else if (f.kind[t] == 0) return false;   // Repeat, but nothing to repeat
         }
-        KTA_INF_SYNC();
+        KTA_LANE_SYNC();
 #pragma unroll
         for (int t = 0; t < 3; t++) {       // lane t builds table t
-            if (!((build >> t) & 1u) || (KTA_INF_LANES > 1 && lane != t)) continue;
+            if (!((build >> t) & 1u) || (KTA_LANES > 1 && lane != t)) continue;
             uint32_t *dt = t == 0 ? w.ll : t == 1 ? w.of : w.ml;
             if (nsym[t] == 0) dt[0] = (uint32_t)w.norm[t][0];   // RLE
             else zstd_fse_build(dt, w.norm[t], nsym[t], f.al[t], w.next[t]);
         }
-        KTA_INF_SYNC();
+        KTA_LANE_SYNC();
         // the interleaved bitstream: initial states LL, OF, ML; per sequence the OF, ML, LL extra bits, then the LL, ML, OF
         // state updates (none after the last sequence)
         ZstdBits s;
@@ -479,7 +474,7 @@ __host__ __device__ inline bool zstd_block(const uint8_t *b, uint32_t bs, uint8_
     if ((uint64_t)left > (uint64_t)f.bmax - (f.op - bstart) || (COPY && left > cap - f.op)) return false;
     lz_emit_literals<COPY>(out, f.op, lits + lit_pos, left, lane);
     f.op += left;
-    KTA_INF_SYNC();   // the block's output is complete before the next block reads it
+    KTA_LANE_SYNC();   // the block's output is complete before the next block reads it
     return true;
 }
 
@@ -544,7 +539,7 @@ __host__ __device__ LzWalk zstd_walk(const uint8_t *in, uint32_t n, uint8_t *out
                 if (p >= n) return r;
                 if (COPY) {
                     if (bsz > out_cap - f.op) return r;
-                    for (uint32_t i = lane; i < bsz; i += KTA_INF_LANES) out[f.op + i] = in[p];
+                    for (uint32_t i = lane; i < bsz; i += KTA_LANES) out[f.op + i] = in[p];
                 }
                 f.op += bsz;
                 bound += bsz;
@@ -573,7 +568,7 @@ __host__ __device__ LzWalk zstd_walk(const uint8_t *in, uint32_t n, uint8_t *out
             if (fcs_bytes > 0 && f.op - f.start != fcs) return r;
             r.out_len = f.op;
         }
-        KTA_INF_SYNC();
+        KTA_LANE_SYNC();
     }
     r.ok = true;
     return r;

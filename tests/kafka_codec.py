@@ -70,7 +70,8 @@ def compress_records(recs: bytes, codec: str) -> bytes:
     raise ValueError(codec)
 
 
-CODEC_BITS = {None: 0, "gzip": 1, "snappy": 2, "snappy-xerial": 2, "lz4": 3, "zstd": 4}
+# Kafka's compression codec ids (attributes & 7), by the names these encoders take
+CODEC_BITS = {None: 0, "gzip": 1, "snappy": 2, "snappy-xerial": 2, "lz4": 3, "zstd": 4, "zstd-stream": 4}
 
 
 def encode_batch(base_offset, base_ts, records, attributes=0, max_ts=None, compression=None):

@@ -1,13 +1,12 @@
-"""Build recipe of the native test programs the GPU tests run — TEST INFRASTRUCTURE.
+"""Build recipe of the native test programs — TEST INFRASTRUCTURE.
 
   logdecomp_probe  tests/native/logdecomp_probe.cu: the product's decompression stage on the GPU, output made visible
                    (sm_90a, the library's nvcc flags without -shared / -fPIC)
-  zstd_harness     tests/native/zstd_harness.cu and lzwalk_harness.cu: the same walks as plain host code, one "lane"
-  lzwalk_harness   (the host tests build their own address-sanitizer copies; these are the plain builds the GPU tests compare with)
+  codec_harness    tests/native/codec_harness.cu: the same codec walks as plain host code, one "lane" (codec_harness.py runs it)
 
-The programs go to tests/native/build/ (git-ignored).  __graft_entry__.build() builds them, because the machine that runs the
-GPU tests may have no nvcc; ensure() rebuilds one when it is older than the sources, and fails when it is missing and cannot be
-built."""
+build() makes the plain programs in tests/native/build/ (git-ignored).  __graft_entry__.build() builds them, because the machine
+that runs the GPU tests may have no nvcc; build() rebuilds one when it is older than the sources, and fails when it is missing
+and cannot be built.  build_sanitized() makes the host tests' address-sanitizer build of the harness."""
 import os
 import shutil
 import subprocess
@@ -17,21 +16,22 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(ROOT, "kafka_topic_analyzer_b200", "csrc")
 NATIVE = os.path.join(HERE, "native")
 OUT = os.path.join(NATIVE, "build")
-PROGRAMS = ("logdecomp_probe", "zstd_harness", "lzwalk_harness")
+PROGRAMS = ("logdecomp_probe", "codec_harness")
+SANITIZE = ["-g", "-Xcompiler", "-fsanitize=address,-fno-omit-frame-pointer"]
 
 
-def _nvcc():
-    nvcc = os.environ.get("NVCC") or "/usr/local/cuda/bin/nvcc"
-    return nvcc if os.path.exists(nvcc) else shutil.which("nvcc")
+def nvcc():
+    path = os.environ.get("NVCC") or "/usr/local/cuda/bin/nvcc"
+    return path if os.path.exists(path) else shutil.which("nvcc")
 
 
-def _command(nvcc, name, exe):
+def _command(nvcc, name, exe, flags=()):
     src = os.path.join(NATIVE, name + ".cu")
     if name == "logdecomp_probe":
         from kafka_topic_analyzer_b200 import _native
-        flags = " ".join(_native.NVCC_FLAGS).replace("-Xcompiler -fPIC", "").replace("-shared", "").split()
-        return [nvcc, *flags, "-o", exe, src]
-    return [nvcc, "-O2", "-std=c++17", "-o", exe, src]
+        lib_flags = " ".join(_native.NVCC_FLAGS).replace("-Xcompiler -fPIC", "").replace("-shared", "").split()
+        return [nvcc, *lib_flags, "-o", exe, src]
+    return [nvcc, "-O1", "-std=c++17", *flags, "-o", exe, src]
 
 
 def _stale(name, exe):
@@ -45,13 +45,13 @@ def build(name, force=False):
     exe = os.path.join(OUT, name)
     if not force and not _stale(name, exe):
         return exe
-    nvcc = _nvcc()
-    if not nvcc:
+    cc = nvcc()
+    if not cc:
         if os.path.exists(exe):
             return exe                   # older than the sources, but nothing here can rebuild it: used as it is
         raise RuntimeError("%s is missing and there is no nvcc to build it (run __graft_entry__.build())" % exe)
     os.makedirs(OUT, exist_ok=True)
-    r = subprocess.run(_command(nvcc, name, exe), capture_output=True, text=True)
+    r = subprocess.run(_command(cc, name, exe), capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError("nvcc failed for %s:\n%s%s" % (name, r.stdout, r.stderr))
     return exe
@@ -59,3 +59,23 @@ def build(name, force=False):
 
 def build_all(force=False):
     return [build(n, force) for n in PROGRAMS]
+
+
+_sanitized = {}
+
+
+def build_sanitized(name, out_dir):
+    """`name` built into out_dir with the address sanitizer, so that a read or write outside a buffer ends the program with a
+    report; plainly when this toolchain has no sanitizer runtime.  Built once per out_dir.  Returns (exe, which build it is)."""
+    key = (name, out_dir)
+    if key not in _sanitized:
+        cc = nvcc()
+        exe = os.path.join(out_dir, name + "_asan")
+        r = subprocess.run(_command(cc, name, exe, SANITIZE), capture_output=True, text=True)
+        how = "%s: address-sanitizer build" % name
+        if r.returncode != 0:
+            exe = os.path.join(out_dir, name)
+            subprocess.run(_command(cc, name, exe), check=True, capture_output=True)
+            how = "%s: plain build, no address sanitizer (%s)" % (name, (r.stderr.strip().splitlines() or ["nvcc failed"])[-1])
+        _sanitized[key] = (exe, how)
+    return _sanitized[key]

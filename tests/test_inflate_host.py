@@ -1,42 +1,27 @@
-"""The gzip / DEFLATE decoder of the RecordBatch path (csrc/kta_inflate.cuh) against zlib, on the host: the same
-__host__ __device__ statements log_decompress_kernel runs per warp on the GPU, compiled by nvcc as a plain host program
-(tests/native/inflate_harness.cu), one lane with its own output object.  The warp-cooperative output side (InfWarpOut,
-gzip_walk: lane 0's literals, the 32-lane matches) runs only on the GPU: test_logdecomp_gpu.py compares its output with
-zlib's, over these payloads among others."""
+"""The gzip / DEFLATE decoder of the RecordBatch path (csrc/kta_inflate.cuh) against zlib, on the host: the product's
+gzip_size and gzip_walk, the same __host__ __device__ statements log_unc_size_kernel and log_decompress_kernel run on the GPU,
+compiled by nvcc as a plain host program with the address sanitizer (tests/native/codec_harness.cu, one lane, exact-size
+buffers).  The lane split (lane 0's literals, the 32-lane matches) runs only on the GPU: test_logdecomp_gpu.py compares its
+output with zlib's, over these payloads among others."""
 import gzip
-import os
-import shutil
 import struct
-import subprocess
 import zlib
 
 import numpy as np
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-NVCC = os.environ.get("NVCC") or "/usr/local/cuda/bin/nvcc"
+import codec_harness as ch
+import kafka_codec as kc
 
 
 @pytest.fixture(scope="module")
 def harness(tmp_path_factory):
-    if not (os.path.exists(NVCC) or shutil.which("nvcc")):
-        pytest.skip("nvcc not available")
-    exe = str(tmp_path_factory.mktemp("inflate") / "inflate_harness")
-    subprocess.run([NVCC if os.path.exists(NVCC) else "nvcc", "-O2", "-std=c++17", "-o", exe, os.path.join(HERE, "native", "inflate_harness.cu")],
-                   check=True, capture_output=True)
-    return exe
+    return ch.sanitized(tmp_path_factory)
 
 
 def run_cases(exe, cases):
-    blob = b"".join(struct.pack("<I", len(c)) + c for c in cases)
-    out = subprocess.run([exe], input=blob, capture_output=True, check=True).stdout
-    res, at = [], 0
-    for _ in cases:
-        ok, n = out[at], struct.unpack_from("<I", out, at + 1)[0]
-        res.append((bool(ok), out[at + 5:at + 5 + n]))
-        at += 5 + n
-    assert at == len(out)
-    return res
+    """gzip members → per case (ok, size-pass length, output)"""
+    return ch.run_cases(exe, [(kc.CODEC_BITS["gzip"], c) for c in cases])
 
 
 def gz(data, level=6, strategy=zlib.Z_DEFAULT_STRATEGY, memlevel=8):
@@ -73,8 +58,8 @@ def test_inflate_matches_zlib(harness):
         cases.append(gz(data, 9, memlevel=1))                   # tiny hash table: many small dynamic blocks
         want.append(data)
     got = run_cases(harness, cases)
-    for i, ((ok, out), w) in enumerate(zip(got, want)):
-        assert ok and out == w, i
+    for i, ((ok, size_len, out), w) in enumerate(zip(got, want)):
+        assert ok and size_len == len(w) and out == w, i
 
 
 def test_gzip_header_fields(harness):
@@ -89,8 +74,8 @@ def test_gzip_header_fields(harness):
         b"\x1f\x8b\x08\x08" + bytes(6) + b"name.log\x00" + raw + trailer,
         b"\x1f\x8b\x08\x1e" + bytes(6) + struct.pack("<H", 2) + b"xy" + b"n\x00" + b"comment\x00" + b"\x12\x34" + raw + trailer,
     ]
-    for ok, out in run_cases(harness, cases):
-        assert ok and out == data
+    for ok, size_len, out in run_cases(harness, cases):
+        assert ok and size_len == len(data) and out == data
 
 
 def test_corrupt_streams_fail_cleanly(harness):
@@ -112,8 +97,8 @@ def test_corrupt_streams_fail_cleanly(harness):
         b[int(rng.integers(10, len(good) - 8))] ^= 1 << int(rng.integers(0, 8))
         cases.append(bytes(b))
     res = run_cases(harness, cases)
-    for ok, out in res[:8]:
+    for ok, _, out in res[:8]:
         assert not ok
-    for ok, out in res[8:]:                                     # damage may survive as different bytes; what matters is that the
+    for ok, _, out in res[8:]:                                     # damage may survive as different bytes; what matters is that the
         if ok:                                                  # walk terminates inside its bounds and still honours ISIZE
             assert len(out) == len(data)

@@ -16,6 +16,7 @@ import zlib
 import numpy as np
 import pytest
 
+import codec_harness as ch
 import kafka_codec as kc
 import native_build
 import np_oracle
@@ -28,7 +29,6 @@ from parity import assert_parity
 
 NOW = (4102444800, 123456789)
 LOGB_OK, LOGB_BAD = 0, 2
-BITS = {"gzip": 1, "snappy": 2, "lz4": 3, "zstd": 4}
 STRATEGIES = (zlib.Z_DEFAULT_STRATEGY, zlib.Z_FIXED, zlib.Z_HUFFMAN_ONLY, zlib.Z_RLE, zlib.Z_FILTERED)
 
 
@@ -190,7 +190,7 @@ def host_corpus():
         for codec in ("gzip", "lz4", "snappy", "snappy-xerial"):
             if codec != "gzip" and not data:
                 continue
-            out.append(("lzwalk-%s/%s" % (name, codec), with_section(unc, kc.compress_records(data, codec), lh.CODEC[codec]), unc))
+            out.append(("lzwalk-%s/%s" % (name, codec), with_section(unc, kc.compress_records(data, codec), kc.CODEC_BITS[codec]), unc))
     return out
 
 
@@ -230,7 +230,7 @@ def test_many_batches_per_launch(probe):
                 for _ in range(int(rng.integers(1, 5)))]
         unc = records_batch(recs, base_offset=b * 10)
         codec = codecs[b % len(codecs)]
-        comp = unc if codec is None else with_section(unc, zc.compress_records(unc[61:], codec), zc.CODEC_BITS[codec])
+        comp = unc if codec is None else with_section(unc, zc.compress_records(unc[61:], codec), kc.CODEC_BITS[codec])
         items.append(("batch-%d/%s" % (b, codec), comp, unc, codec))
     got = run_probe(probe, [b"".join(c for _, c, _, _ in items)])[0]
     assert len(got) == len(items)
@@ -243,22 +243,19 @@ def test_many_batches_per_launch(probe):
 def test_damaged_sections_agree_with_the_host_walks(probe):
     """The damaged sections of the host tests (900 zstd frames, 1200 gzip / LZ4 / Snappy sections), once, in one launch: the
     GPU accepts exactly the ones the host walk accepts, with the same bytes.  recordsCount is 0, so that only the walks decide."""
-    zcases = zh.damaged_frames()
-    lcases = lh.damaged_sections()
-    zhost = zh.run_cases(native_build.build("zstd_harness"), zcases)
-    lhost = lh.run_cases(native_build.build("lzwalk_harness"), lcases)
+    cases = [(kc.CODEC_BITS["zstd"], f) for f in zh.damaged_frames()] + lh.damaged_sections()
+    host = ch.run_cases(native_build.build("codec_harness"), cases)
     base = payload_batch(b"")
-    batches = [with_section(base, f, 4) for f in zcases] + [with_section(base, s, c) for c, s in lcases]
-    got = run_probe(probe, [b"".join(batches)])[0]
-    assert len(got) == len(batches)
+    got = run_probe(probe, [b"".join(with_section(base, s, c) for c, s in cases)])[0]
+    assert len(got) == len(cases)
     disagree = []
-    for i, ((ok, _, out), (flags, slot, img)) in enumerate(zip(zhost + lhost, got)):
+    for i, ((ok, _, out), (flags, slot, img)) in enumerate(zip(host, got)):
         assert flags in (LOGB_OK, LOGB_BAD), (i, flags)
         if ok != (flags == LOGB_OK) or (ok and (img[61:] != out or slot != (61 + len(out) + 15) & ~15)):
-            disagree.append((i, "zstd" if i < len(zcases) else "codec %d" % lcases[i - len(zcases)][0], ok, flags, len(out), len(img)))
+            disagree.append((i, "codec %d" % cases[i][0], ok, flags, len(out), len(img)))
     assert not disagree, disagree[:20]
-    assert sum(ok for ok, _, _ in zhost + lhost) > 50          # both outcomes are exercised
-    assert sum(not ok for ok, _, _ in zhost + lhost) > 500
+    assert sum(ok for ok, _, _ in host) > 50          # both outcomes are exercised
+    assert sum(not ok for ok, _, _ in host) > 500
 
 
 @pytest.mark.gpu

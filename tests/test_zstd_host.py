@@ -1,51 +1,29 @@
-"""The zstd walk of the RecordBatch decoder (csrc/kta_zstd.cuh) on the host, compiled by nvcc with the address sanitizer: the
-same statements the GPU runs per warp, against pyarrow's zstd, over hand-assembled frames, and under random damage — a
-damaged section must be rejected or decode to SOMETHING of the size the size pass announced, never read or write outside
-its buffers (the harness allocates input, output and literal buffers at their exact sizes)."""
+"""The zstd walk of the RecordBatch decoder (csrc/kta_zstd.cuh) on the host, compiled by nvcc with the address sanitizer
+(tests/native/codec_harness.cu): the same statements the GPU runs per warp, against pyarrow's zstd, over hand-assembled frames,
+and under random damage — a damaged section must be rejected or decode to SOMETHING of the size the size pass announced, never
+read or write outside its buffers (the harness allocates input, output and literal buffers at their exact sizes)."""
 import collections
-import os
-import shutil
 import struct
-import subprocess
 
 import numpy as np
 import pytest
 
+import codec_harness as ch
 import kafka_codec as kc
 import zstd_codec as zc
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-NVCC = os.environ.get("NVCC") or "/usr/local/cuda/bin/nvcc"
 LEVELS = (-5, 1, 3, 9, 19, 22)
 MAGIC = b"\x28\xb5\x2f\xfd"
 
 
 @pytest.fixture(scope="module")
 def harness(tmp_path_factory):
-    nvcc = NVCC if os.path.exists(NVCC) else shutil.which("nvcc")
-    if not nvcc:
-        pytest.skip("nvcc not available")
-    exe = str(tmp_path_factory.mktemp("zstd") / "zstd_harness")
-    src = os.path.join(HERE, "native", "zstd_harness.cu")
-    r = subprocess.run([nvcc, "-O1", "-g", "-std=c++17", "-Xcompiler", "-fsanitize=address,-fno-omit-frame-pointer", "-o", exe, src],
-                       capture_output=True, text=True)
-    if r.returncode != 0:        # no sanitizer runtime in this toolchain: the plain build still checks the results
-        subprocess.run([nvcc, "-O1", "-std=c++17", "-o", exe, src], check=True, capture_output=True)
-    return exe
+    return ch.sanitized(tmp_path_factory)
 
 
-def run_cases(exe, cases):
-    blob = b"".join(struct.pack("<I", len(d)) + d for d in cases)
-    env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0:protect_shadow_gap=0")
-    r = subprocess.run([exe], input=blob, capture_output=True, env=env)
-    assert r.returncode == 0, r.stderr.decode("utf-8", "replace")[-3000:]
-    out, res, at = r.stdout, [], 0
-    for _ in cases:
-        ok, size_len, n = out[at], *struct.unpack_from("<II", out, at + 1)
-        res.append((bool(ok), size_len, out[at + 9:at + 9 + n]))
-        at += 9 + n
-    assert at == len(out)
-    return res
+def run_cases(exe, frames):
+    """zstd sections → per case (ok, size-pass length, output)"""
+    return ch.run_cases(exe, [(kc.CODEC_BITS["zstd"], f) for f in frames])
 
 
 def sections():

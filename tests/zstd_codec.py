@@ -9,9 +9,6 @@ import struct
 
 import kafka_codec as kc
 
-CODEC_BITS = {None: 0, "gzip": 1, "snappy": 2, "snappy-xerial": 2, "lz4": 3, "zstd": 4, "zstd-stream": 4}
-
-
 def compress_records(recs: bytes, codec: str) -> bytes:
     import pyarrow as pa
     if codec == "zstd":
@@ -35,7 +32,7 @@ def recompress(seg: bytes, pick) -> bytes:
         if codec:
             body = compress_records(body, codec)
             hdr[8:12] = struct.pack(">i", 49 + len(body))
-            hdr[22] |= CODEC_BITS[codec]
+            hdr[22] |= kc.CODEC_BITS[codec]
         out += hdr + body
         pos += 12 + bl
     return bytes(out)
