@@ -87,6 +87,15 @@ def encode_batch(base_offset, base_ts, records, attributes=0, max_ts=None, compr
     return struct.pack(">qi", base_offset, len(after_len)) + after_len
 
 
+def batch_offsets(seg):
+    """where every batch of a segment starts: the walk from batch header to batch header by batchLength"""
+    seg, offs, pos = bytes(seg), [], 0
+    while pos + 61 <= len(seg):
+        offs.append(pos)
+        pos += 12 + int.from_bytes(seg[pos + 8:pos + 12], "big", signed=True)
+    return offs
+
+
 def encode_partition(partition_records, rng, max_batch=40, log_append_time=False, compression=None):
     """partition_records: list of (ts_ms, key|None, value_len|None) in offset order → one log segment (bytes).
     ts_ms == -1 (not available) forces a batch with base timestamp -1."""

@@ -6,8 +6,9 @@ handling as a scan."""
 import numpy as np
 import pytest
 
+from feed import alive_import, engine, unmix32
 from kafka_topic_analyzer_b200 import KtaError
-from test_alive_seen_cache import assert_same_map, dev, engine, exported, unmix32
+from parity import assert_same_map, exported, last_writer
 
 
 def stamped(rng, hashes, copies):
@@ -18,19 +19,9 @@ def stamped(rng, hashes, copies):
     return h, seq
 
 
-def last_writer(h, seq, alive):
-    """Sorted (hash, stamp) arrays: the largest stamp of every hash."""
-    stamp = ((seq + np.uint64(1)) << np.uint64(1)) | alive.astype(np.uint64)
-    order = np.lexsort((stamp, h))
-    h, stamp = h[order], stamp[order]
-    last = np.ones(h.size, dtype=bool)
-    last[:-1] = h[1:] != h[:-1]
-    return h[last], stamp[last]
-
-
 def import_list(e, h, seq, alive):
     stamp = ((seq + np.uint64(1)) << np.uint64(1)) | alive.astype(np.uint64)
-    e.alive_import(dev(h.view(np.int32)), dev(stamp), h.size)
+    alive_import(e, h.view(np.int32), stamp)
 
 
 @pytest.mark.gpu

@@ -10,17 +10,16 @@ pattern, or a run of consecutive x that share a home pair at every table size.""
 import numpy as np
 import pytest
 
-from kafka_topic_analyzer_b200 import KtaEngine, KtaError, synth
+from kafka_topic_analyzer_b200 import KtaError, synth
 from kafka_topic_analyzer_b200.synth import HostTopic, tile_base_from_key_len
+from feed import MASK32, NOW, alive_import, engine, fmix32, gather, push_host, scan, settle, take, unmix32
 from oracle_lib import Oracle, fnv32, olib
-from parity import assert_parity
+from parity import assert_parity, assert_same_map, exported, last_writer
 import np_oracle
 
-NOW = (4102444800, 123456789)   # 2100-01-01: later than every record
-HLL_P = 12
-P = 8
+HLL_P = 12                      # feed.engine's
+P = 8                           # feed.engine's default
 M20 = 1 << 20
-MASK32 = 0xFFFFFFFF
 FNV = 0x811C9DC5                # basis and multiplier of the reference hash (src/fnv32.rs)
 FNV_INV = pow(FNV, -1, 1 << 32)
 
@@ -28,23 +27,6 @@ FNV_INV = pow(FNV, -1, 1 << 32)
 # ------------------------------------------------------------------------------------------------
 # crafted keys
 # ------------------------------------------------------------------------------------------------
-def fmix32(h):
-    h ^= h >> 16
-    h = (h * 0x85EBCA6B) & MASK32
-    h ^= h >> 13
-    h = (h * 0xC2B2AE35) & MASK32
-    return h ^ (h >> 16)
-
-
-def unmix32(x):
-    """fmix32^-1 (the constants of hll_unmix, csrc/kta_kernels.cuh)."""
-    x ^= x >> 16
-    x = (x * 0x7ED1B41D) & MASK32
-    x ^= (x >> 13) ^ (x >> 26)
-    x = (x * 0xA5CB9243) & MASK32
-    return x ^ (x >> 16)
-
-
 _forward = None
 
 
@@ -83,16 +65,6 @@ def keys_for_mixed(xs):
 # ------------------------------------------------------------------------------------------------
 # topics
 # ------------------------------------------------------------------------------------------------
-def _gather(blob, off, lens):
-    """Concatenation of blob[off[i] : off[i] + lens[i]] (lens >= 0)."""
-    lens = lens.astype(np.int64)
-    total = int(lens.sum())
-    if total == 0:
-        return np.zeros(0, dtype=np.uint8)
-    starts = np.repeat(off.astype(np.int64) - (np.cumsum(lens) - lens), lens)
-    return blob[starts + np.arange(total, dtype=np.int64)]
-
-
 def pool_topic(rng, ids, pool, alive):
     """Records whose key is pool[ids[i]] (ids < 0: null key); alive[i] False = tombstone."""
     n = ids.size
@@ -101,20 +73,11 @@ def pool_topic(rng, ids, pool, alive):
     blob = np.frombuffer(b"".join(pool) or b"\0", dtype=np.uint8)
     keyed = ids >= 0
     kl = np.where(keyed, plen[np.maximum(ids, 0)], -1).astype(np.int32)
-    kb = _gather(blob, poff[np.maximum(ids, 0)], np.maximum(kl, 0)).copy()
+    kb = gather(blob, poff[np.maximum(ids, 0)], np.maximum(kl, 0)).copy()
     vl = np.where(alive, rng.integers(0, 300, size=n), -1).astype(np.int32)
     part = rng.integers(0, P, size=n).astype(np.int32)
     ts = (1_600_000_000_000 + rng.integers(-10**6, 10**6, size=n)).astype(np.int64)
     return HostTopic(part, np.zeros(n, dtype=np.int64), ts, kl, vl, np.arange(n, dtype=np.uint64), kb, tile_base_from_key_len(kl))
-
-
-def take(t, idx):
-    """The records idx of t, in that order."""
-    kl0 = np.maximum(t.key_len.astype(np.int64), 0)
-    koff = np.cumsum(kl0) - kl0
-    kl = t.key_len[idx]
-    return HostTopic(t.partition[idx], t.offset[idx], t.ts_ms[idx], kl, t.value_len[idx], t.seq[idx],
-                     _gather(t.key_bytes, koff[idx], kl0[idx]).copy(), tile_base_from_key_len(kl))
 
 
 def filler_pool(rng, count, length=8):
@@ -131,40 +94,7 @@ def last_writer_map(t, seq, keep=None, parts=P):
     m = (t.key_len >= 0) & (t.partition >= 0) & (t.partition < parts)
     if keep is not None:
         m &= keep
-    stamp = ((np.asarray(seq, dtype=np.uint64)[m] + np.uint64(1)) << np.uint64(1)) | (t.value_len[m] >= 0).astype(np.uint64)
-    h = h[m]
-    order = np.lexsort((stamp, h))
-    h, stamp = h[order], stamp[order]
-    last = np.ones(h.size, dtype=bool)
-    last[:-1] = h[1:] != h[:-1]
-    return h[last], stamp[last]
-
-
-def exported(e):
-    import torch
-    n = e.alive_export_count()
-    dh = torch.zeros(max(n, 1), dtype=torch.int32, device="cuda")
-    ds = torch.zeros(max(n, 1), dtype=torch.int64, device="cuda")
-    assert e.alive_export(dh, ds, n) == n
-    h = dh[:n].cpu().numpy().view(np.uint32)
-    s = ds[:n].cpu().numpy().view(np.uint64)
-    order = np.argsort(h, kind="stable")
-    return h[order], s[order]
-
-
-def assert_same_map(got, want):
-    gh, gs = got
-    wh, ws = want
-    if np.array_equal(gh, wh) and np.array_equal(gs, ws):
-        return
-    only_got = np.setdiff1d(gh, wh)
-    only_want = np.setdiff1d(wh, gh)
-    common, gi, wi = np.intersect1d(gh, wh, return_indices=True)
-    bad = np.nonzero(gs[gi] != ws[wi])[0]
-    detail = [(hex(int(common[i])), int(gs[gi[i]]), int(ws[wi[i]])) for i in bad[:5]]
-    raise AssertionError("alive table != last-writer map: %d entries exported, %d expected; %d only exported, %d missing, "
-                         "%d with a different stamp, e.g. (hash, got, want) %s"
-                         % (gh.size, wh.size, only_got.size, only_want.size, bad.size, detail))
+    return last_writer(h[m], np.asarray(seq, dtype=np.uint64)[m], t.value_len[m] >= 0)
 
 
 def oracle_of(*topics):
@@ -181,32 +111,6 @@ def check_exact(e, o, want, parts=P):
     assert_parity(e, o, parts, check_alive=True, hll_regs=o.hll_alive_regs(HLL_P))
     _, occupied, _, _ = e.alive_table_stats()
     assert occupied == want[0].size
-
-
-def engine(**kw):
-    return KtaEngine(P, count_alive_keys=True, hll_precision=HLL_P, now=NOW, **kw)
-
-
-def dev(a):
-    import torch
-    a = np.ascontiguousarray(a)
-    return torch.from_numpy(a.view(np.int64) if a.dtype == np.uint64 else a).cuda()
-
-
-def scan(e, t, seq=None, seq_base=None):
-    """One device batch (columns copied to HBM; the engine keeps them until it is confirmed)."""
-    import torch
-    kb = torch.zeros(t.key_bytes.size + 16, dtype=torch.uint8, device="cuda")
-    if t.key_bytes.size:
-        kb[: t.key_bytes.size] = dev(t.key_bytes)
-    e.scan_batch_device(dev(t.partition), dev(t.ts_ms), dev(t.key_len), dev(t.value_len), key_bytes=kb,
-                        key_bytes_len=int(t.key_bytes.size), key_tile_base=dev(t.key_tile_base),
-                        seq=None if seq is None else dev(np.asarray(seq, dtype=np.uint64)), seq_base=seq_base)
-
-
-def push(e, t, seq=None, seq_base=None):
-    e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, t.key_tile_base,
-                      seq=None if seq is None else np.ascontiguousarray(seq, dtype=np.uint64), seq_base=seq_base)
 
 
 def wave_shift(n):
@@ -419,7 +323,7 @@ def test_explicit_seq_with_the_cache(shape, entry):
         assert int(seq[0]) not in (lo, hi) and int(seq[-1]) not in (lo, hi)
     want = last_writer_map(t, seq)
     with engine() as e:
-        (scan if entry == "device" else push)(e, t, seq=seq)
+        (scan if entry == "device" else push_host)(e, t, seq=seq)
         check_exact(e, oracle_of(take(t, np.argsort(seq, kind="stable"))), want)
 
 
@@ -437,7 +341,7 @@ def test_explicit_seq_outside_the_window(entry):
     seq[out] = np.uint64((1 << 31) + 5) + np.arange(int(out.sum()), dtype=np.uint64)
     want = last_writer_map(t, seq, keep=~out)
     with engine() as e:
-        (scan if entry == "device" else push)(e, t, seq=seq)
+        (scan if entry == "device" else push_host)(e, t, seq=seq)
         with pytest.raises(KtaError) as ei:
             e.finalize()
         assert ei.value.code == 1 and "window" in str(ei.value)
@@ -468,7 +372,7 @@ def test_growth_and_stamps_only_rerun_under_the_cache(entry):
             for lo, hi in zip(cuts[:-1], cuts[1:]):
                 scan(e, take(t, np.arange(lo, hi)))
         else:
-            push(e, t)
+            push_host(e, t)
         check_exact(e, oracle_of(t), want)
         slots, occupied, grows, reruns = e.alive_table_stats()
         assert grows >= 1 and reruns >= 1 and occupied * 10 <= slots * 6
@@ -491,7 +395,7 @@ def test_rebase_under_the_cache():
             t = pool_topic(rng, ids, pool, rng.random(M20) < 0.5)
             o.handle_batch(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes)
             seen |= set(np_oracle.fnv32_many(t.key_len, t.key_bytes)[t.key_len >= 0].tolist())
-            (scan if b % 2 == 0 else push)(e, t, seq_base=base)
+            (scan if b % 2 == 0 else push_host)(e, t, seq_base=base)
             e.finalize()
             assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(HLL_P))
             assert e.alive_table_stats()[1] == len(seen)
@@ -512,7 +416,7 @@ def test_sharded_exact_handles_merge_to_the_whole_topic():
     whole = synth.fill_host(spec)
     o = Oracle(count_alive_keys=True, now=NOW)
     o.handle_batch(whole.partition, whole.ts_ms, whole.key_len, whole.value_len, whole.key_bytes)
-    engines = [KtaEngine(P16, count_alive_keys=True, hll_precision=HLL_P, now=NOW, shard=(r, world)) for r in range(world)]
+    engines = [engine(P16, shard=(r, world)) for r in range(world)]
     try:
         words = engines[0].merge_words(world)
         total = torch.zeros(words, dtype=torch.int64, device="cuda")
@@ -523,18 +427,20 @@ def test_sharded_exact_handles_merge_to_the_whole_topic():
             t = take(whole, idx)
             scan(e, t, seq=whole.seq[idx])
             buf = torch.zeros(words, dtype=torch.int64, device="cuda")
-            e.merge_export(r, world, buf)
-            torch.cuda.synchronize()
+            settle()
+            e.merge_export(r, world, buf)                   # returns once the engine's stream has written buf
             total += buf
             cnt = e.alive_export_count()
             h = torch.zeros(cnt, dtype=torch.int32, device="cuda")
             s = torch.zeros(cnt, dtype=torch.int64, device="cuda")
+            settle()
             assert e.alive_export(h, s, cnt) == cnt
             lists.append((h, s, cnt))
         e0 = engines[0]
+        settle()
         e0.merge_import(world, total)
         for h, s, cnt in lists[1:]:
-            e0.alive_import(h, s, cnt)
+            alive_import(e0, h, s, cnt)
         check_exact(e0, o, last_writer_map(whole, whole.seq, parts=P16), parts=P16)
     finally:
         for e in engines:

@@ -2,42 +2,24 @@
 the same seeded inputs — bit-exact for every counter, sum, histogram bucket, extremum, the alive-key
 count and the HLL registers; HLL *estimate* within 4 sigma of the exact count (sigma = 1.04/sqrt(m)).
 At the full BASELINE sizes parity is checked through size-independent invariants."""
-import ctypes as C
 import json
 import os
 
 import numpy as np
 import pytest
 
-from kafka_topic_analyzer_b200 import KtaEngine, KtaError, Message, TopicAnalyzer, lib, synth
-from kafka_topic_analyzer_b200 import metrics as M
+from kafka_topic_analyzer_b200 import KtaEngine, KtaError, Message, TopicAnalyzer, synth
 from kafka_topic_analyzer_b200 import _native as N
-from oracle_lib import Oracle, fnv32, hll_estimate
-from parity import assert_parity, oracle_for, random_topic
+from kafka_topic_analyzer_b200.synth import HostTopic, tile_base_from_key_len
+from feed import (Topic, capture_hashes, device, feed, fixed_width_topic, push_host, push_records, random_topic, scan,
+                  settle, take, to_device)
+from oracle_lib import Oracle
+from parity import assert_parity, expected, oracle_for, replay_demo_row
 import np_oracle
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 NOW = (4102444800, 123456789)  # 2100-01-01: later than every synthetic record
-
-
-def torch_dev(a, dtype=None):
-    import torch
-    t = torch.from_numpy(np.ascontiguousarray(a).view(np.int64) if a.dtype == np.uint64 else np.ascontiguousarray(a))
-    return t.cuda()
-
-
-def scan_device(engine, t, with_tile_base=True, with_seq=False):
-    import torch
-    cols = dict(partition=torch_dev(t.partition), ts_ms=torch_dev(t.ts_ms), key_len=torch_dev(t.key_len),
-                value_len=torch_dev(t.value_len))
-    kb = torch.zeros(t.key_bytes.size + 16, dtype=torch.uint8, device="cuda")
-    kb[: t.key_bytes.size] = torch_dev(t.key_bytes) if t.key_bytes.size else kb[:0]
-    tb = torch_dev(t.key_tile_base) if with_tile_base else None
-    sq = torch_dev(t.seq) if with_seq else None
-    engine.scan_batch_device(cols["partition"], cols["ts_ms"], cols["key_len"], cols["value_len"], key_bytes=kb,
-                             key_bytes_len=int(t.key_bytes.size), key_tile_base=tb, seq=sq)
-    engine.finalize()
 
 
 # ------------------------------------------------------------------------------------------------
@@ -58,23 +40,13 @@ def test_config0_counters(mode):
     t = synth.fill_host(spec)
     o = oracle_for(t, now=NOW)
     with KtaEngine(4, now=NOW, ring_records=16384) as e:
-        if mode == "device":
-            scan_device(e, t)
-        elif mode == "device_no_tile_base":
-            scan_device(e, t, with_tile_base=False)
-        elif mode == "host_batch":
-            e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, t.key_tile_base)
-            e.finalize()
-        else:
-            off = 0
-            for i in range(0, 30_000):
-                kl = int(t.key_len[i])
-                key = None if kl < 0 else t.key_bytes[off:off + kl].tobytes()
-                off += max(kl, 0)
-                e.push(int(t.partition[i]), int(t.offset[i]), int(t.ts_ms[i]), key, int(t.value_len[i]))
-            e.finalize()
+        if mode == "push":
+            push_records(e, t, 30_000)
             o = Oracle(now=NOW)
             o.handle_batch(t.partition[:30000], t.ts_ms[:30000], t.key_len[:30000], t.value_len[:30000], t.key_bytes)
+        else:
+            feed(e, t, mode)
+        e.finalize()
         assert_parity(e, o, 4)
 
 
@@ -87,7 +59,8 @@ def test_fused_alive_exact_and_hll(key_mode, run_len, P):
     t = synth.fill_host(spec)
     o = oracle_for(t, count_alive_keys=True, now=NOW)
     with KtaEngine(P, count_alive_keys=True, hll_precision=12, now=NOW) as e:
-        scan_device(e, t)
+        scan(e, t)
+        e.finalize()
         assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(12))
         exact = e.alive_keys()
         assert abs(e.alive_keys_hll() - exact) <= max(4 * 1.04 / 64 * exact, 3)
@@ -103,14 +76,12 @@ def test_stress_distributions_hot_keys_and_value_tail(key_mode, P):
                            null_key_per_10k=200, zipf_keys=True, geometric_values=True)
     t = synth.fill_host(spec)
     assert int(t.value_len.max()) > (1 << 16) and int((t.value_len < (1 << 16)).sum()) > n // 2
-    o = oracle_for(t, count_alive_keys=True, now=NOW)
-    with KtaEngine(P, count_alive_keys=True, hll_precision=12, now=NOW) as e:
-        scan_device(e, t)
-        assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(12))
-    os_ = oracle_for(t, track_stream=True, now=NOW)
-    with KtaEngine(P, hll_precision=12, now=NOW) as e:          # in-stream sketch (no -c): the fused bench mode
-        scan_device(e, t)
-        assert_parity(e, os_, P, hll_regs=os_.hll_stream_regs(12))
+    for mode in ("exact", "hll"):                                # hll: the in-stream sketch (no -c), the fused bench mode
+        o, kw = expected(mode, t, 12)
+        with KtaEngine(P, count_alive_keys=mode == "exact", hll_precision=12, now=NOW) as e:
+            scan(e, t)
+            e.finalize()
+            assert_parity(e, o, P, **kw)
 
 
 @pytest.mark.parametrize("seed", [1, 2, 3])
@@ -126,16 +97,9 @@ def test_random_ragged_batches(seed):
             t = random_topic(rng, int(rng.integers(1, 9000)), P, big=True)
             o.handle_batch(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes)
             if b % 2 == 0:
-                e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes,
-                                  t.key_tile_base if b == 0 else None, seq_base=base)
+                push_host(e, t, tile_base=b == 0, seq_base=base)
             else:
-                import torch
-                kb = torch.zeros(t.key_bytes.size + 16, dtype=torch.uint8, device="cuda")
-                if t.key_bytes.size:
-                    kb[: t.key_bytes.size] = torch_dev(t.key_bytes)
-                e.scan_batch_device(torch_dev(t.partition), torch_dev(t.ts_ms), torch_dev(t.key_len),
-                                    torch_dev(t.value_len), key_bytes=kb, key_bytes_len=int(t.key_bytes.size),
-                                    key_tile_base=None, seq_base=base)
+                scan(e, t, tile_base=False, seq_base=base)
             base += t.n
         e.finalize()
         assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(10))
@@ -144,18 +108,11 @@ def test_random_ragged_batches(seed):
 @pytest.mark.parametrize("L", [1, 9, 16, 17, 40, 100, 200])
 def test_fixed_width_keys(L):
     """Fixed-width keys of any length take the ballot-offset path (16-byte aligned ones the LDS.128 path)."""
-    from kafka_topic_analyzer_b200.synth import HostTopic, tile_base_from_key_len
-    rng = np.random.default_rng(L)
-    n = 20_000
-    kl = np.where(rng.random(n) < 0.03, -1, L).astype(np.int32)
-    pool = rng.integers(0, 256, size=(500, L), dtype=np.uint8)
-    kb = pool[rng.integers(0, 500, size=int((kl >= 0).sum()))].reshape(-1)
-    t = HostTopic(rng.integers(0, 5, size=n).astype(np.int32), np.zeros(n, dtype=np.int64),
-                  (1_600_000_000_000 + np.arange(n)).astype(np.int64), kl, rng.integers(-1, 300, size=n).astype(np.int32),
-                  np.arange(n, dtype=np.uint64), kb, tile_base_from_key_len(kl))
+    t = fixed_width_topic(np.random.default_rng(L), 20_000, 5, L, 0.03, 500)
     o = oracle_for(t, count_alive_keys=True, now=NOW)
     with KtaEngine(5, count_alive_keys=True, hll_precision=9, now=NOW) as e:
-        scan_device(e, t)
+        scan(e, t)
+        e.finalize()
         assert_parity(e, o, 5, check_alive=True, hll_regs=o.hll_alive_regs(9))
 
 
@@ -167,9 +124,10 @@ def test_hash_capture_matches_oracle_per_record():
     want = np_oracle.fnv32_many(t.key_len, t.key_bytes)
     with KtaEngine(3, hll_precision=8, now=NOW) as e:
         out = torch.full((t.n,), 0xFFFFFFFF, dtype=torch.int64, device="cuda").to(torch.int32)
-        lib().kta_set_hash_capture(e.handle, out.data_ptr())
-        scan_device(e, t)
-        lib().kta_set_hash_capture(e.handle, None)
+        capture_hashes(e, out)
+        scan(e, t)
+        e.finalize()
+        capture_hashes(e, None)
         got = out.cpu().numpy().view(np.uint32)
     assert np.array_equal(got, want)
 
@@ -180,7 +138,8 @@ def test_hll_in_stream_registers():
     t = synth.fill_host(spec)
     o = oracle_for(t, track_stream=True, now=NOW)
     with KtaEngine(64, hll_precision=14, now=NOW) as e:
-        scan_device(e, t)
+        scan(e, t)
+        e.finalize()
         assert_parity(e, o, 64, hll_regs=o.hll_stream_regs(14))
         distinct = len(set(np_oracle.fnv32_many(t.key_len, t.key_bytes)[(t.key_len >= 0) & (t.value_len >= 0)].tolist()))
         assert abs(e.alive_keys_hll() - distinct) <= 4 * 1.04 / 128 * distinct
@@ -219,13 +178,14 @@ def test_reset_forgets_the_alive_table():
     with KtaEngine(8, count_alive_keys=True, hll_precision=10, now=NOW) as e:
         for t in (ta, tb, ta):
             e.reset()
-            scan_device(e, t)
+            scan(e, t)
+            e.finalize()
             o = oracle_for(t, count_alive_keys=True, now=NOW)
             assert_parity(e, o, 8, check_alive=True, hll_regs=o.hll_alive_regs(10))
         # and without a reset the second topic continues the first (seq keeps counting)
         e.reset()
-        e.push_batch_host(ta.partition, ta.ts_ms, ta.key_len, ta.value_len, ta.key_bytes, ta.key_tile_base, seq_base=0)
-        e.push_batch_host(tb.partition, tb.ts_ms, tb.key_len, tb.value_len, tb.key_bytes, tb.key_tile_base, seq_base=ta.n)
+        push_host(e, ta, seq_base=0)
+        push_host(e, tb, seq_base=ta.n)
         e.finalize()
         o = Oracle(count_alive_keys=True, now=NOW)
         o.handle_batch(ta.partition, ta.ts_ms, ta.key_len, ta.value_len, ta.key_bytes)
@@ -251,7 +211,7 @@ def test_byte_sums_survive_u32_wraparound(layout):
     kl = torch.full((n,), klv, dtype=torch.int32, device="cuda")
     vl = torch.full((n,), vlv, dtype=torch.int32, device="cuda")
     with KtaEngine(P, now=NOW) as e:
-        e.scan_batch_device(part, ts, kl, vl)
+        scan(e, Topic(part, ts, kl, vl, None, 0), tile_base=False)
         e.finalize()
         mm = e.message_metrics
         for p in range(P):
@@ -281,7 +241,7 @@ def test_timestamp_extrema_across_high_word_boundaries(case):
     o = Oracle(now=NOW)
     o.handle_batch(part, ts, kl, vl, np.zeros(0, dtype=np.uint8))
     with KtaEngine(P, now=NOW) as e:
-        e.scan_batch_device(torch_dev(part), torch_dev(ts), torch_dev(kl), torch_dev(vl))
+        scan(e, Topic(*(device(c) for c in (part, ts, kl, vl)), None, 0), tile_base=False)
         e.finalize()
         assert_parity(e, o, P)
         mm = e.message_metrics
@@ -311,23 +271,17 @@ def test_out_of_range_partitions_are_left_out_of_every_metric():
     ts, vl = t.ts_ms.copy(), t.value_len.copy()
     ts[badp] = np.where(rng.random(int(badp.sum())) < 0.5, 1, 4_000_000_000_000)
     vl[badp] = (1 << 31) - 1
-    from kafka_topic_analyzer_b200.synth import HostTopic
     tb = HostTopic(part, t.offset, ts, t.key_len, vl, t.seq, t.key_bytes, t.key_tile_base)
     # oracle: the in-range records only, in order
-    good = ~badp
-    kl0 = np.maximum(t.key_len, 0).astype(np.int64)
-    koff = np.concatenate([[0], np.cumsum(kl0)])
-    keep = np.concatenate([t.key_bytes[koff[i]:koff[i + 1]] for i in np.nonzero(good)[0]] or [np.zeros(0, np.uint8)])
-    o = Oracle(count_alive_keys=True, now=NOW)
-    o.handle_batch(part[good], ts[good], t.key_len[good], vl[good], keep.astype(np.uint8))
+    o = oracle_for(take(tb, np.nonzero(~badp)[0]), count_alive_keys=True, now=NOW)
     for mode in ("device", "host"):
         with KtaEngine(P, count_alive_keys=True, hll_precision=10, now=NOW, ring_records=8192) as e:
             with pytest.raises(KtaError) as ei:
                 if mode == "device":
-                    scan_device(e, tb)
+                    scan(e, tb)
                 else:
-                    e.push_batch_host(tb.partition, tb.ts_ms, tb.key_len, tb.value_len, tb.key_bytes, None)
-                    e.finalize()
+                    push_host(e, tb, tile_base=False)
+                e.finalize()
             assert ei.value.code == 4
             assert e.bad_partition_records() == int(badp.sum())
             assert e.finalize(strict=False) == int(badp.sum())     # the same as a warning: the count, no exception
@@ -347,32 +301,17 @@ def test_alive_table_grows_and_restamps(mode):
     o = oracle_for(t, count_alive_keys=True, now=NOW)
     with KtaEngine(P, count_alive_keys=True, hll_precision=11, now=NOW, ring_records=4096, alive_table_kib=1) as e:
         assert e.alive_table_stats()[0] == 128
-        if mode == "device":
-            scan_device(e, t)
-        elif mode == "host_batch":
-            e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, t.key_tile_base)   # 30 ring chunks
-            e.finalize()
-        elif mode == "push":
-            off = 0
-            for i in range(n):
-                kl = int(t.key_len[i])
-                key = None if kl < 0 else t.key_bytes[off:off + kl].tobytes()
-                off += max(kl, 0)
-                e.push(int(t.partition[i]), int(t.offset[i]), int(t.ts_ms[i]), key, int(t.value_len[i]))
-            e.finalize()
+        if mode != "device_batches":
+            feed(e, t, mode)                                # host_batch: 30 ring chunks
         else:
             # several device batches queued before the first confirmation: all of them are re-run
-            import torch
             T = N.KTA_KEY_TILE
-            kb = torch.zeros(t.key_bytes.size + 16, dtype=torch.uint8, device="cuda")
-            kb[: t.key_bytes.size] = torch_dev(t.key_bytes)
-            cols = [torch_dev(c) for c in (t.partition, t.ts_ms, t.key_len, t.value_len)]
-            tb = torch_dev(t.key_tile_base)
+            d = to_device(t)
             cuts = [0, 40 * T, 300 * T, 301 * T, n]
             for lo, hi in zip(cuts[:-1], cuts[1:]):
-                e.scan_batch_device(*[c[lo:hi] for c in cols], key_bytes=kb, key_bytes_len=int(t.key_bytes.size),
-                                    key_tile_base=tb[lo // T:])
-            e.finalize()
+                scan(e, Topic(*(c[lo:hi] for c in (d.partition, d.ts_ms, d.key_len, d.value_len)), d.key_bytes, d.kbl,
+                              key_tile_base=d.key_tile_base[lo // T:]))
+        e.finalize()
         slots, occupied, grows, reruns = e.alive_table_stats()
         assert grows >= 1 and reruns >= 1 and occupied * 10 <= slots * 7
         distinct = len(set(np_oracle.fnv32_many(t.key_len, t.key_bytes)[t.key_len >= 0].tolist()))
@@ -380,7 +319,7 @@ def test_alive_table_grows_and_restamps(mode):
         assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(11))
         # and the grown table keeps working: the same topic again (new sequence numbers) changes nothing but the counters
         before = e.alive_keys()
-        e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, t.key_tile_base)
+        push_host(e, t)
         e.finalize()
         assert e.alive_keys() == before and e.message_metrics.overall_count() == 2 * n
 
@@ -397,19 +336,15 @@ def test_alive_table_rebase_keeps_last_writer_across_the_seq_window():
             t = random_topic(rng, 6000, P, max_key=6)      # short keys: plenty of overwrites between batches
             o.handle_batch(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes)
             if b % 2:
-                e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, t.key_tile_base, seq_base=base)
+                push_host(e, t, seq_base=base)
             else:
-                import torch
-                kb = torch.zeros(t.key_bytes.size + 16, dtype=torch.uint8, device="cuda")
-                kb[: t.key_bytes.size] = torch_dev(t.key_bytes)
-                e.scan_batch_device(torch_dev(t.partition), torch_dev(t.ts_ms), torch_dev(t.key_len), torch_dev(t.value_len),
-                                    key_bytes=kb, key_bytes_len=int(t.key_bytes.size), seq_base=base)
+                scan(e, t, tile_base=False, seq_base=base)
             e.finalize()
             assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(9))
         # a batch that goes back before the window: refused, state untouched
         t = random_topic(rng, 100, P)
         with pytest.raises(KtaError) as ei:
-            e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, t.key_tile_base, seq_base=5)
+            push_host(e, t, seq_base=5)
         assert ei.value.code == 1
         e.finalize()
         assert_parity(e, o, P, check_alive=True)
@@ -429,23 +364,18 @@ def test_seq_contract():
             t = random_topic(rng, 3000, P, max_key=5)
             o.handle_batch(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes)
             if b == 1:     # per-record pushes in between: the batches after them must count on from there
-                off = 0
-                for i in range(t.n):
-                    kl = int(t.key_len[i])
-                    e.push(int(t.partition[i]), 0, int(t.ts_ms[i]), None if kl < 0 else t.key_bytes[off:off + kl].tobytes(),
-                           int(t.value_len[i]))
-                    off += max(kl, 0)
+                push_records(e, t)
             else:
-                e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, t.key_tile_base)   # seq_base=None
+                push_host(e, t)                             # seq_base=None
         e.finalize()
         assert_parity(e, o, P, check_alive=True)
         t = random_topic(rng, 500, P)
         with pytest.raises(KtaError) as ei:
-            e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, t.key_tile_base, seq_base=0)
+            push_host(e, t, seq_base=0)
         assert ei.value.code == 1 and "seq_base" in str(ei.value)
         # explicit seq outside the window: reported by finalize, the offending records are left out of the table
         seq = np.arange(t.n, dtype=np.uint64) + np.uint64((1 << 31) + 10)
-        e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, t.key_tile_base, seq=seq)
+        push_host(e, t, seq=seq)
         with pytest.raises(KtaError) as ei:
             e.finalize()
         assert ei.value.code == 1 and "window" in str(ei.value)
@@ -455,26 +385,18 @@ def test_seq_contract():
 def test_host_batch_whose_keys_exceed_the_staging_ring(L, with_tile_base):
     """kta_push_batch_host splits a batch into chunks whose key bytes fit ring_key_bytes; tiles heavier than 64 B per
     record used to trip the split (ADVICE r1).  Fixed-length L-byte keys, total far above the ring's key capacity."""
-    from kafka_topic_analyzer_b200.synth import HostTopic, tile_base_from_key_len
-    rng = np.random.default_rng(L)
-    n = 40_000 if L < 10_000 else 1500
-    kl = np.where(rng.random(n) < 0.02, -1, L).astype(np.int32)
-    pool = rng.integers(0, 256, size=(300, L), dtype=np.uint8)
-    kb = pool[rng.integers(0, 300, size=int((kl >= 0).sum()))].reshape(-1)
-    t = HostTopic(rng.integers(0, 4, size=n).astype(np.int32), np.zeros(n, dtype=np.int64),
-                  (1_600_000_000_000 + np.arange(n)).astype(np.int64), kl, rng.integers(-1, 300, size=n).astype(np.int32),
-                  np.arange(n, dtype=np.uint64), kb, tile_base_from_key_len(kl))
+    t = fixed_width_topic(np.random.default_rng(L), 40_000 if L < 10_000 else 1500, 4, L, 0.02, 300)
     o = oracle_for(t, count_alive_keys=True, now=NOW)
     ring_kb = 1 << 20 if L < 10_000 else 6 << 20       # one 128-record tile of 40 KB keys is 5 MB
-    assert kb.size > 4 * ring_kb
+    assert t.key_bytes.size > 4 * ring_kb
     with KtaEngine(4, count_alive_keys=True, now=NOW, ring_records=16384, ring_key_bytes=ring_kb) as e:
-        e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, t.key_tile_base if with_tile_base else None)
+        push_host(e, t, tile_base=with_tile_base)
         e.finalize()
         assert_parity(e, o, 4, check_alive=True)
     # a single tile that cannot fit is the one case that is refused, and it says so
     with KtaEngine(4, count_alive_keys=True, now=NOW, ring_records=16384, ring_key_bytes=100 * L) as e:
         with pytest.raises(KtaError) as ei:
-            e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, None)
+            push_host(e, t, tile_base=False)
         assert ei.value.code == 1 and "ring_key_bytes" in str(ei.value)
 
 
@@ -482,7 +404,6 @@ def test_long_keys_fall_back_to_global_reads():
     """A tile whose keys exceed the 20 KiB staging buffer takes the direct-global path; results equal."""
     rng = np.random.default_rng(5)
     n = 3000
-    from kafka_topic_analyzer_b200.synth import HostTopic, tile_base_from_key_len
     kl = rng.integers(0, 300, size=n).astype(np.int32)
     kl[100] = 70_000
     kb = rng.integers(0, 256, size=int(np.maximum(kl, 0).sum()), dtype=np.uint8)
@@ -491,10 +412,11 @@ def test_long_keys_fall_back_to_global_reads():
                   np.arange(n, dtype=np.uint64), kb, tile_base_from_key_len(kl))
     o = oracle_for(t, count_alive_keys=True, now=NOW)
     with KtaEngine(3, count_alive_keys=True, now=NOW, ring_key_bytes=1 << 20) as e:
-        scan_device(e, t)
+        scan(e, t)
+        e.finalize()
         assert_parity(e, o, 3, check_alive=True)
         e.reset()
-        e.push_batch_host(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes, None)
+        push_host(e, t, tile_base=False)
         e.finalize()
         assert_parity(e, o, 3, check_alive=True)
 
@@ -516,13 +438,10 @@ def test_topic_analyzer_interface():
 
 def test_demo_output_row8_replay_on_gpu():
     """Row 8 of demo_output.png replayed through the GPU path: 20 021 871 records."""
-    from test_oracle_golden import replay_demo_row
     demo = json.load(open(os.path.join(GOLD, "demo_output.json")))
     row = demo["rows"][8]
     with KtaEngine(10, now=NOW) as e:
-        def feed(part, ts, kl, vl):
-            e.push_batch_host(part, ts, kl, vl)
-        replay_demo_row(row, demo, feed)
+        replay_demo_row(row, demo, lambda part, ts, kl, vl: e.push_batch_host(part, ts, kl, vl))
         e.finalize()
         mm = e.message_metrics
         assert (mm.total(8), mm.alive(8), mm.tombstones(8), mm.key_null(8)) == (row["total"], row["alive"], 0, 0)
@@ -598,11 +517,11 @@ def test_alive_keys_large_vs_exact_set():
     topic = synth.DeviceTopic(spec)
     hashes = torch.empty(n, dtype=torch.int32, device="cuda")
     with KtaEngine(P, count_alive_keys=True, hll_precision=14, now=NOW) as e:
-        lib().kta_set_hash_capture(e.handle, hashes.data_ptr())
+        capture_hashes(e, hashes)
         e.scan_batch_device(topic.partition, topic.ts_ms, topic.key_len, topic.value_len, key_bytes=topic.key_bytes,
                             key_bytes_len=topic.key_bytes_len, key_tile_base=topic.key_tile_base)
         e.finalize()
-        lib().kta_set_hash_capture(e.handle, None)
+        capture_hashes(e, None)
         got = e.alive_keys()
         est = e.alive_keys_hll()
     want, _ = _alive_by_sort(hashes, topic.value_len, None)
@@ -640,11 +559,11 @@ def test_config2_full_size_alive_exact():
     topic = synth.DeviceTopic(spec)
     hashes = torch.empty(n, dtype=torch.int32, device="cuda")
     with KtaEngine(P, count_alive_keys=True, hll_precision=14, now=NOW) as e:
-        lib().kta_set_hash_capture(e.handle, hashes.data_ptr())
+        capture_hashes(e, hashes)
         e.scan_batch_device(topic.partition, topic.ts_ms, topic.key_len, topic.value_len, key_bytes=topic.key_bytes,
                             key_bytes_len=topic.key_bytes_len, key_tile_base=topic.key_tile_base)
         e.finalize()
-        lib().kta_set_hash_capture(e.handle, None)
+        capture_hashes(e, None)
         got, est = e.alive_keys(), e.alive_keys_hll()
         slots, occupied, grows, reruns = e.alive_table_stats()
         assert e.message_metrics.overall_count() == n
@@ -715,23 +634,17 @@ def test_partition_sharded_engines_merge_to_the_whole_topic(P, world, run_len):
         total = torch.zeros(words, dtype=torch.int64, device="cuda")
         for r, e in enumerate(engines):
             # shard r of the topic = the records whose partition is r mod world, in seq order
-            sel = (whole.partition % world) == r
-            kl0 = np.maximum(whole.key_len, 0).astype(np.int64)
-            koff = np.concatenate([[0], np.cumsum(kl0)])
-            idx = np.nonzero(sel)[0]
-            kb = np.concatenate([whole.key_bytes[koff[i]:koff[i + 1]] for i in idx] or [np.zeros(0, np.uint8)]).astype(np.uint8)
-            from kafka_topic_analyzer_b200.synth import HostTopic, tile_base_from_key_len
-            t = HostTopic(whole.partition[sel], whole.offset[sel], whole.ts_ms[sel], whole.key_len[sel], whole.value_len[sel],
-                          whole.seq[sel], kb, tile_base_from_key_len(whole.key_len[sel]))
-            scan_device(e, t)
+            scan(e, take(whole, np.nonzero(whole.partition % world == r)[0]))
+            e.finalize()
             # the shard alone: its own partitions as the oracle sees them, the others untouched
             mm = e.message_metrics
             for p in range(P):
                 assert mm.total(p) == (o.counter("total", p) if p % world == r else 0)
             buf = torch.zeros(words, dtype=torch.int64, device="cuda")
-            e.merge_export(r, world, buf)
-            torch.cuda.synchronize()
+            settle()
+            e.merge_export(r, world, buf)                   # returns once the engine's stream has written buf
             total += buf
+        settle()
         engines[0].merge_import(world, total)
         engines[0].finalize()
         assert_parity(engines[0], o, P, hll_regs=o.hll_stream_regs(11))

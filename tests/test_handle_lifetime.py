@@ -5,11 +5,13 @@ import shutil
 import subprocess
 import sys
 
+import numpy as np
 import pytest
 
+import kafka_codec as kc
+from feed import NOW, partition_lists
 from kafka_topic_analyzer_b200 import KtaEngine, lib, synth
-from parity import assert_parity
-from test_logdecode import NOW, _oracle_over, _partition_lists
+from parity import assert_parity, oracle_over
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -40,11 +42,7 @@ def test_destroy_releases_everything_the_handle_allocated():
 
 
 def _longest_batch(seg):
-    raw, pos, longest = seg.tobytes(), 0, 0
-    while pos + 12 <= len(raw):
-        n = 12 + int.from_bytes(raw[pos + 8:pos + 12], "big", signed=True)
-        longest, pos = max(longest, n), pos + n
-    return longest
+    return int(np.diff(kc.batch_offsets(seg) + [seg.size]).max())
 
 
 @pytest.mark.gpu
@@ -56,7 +54,7 @@ def test_log_decode_on_two_devices_in_one_process():
     segs = [(p, synth.encode_segment(spec, p, batch_records=100)) for p in range(P)]
     # batches of about 16 KB are staged, and 4 warps' stages of >= 12 KiB need the opt-in shared memory
     assert 12 * 1024 <= max(_longest_batch(s) for _, s in segs) <= 40 * 1024
-    o = _oracle_over(_partition_lists(synth.fill_host(spec)), count_alive_keys=True)
+    o = oracle_over(partition_lists(synth.fill_host(spec)), count_alive_keys=True)
     for device in (0, 1):
         with KtaEngine(P, count_alive_keys=True, hll_precision=10, device=device, now=NOW) as e:
             assert e.push_log_segments(segs) == spec.n_total

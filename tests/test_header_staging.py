@@ -4,23 +4,20 @@ pointers in each mode, must match the CPU oracle both times."""
 import numpy as np
 import pytest
 
+from feed import device, fixed_width_topic, scan, to_device
 from kafka_topic_analyzer_b200 import KtaEngine, synth
-from parity import assert_parity, oracle_for
+from parity import assert_parity, expected
 
 pytestmark = pytest.mark.gpu
 NOW = (4102444800, 123456789)
 P = 16
 
 
-def _column(a, shift):
-    """`a` on the device, starting `shift` elements into a 16-byte-aligned allocation."""
-    import torch
-    src = torch.from_numpy(np.ascontiguousarray(a))
-    buf = torch.zeros(a.size + 4, dtype=src.dtype, device="cuda")
-    col = buf[shift:shift + a.size]
-    col.copy_(src)
-    assert (buf.data_ptr() % 16 == 0) and ((col.data_ptr() % 16 == 0) == (shift == 0))
-    return col
+def scan_from(e, t, shift):
+    """t's header columns from `shift` elements past a 16-byte-aligned base, its keys and tile bases as they are"""
+    d = to_device(t)
+    scan(e, d, cols=[device(c, shift) for c in (t.partition, t.ts_ms, t.key_len, t.value_len)])
+    e.finalize()
 
 
 @pytest.fixture(scope="module")
@@ -34,23 +31,9 @@ def topic():
 @pytest.mark.parametrize("shift", [0, 1])
 @pytest.mark.parametrize("mode", ["counters", "hll", "alive"])
 def test_scan_from_aligned_and_misaligned_columns(topic, mode, shift):
-    import torch
-    t = topic
-    kb = torch.zeros(t.key_bytes.size + 16, dtype=torch.uint8, device="cuda")
-    kb[: t.key_bytes.size] = torch.from_numpy(t.key_bytes)
-    tb = torch.from_numpy(t.key_tile_base.view(np.int64)).cuda()
-    if mode == "counters":
-        engine, o, kw = KtaEngine(P, now=NOW), oracle_for(t, now=NOW), {}
-    elif mode == "hll":
-        o = oracle_for(t, track_stream=True, now=NOW)
-        engine, kw = KtaEngine(P, hll_precision=12, now=NOW), dict(hll_regs=o.hll_stream_regs(12))
-    else:
-        o = oracle_for(t, count_alive_keys=True, now=NOW)
-        engine, kw = KtaEngine(P, count_alive_keys=True, hll_precision=12, now=NOW), dict(check_alive=True, hll_regs=o.hll_alive_regs(12))
-    with engine as e:
-        e.scan_batch_device(_column(t.partition, shift), _column(t.ts_ms, shift), _column(t.key_len, shift),
-                            _column(t.value_len, shift), key_bytes=kb, key_bytes_len=int(t.key_bytes.size), key_tile_base=tb)
-        e.finalize()
+    o, kw = expected({"alive": "exact"}.get(mode, mode), topic, 12)
+    with KtaEngine(P, count_alive_keys=mode == "alive", hll_precision=0 if mode == "counters" else 12, now=NOW) as e:
+        scan_from(e, topic, shift)
         assert_parity(e, o, P, **kw)
 
 
@@ -59,24 +42,9 @@ def test_launch_shapes_for_many_partitions_and_long_keys(P, L):
     """Shapes away from the 12 warps x 3 stages of 16-byte keys on 64 partitions: the counter rows of 512 partitions leave
     room for key-only stages only, 700 partitions keep their counters in global memory, 36- and 64-byte keys need larger
     key stages (2 stages with headers, or keys only).  Both hashing modes, vs the oracle."""
-    from kafka_topic_analyzer_b200.synth import HostTopic, tile_base_from_key_len
-    import torch
-    rng = np.random.default_rng(P * 100 + L)
-    n = 40_000 + 37
-    kl = np.where(rng.random(n) < 0.02, -1, L).astype(np.int32)
-    pool = rng.integers(0, 256, size=(3000, L), dtype=np.uint8)
-    kb = pool[rng.integers(0, 3000, size=int((kl >= 0).sum()))].reshape(-1)
-    t = HostTopic(rng.integers(0, P, size=n).astype(np.int32), np.zeros(n, dtype=np.int64),
-                  (1_600_000_000_000 + np.arange(n)).astype(np.int64), kl, rng.integers(-1, 300, size=n).astype(np.int32),
-                  np.arange(n, dtype=np.uint64), kb, tile_base_from_key_len(kl))
-    keys = torch.zeros(kb.size + 16, dtype=torch.uint8, device="cuda")
-    keys[: kb.size] = torch.from_numpy(kb)
-    tb = torch.from_numpy(t.key_tile_base.view(np.int64)).cuda()
-    for alive in (False, True):
-        o = oracle_for(t, count_alive_keys=alive, track_stream=not alive, now=NOW)
-        regs = o.hll_alive_regs(12) if alive else o.hll_stream_regs(12)
-        with KtaEngine(P, count_alive_keys=alive, hll_precision=12, now=NOW) as e:
-            e.scan_batch_device(_column(t.partition, 0), _column(t.ts_ms, 0), _column(t.key_len, 0), _column(t.value_len, 0),
-                                key_bytes=keys, key_bytes_len=int(kb.size), key_tile_base=tb)
-            e.finalize()
-            assert_parity(e, o, P, check_alive=alive, hll_regs=regs)
+    t = fixed_width_topic(np.random.default_rng(P * 100 + L), 40_000 + 37, P, L, 0.02, 3000)
+    for mode in ("hll", "exact"):
+        o, kw = expected(mode, t, 12)
+        with KtaEngine(P, count_alive_keys=mode == "exact", hll_precision=12, now=NOW) as e:
+            scan_from(e, t, 0)
+            assert_parity(e, o, P, **kw)

@@ -14,6 +14,7 @@ import numpy as np
 import pytest
 
 import kafka_codec as kc
+from feed import scan_log_batches, scan_log_segment, stage_batches
 from kafka_topic_analyzer_b200 import KtaEngine, KtaError
 from oracle_lib import Oracle
 from parity import assert_parity
@@ -299,31 +300,9 @@ def _interleaved(t):
     return out
 
 
-def _device_buffer(batches):
-    import torch
-    offs, at = [], 0
-    for b in batches:
-        offs.append(at)
-        at += len(b.raw)
-    buf = torch.from_numpy(np.frombuffer(b"".join(b.raw for b in batches), dtype=np.uint8).copy()).cuda()
-    return (buf, at, torch.tensor(offs, dtype=torch.int64).cuda(), torch.tensor([b.p for b in batches], dtype=torch.int32).cuda(),
-            len(batches))
-
-
-def _scan_segment_device(e, p, seg: bytes):
-    import ctypes as C
-    import torch
-    from kafka_topic_analyzer_b200._native import check, lib
-    offs, pos = [], 0
-    while pos + 61 <= len(seg):
-        offs.append(pos)
-        pos += 12 + int.from_bytes(seg[pos + 8:pos + 12], "big", signed=True)
-    buf = torch.from_numpy(np.frombuffer(seg, dtype=np.uint8).copy()).cuda()
-    d_off = torch.tensor(offs, dtype=torch.int64).cuda()
-    n = C.c_int64()
-    check(lib().kta_scan_log_segment_device(e.handle, p, buf.data_ptr(), len(seg), d_off.data_ptr(), len(offs), C.byref(n)))
-    e.sync()
-    return n.value
+def _staged(batches):
+    """Bt batches, in this order, in one device buffer"""
+    return stage_batches([(b.p, b.raw) for b in batches])
 
 
 @pytest.mark.gpu
@@ -350,9 +329,9 @@ def test_four_entry_points(entry):
                 total = e.push_log_segments([(p, t.segment(p)) for p in range(P)])
             elif entry == "segment_device":
                 for p in range(P):
-                    total += _scan_segment_device(e, p, t.segment(p))
+                    total += scan_log_segment(e, p, t.segment(p))
             else:
-                total = e.scan_log_batches_device(*_device_buffer(calls[0]))
+                total = scan_log_batches(e, _staged(calls[0]))
             e.finalize()
             exp = want if level == "read_committed" else _all_records(calls)
             o = _oracle(exp)
@@ -531,7 +510,7 @@ def test_many_transactional_batches_in_one_call():
     assert sum(1 for _, (raw, _r) in inter if raw[22] == 0x10) == 1 << 17
     want = [(p, rec) for p, (_, rec) in inter if rec is not None]
     with KtaEngine(P, count_alive_keys=True, now=NOW, isolation_level="read_committed") as e:
-        n = e.scan_log_batches_device(*_device_buffer([Bt(p, 0, 0, 0, None, raw=raw) for p, (raw, _) in inter]))
+        n = scan_log_batches(e, stage_batches([(p, raw) for p, (raw, _) in inter]))
         e.finalize()
         assert n == len(want)
         assert e.log_txn_stats() == (n_ab, n_ab, 0)

@@ -3,9 +3,10 @@ with the same records (what librdkafka would have delivered message by message).
 import numpy as np
 import pytest
 
+from feed import partition_lists, scan_log_batches, scan_log_segment, stage_batches
 from kafka_topic_analyzer_b200 import KtaEngine, KtaError, synth
 from oracle_lib import Oracle
-from parity import assert_parity
+from parity import assert_parity, expected, oracle_over
 import kafka_codec as kc
 
 NOW = (4102444800, 123456789)
@@ -31,26 +32,6 @@ def test_smallest_record_is_seven_bytes():
     assert count == 100 and count * 7 + 49 == batch_len == len(b) - 12
 
 
-def _partition_lists(t):
-    """per-partition record lists (ts, key, value_len) in offset order, from a HostTopic"""
-    kl = t.key_len
-    koff = np.concatenate([[0], np.cumsum(np.maximum(kl, 0))])
-    per = {}
-    for i in range(t.n):
-        key = None if kl[i] < 0 else t.key_bytes[koff[i]:koff[i] + kl[i]].tobytes()
-        vl = None if t.value_len[i] < 0 else int(t.value_len[i])
-        per.setdefault(int(t.partition[i]), []).append((int(t.ts_ms[i]), key, vl))
-    return per
-
-
-def _oracle_over(per, **kw):
-    o = Oracle(now=NOW, **kw)
-    for p in sorted(per):
-        for ts, key, vl in per[p]:
-            o.handle_message(p, None if ts == -1 else ts, key, vl)
-    return o
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("key_mode,exact", [(0, True), (2, True), (1, False)])
 def test_segments_decode_and_scan(key_mode, exact):
@@ -58,8 +39,8 @@ def test_segments_decode_and_scan(key_mode, exact):
     P = 6
     spec = synth.make_spec(P * 1500, P, key_mode=key_mode, distinct_keys=600, tombstone_per_10k=2000, null_key_per_10k=400,
                            ts_missing_per_10k=300, empty_value_per_10k=200, value_mean=40)
-    per = _partition_lists(synth.fill_host(spec))
-    o = _oracle_over(per, count_alive_keys=exact, track_stream=not exact)
+    per = partition_lists(synth.fill_host(spec))
+    o, kw = expected("exact" if exact else "hll", per, 10)
     with KtaEngine(P, count_alive_keys=exact, hll_precision=10, now=NOW) as e:
         total = 0
         for p in sorted(per):
@@ -67,7 +48,7 @@ def test_segments_decode_and_scan(key_mode, exact):
             total += e.push_log_segment(p, seg + b"\x00" * 17)      # + a truncated tail, as in a partial fetch
         e.finalize()
         assert total == spec.n_total
-        assert_parity(e, o, P, check_alive=exact, hll_regs=o.hll_alive_regs(10) if exact else o.hll_stream_regs(10))
+        assert_parity(e, o, P, **kw)
 
 
 @pytest.mark.gpu
@@ -127,7 +108,7 @@ def test_cli_log_dir(tmp_path):
     rng = np.random.default_rng(21)
     P = 3
     spec = synth.make_spec(P * 2000, P, key_mode=1, distinct_keys=300, tombstone_per_10k=3000, value_mean=30)
-    per = _partition_lists(synth.fill_host(spec))
+    per = partition_lists(synth.fill_host(spec))
     for p, recs in per.items():
         d = tmp_path / ("orders-%d" % p)
         d.mkdir()
@@ -146,7 +127,7 @@ def test_cli_log_dir(tmp_path):
     r = subprocess.run([os.path.join(CLI_DIR, "kafka-topic-analyzer"), "-t", "orders", "-b", "unused:9092", "-c", "--log-dir",
                         str(tmp_path)], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
-    o = _oracle_over(per, count_alive_keys=True)
+    o = oracle_over(per, count_alive_keys=True)
     lines = r.stdout.splitlines()
     assert "Alive keys: %d" % o.scalar("sum_all_alive") in lines
     assert "Topic Size: %d bytes" % o.scalar("overall_size") in lines
@@ -234,44 +215,24 @@ def test_device_entry_points_one_buffer_many_partitions(batch_records):
     """kta_scan_log_batches_device: the batches of all partitions in ONE device buffer, decoded and scanned in one go; and
     kta_scan_log_segment_device per partition.  40 records per batch (≈ 12 KB: staged in shared memory by a bulk copy) and 300
     (≈ 90 KB: read in place); the buffer has no slack behind its last byte, so the last batch is read in place too."""
-    import torch
     P = 5
     spec = synth.make_spec(P * 12_000, P, distinct_keys=3000, tombstone_per_10k=2000, key_mode=1)
     o = Oracle(count_alive_keys=True, now=NOW)
-    chunks, offs, parts, total = [], [], [], 0
+    segs = []
     for p in range(P):
         t = synth.fill_host(spec, rank=p, world=P)
         o.handle_batch(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes)
-        s = synth.encode_segment(spec, p, batch_records=batch_records)
-        pos = 0
-        while pos + 61 <= s.size:
-            offs.append(total + pos)
-            parts.append(p)
-            pos += 12 + int.from_bytes(s[pos + 8:pos + 12].tobytes(), "big", signed=True)
-        chunks.append(s)
-        total += s.size                       # packed back to back: batches start at arbitrary alignments
-    buf = torch.from_numpy(np.concatenate(chunks)).cuda()
-    assert buf.numel() == total
-    d_off = torch.tensor(offs, dtype=torch.int64).cuda()
-    d_part = torch.tensor(parts, dtype=torch.int32).cuda()
+        segs.append((p, synth.encode_segment(spec, p, batch_records=batch_records)))
+    staged = stage_batches(segs)              # packed back to back: batches start at arbitrary alignments
+    assert staged[0].numel() == staged[1] == sum(s.size for _, s in segs)
     with KtaEngine(P, count_alive_keys=True, hll_precision=10, now=NOW) as e:
-        assert e.scan_log_batches_device(buf, total, d_off, d_part, len(offs)) == spec.n_total
+        assert scan_log_batches(e, staged) == spec.n_total
         e.finalize()
         assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(10))
         # partition by partition through the single-partition entry point: the result is the same
         e.reset()
-        import ctypes as C
-        at, b0 = 0, 0
-        for p in range(P):
-            nb = parts.count(p)
-            n = C.c_int64()
-            rel = (d_off[b0:b0 + nb] - at).contiguous()
-            seg = buf[at:at + chunks[p].size].clone()
-            from kafka_topic_analyzer_b200._native import check, lib
-            check(lib().kta_scan_log_segment_device(e.handle, p, seg.data_ptr(), seg.numel(), rel.data_ptr(), nb, C.byref(n)))
-            assert n.value == spec.n_total // P
-            at += chunks[p].size
-            b0 += nb
+        for p, s in segs:
+            assert scan_log_segment(e, p, s) == spec.n_total // P
         e.finalize()
         assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(10))
 
@@ -305,8 +266,8 @@ def test_compressed_segments_decode_and_scan(codec):
     P = 5
     spec = synth.make_spec(P * 4000, P, key_mode=1, distinct_keys=900, tombstone_per_10k=2000, null_key_per_10k=300,
                            empty_value_per_10k=100, value_mean=120)
-    per = _partition_lists(synth.fill_host(spec))
-    o = _oracle_over(per, count_alive_keys=True)
+    per = partition_lists(synth.fill_host(spec))
+    o = oracle_over(per, count_alive_keys=True)
     comp = ["gzip", "lz4", "snappy", "snappy-xerial", None] if codec == "mixed" else codec
     with KtaEngine(P, count_alive_keys=True, hll_precision=10, now=NOW) as e:
         total = 0

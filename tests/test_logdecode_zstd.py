@@ -6,9 +6,9 @@ import subprocess
 import numpy as np
 import pytest
 
+from feed import partition_lists, scan_log_batches, stage_batches
 from kafka_topic_analyzer_b200 import KtaEngine, KtaError, synth
-from oracle_lib import Oracle
-from parity import assert_parity
+from parity import assert_parity, oracle_over
 import kafka_codec as kc
 import zstd_codec as zc
 
@@ -16,37 +16,9 @@ NOW = (4102444800, 123456789)
 MIXED = ["zstd", "zstd-stream", "gzip", "lz4", "snappy", None]
 
 
-def _partition_lists(t):
-    kl = t.key_len
-    koff = np.concatenate([[0], np.cumsum(np.maximum(kl, 0))])
-    per = {}
-    for i in range(t.n):
-        key = None if kl[i] < 0 else t.key_bytes[koff[i]:koff[i] + kl[i]].tobytes()
-        vl = None if t.value_len[i] < 0 else int(t.value_len[i])
-        per.setdefault(int(t.partition[i]), []).append((int(t.ts_ms[i]), key, vl))
-    return per
-
-
-def _oracle_over(per):
-    o = Oracle(count_alive_keys=True, now=NOW)
-    for p in sorted(per):
-        for ts, key, vl in per[p]:
-            o.handle_message(p, None if ts == -1 else ts, key, vl)
-    return o
-
-
-def _batch_offsets(seg):
-    offs, pos = [], 0
-    while pos + 61 <= len(seg):
-        offs.append(pos)
-        pos += 12 + int.from_bytes(seg[pos + 8:pos + 12], "big", signed=True)
-    return offs
-
-
 def _check_all_entry_points(P, per, segs, hll_p=10):
     """push_log_segment per partition, push_log_segments in one call, scan_log_batches_device over one device buffer"""
-    import torch
-    o = _oracle_over(per)
+    o = oracle_over(per, count_alive_keys=True)
     n = sum(len(v) for v in per.values())
     with KtaEngine(P, count_alive_keys=True, hll_precision=hll_p, now=NOW) as e:
         assert sum(e.push_log_segment(p, s) for p, s in segs) == n
@@ -57,15 +29,7 @@ def _check_all_entry_points(P, per, segs, hll_p=10):
         e.finalize()
         assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(hll_p))
         e.reset()
-        offs, parts, at = [], [], 0
-        for p, s in segs:
-            offs += [at + x for x in _batch_offsets(s)]
-            parts += [p] * len(_batch_offsets(s))
-            at += len(s)
-        buf = torch.from_numpy(np.frombuffer(b"".join(s for _, s in segs), dtype=np.uint8).copy()).cuda()
-        d_off = torch.tensor(offs, dtype=torch.int64).cuda()
-        d_part = torch.tensor(parts, dtype=torch.int32).cuda()
-        assert e.scan_log_batches_device(buf, at, d_off, d_part, len(offs)) == n
+        assert scan_log_batches(e, stage_batches(segs)) == n
         e.finalize()
         assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(hll_p))
 
@@ -79,7 +43,7 @@ def test_zstd_segments_decode_and_scan(codec):
     P = 5
     spec = synth.make_spec(P * 4000, P, key_mode=1, distinct_keys=900, tombstone_per_10k=2000, null_key_per_10k=300,
                            empty_value_per_10k=100, value_mean=120)
-    per = _partition_lists(synth.fill_host(spec))
+    per = partition_lists(synth.fill_host(spec))
     comp = MIXED if codec == "mixed" else codec
     segs = [(p, zc.encode_partition(per[p], rng, max_batch=200, compression=comp)) for p in sorted(per)]
     raw = sum(len(kc.encode_partition(per[p], np.random.default_rng(1), max_batch=200)) for p in per)
@@ -106,14 +70,14 @@ def test_large_zstd_batches(codec):
     default message.max.bytes)"""
     P = 3
     spec = synth.make_spec(P * 9000, P, key_mode=1, distinct_keys=4000, tombstone_per_10k=1500, value_mean=120)
-    per = _partition_lists(synth.fill_host(spec))
+    per = partition_lists(synth.fill_host(spec))
     sizes = {0: 450, 1: 1100, 2: 9000}                             # records per batch: ~60 KB, ~150 KB, ~1.1 MB
     segs = []
     for p in sorted(per):
         seg = _fixed_batches(per[p], sizes[p], codec)
         segs.append((p, seg))
     big = _fixed_batches(per[2], sizes[2], None)
-    assert len(big) > 1_000_000 and len(_batch_offsets(big)) == 1
+    assert len(big) > 1_000_000 and len(kc.batch_offsets(big)) == 1
     assert len(_fixed_batches(per[0][:450], 450, None)) > 48 * 1024
     assert len(_fixed_batches(per[1][:1100], 1100, None)) > 128 * 1024
     _check_all_entry_points(P, per, segs)
@@ -166,7 +130,7 @@ def test_cli_log_dir_zstd(tmp_path):
     rng = np.random.default_rng(23)
     P = 3
     spec = synth.make_spec(P * 2000, P, key_mode=1, distinct_keys=300, tombstone_per_10k=3000, value_mean=30)
-    per = _partition_lists(synth.fill_host(spec))
+    per = partition_lists(synth.fill_host(spec))
     reports = []
     for comp in (None, ["zstd", "zstd-stream"]):
         root = tmp_path / ("zstd" if comp else "plain")
@@ -179,7 +143,7 @@ def test_cli_log_dir_zstd(tmp_path):
         assert r.returncode == 0, r.stderr
         reports.append(r.stdout.splitlines())
     plain, zstd = reports
-    o = _oracle_over(per)
+    o = oracle_over(per, count_alive_keys=True)
     assert "Alive keys: %d" % o.scalar("sum_all_alive") in zstd
     rows = [l for l in zstd if l.startswith("| ") and l[2].isdigit()]
     assert len(rows) == P

@@ -24,8 +24,8 @@ import test_inflate_host as ih
 import test_lzwalk_host as lh
 import test_zstd_host as zh
 import zstd_codec as zc
-from oracle_lib import Oracle
-from parity import assert_parity
+from feed import capture_hashes, scan_log_batches, stage_batches
+from parity import assert_parity, oracle_over
 
 NOW = (4102444800, 123456789)
 LOGB_OK, LOGB_BAD = 0, 2
@@ -265,7 +265,6 @@ def test_every_decompressed_byte_is_a_key_byte():
     inside the fused scan) check the decompression through the product's own entry points and buffers."""
     import torch
     from kafka_topic_analyzer_b200 import KtaEngine
-    from kafka_topic_analyzer_b200._native import lib
     rng = np.random.default_rng(59)
     codecs = ["gzip", "lz4", "snappy", "snappy-xerial", "zstd", "zstd-stream", None]
     P = 4
@@ -289,35 +288,22 @@ def test_every_decompressed_byte_is_a_key_byte():
         segs.append((p, bytes(seg)))
     kl = np.array([-1 if k is None else len(k) for k in order], dtype=np.int32)
     want = np_oracle.fnv32_many(kl, np.frombuffer(b"".join(k for k in order if k), dtype=np.uint8))
-    o = Oracle(count_alive_keys=True, now=NOW)
-    for p in range(P):
-        for ts, key, vl in per[p]:
-            o.handle_message(p, ts, key, vl)
+    o = oracle_over(per, count_alive_keys=True)
     n = len(order)
     with KtaEngine(P, count_alive_keys=True, hll_precision=10, now=NOW) as e:
         cap = torch.zeros(n, dtype=torch.int32, device="cuda")
-        lib().kta_set_hash_capture(e.handle, cap.data_ptr())
+        capture_hashes(e, cap)
         assert e.push_log_segments(segs) == n
-        lib().kta_set_hash_capture(e.handle, None)
+        capture_hashes(e, None)
         e.finalize()
         assert np.array_equal(cap.cpu().numpy().view(np.uint32), want)
         assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(10))
         # the same batches in one device buffer, through kta_scan_log_batches_device
         e.reset()
-        offs, parts, at = [], [], 0
-        for p, s in segs:
-            pos = 0
-            while pos + 61 <= len(s):
-                offs.append(at + pos)
-                parts.append(p)
-                pos += 12 + int.from_bytes(s[pos + 8:pos + 12], "big", signed=True)
-            at += len(s)
-        buf = torch.from_numpy(np.frombuffer(b"".join(s for _, s in segs), dtype=np.uint8).copy()).cuda()
         cap.fill_(0)
-        lib().kta_set_hash_capture(e.handle, cap.data_ptr())
-        assert e.scan_log_batches_device(buf, at, torch.tensor(offs, dtype=torch.int64).cuda(),
-                                         torch.tensor(parts, dtype=torch.int32).cuda(), len(offs)) == n
-        lib().kta_set_hash_capture(e.handle, None)
+        capture_hashes(e, cap)
+        assert scan_log_batches(e, stage_batches(segs)) == n
+        capture_hashes(e, None)
         e.finalize()
         assert np.array_equal(cap.cpu().numpy().view(np.uint32), want)
         assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(10))

@@ -10,6 +10,7 @@ import pytest
 
 import np_oracle
 from oracle_lib import Oracle, fnv32, hll_estimate, olib
+from parity import replay_demo_row
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 
@@ -65,25 +66,6 @@ def test_demo_output_table_getters():
         assert o.avg("value_size_avg", p) == r["value_size_avg"]
         assert o.avg("message_size_avg", p) == r["message_size_avg"]
         assert "%.4f" % o.dirty_ratio(p) == r["dirty_ratio"]
-
-
-def replay_demo_row(row, demo, handler):
-    """Re-creates one partition of the demo topic as records: 9-byte keys (K-Bytes / Total == 9 exactly),
-    values spread so that V-Bytes matches, one smallest (139) and one largest (750) message."""
-    n, vsum = row["total"], row["v_bytes"]
-    vl = np.full(n, 0, dtype=np.int64)
-    vl[0], vl[1] = demo["smallest_message"] - 9, demo["largest_message"] - 9
-    rest = vsum - int(vl[0]) - int(vl[1])
-    base, extra = divmod(rest, n - 2)
-    vl[2:] = base
-    vl[2:2 + extra] += 1
-    assert int(vl.sum()) == vsum and vl.min() >= 130 and vl.max() <= 741
-    ts = np.full(n, demo["earliest_message_s"] * 1000 + 500, dtype=np.int64)
-    ts[n // 2] = demo["earliest_message_s"] * 1000 + 999      # still the same second (truncation)
-    ts[-1] = demo["latest_message_s"] * 1000 + 1
-    kl = np.full(n, 9, dtype=np.int32)
-    part = np.full(n, row["P"], dtype=np.int32)
-    handler(part, ts, kl, vl.astype(np.int32))
 
 
 def test_demo_output_replay_row8():

@@ -18,8 +18,9 @@ import pytest
 import torch
 
 import scan_ref as R
-from kafka_topic_analyzer_b200 import KtaEngine, lib, synth
+from kafka_topic_analyzer_b200 import KtaEngine, synth
 from kafka_topic_analyzer_b200 import _native as N
+from feed import Topic, alive_import, capture_hashes, device, push_host, rekey, scan, settle, take
 from oracle_lib import COUNTERS, fnv32 as oracle_fnv32
 
 NOW = (4102444800, 123456789)
@@ -91,83 +92,12 @@ def _budget(request):
 # ------------------------------------------------------------------------------------------------
 # topics in HBM
 # ------------------------------------------------------------------------------------------------
-class Topic:
-    """SoA columns on the device, keys packed in record order with 64 bytes of slack, key_tile_base from key_len."""
-
-    def __init__(self, partition, ts_ms, key_len, value_len, key_bytes, key_bytes_len, seq=None):
-        self.partition, self.ts_ms, self.key_len, self.value_len = partition, ts_ms, key_len, value_len
-        self.key_bytes, self.kbl, self.seq = key_bytes, int(key_bytes_len), seq
-        self.n = int(partition.numel())
-        self.key_tile_base = tile_base(key_len)
-
-    @property
-    def keys(self):
-        return self.key_bytes[: self.kbl]
-
-
-def tile_base(key_len):
-    kl = key_len.to(torch.int64).clamp(min=0)
-    nt = -(-kl.numel() // T)
-    sums = torch.cat([kl, kl.new_zeros(nt * T - kl.numel())]).view(nt, T).sum(1)
-    return torch.cat([kl.new_zeros(1), torch.cumsum(sums, 0)])
-
-
 def generate(n, P, run_len=1, **kw):
     """the first n records of a synthetic topic, generated in HBM"""
     unit = P * run_len
     spec = synth.make_spec(-(-n // unit) * unit, P, run_len=run_len, **kw)
     d = synth.DeviceTopic(spec, count=n)
     return Topic(d.partition, d.ts_ms, d.key_len, d.value_len, d.key_bytes, d.key_bytes_len)
-
-
-def made_byte(r, pos):
-    return ((r * 2654435761 + pos * 40503 + (pos >> 8) * 97) >> 5) & 0xFF
-
-
-def pack_keys(kb_src, src_off, lens, made=None, chunk=1 << 21):
-    """Packed key bytes (+ 64 B of slack): record i's key is lens[i] bytes from kb_src[src_off[i]:], or where made[i],
-    bytes made from i and the position.  Chunked over records, so no index tensor spans the whole key buffer."""
-    lens = lens.to(torch.int64).clamp(min=0)
-    dst = torch.cumsum(lens, 0) - lens
-    total = int(lens.sum())
-    out = torch.zeros(total + 64, dtype=torch.uint8, device=lens.device)
-    for a in range(0, lens.numel(), chunk):
-        b = min(lens.numel(), a + chunk)
-        cnt = int(lens[a:b].sum())
-        if not cnt:
-            continue
-        r = torch.repeat_interleave(torch.arange(a, b, device=lens.device), lens[a:b])
-        pos = torch.arange(cnt, device=lens.device) - (dst[r] - dst[a])
-        if made is None:
-            val = kb_src[src_off[r] + pos]
-        else:
-            m = made[r]
-            val = kb_src[torch.where(m, 0, src_off[r] + pos)].to(torch.int64)
-            val = torch.where(m, made_byte(r, pos), val).to(torch.uint8)
-        out[dst[a]: dst[a] + cnt] = val
-        del r, pos, val
-    return out, total
-
-
-def rekey(t, new_kl):
-    """t with key lengths new_kl: a record whose length is unchanged keeps its key, any other gets made bytes"""
-    kb, total = pack_keys(t.keys, R.key_offsets(t.key_len), new_kl, made=new_kl != t.key_len)
-    return Topic(t.partition, t.ts_ms, new_kl.to(torch.int32), t.value_len, kb, total, t.seq)
-
-
-def take(t, idx):
-    """the records idx of t, in that order, with their keys; seq = idx (their place in t)"""
-    kb, total = pack_keys(t.keys, R.key_offsets(t.key_len)[idx], t.key_len[idx])
-    return Topic(t.partition[idx], t.ts_ms[idx], t.key_len[idx], t.value_len[idx], kb, total, seq=idx.to(torch.int64))
-
-
-def shifted(a, shift):
-    """a copy of a whose base lies `shift` elements past a 16-byte-aligned address"""
-    buf = torch.zeros(a.numel() + 16, dtype=a.dtype, device=a.device)
-    col = buf[shift: shift + a.numel()]
-    col.copy_(a)
-    assert (col.data_ptr() % 16 == 0) == (shift == 0)
-    return col
 
 
 def long_fn(kb):
@@ -185,20 +115,6 @@ def engine(mode, P, shard=None, hll_p=HLL_P, **kw):
     if mode == "counters":
         return KtaEngine(P, now=NOW, shard=shard, **kw)
     return KtaEngine(P, count_alive_keys=mode == "exact", hll_precision=hll_p, now=NOW, shard=shard, **kw)
-
-
-def scan(e, t, seq=False, seq_base=None, cols=None, key_bytes=None):
-    # the engine scans on its own stream: the columns torch has just written must have landed first
-    torch.cuda.synchronize()
-    c = cols or (t.partition, t.ts_ms, t.key_len, t.value_len)
-    e.scan_batch_device(*c, key_bytes=t.key_bytes if key_bytes is None else key_bytes, key_bytes_len=t.kbl,
-                        key_tile_base=t.key_tile_base, seq=t.seq if seq else None, seq_base=seq_base)
-
-
-def push_host(e, t):
-    h = lambda a: a.cpu().numpy()
-    e.push_batch_host(h(t.partition), h(t.ts_ms), h(t.key_len), h(t.value_len), h(t.keys),
-                      h(t.key_tile_base).view(np.uint64))
 
 
 def first_mismatch(got, want):
@@ -255,14 +171,14 @@ def run(mode, t, P, hll_p=HLL_P, capture=False, host=False, cols=None, key_bytes
         out = None
         if capture:
             out = torch.full((t.n,), -1, dtype=torch.int32, device="cuda")
-            assert lib().kta_set_hash_capture(e.handle, out.data_ptr()) == 0
+            capture_hashes(e, out)
         if host:
             push_host(e, t)
         else:
             scan(e, t, cols=cols, key_bytes=key_bytes)
         e.finalize()
         if capture:
-            assert lib().kta_set_hash_capture(e.handle, None) == 0
+            capture_hashes(e, None)
             got = out.to(torch.int64) & R.M32
             bad = torch.nonzero(got != h).flatten()
             if bad.numel():
@@ -319,26 +235,27 @@ def test_instance_at_depth(mode, P, world, smem):
             s = take(t, idx[r]) if mode != "counters" else \
                 Topic(*(c[idx[r]] for c in (t.partition, t.ts_ms, t.key_len, t.value_len)), t.key_bytes, 0)
             assert_depth(s.n, mode)
-            scan(e, s, seq=mode == "exact")
+            scan(e, s, seq=s.seq if mode == "exact" else None)
             if mode != "exact":
                 e.finalize()
             buf = torch.zeros(words, dtype=torch.int64, device="cuda")
-            e.merge_export(r, world, buf)
-            torch.cuda.synchronize()
+            settle()
+            e.merge_export(r, world, buf)               # returns once the engine's stream has written buf
             total += buf
             if mode == "exact":
                 cnt = e.alive_export_count()
                 h = torch.zeros(cnt, dtype=torch.int32, device="cuda")
                 st = torch.zeros(cnt, dtype=torch.int64, device="cuda")
+                settle()
                 assert e.alive_export(h, st, cnt) == cnt
                 e.sync()
                 lists.append((h, st, cnt))
             del s
         e0 = engines[0]
-        torch.cuda.synchronize()
+        settle()
         e0.merge_import(world, total)
         for h, st, cnt in lists[1:]:
-            e0.alive_import(h, st, cnt)
+            alive_import(e0, h, st, cnt)
         e0.finalize()
         check(e0, mm, P, regs, alive)
     finally:
@@ -376,8 +293,8 @@ def test_stage_bookkeeping_at_depth(mode, hdr_shift, key_shift):
     n = depth_n(mode)
     assert_depth(n, mode)
     t = generate(n, 64, key_mode=0, distinct_keys=1_000_000, tombstone_per_10k=1500)
-    cols = [shifted(c, hdr_shift) for c in (t.partition, t.ts_ms, t.key_len, t.value_len)]
-    kb = shifted(t.key_bytes, key_shift)
+    cols = [device(c, hdr_shift) for c in (t.partition, t.ts_ms, t.key_len, t.value_len)]
+    kb = device(t.key_bytes, key_shift)
     run(mode, t, 64, cols=cols, key_bytes=kb, smem=True)
 
 

@@ -7,8 +7,9 @@ import torch
 import np_oracle
 import scan_ref as R
 from kafka_topic_analyzer_b200 import synth
-from oracle_lib import COUNTERS, Oracle
-from parity import random_topic
+from feed import random_topic, take
+from oracle_lib import COUNTERS
+from parity import oracle_for
 
 NOW = (4102444800, 123456789)
 N = 1 << 16
@@ -44,10 +45,7 @@ def test_reference_equals_the_oracle(name, t, P):
         assert (t.key_len == 0).any() and (t.key_len < 0).any() and (t.value_len == 0).any() and (t.value_len < 0).any()
     # the oracle sees the in-range records only, in order (out-of-range records take part in nothing)
     good = (t.partition >= 0) & (t.partition < P)
-    koff = np.concatenate([[0], np.cumsum(np.maximum(t.key_len, 0).astype(np.int64))])
-    keep = np.concatenate([t.key_bytes[koff[i]:koff[i + 1]] for i in np.nonzero(good)[0]] or [np.zeros(0, np.uint8)])
-    o = Oracle(count_alive_keys=True, track_stream=True, now=NOW)
-    o.handle_batch(t.partition[good], t.ts_ms[good], t.key_len[good], t.value_len[good], keep.astype(np.uint8))
+    o = oracle_for(take(t, np.nonzero(good)[0]), count_alive_keys=True, track_stream=True, now=NOW)
 
     mm = R.message_metrics(P, cols["partition"], cols["ts_ms"], cols["key_len"], cols["value_len"])
     assert mm["bad"] == int((~good).sum())

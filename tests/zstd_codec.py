@@ -24,17 +24,15 @@ def compress_records(recs: bytes, codec: str) -> bytes:
 def recompress(seg: bytes, pick) -> bytes:
     """every batch of an uncompressed segment with its records section compressed by pick() (a codec name, or None to
     leave the batch as it is); batchLength and the attributes' codec bits follow"""
-    out, pos = bytearray(), 0
-    while pos + 61 <= len(seg):
-        bl = int.from_bytes(seg[pos + 8:pos + 12], "big", signed=True)
-        hdr, body = bytearray(seg[pos:pos + 61]), seg[pos + 61:pos + 12 + bl]
+    out, offs = bytearray(), kc.batch_offsets(seg)
+    for pos, end in zip(offs, offs[1:] + [len(seg)]):
+        hdr, body = bytearray(seg[pos:pos + 61]), seg[pos + 61:end]
         codec = pick()
         if codec:
             body = compress_records(body, codec)
             hdr[8:12] = struct.pack(">i", 49 + len(body))
             hdr[22] |= kc.CODEC_BITS[codec]
         out += hdr + body
-        pos += 12 + bl
     return bytes(out)
 
 
