@@ -211,7 +211,8 @@ int kta_alive_import_device(kta_handle *h, const uint32_t *dev_hash, const uint6
  * columns above (what librdkafka's parser + BorrowedMessage accessors do per message, src/kafka.rs:93,
  * src/metric.rs:208-209,218,233) and scans it.  Control batches are skipped, LogAppendTime batches use
  * maxTimestamp, a record's timestamp is baseTimestamp + timestampDelta (only a result of -1 is "not available"),
- * CRCs are not verified (librdkafka default check.crcs=false).  gzip, LZ4 (frame format), Snappy (raw or
+ * CRCs are verified only when check.crcs is switched on (kta_log_set_check_crcs; off by default, like librdkafka's
+ * check.crcs=false).  gzip, LZ4 (frame format), Snappy (raw or
  * xerial-framed) and zstd batches are decompressed on the GPU; the checksums inside a compressed section (gzip's
  * CRC32, zstd's Content_Checksum) are skipped, not verified, like the batch CRC.  zstd frames with a Dictionary_ID and
  * the unassigned codecs 5-7 are rejected (KTA_ERR_INVALID).
@@ -250,6 +251,37 @@ int kta_log_add_txn_index_host(kta_handle *h, int32_t partition, const uint8_t *
  * the batches and records left out as aborted, and the records of undecided transactional batches that were delivered
  * (any pointer may be NULL) */
 int kta_log_txn_stats(kta_handle *h, uint64_t *aborted_batches, uint64_t *aborted_records, uint64_t *undecided_records);
+
+/* check.crcs: verify every record batch's CRC-32C and skip the batches that fail it.
+ * The checksum is CRC-32C (Castagnoli, reflected polynomial 0x82F63B78, init and xorout 0xFFFFFFFF) over the batch from
+ * `attributes` (byte 21) to its end (byte 12 + batchLength), computed over the bytes as stored (the compressed ones for a
+ * compressed batch), compared with the big-endian u32 at bytes 17-20.
+ * Off (the default, as librdkafka's check.crcs=false): nothing changes.  On: the check runs on the GPU before anything
+ * reads a CRC-covered field.  A batch that fails it is not decompressed, decoded, or classified as transactional data or
+ * as a marker: it delivers no records, takes no sequence numbers and raises no error, so an unknown codec, an implausible
+ * recordsCount, a section that does not decompress, a malformed record, an unreadable marker or a producer's baseOffset
+ * order inside it no longer refuse the call.  It is counted as a CRC failure only, never as aborted; under
+ * read_committed a failed marker is not seen (its transaction is decided by the registered ranges, or is undecided).
+ * The fields outside the CRC frame the batch and still refuse the call as before: the batch must fit the buffer,
+ * batchLength >= 49 and magic == 2.  A batch that passes goes through every other check unchanged (a valid CRC over a
+ * malformed record is a producer bug, not damage: KTA_ERR_INVALID).  librdkafka reports such a batch as a consumer error
+ * (RD_KAFKA_RESP_ERR__BAD_MSG, "failed CRC32C check") and goes on with the next one; kta_log_crc_failures lists them. */
+#define KTA_LOG_CRC_KEEP 4096   /* failures kept per handle (kta_log_crc_failures) */
+typedef struct kta_log_crc_failure {
+    int32_t partition;
+    uint32_t batch_bytes;        /* 12 + batchLength */
+    int64_t base_offset;
+    uint32_t stored_crc;         /* bytes 17-20 of the batch */
+    uint32_t computed_crc;
+} kta_log_crc_failure;           /* 24 bytes */
+/* enabled: 0 or 1 (anything else is KTA_ERR_INVALID); applies to every later log call; kta_reset keeps it */
+int kta_log_set_check_crcs(kta_handle *h, int enabled);
+/* totals over the successful log calls since create / reset: batches checked (while the switch was on), batches that
+ * failed, and their bytes (12 + batchLength each).  Any pointer may be NULL; valid whether the switch is on or off. */
+int kta_log_crc_stats(kta_handle *h, uint64_t *checked_batches, uint64_t *failed_batches, uint64_t *failed_bytes);
+/* the first KTA_LOG_CRC_KEEP failures of successful calls since create / reset, in call order and, within a call, in
+ * batch order: min(cap, kept) of them are copied to out; *count (may be NULL) = the number kept.  kta_reset clears them. */
+int kta_log_crc_failures(kta_handle *h, kta_log_crc_failure *out, int64_t cap, int64_t *count);
 
 /* ---- introspection for benchmarks ---- */
 /* kernels launched by this handle since create/reset, and device time of the scan kernels (ms,

@@ -100,6 +100,16 @@ class SynthSpec(C.Structure):
     ]
 
 
+class CrcFailure(C.Structure):
+    _fields_ = [
+        ("partition", C.c_int32), ("batch_bytes", C.c_uint32), ("base_offset", C.c_int64),
+        ("stored_crc", C.c_uint32), ("computed_crc", C.c_uint32),
+    ]
+
+
+LOG_CRC_KEEP = 4096   # include/kta.h KTA_LOG_CRC_KEEP
+
+
 # every symbol include/kta.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -139,6 +149,9 @@ SYMBOLS = {
     "kta_push_log_segments_host": (C.c_int, [_P, C.c_int32, _P, _P, _P, C.POINTER(C.c_int64)]),
     "kta_log_add_txn_index_host": (C.c_int, [_P, C.c_int32, _P, C.c_int64]),
     "kta_log_txn_stats": (C.c_int, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "kta_log_set_check_crcs": (C.c_int, [_P, C.c_int]),
+    "kta_log_crc_stats": (C.c_int, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "kta_log_crc_failures": (C.c_int, [_P, C.POINTER(CrcFailure), C.c_int64, C.POINTER(C.c_int64)]),
     "kta_stats": (C.c_int, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "kta_set_timing": (C.c_int, [_P, C.c_int]),
     "kta_scan_time_ms": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),

@@ -14,6 +14,10 @@
 //                              consumer: records of transactions still open at the end of the files are counted (with a
 //                              warning) instead of waiting at the last stable offset, and legacy magic 0/1 message sets are
 //                              reported as malformed.
+//                              --librdkafka check.crcs=true (default false, as librdkafka's) verifies every batch's
+//                              CRC-32C on the GPU: a batch that fails it is skipped, and reported on stderr in librdkafka's
+//                              words ("... failed CRC32C check ..."); the report covers the rest and the exit status stays
+//                              0, as the reference logs a failed poll and goes on (src/kafka.rs:95-97).
 //   --feed push|batch|device   how records reach the handlers: kta_push per record (the reference's call shape),
 //                              kta_push_batch_host, or generated and scanned in HBM
 //
@@ -67,7 +71,23 @@ static bool read_file(const std::string &path, std::vector<uint8_t> &out) {
 static int print_report(kta_handle *h, const std::string &topic, const std::vector<int> &partitions, const std::vector<int64_t> &start_offsets,
                         const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs);
 
-static int analyze_log_dir(const std::string &topic, const std::string &dir, bool alive, int hll, bool read_committed,
+// check.crcs: every kept failure as librdkafka words the consumer error it raises (RD_KAFKA_RESP_ERR__BAD_MSG), logged as
+// the reference logs a failed poll; the failures beyond those kept in one line
+static void warn_crc_failures(kta_handle *h) {
+    uint64_t failed = 0;
+    KTA(kta_log_crc_stats(h, nullptr, &failed, nullptr));
+    if (!failed) return;
+    std::vector<kta_log_crc_failure> f(KTA_LOG_CRC_KEEP);
+    int64_t kept = 0;
+    KTA(kta_log_crc_failures(h, f.data(), (int64_t)f.size(), &kept));
+    for (int64_t i = 0; i < kept; i++)
+        fprintf(stderr, "warning: Kafka error: MessageSet at offset %lld (%u bytes) of partition %d failed CRC32C check (original 0x%08x != calculated 0x%08x)\n",
+                (long long)f[(size_t)i].base_offset, f[(size_t)i].batch_bytes, f[(size_t)i].partition, f[(size_t)i].stored_crc, f[(size_t)i].computed_crc);
+    if (failed > (uint64_t)kept)
+        fprintf(stderr, "warning: %llu more record batch(es) failed CRC32C check and were skipped\n", (unsigned long long)(failed - (uint64_t)kept));
+}
+
+static int analyze_log_dir(const std::string &topic, const std::string &dir, bool alive, int hll, bool read_committed, bool check_crcs,
                            std::chrono::steady_clock::time_point start_time) {
     // get_topic_offsets (src/kafka.rs:60-72) from the files: partitions = <topic>-<n> directories, low watermark =
     // first batch's baseOffset, high watermark = last batch's baseOffset + lastOffsetDelta + 1
@@ -106,6 +126,7 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
     cfg.isolation_level = read_committed ? KTA_READ_COMMITTED : KTA_READ_UNCOMMITTED;
     kta_handle *h = nullptr;
     KTA(kta_create(&cfg, &h));
+    if (check_crcs) KTA(kta_log_set_check_crcs(h, 1));
     // read_committed: every partition's aborted transactions are known before any segment is decoded, so a transaction
     // whose marker lies in a later group of segments is decided exactly
     if (read_committed)
@@ -156,6 +177,7 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
         }
     }
     flush();
+    if (check_crcs) warn_crc_failures(h);
     if (std::all_of(end_offsets.begin(), end_offsets.end(), [](int64_t v) { return v == 0; })) {
         fprintf(stderr, "Given topic has no content, no analysis possible. Exiting.\n");  // main.rs:98-101
         return 254;
@@ -201,6 +223,9 @@ int main(int argc, char **argv) {
                  "                                                 (this build reads isolation.level=read_committed|read_uncommitted\n"
                  "                                                 for --log-dir; its default is read_uncommitted, librdkafka's is\n"
                  "                                                 read_committed: pass isolation.level=read_committed to match it)\n"
+                 "                                                 and check.crcs=true|false for --log-dir (default false, as\n"
+                 "                                                 librdkafka's): true verifies every batch's CRC-32C, skips and\n"
+                 "                                                 reports the batches that fail it, and reports the rest\n"
                  "        --log-dir <DIR>                          read <DIR>/<TOPIC>-<partition>/*.log (and, read_committed,\n"
                  "                                                 *.txnindex) instead of a broker\n"
                  "    -t, --topic <TOPIC>                          The topic to analyze\n"
@@ -217,8 +242,8 @@ int main(int argc, char **argv) {
         fprintf(stderr, "Error fetching metadata: this build has no librdkafka client (no broker access); pass --log-dir DIR or --synthetic n=...,partitions=...\n");
         return 101;  // the reference panics here (src/kafka.rs:61)
     }
-    // --librdkafka k=v,k=v (src/main.rs:84-93).  Without a client only isolation.level has a meaning here.
-    bool read_committed = false;
+    // --librdkafka k=v,k=v (src/main.rs:84-93).  Without a client only isolation.level and check.crcs have a meaning here.
+    bool read_committed = false, check_crcs = false;
     for (size_t p = 0; !librdkafka.empty() && p <= librdkafka.size();) {
         size_t e = librdkafka.find(',', p);
         if (e == std::string::npos) e = librdkafka.size();
@@ -232,11 +257,19 @@ int main(int argc, char **argv) {
                 return 2;
             }
             read_committed = v == "read_committed";
+        } else if (item.substr(0, q) == "check.crcs") {
+            const std::string v = item.substr(q + 1);
+            if (v != "true" && v != "false") {
+                fprintf(stderr, "error: --librdkafka: check.crcs must be true or false, not '%s'\n", v.c_str());
+                return 2;
+            }
+            check_crcs = v == "true";
         }
         p = e + 1;
     }
     const auto start_time = std::chrono::steady_clock::now();  // main.rs:69
-    if (!log_dir.empty()) return analyze_log_dir(topic, log_dir, count_alive_occurrences == 1, hll, read_committed, start_time);
+    if (!log_dir.empty())
+        return analyze_log_dir(topic, log_dir, count_alive_occurrences == 1, hll, read_committed, check_crcs, start_time);
 
     std::map<std::string, std::string> kv;
     for (size_t p = 0; p < synthetic.size();) {

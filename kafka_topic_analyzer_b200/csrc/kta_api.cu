@@ -22,6 +22,7 @@
 #include <cub/device/device_radix_sort.cuh>
 
 #include "kta_kernels.cuh"
+#include "kta_logcrc.cuh"
 #include "kta_logdecode.cuh"
 #include "kta_logdecode_launch.cuh"
 #include "kta_logtxn.cuh"
@@ -163,6 +164,17 @@ struct TxnState {
     uint64_t totals[3] = {0, 0, 0};                  // the stats of every successful call since create / reset
 };
 
+// check.crcs of the log entry points (kta_logcrc.cuh): the switch, the passes' buffers, and what successful calls found
+struct CrcState {
+    bool on = false;
+    DevBuf<uint64_t> d_spans;                        // per batch: spans of its CRC region, then their inclusive scan
+    DevBuf<uint32_t> d_acc;                          // per batch: the xor of its spans' shares of the register
+    DevBuf<LogCrcFail> d_fails;                      // the call's failures, in the order the header pass met them
+    DevBuf<LogCrcTables> d_tables;                   // built on the first call with the switch on
+    uint64_t totals[3] = {0, 0, 0};                  // checked batches, failed batches, failed bytes
+    std::vector<kta_log_crc_failure> kept;           // the first KTA_LOG_CRC_KEEP failures
+};
+
 // State of the log entry points (Kafka RecordBatch v2 segments → SoA → scan), reused from call to call
 struct LogScan {
     DevBuf<uint8_t> bytes;                   // segments staged from the host (kta_push_log_segments_host)
@@ -170,7 +182,7 @@ struct LogScan {
     DevBuf<int32_t> part;                    // and each batch's partition
     DevBuf<LogBatchInfo> info;               // per batch, from the header pass
     DevBuf<uint64_t> cnt;                    // records per batch, then their inclusive scan
-    DevBuf<uint32_t> err;                    // [0] error flags, [1] longest batch
+    DevBuf<uint32_t> err;                    // [0] error flags, [1] longest batch; check.crcs: [2] failures, [4..5] their bytes
     DevBuf<int32_t> dec_part, dec_klen, dec_vlen;   // the decoded columns
     DevBuf<int64_t> dec_ts;
     DevBuf<uint64_t> dec_ksrc;               // per decoded record: where its key bytes lie in the segment buffer
@@ -180,6 +192,7 @@ struct LogScan {
     DevBuf<uint64_t> unc_slot;               // per compressed batch: offset of its image in unc
     bool read_committed = false;
     TxnState txn;
+    CrcState crc;
 };
 
 struct kta_handle {
@@ -884,25 +897,62 @@ static int txn_passes(kta_handle *h, int32_t partition, const uint8_t *dev_bytes
     return KTA_OK;
 }
 
-// What the header pass (and read_committed's passes) found in one call's batches
+// What the header pass (and read_committed's passes and the CRC check) found in one call's batches
 struct LogHeaders {
     uint64_t nrec = 0;                               // records in all
-    uint32_t err[2] = {0, 0};                        // the header pass's error word: [0] LOGB_* flags, [1] longest batch
+    uint32_t err[6] = {0, 0, 0, 0, 0, 0};            // the header pass's error word: [0] LOGB_* flags, [1] longest batch;
+                                                     // check.crcs: [2] failed batches, [4..5] their bytes (u64)
     unsigned long long txn_stats[3] = {0, 0, 0};     // this call's aborted batches, aborted records, undecided records
+    std::vector<kta_log_crc_failure> crc_fails;      // check.crcs: this call's failures, in batch order, as many as are kept
 };
 
+// check.crcs: the passes of kta_logcrc.cuh that precede the header pass (span counts, their scan, the spans' CRCs).  No
+// host round trip: the span kernel reads the total from the scan, and its grid is bounded by the call's bytes.
+static int log_crc_spans(kta_handle *h, const uint8_t *dev_bytes, int64_t len, const uint64_t *dev_batch_off, int64_t nbatches) {
+    CrcState &c = h->log.crc;
+    cudaStream_t s = h->stream;
+    int rc;
+    if (!c.d_tables) {
+        LogCrcTables t;
+        log_crc_tables_host(t);
+        if ((rc = c.d_tables.alloc(1))) return rc;
+        CU(cudaMemcpyAsync(c.d_tables, &t, sizeof t, cudaMemcpyHostToDevice, s));
+        CU(cudaStreamSynchronize(s));   // `t` lives on this stack frame
+        CU(cudaFuncSetAttribute(log_crc_span_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LOG_CRC_SMEM));
+    }
+    if ((rc = c.d_spans.grow(s, nbatches + 1)) || (rc = c.d_acc.grow(s, nbatches)) || (rc = c.d_fails.grow(s, nbatches))) return rc;
+    log_crc_count_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, c.d_spans, c.d_acc);
+    tile_base_scan_kernel<<<1, 1024, 0, s>>>(c.d_spans, nbatches);
+    // at most len / S + nbatches spans, one per thread at least: a small call gets a small grid
+    const int64_t max_spans = len / LOG_CRC_SPAN + nbatches;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((max_spans + LOG_CRC_THREADS - 1) / LOG_CRC_THREADS, h->sm_count));
+    log_crc_span_kernel<<<grid, LOG_CRC_THREADS, LOG_CRC_SMEM, s>>>(dev_bytes, dev_batch_off, nbatches, c.d_spans, c.d_tables, c.d_acc);
+    CU(cudaGetLastError());
+    h->launches += 3;
+    return KTA_OK;
+}
+
 // The header pass, read_committed's passes and the scan of the record counts.  One host round trip (two under
-// read_committed); refuses the call for its headers and for the order of a producer's batches.
+// read_committed); refuses the call for its headers and for the order of a producer's batches.  With check.crcs the CRC
+// passes come first and the failures are counted in the same round trip; only a call with failures makes one more, for
+// their list.
 static int log_headers(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes, int64_t len,
                        const uint64_t *dev_batch_off, int64_t nbatches, LogHeaders &out) {
     LogScan &L = h->log;
     cudaStream_t s = h->stream;
     int rc;
     if ((rc = L.info.grow(s, nbatches + 1)) || (rc = L.cnt.grow(s, nbatches + 1))) return rc;
-    if (!L.err && (rc = L.err.alloc(2))) return rc;
-    CU(cudaMemsetAsync(L.err, 0, 8, s));
-    log_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, partition,
-                                                                            dev_batch_partition, L.info, L.cnt, L.err);
+    if (!L.err && (rc = L.err.alloc(6))) return rc;
+    const bool crc = L.crc.on;
+    const size_t err_bytes = crc ? 24 : 8;
+    if (crc && (rc = log_crc_spans(h, dev_bytes, len, dev_batch_off, nbatches))) return rc;
+    CU(cudaMemsetAsync(L.err, 0, err_bytes, s));
+    if (crc)
+        log_crc_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(
+            dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, L.info, L.cnt, L.err, L.crc.d_acc, L.crc.d_fails);
+    else
+        log_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, partition,
+                                                                                dev_batch_partition, L.info, L.cnt, L.err);
     CU(cudaGetLastError());
     bool txn = false;   // read_committed and the call has transactional batches
     if (L.read_committed && (rc = txn_passes(h, partition, dev_bytes, nbatches, &txn))) return rc;
@@ -911,7 +961,7 @@ static int log_headers(kta_handle *h, int32_t partition, const int32_t *dev_batc
     h->launches += 2;
     uint32_t txn_word[2] = {0, 0};
     CU(cudaMemcpyAsync(&out.nrec, L.cnt + nbatches, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(out.err, L.err, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(out.err, L.err, err_bytes, cudaMemcpyDeviceToHost, s));
     if (txn) {
         CU(cudaMemcpyAsync(txn_word, L.txn.d_word, 8, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(out.txn_stats, L.txn.d_stats, 24, cudaMemcpyDeviceToHost, s));
@@ -922,6 +972,17 @@ static int log_headers(kta_handle *h, int32_t partition, const int32_t *dev_batc
     if (out.err[0] & LOGB_BAD) return fail(KTA_ERR_INVALID, "malformed record batch header in partition %d", partition);
     if (txn_word[1] & TXN_ERR_ORDER)
         return fail(KTA_ERR_INVALID, "the batches of one producer in partition %d are not in increasing baseOffset order", partition);
+    // the failures to keep: the first ones in batch order, as many as the handle's list still has room for
+    const uint32_t nfail = out.err[2];
+    const size_t room = KTA_LOG_CRC_KEEP - L.crc.kept.size();
+    if (nfail && room) {
+        std::vector<LogCrcFail> f(nfail);
+        CU(cudaMemcpyAsync(f.data(), L.crc.d_fails, (size_t)nfail * sizeof(LogCrcFail), cudaMemcpyDeviceToHost, s));
+        CU(cudaStreamSynchronize(s));
+        std::sort(f.begin(), f.end(), [](const LogCrcFail &a, const LogCrcFail &b) { return a.batch < b.batch; });
+        for (size_t i = 0; i < std::min<size_t>(room, f.size()); i++)
+            out.crc_fails.push_back(kta_log_crc_failure{f[i].partition, f[i].batch_bytes, f[i].base_offset, f[i].stored, f[i].computed});
+    }
     return KTA_OK;
 }
 
@@ -1031,8 +1092,15 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
         if ((rc = log_gather_keys(h, partition, dev_bytes, keys, b))) return rc;
         if ((rc = scan_device_batch(h, &b))) return rc;
     }
-    // the call succeeded: its transaction counters join the handle's totals
+    // the call succeeded: its transaction counters and CRC results join the handle's totals
     for (int i = 0; i < 3; i++) h->log.txn.totals[i] += hd.txn_stats[i];
+    CrcState &c = h->log.crc;
+    if (c.on) {
+        c.totals[0] += (uint64_t)nbatches;
+        c.totals[1] += hd.err[2];
+        c.totals[2] += (uint64_t)hd.err[4] | ((uint64_t)hd.err[5] << 32);
+        c.kept.insert(c.kept.end(), hd.crc_fails.begin(), hd.crc_fails.end());
+    }
     if (records_out) *records_out = (int64_t)hd.nrec;
     return KTA_OK;
 }
@@ -1148,6 +1216,30 @@ extern "C" int kta_log_txn_stats(kta_handle *h, uint64_t *aborted_batches, uint6
     if (aborted_batches) *aborted_batches = h->log.txn.totals[0];
     if (aborted_records) *aborted_records = h->log.txn.totals[1];
     if (undecided_records) *undecided_records = h->log.txn.totals[2];
+    return KTA_OK;
+}
+
+extern "C" int kta_log_set_check_crcs(kta_handle *h, int enabled) {
+    if (!h) return fail(KTA_ERR_INVALID, "null handle");
+    if (enabled != 0 && enabled != 1) return fail(KTA_ERR_INVALID, "check_crcs %d is neither 0 nor 1", enabled);
+    h->log.crc.on = enabled == 1;
+    return KTA_OK;
+}
+
+extern "C" int kta_log_crc_stats(kta_handle *h, uint64_t *checked_batches, uint64_t *failed_batches, uint64_t *failed_bytes) {
+    if (!h) return fail(KTA_ERR_INVALID, "null handle");
+    if (checked_batches) *checked_batches = h->log.crc.totals[0];
+    if (failed_batches) *failed_batches = h->log.crc.totals[1];
+    if (failed_bytes) *failed_bytes = h->log.crc.totals[2];
+    return KTA_OK;
+}
+
+extern "C" int kta_log_crc_failures(kta_handle *h, kta_log_crc_failure *out, int64_t cap, int64_t *count) {
+    if (!h || cap < 0 || (cap && !out)) return fail(KTA_ERR_INVALID, "bad argument");
+    const std::vector<kta_log_crc_failure> &kept = h->log.crc.kept;
+    const size_t n = std::min<size_t>((size_t)cap, kept.size());
+    if (n) memcpy(out, kept.data(), n * sizeof(kta_log_crc_failure));
+    if (count) *count = (int64_t)kept.size();
     return KTA_OK;
 }
 
@@ -1387,6 +1479,8 @@ extern "C" int kta_reset(kta_handle *h) {
     h->records = 0;
     h->log.txn.ranges.clear();
     for (uint64_t &v : h->log.txn.totals) v = 0;
+    for (uint64_t &v : h->log.crc.totals) v = 0;   // (the check.crcs switch itself stays as it is)
+    h->log.crc.kept.clear();
     return state_reset_device(h);
 }
 

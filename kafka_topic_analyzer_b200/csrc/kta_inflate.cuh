@@ -301,7 +301,7 @@ __host__ __device__ inline uint32_t gzip_isize(const uint8_t *in, uint32_t n) {
 
 // gzip: one member (what producers write: the records section is one gzip stream).  The size pass trusts ISIZE, but not
 // beyond what DEFLATE can expand n bytes to (a forged trailer must not size the scratch buffer); the copy pass is bounded by
-// it and must produce exactly that many bytes.  The CRC32 of the trailer is not verified (like the batch CRC: check.crcs=false).
+// it and must produce exactly that many bytes.  The CRC32 of the trailer is not verified (the batch CRC is, with check.crcs on).
 __host__ __device__ inline LzWalk gzip_size(const uint8_t *in, uint32_t n) {
     if (gzip_header_len(in, n) && (uint64_t)gzip_isize(in, n) <= (uint64_t)n * 1032u + 64u) return LzWalk{gzip_isize(in, n), true};
     return LzWalk{0, false};

@@ -12,7 +12,8 @@
 // Semantics kept from the consumer: control batches (attributes bit 5) are not delivered to the application;
 // LogAppendTime batches (attributes bit 3) stamp every record with maxTimestamp; a record's timestamp is baseTimestamp +
 // timestampDelta as the consumer computes it, and only a RESULT of -1 means "not available"; key/value length -1 means
-// null.  CRCs are not verified (librdkafka's default check.crcs=false).
+// null.  CRCs are verified only when the handle's check.crcs switch is on (kta_logcrc.cuh; off by default, like librdkafka's
+// check.crcs=false).
 // Compression (attributes bits 0-2, librdkafka decompresses inside poll, src/kafka.rs:93): gzip (kta_inflate.cuh), LZ4 (frame
 // format), Snappy (raw or xerial-framed; both kta_lz4_snappy.cuh) and zstd (kta_zstd.cuh) batches are decompressed on the GPU
 // into a scratch buffer and then decoded like the others; the unassigned codes 5-7 are rejected.  Checksums inside the
@@ -37,9 +38,10 @@ constexpr int LOG_HEADER_BYTES = 61;
 // LOGB_COMPRESSED: an unknown compression codec (the unassigned codes 5-7).  LOGB_LZ4 / LOGB_SNAPPY / LOGB_GZIP / LOGB_ZSTD: the
 // records section must be decompressed first (log_unc_size_kernel, log_zstd_size_kernel for zstd, and log_decompress_kernel
 // turn such a batch into LOGB_OK).  LOGB_SKIP_ABORTED: a batch of an aborted transaction (read_committed only,
-// kta_logtxn.cuh); it replaces any codec flag, so no later pass touches the batch.
+// kta_logtxn.cuh); it replaces any codec flag, so no later pass touches the batch.  LOGB_SKIP_CRC: a batch whose CRC-32C
+// failed (check.crcs only, kta_logcrc.cuh); nothing CRC-covered of it is read, by the header pass or any later one.
 enum LogBatchFlags { LOGB_OK = 0, LOGB_SKIP_CONTROL = 1, LOGB_BAD = 2, LOGB_COMPRESSED = 4, LOGB_LZ4 = 8, LOGB_SNAPPY = 16, LOGB_GZIP = 32,
-                     LOGB_ZSTD = 64, LOGB_SKIP_ABORTED = 128 };
+                     LOGB_ZSTD = 64, LOGB_SKIP_ABORTED = 128, LOGB_SKIP_CRC = 256 };
 constexpr uint32_t LOGB_CODECS = LOGB_LZ4 | LOGB_SNAPPY | LOGB_GZIP | LOGB_ZSTD;   // batches log_decompress_kernel turns into LOGB_OK
 
 // the flag of Kafka's compression codec id 0-4 (attributes & 7: none, gzip, Snappy, LZ4, zstd)
@@ -71,10 +73,16 @@ struct LogBatchInfo {      // one per record batch, filled by log_header_kernel
     uint32_t pad;
 };
 
-// thread per batch: validate + read the header
-__global__ void log_header_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches,
-                                  int32_t partition, const int32_t *batch_partition /* per batch, or NULL = `partition` */,
-                                  LogBatchInfo *info, uint64_t *rec_count /*[nbatches+1], [b+1]*/, uint32_t *error_flags) {
+// The header pass, thread per batch: validate + read the header.  crc_failed(p, len, b, partition) is asked first for a
+// framed batch (magic 2, batchLength >= 49, inside the buffer); when it says so, the batch is LOGB_SKIP_CRC and none of
+// its CRC-covered fields is read (check.crcs, kta_logcrc.cuh).  log_header_kernel asks NoCrcCheck, which never says so.
+struct NoCrcCheck {
+    __device__ __forceinline__ bool operator()(const uint8_t *, uint32_t, int64_t, int32_t) const { return false; }
+};
+template <typename CrcCheck>
+__device__ __forceinline__ void log_header_pass(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches,
+                                                int32_t partition, const int32_t *batch_partition, LogBatchInfo *info,
+                                                uint64_t *rec_count, uint32_t *error_flags, const CrcCheck &crc_failed) {
     for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nbatches; b += (int64_t)gridDim.x * blockDim.x) {
         LogBatchInfo bi{};
         bi.off = batch_off[b];
@@ -89,9 +97,13 @@ __global__ void log_header_kernel(const uint8_t *bytes, int64_t nbytes, const ui
             // recordsCount sizes the output columns, so it must be plausible before anything is allocated for it: the
             // smallest record is 7 bytes (length, attributes, two deltas, key length, value length, header count)
             const uint32_t codec = attrs & 0x7u;
-            // (for a compressed batch the 7-bytes-per-record bound is checked against the uncompressed size later)
-            if (magic == 2 && batch_len >= LOG_HEADER_BYTES - 12 && bi.off + 12 + (uint64_t)batch_len <= (uint64_t)nbytes && count >= 0 &&
-                (codec != 0 || (uint64_t)count * 7u + (uint64_t)(LOG_HEADER_BYTES - 12) <= (uint64_t)batch_len)) {
+            const bool framed = magic == 2 && batch_len >= LOG_HEADER_BYTES - 12 && bi.off + 12 + (uint64_t)batch_len <= (uint64_t)nbytes;
+            if (framed && crc_failed(p, 12u + (uint32_t)batch_len, b, bi.partition)) {
+                bi.flags = LOGB_SKIP_CRC;
+                bi.len = 12u + (uint32_t)batch_len;
+                bi.base_offset = (int64_t)be_u64(p);
+            } else if (framed && count >= 0 &&   // (for a compressed batch the bound is checked against its uncompressed size later)
+                       (codec != 0 || (uint64_t)count * 7u + (uint64_t)(LOG_HEADER_BYTES - 12) <= (uint64_t)batch_len)) {
                 bi.len = 12u + (uint32_t)batch_len;
                 bi.base_offset = (int64_t)be_u64(p);
                 bi.base_ts = (int64_t)be_u64(p + 27);
@@ -110,6 +122,12 @@ __global__ void log_header_kernel(const uint8_t *bytes, int64_t nbytes, const ui
         rec_count[b + 1] = (uint64_t)bi.records;
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) rec_count[0] = 0;
+}
+
+__global__ void log_header_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches,
+                                  int32_t partition, const int32_t *batch_partition /* per batch, or NULL = `partition` */,
+                                  LogBatchInfo *info, uint64_t *rec_count /*[nbatches+1], [b+1]*/, uint32_t *error_flags) {
+    log_header_pass(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count, error_flags, NoCrcCheck{});
 }
 
 // The records section in[0, n) of a gzip, LZ4 or Snappy batch (flags: its LOGB_GZIP / LOGB_LZ4 / LOGB_SNAPPY): its uncompressed

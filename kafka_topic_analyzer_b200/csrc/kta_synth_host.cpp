@@ -3,6 +3,7 @@
 // includes it) and, on its own, into libkta_synth.so, so that CPU-only users — the oracle tests and bench.py's
 // reference arm — generate the same topic without mapping the GPU library.
 #include <algorithm>
+#include <array>
 #include <cstdio>
 #include <cstring>
 #include <vector>
@@ -62,6 +63,21 @@ static inline void put_varint(std::vector<uint8_t> &o, int64_t n) {
     o.push_back((uint8_t)u);
 }
 
+// CRC-32C (Castagnoli, reflected polynomial 0x82F63B78), byte at a time: the register after [p, p + n) from `crc`
+static uint32_t crc32c_update(uint32_t crc, const uint8_t *p, size_t n) {
+    static const std::array<uint32_t, 256> table = [] {
+        std::array<uint32_t, 256> t{};
+        for (uint32_t i = 0; i < 256; i++) {
+            uint32_t c = i;
+            for (int k = 0; k < 8; k++) c = (c >> 1) ^ ((c & 1u) ? 0x82F63B78u : 0u);
+            t[i] = c;
+        }
+        return t;
+    }();
+    for (size_t i = 0; i < n; i++) crc = table[(crc ^ p[i]) & 0xffu] ^ (crc >> 8);
+    return crc;
+}
+
 // Encodes records [start, start+count) (offset order) of partition `partition` as record batches of
 // `batch_records` records.  *len receives the bytes needed; nothing is written beyond cap (call twice to size).
 extern "C" int kta_synth_encode_segment_host(const kta_synth_spec *s, int32_t partition, int64_t start, int64_t count,
@@ -113,7 +129,7 @@ extern "C" int kta_synth_encode_segment_host(const kta_synth_spec *s, int32_t pa
         put_be(batch, (uint64_t)(49 + recs.size()), 4);
         put_be(batch, 0, 4);            // partitionLeaderEpoch
         batch.push_back(2);             // magic
-        put_be(batch, 0, 4);            // crc (not verified by the consumer path, check.crcs=false)
+        put_be(batch, 0, 4);            // crc: written below, once the bytes it covers are known
         put_be(batch, 0, 2);            // attributes: uncompressed, CreateTime
         put_be(batch, (uint64_t)(nb - 1), 4);
         put_be(batch, (uint64_t)base_ts, 8);
@@ -122,6 +138,9 @@ extern "C" int kta_synth_encode_segment_host(const kta_synth_spec *s, int32_t pa
         put_be(batch, 0xffff, 2);       // producerEpoch -1
         put_be(batch, 0xffffffffu, 4);  // baseSequence -1
         put_be(batch, (uint64_t)nb, 4);
+        // the CRC-32C a broker stores: from attributes (byte 21) to the end of the batch
+        const uint32_t crc = ~crc32c_update(crc32c_update(0xffffffffu, batch.data() + 21, batch.size() - 21), recs.data(), recs.size());
+        for (int i = 0; i < 4; i++) batch[17 + i] = (uint8_t)(crc >> (24 - 8 * i));
         if (out && total + (int64_t)(batch.size() + recs.size()) <= cap) {
             memcpy(out + total, batch.data(), batch.size());
             memcpy(out + total + batch.size(), recs.data(), recs.size());

@@ -4,7 +4,7 @@
 //
 // Accepted: any number of frames, with or without Frame_Content_Size (one-shot compressors write it, streaming ones such as
 // the Java client's do not), skippable frames among them, Raw / RLE / Compressed blocks, every literals and sequences mode.
-// The Content_Checksum (XXH64) is skipped, not verified, like the batch CRC and gzip's CRC32 (check.crcs=false).  Dictionaries
+// The Content_Checksum (XXH64) is skipped, not verified, like gzip's CRC32 (the batch CRC is, with check.crcs on).  Dictionaries
 // (a non-zero Dictionary_ID) are rejected: Kafka does not use them.
 //
 // Shape (like kta_inflate.cuh): every lane of the warp reads the same headers and bitstreams (lane-uniform control flow,

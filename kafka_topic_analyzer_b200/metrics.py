@@ -54,10 +54,11 @@ class KtaEngine:
     def __init__(self, num_partitions: int, count_alive_keys: bool = False, hll_precision: int = 0,
                  device: int = -1, ring_records: int = 0, ring_key_bytes: int = 0,
                  now: Optional[tuple] = None, alive_table_kib: int = 0, shard: Optional[tuple] = None,
-                 isolation_level: str = "read_uncommitted"):
+                 isolation_level: str = "read_uncommitted", check_crcs: bool = False):
         """shard = (rank, world): this engine scans only partitions p with p % world == rank (a partition-sharded job).
         isolation_level: "read_uncommitted" (every data batch of a log segment is delivered) or "read_committed" (records
-        of aborted transactions are left out, include/kta.h)."""
+        of aborted transactions are left out, include/kta.h).  check_crcs: verify every record batch's CRC-32C and skip
+        the batches that fail it (librdkafka's check.crcs; see set_check_crcs)."""
         levels = {"read_uncommitted": N.READ_UNCOMMITTED, "read_committed": N.READ_COMMITTED}
         if isolation_level not in levels:
             raise ValueError("isolation_level must be 'read_uncommitted' or 'read_committed', not %r" % (isolation_level,))
@@ -80,6 +81,8 @@ class KtaEngine:
         self._h = C.c_void_p()
         self._keep = []  # device buffers that must outlive queued scans
         check(lib().kta_create(C.byref(cfg), C.byref(self._h)))
+        if check_crcs:
+            self.set_check_crcs(True)
         self.num_partitions = num_partitions
         self.count_alive_keys = bool(count_alive_keys)
         self.hll_precision = hll_precision
@@ -192,6 +195,26 @@ class KtaEngine:
         v = [C.c_uint64() for _ in range(3)]
         check(lib().kta_log_txn_stats(self._h, *[C.byref(x) for x in v]))
         return tuple(x.value for x in v)
+
+    def set_check_crcs(self, enabled: bool) -> None:
+        """check.crcs for every later log call: a record batch whose CRC-32C does not match is skipped unread and
+        listed (log_crc_failures) instead of being decoded.  Off by default; reset() keeps the setting."""
+        check(lib().kta_log_set_check_crcs(self._h, 1 if enabled else 0))
+
+    def log_crc_stats(self):
+        """(checked batches, failed batches, failed bytes) over the successful log calls since create / reset."""
+        v = [C.c_uint64() for _ in range(3)]
+        check(lib().kta_log_crc_stats(self._h, *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
+
+    def log_crc_failures(self):
+        """The kept failures (the first N.LOG_CRC_KEEP since create / reset), in call order and, within a call, in batch
+        order: [(partition, batch bytes, base offset, stored crc, computed crc)]."""
+        n = C.c_int64()
+        check(lib().kta_log_crc_failures(self._h, None, 0, C.byref(n)))
+        buf = (N.CrcFailure * max(n.value, 1))()
+        check(lib().kta_log_crc_failures(self._h, buf, n.value, C.byref(n)))
+        return [(f.partition, f.batch_bytes, f.base_offset, f.stored_crc, f.computed_crc) for f in buf[:n.value]]
 
     def sync(self) -> None:
         check(lib().kta_sync(self._h))

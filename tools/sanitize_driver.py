@@ -11,7 +11,7 @@ from kafka_topic_analyzer_b200 import synth
 from parity import assert_parity, oracle_for
 
 NOW = (4102444800, 1)
-which = sys.argv[1:] or ["counters", "hll", "exact", "ragged", "ring", "log", "logz", "logzstd", "logtxn"]
+which = sys.argv[1:] or ["counters", "hll", "exact", "ragged", "ring", "log", "logz", "logzstd", "logtxn", "logcrc"]
 
 
 def compress_segment(seg, b0=0):
@@ -76,6 +76,25 @@ for name in which:
             e.finalize()
             assert e.log_txn_stats() == stats and e.message_metrics.overall_count() == len(want)
         print(name, "ok", stats)
+        continue
+    if name == "logcrc":   # check.crcs: batches of one to many spans at odd offsets, every third one damaged
+        import crc_codec as cc
+        import kafka_codec as kc
+        segs, bad, nb = [], 0, 0
+        for p in range(P):
+            s = bytearray(cc.set_crcs(compress_segment(synth.encode_segment(synth.make_spec(n, P), p, 0, n // P,
+                                                                             batch_records=7 + 60 * p), p)))
+            for i, o in enumerate(kc.batch_offsets(s)):
+                nb += 1
+                if i % 3 == 0:
+                    s[o + 40] ^= 1
+                    bad += 1
+            segs.append((p, bytes(s) + b"\x00" * (p % 3)))
+        with kta.KtaEngine(P, count_alive_keys=True, device=0, now=NOW, check_crcs=True) as e:
+            e.push_log_segments(segs)
+            e.finalize()
+            assert e.log_crc_stats()[:2] == (nb, bad), (e.log_crc_stats(), nb, bad)
+        print(name, "ok", nb, bad)
         continue
     key_mode = 2 if name in ("ragged", "ring") else 0
     spec = synth.make_spec(n, P, key_mode=key_mode, distinct_keys=3000, tombstone_per_10k=2500, ts_missing_per_10k=20,
