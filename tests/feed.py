@@ -295,3 +295,38 @@ def scan_log_segment(e, p, seg):
     N.check(lib().kta_scan_log_segment_device(e.handle, p, buf.data_ptr(), length, offs.data_ptr(), nb, C.byref(n)))
     e.sync()
     return n.value
+
+
+def interleaved(parts):
+    """the batches of {partition: [batch]}, round-robin over the partitions, each partition's in its order"""
+    lists = [list(parts[p]) for p in sorted(parts)]
+    out = []
+    while any(lists):
+        for l in lists:
+            if l:
+                out.append(l.pop(0))
+    return out
+
+
+LOG_ENTRIES = ("segment_host", "segments_host", "segment_device", "batches_device")
+
+
+def scan_log(e, entry, parts):
+    """{partition: [batch]} (anything with .p and .raw bytes) through one log entry point: segment_host and
+    segment_device take each partition's batches as one segment, one call per partition; segments_host takes every
+    partition's segment in one call; batches_device takes every batch, interleaved, in one device buffer.  Returns
+    (records delivered, the batches in the order they were scanned)."""
+    order = [b for p in sorted(parts) for b in parts[p]]
+    segs = [(p, b"".join(b.raw for b in parts[p])) for p in sorted(parts)]
+    if entry == "segment_host":
+        n = sum(e.push_log_segment(p, s) for p, s in segs)
+    elif entry == "segments_host":
+        n = e.push_log_segments(segs)
+    elif entry == "segment_device":
+        n = sum(scan_log_segment(e, p, s) for p, s in segs)
+    elif entry == "batches_device":
+        order = interleaved(parts)
+        n = scan_log_batches(e, stage_batches([(b.p, b.raw) for b in order]))
+    else:
+        raise ValueError(entry)
+    return n, order

@@ -12,8 +12,8 @@ sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import numpy as np  # noqa: E402
 
 from kafka_topic_analyzer_b200 import KtaEngine, KtaError, synth  # noqa: E402
+import kafka_codec as kc  # noqa: E402
 import test_log_txn as lt  # noqa: E402
-import zstd_codec as zc  # noqa: E402
 
 NOW = (4102444800, 1)
 P = 8
@@ -75,7 +75,7 @@ def one_round():
     host = synth.fill_host(spec)
     n = host.n
     codec = itertools.cycle(["gzip", "zstd", None])
-    segs = [(p, zc.recompress(synth.encode_segment(spec, p, 0, 256, batch_records=50).tobytes(), lambda: next(codec)))
+    segs = [(p, kc.recompress(synth.encode_segment(spec, p, 0, 256, batch_records=50).tobytes(), lambda: next(codec)))
             for p in range(P)]
     with Dev() as dev, KtaEngine(P, count_alive_keys=True, hll_precision=10, device=0, now=NOW, ring_records=1024,
                                  alive_table_kib=1) as e:   # a 1 KiB alive-key table: it grows
@@ -106,7 +106,7 @@ def one_round():
     t = lt.gen_topic(3, P=P, steps=80)
     with KtaEngine(P, count_alive_keys=True, device=0, now=NOW, alive_table_kib=1, isolation_level="read_committed") as e:
         for p in range(P):
-            e.push_txn_index(p, lt.txn_index(t.aborted[p]))
+            e.push_txn_index(p, kc.txn_index(t.aborted[p]))
         e.push_log_segments([(p, t.segment(p)) for p in range(P)])
         e.finalize()
         assert e.log_txn_stats() == lt.rule_model([[b for p in range(P) for b in t.batches[p]]], t.aborted)[1]

@@ -24,6 +24,15 @@ def oracle_over(per, count_alive_keys=False, track_stream=False, now=NOW):
     return o
 
 
+def oracle_in_order(records, count_alive_keys=True, now=NOW):
+    """The CPU oracle over (partition, ts, key, value_len) records in the order given, which must be the order the
+    engine delivered them: the exact alive-key count of a hash that several partitions write depends on it."""
+    o = Oracle(count_alive_keys=count_alive_keys, now=now)
+    for p, ts, key, vl in records:
+        o.handle_message(p, ts, key, vl)
+    return o
+
+
 def expected(mode, t, hll_p):
     """(oracle, assert_parity keywords) for a scan of t in mode counters, hll (the in-stream sketch) or exact (-c); t is
     a HostTopic or partition lists"""

@@ -12,13 +12,10 @@ from dataclasses import dataclass, field
 import numpy as np
 import pytest
 
-import crc_codec as cc
 import kafka_codec as kc
-import zstd_codec as zc
-from feed import scan_log_batches, scan_log_segment, stage_batches
+from feed import LOG_ENTRIES, interleaved, scan_log, scan_log_batches, scan_log_segment, stage_batches
 from kafka_topic_analyzer_b200 import KtaEngine, KtaError, _native, lib, synth
-from oracle_lib import Oracle
-from parity import assert_parity
+from parity import assert_parity, oracle_in_order
 
 NOW = (4102444800, 123456789)
 TS0 = 1_700_000_000_000
@@ -26,7 +23,6 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 # the span size of the device pass (every span but a batch's first is this long): the region lengths below straddle it
 SPAN = int(re.search(r"LOG_CRC_SPAN = (\d+)", open(os.path.join(ROOT, "kafka_topic_analyzer_b200", "csrc", "kta_logcrc.cuh")).read()).group(1))
 CODECS = (None, "gzip", "snappy", "snappy-xerial", "lz4", "zstd", "zstd-stream")
-ENTRIES = ["segment_host", "segments_host", "segment_device", "batches_device"]
 
 
 # ---- batches whose delivered records are known ------------------------------------------------------------------------
@@ -50,7 +46,7 @@ def batch(p, off, recs, codec=None, values=None):
     """recs [(ts, key, value_len)] as one batch at baseOffset `off` with its real CRC; values: explicit value bytes"""
     base = recs[0][0] if recs else TS0 + off
     rows = [(j, ts - base, k, vl, (), None if values is None else values[j]) for j, (ts, k, vl) in enumerate(recs)]
-    return B(p, cc.set_crcs(zc.encode_batch(off, base, rows, compression=codec)), list(recs))
+    return B(p, kc.set_crcs(kc.encode_batch(off, base, rows, compression=codec)), list(recs))
 
 
 def random_recs(rng, n, off, keys=30):
@@ -95,43 +91,9 @@ def seg(batches):
     return b"".join(b.raw for b in batches)
 
 
-def interleaved(parts):
-    lists = [list(parts[p]) for p in sorted(parts)]
-    out = []
-    while any(lists):
-        for l in lists:
-            if l:
-                out.append(l.pop(0))
-    return out
-
-
-def run(e, entry, parts):
-    """parts {p: [B]} through one entry point; returns (records delivered, the batches in the order they were scanned)"""
-    P = sorted(parts)
-    order = [b for p in P for b in parts[p]]
-    if entry == "segment_host":
-        n = sum(e.push_log_segment(p, seg(parts[p])) for p in P)
-    elif entry == "segments_host":
-        n = e.push_log_segments([(p, seg(parts[p])) for p in P])
-    elif entry == "segment_device":
-        n = sum(scan_log_segment(e, p, seg(parts[p])) for p in P)
-    else:
-        order = interleaved(parts)
-        n = scan_log_batches(e, stage_batches([(b.p, b.raw) for b in order]))
-    return n, order
-
-
-def oracle(batches, exact=True):
-    o = Oracle(count_alive_keys=exact, now=NOW)
-    for b in batches:
-        if not b.bad:
-            for ts, key, vl in b.recs:
-                o.handle_message(b.p, ts, key, vl)
-    return o
-
-
-def delivered(batches):
-    return sum(len(b.recs) for b in batches if not b.bad)
+def passed(batches):
+    """the (partition, ts, key, value_len) records of the batches that pass, in order"""
+    return [(b.p, *r) for b in batches if not b.bad for r in b.recs]
 
 
 def failure(b: B, computed):
@@ -144,11 +106,11 @@ def engine(P, **kw):
 
 # ---- CPU ------------------------------------------------------------------------------------------------------------
 def test_crc32c_known_answers():
-    assert cc.crc32c(b"123456789") == 0xE3069283
-    assert cc.crc32c(bytes(32)) == 0x8A9136AA                        # RFC 3720 B.4
-    assert cc.crc32c(b"\xff" * 32) == 0x62A8AB43
-    assert cc.crc32c(bytes(range(32))) == 0x46DD794E
-    assert cc.crc32c(bytes(range(31, -1, -1))) == 0x113FDB5C
+    assert kc.crc32c(b"123456789") == 0xE3069283
+    assert kc.crc32c(bytes(32)) == 0x8A9136AA                        # RFC 3720 B.4
+    assert kc.crc32c(b"\xff" * 32) == 0x62A8AB43
+    assert kc.crc32c(bytes(range(32))) == 0x46DD794E
+    assert kc.crc32c(bytes(range(31, -1, -1))) == 0x113FDB5C
 
 
 @pytest.mark.parametrize("key_mode,batch_records", [(0, 100), (1, 333), (2, 1000)])
@@ -159,8 +121,8 @@ def test_synth_encoder_writes_real_crcs(key_mode, batch_records):
         offs = kc.batch_offsets(s)
         assert len(offs) == -(-2000 // batch_records)
         for o in offs:
-            assert struct.unpack(">I", s[o + 17:o + 21])[0] == cc.batch_crc(s, o)
-        assert cc.set_crcs(s) == s
+            assert struct.unpack(">I", s[o + 17:o + 21])[0] == kc.batch_crc(s, o)
+        assert kc.set_crcs(s) == s
 
 
 def test_set_crcs_round_trip():
@@ -169,15 +131,15 @@ def test_set_crcs_round_trip():
     s = kc.encode_partition(recs, rng, max_batch=40)                  # CRC fields 0
     offs = kc.batch_offsets(s)
     assert all(s[o + 17:o + 21] == bytes(4) for o in offs)
-    t = cc.set_crcs(s)
+    t = kc.set_crcs(s)
     assert len(t) == len(s) and kc.batch_offsets(t) == offs
     for o in offs:
         assert t[o:o + 17] == s[o:o + 17] and t[o + 21:o + 61] == s[o + 21:o + 61]
-        assert struct.unpack(">I", t[o + 17:o + 21])[0] == cc.crc32c(t[o + 21:o + 12 + struct.unpack(">i", t[o + 8:o + 12])[0]])
-    assert cc.set_crcs(t) == t
+        assert struct.unpack(">I", t[o + 17:o + 21])[0] == kc.crc32c(t[o + 21:o + 12 + struct.unpack(">i", t[o + 8:o + 12])[0]])
+    assert kc.set_crcs(t) == t
     u = bytearray(t)
     u[offs[1] + 17:offs[1] + 21] = b"\xde\xad\xbe\xef"
-    assert cc.set_crcs(bytes(u)) == t
+    assert kc.set_crcs(bytes(u)) == t
 
 
 def test_cli_rejects_a_bad_check_crcs_value(tmp_path):
@@ -191,15 +153,15 @@ def test_cli_rejects_a_bad_check_crcs_value(tmp_path):
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-@pytest.mark.parametrize("entry", ENTRIES)
+@pytest.mark.parametrize("entry", LOG_ENTRIES)
 def test_valid_crcs_deliver_everything(entry):
     parts = gen(11)
     nb = sum(len(v) for v in parts.values())
     with engine(4) as e:
-        n, order = run(e, entry, parts)
+        n, order = scan_log(e, entry, parts)
         e.finalize()
-        o = oracle(order)
-        assert n == delivered(order)
+        o = oracle_in_order(passed(order))
+        assert n == len(passed(order))
         assert_parity(e, o, 4, check_alive=True, hll_regs=o.hll_alive_regs(10))
         assert e.log_crc_stats() == (nb, 0, 0) and e.log_crc_failures() == []
 
@@ -213,7 +175,7 @@ def test_every_crc_flipped_delivers_nothing(entry):
         for b in v:
             flip_crc(b)
     with engine(4) as e:
-        n, order = run(e, entry, parts)
+        n, order = scan_log(e, entry, parts)
         e.finalize()
         assert n == 0 and e.message_metrics.overall_count() == 0
         assert e.log_crc_failures() == [failure(b, ref[id(b)]) for b in order]
@@ -224,9 +186,9 @@ def sized_batch(p, off, region, rng):
     """a batch whose CRC region (attributes to the end) is `region` bytes long: below one record (47 bytes), a batch
     without records followed by unread bytes; else one record whose value fills the rest"""
     if region < 47:
-        raw = bytearray(zc.encode_batch(off, TS0 + off, [])) + rng.bytes(region - 40)
+        raw = bytearray(kc.encode_batch(off, TS0 + off, [])) + rng.bytes(region - 40)
         raw[8:12] = struct.pack(">i", len(raw) - 12)
-        return B(p, cc.set_crcs(bytes(raw)))
+        return B(p, kc.set_crcs(bytes(raw)))
     v = max(0, region - 49)
     for _ in range(4):
         b = batch(p, off, [(TS0 + off, None, v)], values=[rng.bytes(v)])
@@ -261,8 +223,8 @@ def test_crc_region_lengths():
         with engine(1) as e:
             n = scan_log_batches(e, stage_batches([(0, seg(out))]))
             e.finalize()
-            assert n == delivered(out)
-            assert_parity(e, oracle(out), 1, check_alive=True)
+            assert n == len(passed(out))
+            assert_parity(e, oracle_in_order(passed(out)), 1, check_alive=True)
             want = [failure(b, c) for b, c in zip(out, ref)] if flipped else []
             assert e.log_crc_failures() == want
 
@@ -280,11 +242,11 @@ def test_batches_at_odd_byte_offsets():
     with engine(3) as e:
         n = scan_log_batches(e, staged)
         e.finalize()
-        assert n == delivered(order)
-        assert_parity(e, oracle(order), 3, check_alive=True)
+        assert n == len(passed(order))
+        assert_parity(e, oracle_in_order(passed(order)), 3, check_alive=True)
         bad = [b for b in order if b.bad]
         assert [f[:4] for f in e.log_crc_failures()] == [failure(b, 0)[:4] for b in bad]
-        assert [f[4] for f in e.log_crc_failures()] == [cc.batch_crc(b.raw, 0) for b in bad]
+        assert [f[4] for f in e.log_crc_failures()] == [kc.batch_crc(b.raw, 0) for b in bad]
 
 
 def _damaged(kind, rng):
@@ -306,9 +268,9 @@ def _damaged(kind, rng):
 def test_single_bit_damage(kind):
     batches, msg = _damaged(kind, np.random.default_rng(21))
     with engine(1) as e:
-        assert e.push_log_segment(0, seg(batches)) == delivered(batches)
+        assert e.push_log_segment(0, seg(batches)) == len(passed(batches))
         e.finalize()
-        assert_parity(e, oracle(batches), 1, check_alive=True)
+        assert_parity(e, oracle_in_order(passed(batches)), 1, check_alive=True)
         assert e.log_crc_stats() == (len(batches), 1, len(batches[2].raw))
     with KtaEngine(1, count_alive_keys=True, now=NOW) as e:
         with pytest.raises(KtaError, match=msg):
@@ -316,24 +278,13 @@ def test_single_bit_damage(kind):
 
 
 # ---- read_committed ---------------------------------------------------------------------------------------------------
-def with_producer(raw: bytes, pid: int) -> bytes:
-    b = bytearray(raw)
-    b[43:57] = struct.pack(">qhi", pid, 0, 0)
-    return bytes(b)
-
-
 def txn(p, off, recs, pid):
     rows = [(j, ts - recs[0][0], k, vl) for j, (ts, k, vl) in enumerate(recs)]
-    return B(p, cc.set_crcs(with_producer(kc.encode_batch(off, recs[0][0], rows, attributes=0x10), pid)), list(recs))
+    return B(p, kc.set_crcs(kc.txn_batch(off, recs[0][0], rows, pid)), list(recs))
 
 
-def marker(p, off, pid, commit):
-    rec = [(0, 0, struct.pack(">hh", 0, 1 if commit else 0), None, (), struct.pack(">hi", 0, 3))]
-    return B(p, cc.set_crcs(with_producer(kc.encode_batch(off, TS0, rec, attributes=0x30), pid)))
-
-
-def txn_index(entries) -> bytes:
-    return b"".join(struct.pack(">hqqqq", 0, q, f, l, l + 1) for q, f, l in entries)
+def abort_marker(p, off, pid):
+    return B(p, kc.set_crcs(kc.marker(off, pid, 0, False, TS0)))
 
 
 @pytest.mark.gpu
@@ -342,10 +293,10 @@ def test_read_committed_corrupted_abort_marker():
     recs = [(TS0 + i, b"k%d" % i, 10) for i in range(4)]
     plain = batch(0, 6, [(TS0 + 6, b"z", 1)])
     for with_index in (False, True):
-        bs = [txn(0, 0, recs, 5), damage(marker(0, 4, 5, commit=False), at=70), plain]
+        bs = [txn(0, 0, recs, 5), damage(abort_marker(0, 4, 5), at=70), plain]
         with engine(1, isolation_level="read_committed") as e:
             if with_index:
-                e.push_txn_index(0, txn_index([(5, 0, 4)]))
+                e.push_txn_index(0, kc.txn_index([(5, 0, 4)]))
             n = e.push_log_segment(0, seg(bs))
             e.finalize()
             if with_index:
@@ -353,20 +304,20 @@ def test_read_committed_corrupted_abort_marker():
                 assert n == 1 and e.log_txn_stats() == (1, 4, 0)
             else:
                 assert n == 5 and e.log_txn_stats() == (0, 0, 4)
-            assert_parity(e, oracle(bs), 1, check_alive=True)
+            assert_parity(e, oracle_in_order(passed(bs)), 1, check_alive=True)
             assert e.log_crc_stats()[1] == 1 and e.log_crc_failures()[0][2] == 4
 
 
 @pytest.mark.gpu
 def test_read_committed_corrupted_aborted_batch_counts_as_crc_failure():
     recs = [(TS0 + i, b"k%d" % i, 10) for i in range(4)]
-    bs = [damage(txn(0, 0, recs, 5), at=61 + 3), marker(0, 4, 5, commit=False), batch(0, 5, [(TS0 + 5, b"z", 1)])]
+    bs = [damage(txn(0, 0, recs, 5), at=61 + 3), abort_marker(0, 4, 5), batch(0, 5, [(TS0 + 5, b"z", 1)])]
     with engine(1, isolation_level="read_committed") as e:
         assert e.push_log_segment(0, seg(bs)) == 1
         e.finalize()
         assert e.log_txn_stats() == (0, 0, 0)
         assert e.log_crc_stats() == (3, 1, len(bs[0].raw))
-        assert_parity(e, oracle(bs), 1, check_alive=True)
+        assert_parity(e, oracle_in_order(passed(bs)), 1, check_alive=True)
 
 
 @pytest.mark.gpu
@@ -378,7 +329,8 @@ def test_alive_keys_skipped_batch_held_the_last_write():
         assert e.push_log_segment(0, seg(bs)) == 2
         e.finalize()
         assert e.alive_keys() == 2
-        assert_parity(e, oracle(bs), 1, check_alive=True, hll_regs=oracle(bs).hll_alive_regs(10))
+        o = oracle_in_order(passed(bs))
+        assert_parity(e, o, 1, check_alive=True, hll_regs=o.hll_alive_regs(10))
     with KtaEngine(1, count_alive_keys=True, now=NOW) as e:
         assert e.push_log_segment(0, seg(bs)) == 4
         e.finalize()
@@ -418,7 +370,7 @@ def test_handle_state():
         assert e.push_log_segments([(1, seg(b))]) == 0
         got = e.log_crc_failures()
         assert len(got) == _native.LOG_CRC_KEEP
-        assert got == [failure(x, cc.batch_crc(x.raw, 0)) for x in (a + b)[:_native.LOG_CRC_KEEP]]
+        assert got == [failure(x, kc.batch_crc(x.raw, 0)) for x in (a + b)[:_native.LOG_CRC_KEEP]]
         assert e.log_crc_stats()[:2] == (6000, 6000)
 
 
@@ -432,10 +384,7 @@ def test_default_off_accepts_zero_crcs():
     with KtaEngine(1, count_alive_keys=True, now=NOW) as e:
         assert e.push_log_segment(0, s) == 400
         e.finalize()
-        o = Oracle(count_alive_keys=True, now=NOW)
-        for ts, k, vl in recs:
-            o.handle_message(0, ts, k, vl)
-        assert_parity(e, o, 1, check_alive=True)
+        assert_parity(e, oracle_in_order((0, *r) for r in recs), 1, check_alive=True)
         e.set_check_crcs(True)
         assert e.push_log_segment(0, s) == 0
         assert e.log_crc_stats()[:2] == (nb, nb)
@@ -465,7 +414,7 @@ def test_cli_check_crcs(tmp_path):
         victim.bad = check
         r = subprocess.run(base + (["--librdkafka", "check.crcs=true"] if check else []), capture_output=True, text=True)
         assert r.returncode == 0, r.stderr
-        o = oracle([b for p in range(P) for b in parts[p]])
+        o = oracle_in_order(passed([b for p in range(P) for b in parts[p]]))
         lines = r.stdout.splitlines()
         assert "Alive keys: %d" % o.scalar("sum_all_alive") in lines
         assert "Topic Size: %d bytes" % o.scalar("overall_size") in lines
@@ -480,6 +429,6 @@ def test_cli_check_crcs(tmp_path):
         if check:
             assert warn == ["warning: Kafka error: MessageSet at offset %d (%d bytes) of partition 1 failed CRC32C check "
                             "(original 0x%08x != calculated 0x%08x)" % (victim.base_offset, len(victim.raw), stored,
-                                                                       cc.batch_crc(victim.raw, 0))]
+                                                                       kc.batch_crc(victim.raw, 0))]
         else:
             assert warn == []

@@ -6,7 +6,6 @@ decided commit, abort or open before its batches are written).  A CPU test check
 walks the encoded bytes as librdkafka does, driven by the aborted-transaction list; the GPU tests compare the engine
 with the oracle fed only the delivered records."""
 import struct
-import zlib
 from dataclasses import dataclass, field
 from typing import Optional
 
@@ -14,44 +13,13 @@ import numpy as np
 import pytest
 
 import kafka_codec as kc
-from feed import scan_log_batches, scan_log_segment, stage_batches
+from feed import LOG_ENTRIES, scan_log, scan_log_batches, stage_batches
+from kafka_codec import marker, marker_record_key, txn_batch, txn_index, with_producer
 from kafka_topic_analyzer_b200 import KtaEngine, KtaError
-from oracle_lib import Oracle
-from parity import assert_parity
+from parity import assert_parity, oracle_in_order
 
 NOW = (4102444800, 123456789)
 TS0 = 1_700_000_000_000
-
-
-# ---- transactional encoder ------------------------------------------------------------------------------------------
-def with_producer(batch: bytes, pid: int, epoch: int = 0, base_seq: int = 0) -> bytes:
-    """a batch of kafka_codec.encode_batch with its producerId / producerEpoch / baseSequence set (header bytes 43-56)"""
-    b = bytearray(batch)
-    b[43:57] = struct.pack(">qhi", pid, epoch, base_seq)
-    return bytes(b)
-
-
-def txn_batch(base_offset, base_ts, records, pid, epoch=0, base_seq=0, compression=None, transactional=True):
-    """records as for kafka_codec.encode_batch; attributes bit 4 = transactional"""
-    return with_producer(kc.encode_batch(base_offset, base_ts, records, attributes=0x10 if transactional else 0,
-                                         compression=compression), pid, epoch, base_seq)
-
-
-def marker_record_key(commit: bool, version: int = 0) -> bytes:
-    return struct.pack(">hh", version, 1 if commit else 0)
-
-
-def marker(offset, pid, epoch, commit, ts=TS0, key=None):
-    """a control batch (attributes bits 4 and 5) holding one ABORT / COMMIT marker record: key version | type, value
-    version | coordinatorEpoch"""
-    key = marker_record_key(commit) if key is None else key
-    return with_producer(kc.encode_batch(offset, ts, [(0, 0, key, None, (), struct.pack(">hi", 0, 3))], attributes=0x30),
-                         pid, epoch)
-
-
-def txn_index(entries) -> bytes:
-    """.txnindex image: (pid, firstOffset, lastOffset[, lastStableOffset]) → 34-byte big-endian entries, version 0"""
-    return b"".join(struct.pack(">hqqqq", 0, e[0], e[1], e[2], e[3] if len(e) > 3 else e[2] + 1) for e in entries)
 
 
 # ---- generator: topics with transactions decided by construction ----------------------------------------------------
@@ -88,7 +56,7 @@ class Topic:
 
 def _encode(b: Bt) -> bytes:
     if b.is_marker:
-        return marker(b.off, b.pid, b.epoch, b.commit, ts=TS0 + b.off)
+        return marker(b.off, b.pid, b.epoch, b.commit, TS0 + b.off)
     if not b.recs:
         return txn_batch(b.off, TS0 + b.off, [], b.pid, b.epoch, transactional=b.txn is not None)
     base = b.recs[0][0]
@@ -183,36 +151,6 @@ def rule_model(calls, ranges):
 
 
 # ---- a second model: the bytes walked as librdkafka's read_committed consumer walks them ----------------------------
-def _uv(b, p):
-    u, sh = 0, 0
-    while True:
-        x = b[p]
-        p += 1
-        u |= (x & 0x7F) << sh
-        sh += 7
-        if not x & 0x80:
-            return (u >> 1) ^ -(u & 1), p
-
-
-def _decompress(codec_bits, data):
-    import pyarrow as pa
-    if codec_bits == 0:
-        return data
-    if codec_bits == 1:
-        return zlib.decompress(data, 31)
-    if codec_bits == 3:
-        return pa.CompressedInputStream(pa.BufferReader(data), "lz4").read()
-    if codec_bits == 2:
-        n, p = 0, 0
-        for sh in range(0, 35, 7):                # raw snappy: uncompressed length first
-            n |= (data[p] & 0x7F) << sh
-            p += 1
-            if not data[p - 1] & 0x80:
-                break
-        return pa.decompress(data, decompressed_size=n, codec="snappy", asbytes=True)
-    raise ValueError(codec_bits)
-
-
 def librdkafka_walk(seg: bytes, aborted_txns):
     """A read_committed consumer over one partition's bytes, given the fetch response's aborted transactions [(pid,
     firstOffset)]: a transactional batch whose producer has a pending aborted transaction starting at or before it is
@@ -220,36 +158,17 @@ def librdkafka_walk(seg: bytes, aborted_txns):
     pending = {}
     for pid, first in sorted(aborted_txns, key=lambda e: e[1]):
         pending.setdefault(pid, []).append(first)
-    out, pos = [], 0
-    while pos + 61 <= len(seg):
-        base_off, bl = struct.unpack(">qi", seg[pos:pos + 12])
-        attrs, = struct.unpack(">h", seg[pos + 21:pos + 23])
-        base_ts, = struct.unpack(">q", seg[pos + 27:pos + 35])
-        pid, = struct.unpack(">q", seg[pos + 43:pos + 51])
-        cnt, = struct.unpack(">i", seg[pos + 57:pos + 61])
-        body = _decompress(attrs & 7, seg[pos + 61:pos + 12 + bl])
-        pos += 12 + bl
-        recs, p = [], 0
-        for _ in range(cnt):
-            ln, p = _uv(body, p)
-            end = p + ln
-            p += 1
-            tsd, p = _uv(body, p)
-            _, p = _uv(body, p)
-            kl, p = _uv(body, p)
-            key = None if kl < 0 else bytes(body[p:p + kl])
-            p += max(kl, 0)
-            vl, p = _uv(body, p)
-            recs.append((base_ts + tsd, key, None if vl < 0 else vl))
-            p = end
-        if attrs & 0x20:
+    out = []
+    for b in kc.read_segment(seg):
+        waiting = pending.get(b.producer_id)
+        if b.attributes & 0x20:
             # an ABORT marker retires the producer's pending aborted transaction that started before it
-            if recs and struct.unpack(">hh", recs[0][1])[1] == 0 and pending.get(pid) and pending[pid][0] <= base_off:
-                pending[pid].pop(0)
+            if b.records and struct.unpack(">hh", b.records[0][2])[1] == 0 and waiting and waiting[0] <= b.base_offset:
+                waiting.pop(0)
             continue
-        if attrs & 0x10 and pending.get(pid) and pending[pid][0] <= base_off:
+        if b.attributes & 0x10 and waiting and waiting[0] <= b.base_offset:
             continue
-        out += recs
+        out += [(ts, key, vl) for _, ts, key, vl in b.records]
     return out
 
 
@@ -259,7 +178,7 @@ def test_encoder_fields_and_index_image():
     b = txn_batch(7, TS0, [(0, 0, b"k", 3)], pid=0x0102030405060708, epoch=9, base_seq=44)
     assert b[:21] == plain[:21] and b[23:43] == plain[23:43] and b[57:] == plain[57:]
     assert b[21:23] == b"\x00\x10" and struct.unpack(">qhi", b[43:57]) == (0x0102030405060708, 9, 44)
-    m = marker(20, 5, 2, commit=False)
+    m = marker(20, 5, 2, commit=False, ts=TS0)
     assert m[21:23] == b"\x00\x30" and struct.unpack(">qh", m[43:53]) == (5, 2)
     assert librdkafka_walk(m, []) == []
     img = txn_index([(5, 10, 20, 21), (6, 1, 2)])
@@ -278,63 +197,24 @@ def test_generated_truth_matches_a_librdkafka_walk_of_the_bytes(seed):
 
 
 # ---- GPU tests --------------------------------------------------------------------------------------------------------
-def _oracle(delivered, exact=True):
-    o = Oracle(count_alive_keys=exact, now=NOW)
-    for p, (ts, key, vl) in delivered:
-        o.handle_message(p, ts, key, vl)
-    return o
-
-
-def _all_records(calls):
-    return [(b.p, r) for call in calls for b in call if not b.is_marker for r in b.recs]
-
-
-def _interleaved(t):
-    """the batches of every partition, round-robin, each partition's in offset order"""
-    lists = [list(t.batches[p]) for p in sorted(t.batches)]
-    out = []
-    while any(lists):
-        for l in lists:
-            if l:
-                out.append(l.pop(0))
-    return out
-
-
-def _staged(batches):
-    """Bt batches, in this order, in one device buffer"""
-    return stage_batches([(b.p, b.raw) for b in batches])
-
-
 @pytest.mark.gpu
-@pytest.mark.parametrize("entry", ["segment_host", "segments_host", "segment_device", "batches_device"])
+@pytest.mark.parametrize("entry", LOG_ENTRIES)
 def test_four_entry_points(entry):
     """every marker in the call: the engine equals the oracle over the delivered records, for read_committed; the same
     bytes on a read_uncommitted handle deliver every data record, as before"""
     t = gen_topic(7, P=4)
     P = 4
-    if entry in ("segments_host", "batches_device"):
-        calls = [_interleaved(t)] if entry == "batches_device" else [[b for p in range(P) for b in t.batches[p]]]
-    else:
-        calls = [t.batches[p] for p in range(P)]
-    want, stats = rule_model(calls, {})
-    assert sorted(map(repr, want)) == sorted(repr((p, r)) for p in range(P) for r in t.truth(p))
-    assert stats[0] > 0 and stats[2] > 0
     for level in ("read_committed", "read_uncommitted"):
         with KtaEngine(P, count_alive_keys=True, hll_precision=10, now=NOW, isolation_level=level) as e:
-            total = 0
-            if entry == "segment_host":
-                for p in range(P):
-                    total += e.push_log_segment(p, t.segment(p))
-            elif entry == "segments_host":
-                total = e.push_log_segments([(p, t.segment(p)) for p in range(P)])
-            elif entry == "segment_device":
-                for p in range(P):
-                    total += scan_log_segment(e, p, t.segment(p))
-            else:
-                total = scan_log_batches(e, _staged(calls[0]))
+            total, order = scan_log(e, entry, t.batches)
             e.finalize()
-            exp = want if level == "read_committed" else _all_records(calls)
-            o = _oracle(exp)
+            # the rule decides a batch by the later markers of its own partition in its call, so one call over `order`
+            # stands for the one call per partition of segment_host and segment_device too
+            want, stats = rule_model([order], {})
+            assert sorted(map(repr, want)) == sorted(repr((p, r)) for p in range(P) for r in t.truth(p))
+            assert stats[0] > 0 and stats[2] > 0
+            exp = want if level == "read_committed" else [(b.p, r) for b in order if not b.is_marker for r in b.recs]
+            o = oracle_in_order((p, *r) for p, r in exp)
             assert total == len(exp)
             assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(10))
             if level == "read_committed":
@@ -363,7 +243,7 @@ def test_markers_in_a_later_call_need_the_index():
             n = e.push_log_segments([(p, t.segment(p, 0, cut[p])) for p in range(P)])
             n += e.push_log_segments([(p, t.segment(p, cut[p])) for p in range(P)])
             e.finalize()
-            o = _oracle(want)
+            o = oracle_in_order((p, *r) for p, r in want)
             assert n == len(want)
             assert_parity(e, o, P, check_alive=True)
             assert e.log_txn_stats() == stats
@@ -380,19 +260,19 @@ def test_same_producer_id_in_two_partitions_and_epoch_bump():
     of the bumped epoch commits; an empty transaction and a zero-record batch change nothing"""
     seg0 = (txn_batch(0, TS0, [(0, 0, b"a", 1), (1, 1, b"b", 2)], pid=77, epoch=3)
             + txn_batch(2, TS0, [(0, 0, b"n", 5)], pid=-1, transactional=False)
-            + marker(3, 77, 4, commit=False)
+            + marker(3, 77, 4, commit=False, ts=TS0)
             + txn_batch(4, TS0 + 4, [(0, 0, b"c", 3)], pid=77, epoch=4)
-            + marker(5, 77, 4, commit=True)
-            + marker(6, 78, 0, commit=True)                                     # empty transaction
+            + marker(5, 77, 4, commit=True, ts=TS0)
+            + marker(6, 78, 0, commit=True, ts=TS0)                             # empty transaction
             + txn_batch(7, TS0 + 7, [], pid=78)                                 # zero records, then aborted
-            + marker(8, 78, 0, commit=False))
+            + marker(8, 78, 0, commit=False, ts=TS0))
     seg1 = (txn_batch(0, TS0, [(0, 0, b"a", 7)], pid=77, epoch=3)
-            + marker(1, 77, 3, commit=True))
-    want = [(0, (TS0, b"n", 5)), (0, (TS0 + 4, b"c", 3)), (1, (TS0, b"a", 7))]
+            + marker(1, 77, 3, commit=True, ts=TS0))
+    want = [(0, TS0, b"n", 5), (0, TS0 + 4, b"c", 3), (1, TS0, b"a", 7)]
     with KtaEngine(2, count_alive_keys=True, now=NOW, isolation_level="read_committed") as e:
         assert e.push_log_segments([(0, seg0), (1, seg1)]) == 3
         e.finalize()
-        assert_parity(e, _oracle(want), 2, check_alive=True)
+        assert_parity(e, oracle_in_order(want), 2, check_alive=True)
         assert e.log_txn_stats() == (2, 2, 0)
 
 
@@ -401,12 +281,12 @@ def test_aborted_overwrite_and_tombstone_do_not_win_the_alive_table():
     seg = (txn_batch(0, TS0, [(0, 0, b"k1", 5), (1, 1, b"k2", 5)], pid=-1, transactional=False)
            + txn_batch(2, TS0, [(0, 0, b"k1", None), (1, 0, b"k3", 4)], pid=9)      # tombstone of k1, new key k3: aborted
            + txn_batch(4, TS0, [(0, 0, b"k2", None)], pid=10)                      # tombstone of k2: committed
-           + marker(5, 9, 0, commit=False) + marker(6, 10, 0, commit=True))
+           + marker(5, 9, 0, commit=False, ts=TS0) + marker(6, 10, 0, commit=True, ts=TS0))
     with KtaEngine(1, count_alive_keys=True, now=NOW, isolation_level="read_committed") as e:
         assert e.push_log_segment(0, seg) == 3
         e.finalize()
         assert e.alive_keys() == 1                                                  # k1 only
-        assert_parity(e, _oracle([(0, (TS0, b"k1", 5)), (0, (TS0 + 1, b"k2", 5)), (0, (TS0, b"k2", None))]), 1, check_alive=True)
+        assert_parity(e, oracle_in_order([(0, TS0, b"k1", 5), (0, TS0 + 1, b"k2", 5), (0, TS0, b"k2", None)]), 1, check_alive=True)
     with KtaEngine(1, count_alive_keys=True, now=NOW) as e:
         assert e.push_log_segment(0, seg) == 5
         e.finalize()
@@ -418,7 +298,8 @@ def test_damaged_aborted_compressed_batch_is_left_out_unread():
     recs = [(i, i, b"key-%d" % i, 30) for i in range(40)]
     bad = bytearray(txn_batch(0, TS0, recs, pid=5, compression="gzip"))
     bad[75] ^= 0xFF                                                                 # inside the deflate stream
-    seg = bytes(bad) + txn_batch(40, TS0, recs[:3], pid=6, compression="lz4") + marker(43, 5, 0, False) + marker(44, 6, 0, True)
+    seg = (bytes(bad) + txn_batch(40, TS0, recs[:3], pid=6, compression="lz4") + marker(43, 5, 0, False, ts=TS0)
+           + marker(44, 6, 0, True, ts=TS0))
     with KtaEngine(1, now=NOW, isolation_level="read_committed") as e:
         assert e.push_log_segment(0, seg) == 3
         e.finalize()
@@ -431,16 +312,16 @@ def test_damaged_aborted_compressed_batch_is_left_out_unread():
 @pytest.mark.gpu
 def test_malformed_markers_order_and_indexes_are_refused():
     d = txn_batch(0, TS0, [(0, 0, b"k", 1)], pid=5)
-    good = d + marker(1, 5, 0, True)
-    comp = bytearray(marker(1, 5, 0, True))
+    good = d + marker(1, 5, 0, True, ts=TS0)
+    comp = bytearray(marker(1, 5, 0, True, ts=TS0))
     comp[22] |= 1                                                                   # a "gzip" control batch
     bad_markers = [
         bytes(comp),
-        marker(1, 5, 0, True, key=b"\x00\x00\x01"),                                 # key length 3
-        marker(1, 5, 0, True, key=marker_record_key(True, version=1)),              # version 1
+        marker(1, 5, 0, True, ts=TS0, key=b"\x00\x00\x01"),                         # key length 3
+        marker(1, 5, 0, True, ts=TS0, key=marker_record_key(True, version=1)),      # version 1
         with_producer(kc.encode_batch(1, TS0, [], attributes=0x30), 5),             # no record
     ]
-    trunc = bytearray(marker(1, 5, 0, True))
+    trunc = bytearray(marker(1, 5, 0, True, ts=TS0))
     trunc[61] = 0x7E                                                                # record length past the batch
     bad_markers.append(bytes(trunc))
     with KtaEngine(1, now=NOW, isolation_level="read_committed") as e:
@@ -501,20 +382,20 @@ def test_many_transactional_batches_in_one_call():
                         rec = (TS0 + off, keys[kidx[step, q]], int(kidx[step, q] % 97))
                         out.append((txn_batch(off, rec[0], [(0, 0, rec[1], rec[2])], pid=pid, epoch=t), None if abort[q] else rec))
                     else:
-                        out.append((marker(off, pid, t, commit=not abort[q]), None))
+                        out.append((marker(off, pid, t, commit=not abort[q], ts=TS0), None))
                         n_ab += 4 * int(abort[q])
                     off += 1
         per.append(out)
     order = rng.permutation(P)                 # the partitions interleaved batch by batch, in a shuffled order
     inter = [(int(p), per[p][i]) for i in range(len(per[0])) for p in order]
     assert sum(1 for _, (raw, _r) in inter if raw[22] == 0x10) == 1 << 17
-    want = [(p, rec) for p, (_, rec) in inter if rec is not None]
+    want = [(p, *rec) for p, (_, rec) in inter if rec is not None]
     with KtaEngine(P, count_alive_keys=True, now=NOW, isolation_level="read_committed") as e:
         n = scan_log_batches(e, stage_batches([(p, raw) for p, (raw, _) in inter]))
         e.finalize()
         assert n == len(want)
         assert e.log_txn_stats() == (n_ab, n_ab, 0)
-        assert_parity(e, _oracle(want), P, check_alive=True)
+        assert_parity(e, oracle_in_order(want), P, check_alive=True)
 
 
 @pytest.mark.gpu
@@ -544,7 +425,7 @@ def test_cli_isolation_level(tmp_path):
         r = subprocess.run([cli, "-t", "orders", "-b", "unused:9092", "-c", "--log-dir", str(tmp_path)] + opts,
                            capture_output=True, text=True)
         assert r.returncode == 0, r.stderr
-        o = _oracle([(p, x) for p in range(P) for x in recs(p)])
+        o = oracle_in_order([(p, *x) for p in range(P) for x in recs(p)])
         lines = r.stdout.splitlines()
         assert "Alive keys: %d" % o.scalar("sum_all_alive") in lines
         assert "Topic Size: %d bytes" % o.scalar("overall_size") in lines

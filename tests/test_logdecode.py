@@ -141,40 +141,12 @@ def test_cli_log_dir(tmp_path):
         assert [int(c[10]), int(c[11])] == [o.counter("key_size_sum", p), o.counter("value_size_sum", p)]
 
 
-def _py_decode(seg):
-    """tiny pure-Python RecordBatch v2 reader (test infra) → list of (offset, ts, key, value_len)"""
-    import struct
-    def uv(b, p):
-        u, sh = 0, 0
-        while True:
-            x = b[p]; p += 1
-            u |= (x & 0x7F) << sh; sh += 7
-            if not x & 0x80:
-                return (u >> 1) ^ -(u & 1), p
-    out, pos, b = [], 0, bytes(seg)
-    while pos + 61 <= len(b):
-        base_off, bl = struct.unpack(">qi", b[pos:pos + 12])
-        base_ts, = struct.unpack(">q", b[pos + 27:pos + 35])
-        cnt, = struct.unpack(">i", b[pos + 57:pos + 61])
-        p = pos + 61
-        for _ in range(cnt):
-            ln, p = uv(b, p); end = p + ln
-            p += 1
-            tsd, p = uv(b, p); od, p = uv(b, p)
-            kl, p = uv(b, p); key = None if kl < 0 else b[p:p + kl]; p += max(kl, 0)
-            vl, p = uv(b, p)
-            out.append((base_off + od, -1 if base_ts == -1 else base_ts + tsd, key, None if vl < 0 else vl))
-            p = end
-        pos += 12 + bl
-    return out
-
-
 def test_cpp_segment_encoder_matches_the_topic():
     """kta_synth_encode_segment_host (the broker-format face of the synthetic topic) against fill_host."""
     P = 8
     spec = synth.make_spec(P * 700, P, key_mode=2, distinct_keys=400, tombstone_per_10k=1500, null_key_per_10k=500)
     for p in (0, 5):
-        got = _py_decode(synth.encode_segment(spec, p, batch_records=33))
+        got = [r for b in kc.read_segment(synth.encode_segment(spec, p, batch_records=33)) for r in b.records]
         t = synth.fill_host(spec, rank=p, world=P)              # partition p's records in offset order
         koff = np.concatenate([[0], np.cumsum(np.maximum(t.key_len, 0))])
         assert len(got) == t.n

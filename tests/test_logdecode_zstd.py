@@ -2,15 +2,15 @@
 oracle fed with the same records, through every log-segment entry point, from ~16 KB batches up to one of about 1 MiB."""
 import os
 import subprocess
+from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
-from feed import partition_lists, scan_log_batches, stage_batches
+from feed import partition_lists, scan_log
 from kafka_topic_analyzer_b200 import KtaEngine, KtaError, synth
 from parity import assert_parity, oracle_over
 import kafka_codec as kc
-import zstd_codec as zc
 
 NOW = (4102444800, 123456789)
 MIXED = ["zstd", "zstd-stream", "gzip", "lz4", "snappy", None]
@@ -20,18 +20,13 @@ def _check_all_entry_points(P, per, segs, hll_p=10):
     """push_log_segment per partition, push_log_segments in one call, scan_log_batches_device over one device buffer"""
     o = oracle_over(per, count_alive_keys=True)
     n = sum(len(v) for v in per.values())
+    parts = {p: [SimpleNamespace(p=p, raw=s)] for p, s in segs}      # each segment as it is
     with KtaEngine(P, count_alive_keys=True, hll_precision=hll_p, now=NOW) as e:
-        assert sum(e.push_log_segment(p, s) for p, s in segs) == n
-        e.finalize()
-        assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(hll_p))
-        e.reset()
-        assert e.push_log_segments(segs) == n
-        e.finalize()
-        assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(hll_p))
-        e.reset()
-        assert scan_log_batches(e, stage_batches(segs)) == n
-        e.finalize()
-        assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(hll_p))
+        for entry in ("segment_host", "segments_host", "batches_device"):
+            e.reset()
+            assert scan_log(e, entry, parts)[0] == n
+            e.finalize()
+            assert_parity(e, o, P, check_alive=True, hll_regs=o.hll_alive_regs(hll_p))
 
 
 @pytest.mark.gpu
@@ -44,8 +39,9 @@ def test_zstd_segments_decode_and_scan(codec):
     spec = synth.make_spec(P * 4000, P, key_mode=1, distinct_keys=900, tombstone_per_10k=2000, null_key_per_10k=300,
                            empty_value_per_10k=100, value_mean=120)
     per = partition_lists(synth.fill_host(spec))
-    comp = MIXED if codec == "mixed" else codec
-    segs = [(p, zc.encode_partition(per[p], rng, max_batch=200, compression=comp)) for p in sorted(per)]
+    # every partition's batch sizes are drawn before their codecs
+    pick = (lambda: MIXED[int(rng.integers(0, len(MIXED)))]) if codec == "mixed" else (lambda: codec)
+    segs = [(p, kc.recompress(kc.encode_partition(per[p], rng, max_batch=200), pick)) for p in sorted(per)]
     raw = sum(len(kc.encode_partition(per[p], np.random.default_rng(1), max_batch=200)) for p in per)
     assert sum(len(s) for _, s in segs) < raw                       # it really was compressed
     if codec != "mixed":
@@ -58,7 +54,7 @@ def _fixed_batches(recs, per_batch, codec):
     while i < len(recs):
         chunk = recs[i:i + per_batch]
         base_ts = chunk[0][0]
-        out += zc.encode_batch(i, base_ts, [(j, r[0] - base_ts, r[1], r[2]) for j, r in enumerate(chunk)], compression=codec)
+        out += kc.encode_batch(i, base_ts, [(j, r[0] - base_ts, r[1], r[2]) for j, r in enumerate(chunk)], compression=codec)
         i += len(chunk)
     return bytes(out)
 
@@ -87,7 +83,7 @@ def test_large_zstd_batches(codec):
 def test_corrupt_zstd_batches_are_rejected():
     recs = [(i, i, b"key-%d" % (i % 5), 30) for i in range(50)]
     with KtaEngine(1, now=NOW) as e:
-        good = zc.encode_batch(0, 1000, recs, compression="zstd")
+        good = kc.encode_batch(0, 1000, recs, compression="zstd")
         assert good[61:65] == b"\x28\xb5\x2f\xfd" and good[65] >> 6 == 1          # one-shot: a 2-byte Frame_Content_Size
         assert e.push_log_segment(0, good) == 50
         bad = bytearray(good)
@@ -95,7 +91,7 @@ def test_corrupt_zstd_batches_are_rejected():
         with pytest.raises(KtaError):
             e.push_log_segment(0, bytes(bad))
         for codec in ("zstd", "zstd-stream"):
-            g = zc.encode_batch(0, 1000, recs, compression=codec)
+            g = kc.encode_batch(0, 1000, recs, compression=codec)
             cut = bytearray(g[:-7])                                               # shorter section under an adjusted batchLength
             cut[8:12] = (len(cut) - 12).to_bytes(4, "big")
             with pytest.raises(KtaError):
@@ -107,7 +103,7 @@ def test_corrupt_zstd_batches_are_rejected():
             with pytest.raises(KtaError):
                 e.push_log_segment(0, bytes(bad))
         for codec in ("zstd", "zstd-stream"):                                     # recordsCount the section cannot hold
-            bad = bytearray(zc.encode_batch(0, 1000, recs, compression=codec))
+            bad = bytearray(kc.encode_batch(0, 1000, recs, compression=codec))
             bad[57:61] = (0x7FFFFFFF).to_bytes(4, "big")
             with pytest.raises(KtaError):
                 e.push_log_segment(0, bytes(bad))
@@ -137,7 +133,11 @@ def test_cli_log_dir_zstd(tmp_path):
         for p, recs in per.items():
             d = root / ("orders-%d" % p)
             d.mkdir(parents=True)
-            (d / "00000000000000000000.log").write_bytes(zc.encode_partition(recs, np.random.default_rng(p), compression=comp))
+            rng = np.random.default_rng(p)
+            seg = kc.encode_partition(recs, rng)
+            if comp:
+                seg = kc.recompress(seg, lambda: comp[int(rng.integers(0, len(comp)))])
+            (d / "00000000000000000000.log").write_bytes(seg)
         r = subprocess.run([os.path.join(CLI_DIR, "kafka-topic-analyzer"), "-t", "orders", "-b", "unused:9092", "-c", "--log-dir",
                             str(root)], capture_output=True, text=True)
         assert r.returncode == 0, r.stderr

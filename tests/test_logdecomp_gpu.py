@@ -23,8 +23,8 @@ import np_oracle
 import test_inflate_host as ih
 import test_lzwalk_host as lh
 import test_zstd_host as zh
-import zstd_codec as zc
 from feed import capture_hashes, scan_log_batches, stage_batches
+from kafka_codec import with_section
 from parity import assert_parity, oracle_over
 
 NOW = (4102444800, 123456789)
@@ -61,14 +61,6 @@ def run_probe(exe, segments):
 # ------------------------------------------------------------------------------------------------
 # batches
 # ------------------------------------------------------------------------------------------------
-def with_section(batch, section, codec_bits):
-    """the batch with its records section replaced; batchLength and the codec bits follow"""
-    hdr = bytearray(batch[:61])
-    hdr[8:12] = struct.pack(">i", 49 + len(section))
-    hdr[22] = (hdr[22] & 0xF8) | codec_bits
-    return bytes(hdr) + section
-
-
 def payload_batch(data):
     """a batch whose records section is `data` as it is, recordsCount 0 (the decompression stage does not parse records)"""
     return with_section(kc.encode_batch(0, 1000, []), data, 0)
@@ -95,7 +87,7 @@ def compressors(data, zstd_levels=range(-5, 23)):
         out.append(("zstd-%d" % lvl, 4, f))
         if lvl in zh.LEVELS:
             out.append(("zstd-%d-no-fcs" % lvl, 4, zh.without_content_size(f)))
-    out.append(("zstd-stream", 4, zc.compress_records(data, "zstd-stream")))
+    out.append(("zstd-stream", 4, kc.compress_records(data, "zstd-stream")))
     return out
 
 
@@ -230,7 +222,7 @@ def test_many_batches_per_launch(probe):
                 for _ in range(int(rng.integers(1, 5)))]
         unc = records_batch(recs, base_offset=b * 10)
         codec = codecs[b % len(codecs)]
-        comp = unc if codec is None else with_section(unc, zc.compress_records(unc[61:], codec), kc.CODEC_BITS[codec])
+        comp = kc.recompress(unc, lambda: codec)
         items.append(("batch-%d/%s" % (b, codec), comp, unc, codec))
     got = run_probe(probe, [b"".join(c for _, c, _, _ in items)])[0]
     assert len(got) == len(items)
@@ -283,7 +275,7 @@ def test_every_decompressed_byte_is_a_key_byte():
                 recs.append((j, ts - 1_700_000_000_000, key, value))
                 per[p].append((ts, key, value))
                 order.append(key)
-            seg += zc.encode_batch(off, 1_700_000_000_000, recs, compression=codecs[(p + b) % len(codecs)])
+            seg += kc.encode_batch(off, 1_700_000_000_000, recs, compression=codecs[(p + b) % len(codecs)])
             off += len(recs)
         segs.append((p, bytes(seg)))
     kl = np.array([-1 if k is None else len(k) for k in order], dtype=np.int32)

@@ -10,7 +10,6 @@ import pytest
 
 import codec_harness as ch
 import kafka_codec as kc
-import zstd_codec as zc
 
 LEVELS = (-5, 1, 3, 9, 19, 22)
 MAGIC = b"\x28\xb5\x2f\xfd"
@@ -246,9 +245,9 @@ def corpus():
             f = one_shot(data, lvl)
             out.append((f, data))
             out.append((without_content_size(f), data))
-        out.append((zc.compress_records(data, "zstd-stream"), data))
+        out.append((kc.compress_records(data, "zstd-stream"), data))
     recs, text = sections()["records"], sections()["text"]
-    a, b = one_shot(recs, 3), zc.compress_records(text[:50_000], "zstd-stream")
+    a, b = one_shot(recs, 3), kc.compress_records(text[:50_000], "zstd-stream")
     skip = struct.pack("<II", 0x184D2A53, 5) + b"hello"
     out.append((a + b, recs + text[:50_000]))                                   # two frames
     out.append((skip + a + skip + b, recs + text[:50_000]))                     # skippable frames before and between
@@ -347,7 +346,7 @@ def damaged_frames():
     rng = np.random.default_rng(9)
     s = sections()
     data = s["records"] + s["text"][:20_000]
-    goods = (one_shot(data, 3), zc.compress_records(data, "zstd-stream"), one_shot(data, 19))
+    goods = (one_shot(data, 3), kc.compress_records(data, "zstd-stream"), one_shot(data, 19))
     cases = []
     for good in goods:
         for i in range(300):

@@ -11,7 +11,6 @@ and the range over the repetitions are printed.  A separate torch.profiler pass 
 over the call's bytes as a share of the H100's 3.35 TB/s.  The card's name and power limit are printed first.
 usage: python tools/logcrc_bench.py [reps]"""
 import os
-import struct
 import subprocess
 import sys
 import time
@@ -22,47 +21,14 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np
 import torch
 
+import kafka_codec as kc
 import kafka_topic_analyzer_b200 as kta
+from feed import stage_batches
 from kafka_topic_analyzer_b200 import synth
 
 P, N, VM = 16, 8_000_000, 256
 HBM = 3.35e12
 REPS = int(sys.argv[1]) if len(sys.argv) > 1 else 9
-
-
-def batches_of(raw: bytes):
-    out, pos = [], 0
-    while pos + 61 <= len(raw):
-        bl = int.from_bytes(raw[pos + 8:pos + 12], "big", signed=True)
-        out.append(raw[pos:pos + 12 + bl])
-        pos += 12 + bl
-    return out
-
-
-def zstd_batches(batches):
-    import pyarrow as pa
-    import crc_codec as cc
-    out = []
-    for b in batches:
-        body = pa.compress(b[61:], codec="zstd", asbytes=True)
-        hdr = bytearray(b[:61])
-        hdr[8:12] = struct.pack(">i", 49 + len(body))
-        hdr[22] |= 4
-        out.append(cc.set_crcs(bytes(hdr) + body))   # one batch: its CRC over the compressed bytes
-    return out
-
-
-def stage(per_partition):
-    offs, parts, blobs, at = [], [], [], 0
-    for p, bs in enumerate(per_partition):
-        for b in bs:
-            offs.append(at)
-            parts.append(p)
-            blobs.append(b)
-            at += len(b)
-    buf = torch.zeros(at + 64, dtype=torch.uint8, device="cuda")
-    buf[:at] = torch.from_numpy(np.frombuffer(b"".join(blobs), dtype=np.uint8).copy()).cuda()
-    return buf, at, torch.tensor(offs, dtype=torch.int64).cuda(), torch.tensor(parts, dtype=torch.int32).cuda(), len(offs)
 
 
 def main():
@@ -71,10 +37,10 @@ def main():
     print("card:", card, flush=True)
     spec = synth.make_spec(N, P, value_mean=VM, distinct_keys=1_000_000)
     work = {}
-    small = [batches_of(synth.encode_segment(spec, p, batch_records=56).tobytes()) for p in range(P)]
-    work["16k"] = stage(small)
-    work["240k"] = stage([batches_of(synth.encode_segment(spec, p, batch_records=840).tobytes()) for p in range(P)])
-    work["16k-zstd"] = stage([zstd_batches(bs) for bs in small])
+    small = [(p, synth.encode_segment(spec, p, batch_records=56)) for p in range(P)]
+    work["16k"] = stage_batches(small)
+    work["240k"] = stage_batches([(p, synth.encode_segment(spec, p, batch_records=840)) for p in range(P)])
+    work["16k-zstd"] = stage_batches([(p, kc.set_crcs(kc.recompress(s, lambda: "zstd"))) for p, s in small])
     for w, s in work.items():
         print("workload %-8s %d records, %d batches, %.3f GB, %.1f KB per batch" % (w, N, s[4], s[1] / 1e9, s[1] / s[4] / 1e3), flush=True)
     modes = [(w, crc) for w in work for crc in (False, True)]

@@ -1,8 +1,10 @@
 """Throughput of the GPU RecordBatch v2 decoder (SURVEY.md §8 f2) on the synthetic topic stored broker-style.
 Segments are encoded on the host (C++), staged to HBM once, then decoded + scanned from device memory."""
 import ctypes as C, os, sys, time
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import numpy as np, torch
+import kafka_codec as kc
 import kafka_topic_analyzer_b200 as kta
 from kafka_topic_analyzer_b200 import synth
 from kafka_topic_analyzer_b200._native import lib, check
@@ -14,30 +16,6 @@ if CODEC:
     N = 2_000_000
 
 
-def compress_segment(seg: np.ndarray, codec: str) -> np.ndarray:
-    """re-writes every batch of an uncompressed segment with its records section compressed"""
-    import pyarrow as pa
-    raw, out, pos = seg.tobytes(), bytearray(), 0
-    while pos + 61 <= len(raw):
-        bl = int.from_bytes(raw[pos + 8:pos + 12], "big", signed=True)
-        hdr = bytearray(raw[pos:pos + 61])
-        if codec == "gzip":
-            import zlib
-            c = zlib.compressobj(6, zlib.DEFLATED, 31)
-            body = c.compress(raw[pos + 61:pos + 12 + bl]) + c.flush()
-        elif codec == "zstd-stream":   # streaming compressor (as the Java client): no Frame_Content_Size
-            sink = pa.BufferOutputStream()
-            with pa.CompressedOutputStream(sink, "zstd") as z:
-                z.write(raw[pos + 61:pos + 12 + bl])
-            body = sink.getvalue().to_pybytes()
-        else:
-            body = pa.compress(raw[pos + 61:pos + 12 + bl], codec=codec, asbytes=True)
-        hdr[8:12] = (49 + len(body)).to_bytes(4, "big")
-        hdr[22] |= {"gzip": 1, "snappy": 2, "lz4": 3, "zstd": 4, "zstd-stream": 4}[codec]
-        out += hdr + body
-        pos += 12 + bl
-    return np.frombuffer(bytes(out), dtype=np.uint8)
-
 spec = synth.make_spec(N, P, value_mean=VM, distinct_keys=1_000_000)
 chunks, offs, parts = [], [], []
 t0 = time.time()
@@ -46,12 +24,10 @@ for p in range(P):
     s = synth.encode_segment(spec, p, batch_records=BR)
     unc = int(s.size)
     if CODEC:
-        s = compress_segment(s, CODEC)
-    pos = 0
-    while pos + 61 <= s.size:      # batch offsets by hopping headers on the host
-        offs.append(total + pos)
-        parts.append(p)
-        pos += 12 + int.from_bytes(s[pos + 8:pos + 12].tobytes(), "big", signed=True)
+        s = np.frombuffer(kc.recompress(s, lambda: CODEC), dtype=np.uint8)
+    o = kc.batch_offsets(s)
+    offs += [total + x for x in o]
+    parts += [p] * len(o)
     chunks.append(s)
     total += (s.size + 15) // 16 * 16
 raw = sum(int(s.size) for s in chunks)

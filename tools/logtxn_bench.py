@@ -16,11 +16,14 @@ import subprocess
 import sys
 import time
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import numpy as np
 import torch
 
+import kafka_codec as kc
 import kafka_topic_analyzer_b200 as kta
+from feed import stage_batches
 from kafka_topic_analyzer_b200 import synth
 
 P, N, VM, BR = 16, 8_000_000, 256, 56
@@ -29,15 +32,9 @@ REPS = int(sys.argv[1]) if len(sys.argv) > 1 else 9
 OUT = sys.argv[2] if len(sys.argv) > 2 else None
 
 
-def batches_of(seg: np.ndarray):
-    raw, out, pos = seg.tobytes(), [], 0
-    while pos + 61 <= len(raw):
-        bl = int.from_bytes(raw[pos + 8:pos + 12], "big", signed=True)
-        out.append(raw[pos:pos + 12 + bl])
-        pos += 12 + bl
-    return out
-
-
+# The marker and the producer patch of transactional() write other bytes than the test encoders (kafka_codec.marker,
+# with_producer): the marker has baseTimestamp 0, baseSequence -1 and coordinatorEpoch 0, and the patch sets producerId
+# only, leaving producerEpoch and baseSequence as the synthetic encoder wrote them.
 def marker(offset, pid, commit):
     body = bytes([0]) + bytes([0, 0]) + bytes([8]) + struct.pack(">hh", 0, 1 if commit else 0) + bytes([12]) + struct.pack(">hi", 0, 0) + bytes([0])
     rec = bytes([len(body) * 2]) + body
@@ -69,19 +66,6 @@ def transactional(batches, p, rng):
     return out, aborted
 
 
-def stage(per_partition):
-    offs, parts, blobs, at = [], [], [], 0
-    for p, bs in enumerate(per_partition):
-        for b in bs:
-            offs.append(at)
-            parts.append(p)
-            blobs.append(b)
-            at += len(b)
-    buf = torch.zeros(at + 64, dtype=torch.uint8, device="cuda")
-    buf[:at] = torch.from_numpy(np.frombuffer(b"".join(blobs), dtype=np.uint8).copy()).cuda()
-    return buf, at, torch.tensor(offs, dtype=torch.int64).cuda(), torch.tensor(parts, dtype=torch.int32).cuda(), len(offs)
-
-
 def main():
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                           capture_output=True, text=True).stdout.strip()
@@ -90,12 +74,12 @@ def main():
     rng = np.random.default_rng(17)
     plain, txn, n_aborted = [], [], 0
     for p in range(P):
-        bs = batches_of(synth.encode_segment(spec, p, batch_records=BR))
+        bs = kc.split_batches(synth.encode_segment(spec, p, batch_records=BR))
         plain.append(bs)
         t, a = transactional(bs, p, rng)
         txn.append(t)
         n_aborted += a
-    work = {"plain": stage(plain), "txn": stage(txn)}
+    work = {w: stage_batches([(p, b"".join(bs)) for p, bs in enumerate(v)]) for w, v in (("plain", plain), ("txn", txn))}
     print("workloads: %d records, plain %d batches (%.2f GB), txn %d batches, %d records aborted" %
           (N, work["plain"][4], work["plain"][1] / 1e9, work["txn"][4], n_aborted), flush=True)
     modes = [(w, lvl, exact) for exact in (False, True) for w in ("plain", "txn") for lvl in ("read_uncommitted", "read_committed")]

@@ -2,10 +2,10 @@
 exact alive keys (table starting far too small, so growth + stamps-only re-runs happen too), ragged keys, a tail tile,
 the host ring path, the log-segment decoder and its read_committed passes.  Each run is checked against the oracle so a 'clean' sanitizer log is the
 log of a run that also computed the right answer."""
-import os, sys
+import itertools, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
-import numpy as np
+import kafka_codec as kc
 import kafka_topic_analyzer_b200 as kta
 from kafka_topic_analyzer_b200 import synth
 from parity import assert_parity, oracle_for
@@ -14,50 +14,12 @@ NOW = (4102444800, 1)
 which = sys.argv[1:] or ["counters", "hll", "exact", "ragged", "ring", "log", "logz", "logzstd", "logtxn", "logcrc"]
 
 
-def compress_segment(seg, b0=0):
-    """every batch of an uncompressed segment re-written with its records section compressed: gzip, LZ4, Snappy in turn"""
-    import zlib
-    import pyarrow as pa
-    raw, out, pos, b = seg.tobytes(), bytearray(), 0, b0
-    while pos + 61 <= len(raw):
-        bl = int.from_bytes(raw[pos + 8:pos + 12], "big", signed=True)
-        hdr, body = bytearray(raw[pos:pos + 61]), raw[pos + 61:pos + 12 + bl]
-        codec = ("gzip", "lz4", "snappy")[b % 3]
-        if codec == "gzip":
-            c = zlib.compressobj(6, zlib.DEFLATED, 31)
-            body = c.compress(body) + c.flush()
-        else:
-            body = pa.compress(body, codec=codec, asbytes=True)
-        hdr[8:12] = (49 + len(body)).to_bytes(4, "big")
-        hdr[22] |= {"gzip": 1, "snappy": 2, "lz4": 3}[codec]
-        out += hdr + body
-        pos += 12 + bl
-        b += 1
-    return np.frombuffer(bytes(out), dtype=np.uint8)
+def rotate(seg, codecs, first):
+    """every batch of an uncompressed segment with its records section compressed by codecs[(first + i) % len(codecs)]
+    for its index i (None: left uncompressed)"""
+    pick = itertools.islice(itertools.cycle(codecs), first, None)
+    return kc.recompress(seg, lambda: next(pick))
 
-
-def zstd_segment(seg, b0=0):
-    """every batch of an uncompressed segment re-written as zstd: one-shot (Frame_Content_Size), streaming (none) or left
-    uncompressed, in turn"""
-    import pyarrow as pa
-    raw, out, pos, b = seg.tobytes(), bytearray(), 0, b0
-    while pos + 61 <= len(raw):
-        bl = int.from_bytes(raw[pos + 8:pos + 12], "big", signed=True)
-        hdr, body = bytearray(raw[pos:pos + 61]), raw[pos + 61:pos + 12 + bl]
-        if b % 3 == 0:
-            body = pa.compress(body, codec="zstd", asbytes=True)
-        elif b % 3 == 1:
-            sink = pa.BufferOutputStream()
-            with pa.CompressedOutputStream(sink, "zstd") as z:
-                z.write(body)
-            body = sink.getvalue().to_pybytes()
-        if b % 3 != 2:
-            hdr[8:12] = (49 + len(body)).to_bytes(4, "big")
-            hdr[22] |= 4
-        out += hdr + body
-        pos += 12 + bl
-        b += 1
-    return np.frombuffer(bytes(out), dtype=np.uint8)
 
 P = 8
 n = P * 4096 + 0
@@ -70,7 +32,7 @@ for name in which:
         want, stats = lt.rule_model(calls, t.aborted)
         with kta.KtaEngine(P, count_alive_keys=True, device=0, now=NOW, alive_table_kib=1, isolation_level="read_committed") as e:
             for p in range(P):
-                e.push_txn_index(p, lt.txn_index(t.aborted[p]))
+                e.push_txn_index(p, kc.txn_index(t.aborted[p]))
             e.push_log_segments([(p, t.segment(p, 0, cut[p])) for p in range(P)])
             e.push_log_segments([(p, t.segment(p, cut[p])) for p in range(P)])
             e.finalize()
@@ -78,12 +40,10 @@ for name in which:
         print(name, "ok", stats)
         continue
     if name == "logcrc":   # check.crcs: batches of one to many spans at odd offsets, every third one damaged
-        import crc_codec as cc
-        import kafka_codec as kc
         segs, bad, nb = [], 0, 0
         for p in range(P):
-            s = bytearray(cc.set_crcs(compress_segment(synth.encode_segment(synth.make_spec(n, P), p, 0, n // P,
-                                                                             batch_records=7 + 60 * p), p)))
+            s = bytearray(kc.set_crcs(rotate(synth.encode_segment(synth.make_spec(n, P), p, 0, n // P, batch_records=7 + 60 * p),
+                                             ("gzip", "lz4", "snappy"), p)))
             for i, o in enumerate(kc.batch_offsets(s)):
                 nb += 1
                 if i % 3 == 0:
@@ -106,9 +66,9 @@ for name in which:
             per = n // P
             segs = [(p, synth.encode_segment(spec, p, 0, per, batch_records=100)) for p in range(P)]
             if name == "logz":   # gzip / LZ4 / Snappy batches: the decompressors run first
-                segs = [(p, compress_segment(s, p)) for p, s in segs]
+                segs = [(p, rotate(s, ("gzip", "lz4", "snappy"), p)) for p, s in segs]
             if name == "logzstd":   # zstd one-shot / streaming batches and uncompressed ones
-                segs = [(p, zstd_segment(s, p)) for p, s in segs]
+                segs = [(p, rotate(s, ("zstd", "zstd-stream", None), p)) for p, s in segs]
             e.push_log_segments(segs)
             e.finalize()
             got = (e.message_metrics.overall_count(), e.alive_keys())
