@@ -784,11 +784,7 @@ static int derive_tile_base(kta_handle *h, const int32_t *d_klen, int64_t n) {
     const int64_t ntiles = (n + TILE - 1) / TILE;
     int rc;
     if ((rc = h->d_tb_scratch.grow(h->stream, ntiles + 1))) return rc;
-    const int grid = (int)std::min<int64_t>((ntiles + 7) / 8, (int64_t)h->sm_count * 8);
-    tile_key_bytes_kernel<<<grid, 256, 0, h->stream>>>(d_klen, n, ntiles, h->d_tb_scratch);
-    CU(cudaGetLastError());
-    tile_base_scan_kernel<<<1, 1024, 0, h->stream>>>(h->d_tb_scratch, ntiles);
-    CU(cudaGetLastError());
+    CU(log_launch_tile_base(d_klen, n, h->d_tb_scratch, h->sm_count, h->stream));
     h->launches += 2;
     return KTA_OK;
 }
@@ -1023,15 +1019,9 @@ static int log_decode(kta_handle *h, const uint8_t *dev_bytes, int64_t readable,
     if ((rc = L.dec_part.grow(s, (int64_t)nrec)) || (rc = L.dec_klen.grow(s, (int64_t)nrec)) || (rc = L.dec_vlen.grow(s, (int64_t)nrec)) ||
         (rc = L.dec_ts.grow(s, (int64_t)nrec)) || (rc = L.dec_ksrc.grow(s, (int64_t)nrec)))
         return rc;
-    const uint32_t stage = (uint32_t)(((size_t)longest + 16 + 1023) / 1024 * 1024);
-    const bool staged = stage <= 48u * 1024u;
-    const size_t dsm = (size_t)(LOG_DECODE_THREADS / 32) * (LOG_WARP_HEADER + (staged ? stage : 0u));
-    const int per_sm = (int)std::max<size_t>(1, std::min<size_t>(16, h->smem_optin / std::max<size_t>(dsm, 1)));
-    const int dgrid = (int)std::min<int64_t>((nbatches + 3) / 4, (int64_t)h->sm_count * per_sm);
-    const auto decode = staged ? log_decode_kernel<true> : log_decode_kernel<false>;
-    decode<<<dgrid, LOG_DECODE_THREADS, dsm, s>>>(dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, nullptr, L.dec_ts,
-                                                  L.dec_klen, L.dec_vlen, keys ? L.dec_ksrc.get() : nullptr, staged ? stage : 0u, L.err);
-    CU(cudaGetLastError());
+    const LogDecodeShape shape = log_decode_shape(longest, nbatches, h->sm_count, h->smem_optin);
+    CU(log_launch_decode(shape, dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, L.dec_ts, L.dec_klen, L.dec_vlen,
+                         keys ? L.dec_ksrc.get() : nullptr, L.err, s));
     h->launches++;
     b = kta_batch{};
     b.n = (int64_t)nrec;
@@ -1061,9 +1051,7 @@ static int log_gather_keys(kta_handle *h, int32_t partition, const uint8_t *dev_
     if (err[0]) return fail(KTA_ERR_INVALID, "malformed record inside a batch of partition %d", partition);
     if (!keys) return KTA_OK;
     if ((rc = L.dec_keys.grow(s, (int64_t)nkey + 64))) return rc;
-    log_gather_keys_kernel<<<(int)std::min<int64_t>((ntiles + 7) / 8, (int64_t)h->sm_count * 8), 256, 0, s>>>(
-        dev_bytes, L.dec_ksrc, L.dec_klen, b.n, h->d_tb_scratch, L.dec_keys);
-    CU(cudaGetLastError());
+    CU(log_launch_gather_keys(dev_bytes, L.dec_ksrc, L.dec_klen, b.n, h->d_tb_scratch, L.dec_keys, h->sm_count, s));
     h->launches++;
     b.key_bytes = L.dec_keys;
     b.key_bytes_len = (int64_t)nkey;

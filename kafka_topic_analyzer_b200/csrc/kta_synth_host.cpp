@@ -106,8 +106,9 @@ extern "C" int kta_synth_encode_segment_host(const kta_synth_spec *s, int32_t pa
             const kta_synth_record &r = rr[(size_t)i];
             rec.clear();
             rec.push_back(0);
-            // a record without a timestamp inside a batch that has one cannot be expressed: give it the base timestamp
-            put_varint(rec, (have_ts && r.ts_ms != -1) ? r.ts_ms - base_ts : 0);
+            // the consumer's timestamp is baseTimestamp + timestampDelta, and only a result of -1 means "not available": a
+            // record without a timestamp inside a batch that has one gets the delta -1 - baseTimestamp
+            put_varint(rec, !have_ts ? 0 : r.ts_ms != -1 ? r.ts_ms - base_ts : -1 - base_ts);
             put_varint(rec, i);
             if (r.key_len < 0) put_varint(rec, -1);
             else {

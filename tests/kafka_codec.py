@@ -32,31 +32,39 @@ def uvarint(u: int) -> bytes:
             return bytes(out)
 
 
-def varint(n: int) -> bytes:
-    return uvarint(zigzag(n) & 0xFFFFFFFFFFFFFFFF)
+def varint(n: int, width: int = 0) -> bytes:
+    """n zig-zag encoded; width > 0 pads it to that many bytes (up to 10) with empty continuation groups, as a writer that
+    reserves a fixed-width length field may — a non-minimal encoding that readers take as the same value"""
+    b = uvarint(zigzag(n) & 0xFFFFFFFFFFFFFFFF)
+    if width > len(b):
+        assert width <= 10
+        b = b[:-1] + bytes([b[-1] | 0x80]) + b"\x80" * (width - len(b) - 1) + b"\x00"
+    return b
 
 
-def encode_record(offset_delta, ts_delta, key, value_len, headers=(), value=None):
+def encode_record(offset_delta, ts_delta, key, value_len, headers=(), value=None, widths=None):
     """value bytes are synthesised (the metric path never reads them) unless `value` gives them; value_len None (and no
-    value) = tombstone"""
+    value) = tombstone.  widths: {"len", "ts", "key", "value"} → the byte width of the record-length, timestamp-delta,
+    key-length and value-length varints (padded; see varint)"""
+    w = widths or {}
     body = bytearray(b"\x00")                      # record attributes
-    body += varint(ts_delta) + varint(offset_delta)
+    body += varint(ts_delta, w.get("ts", 0)) + varint(offset_delta)
     if key is None:
-        body += varint(-1)
+        body += varint(-1, w.get("key", 0))
     else:
-        body += varint(len(key)) + key
+        body += varint(len(key), w.get("key", 0)) + key
     if value is not None:
         assert value_len is None or value_len == len(value)
-        body += varint(len(value)) + value
+        body += varint(len(value), w.get("value", 0)) + value
     elif value_len is None:
-        body += varint(-1)
+        body += varint(-1, w.get("value", 0))
     else:
-        body += varint(value_len) + bytes((i * 31 + 7) & 0xFF for i in range(value_len))
+        body += varint(value_len, w.get("value", 0)) + bytes((i * 31 + 7) & 0xFF for i in range(value_len))
     body += varint(len(headers))
     for hk, hv in headers:
         body += varint(len(hk)) + hk
         body += varint(-1) if hv is None else varint(len(hv)) + hv
-    return varint(len(body)) + bytes(body)
+    return varint(len(body), w.get("len", 0)) + bytes(body)
 
 
 def compress_records(recs: bytes, codec: str) -> bytes:
@@ -89,15 +97,23 @@ def compress_records(recs: bytes, codec: str) -> bytes:
 CODEC_BITS = {None: 0, "gzip": 1, "snappy": 2, "snappy-xerial": 2, "lz4": 3, "zstd": 4, "zstd-stream": 4}
 
 
+def _int32(x):
+    return (x + (1 << 31)) % (1 << 32) - (1 << 31)
+
+
+def _int64(x):
+    return (x + (1 << 63)) % (1 << 64) - (1 << 63)
+
+
 def encode_batch(base_offset, base_ts, records, attributes=0, max_ts=None, compression=None):
-    """records: list of (offset_delta, ts_delta, key|None, value_len|None[, headers[, value]])"""
+    """records: list of (offset_delta, ts_delta, key|None, value_len|None[, headers[, value[, widths]]])"""
     recs = b"".join(encode_record(*r) for r in records)
     if compression:
         recs = compress_records(recs, compression)
         attributes |= CODEC_BITS[compression]
-    last_delta = max((r[0] for r in records), default=0)
+    last_delta = _int32(max((r[0] for r in records), default=0))
     if max_ts is None:
-        max_ts = max((base_ts + r[1] for r in records), default=base_ts)
+        max_ts = _int64(max((base_ts + r[1] for r in records), default=base_ts))
     after_len = struct.pack(">iBIhiqqqhii", 0, 2, 0, attributes, last_delta, base_ts, max_ts, -1, -1, -1, len(records)) + recs
     return struct.pack(">qi", base_offset, len(after_len)) + after_len
 
@@ -241,7 +257,7 @@ def txn_index(entries) -> bytes:
 
 # ---- reading ----------------------------------------------------------------------------------------------------------
 # one batch as read back: its header fields and its records [(offset, ts, key|None, value_len|None)]
-Batch = namedtuple("Batch", "base_offset attributes base_ts producer_id count records")
+Batch = namedtuple("Batch", "base_offset attributes base_ts producer_id count records max_ts")
 
 
 def _read_varint(b, p):
@@ -282,13 +298,14 @@ def _decompress(codec_bits, data):
 
 
 def read_segment(seg):
-    """every batch of a segment as a Batch; a record's timestamp is -1 when its batch's baseTimestamp is"""
+    """every batch of a segment as a Batch, its records as the consumer computes them: a record's timestamp is
+    baseTimestamp + timestampDelta (in 64-bit arithmetic), and it is -1 ("not available") only when that sum is.  Every
+    batch is read, control and LogAppendTime batches as they are stored (delivered() applies the consumer's rules)."""
     seg, out, pos = bytes(seg), [], 0
     while pos + 61 <= len(seg):
         base_off, bl = struct.unpack(">qi", seg[pos:pos + 12])
         attrs, = struct.unpack(">h", seg[pos + 21:pos + 23])
-        base_ts, = struct.unpack(">q", seg[pos + 27:pos + 35])
-        pid, = struct.unpack(">q", seg[pos + 43:pos + 51])
+        base_ts, max_ts, pid = struct.unpack(">qqq", seg[pos + 27:pos + 51])
         cnt, = struct.unpack(">i", seg[pos + 57:pos + 61])
         body = _decompress(attrs & 7, seg[pos + 61:pos + 12 + bl])
         recs, p = [], 0
@@ -302,8 +319,21 @@ def read_segment(seg):
             key = None if kl < 0 else bytes(body[p:p + kl])
             p += max(kl, 0)
             vl, p = _read_varint(body, p)
-            recs.append((base_off + od, -1 if base_ts == -1 else base_ts + tsd, key, None if vl < 0 else vl))
+            recs.append((base_off + od, _int64(base_ts + tsd), key, None if vl < 0 else vl))
             p = end
-        out.append(Batch(base_off, attrs, base_ts, pid, cnt, recs))
+        out.append(Batch(base_off, attrs, base_ts, pid, cnt, recs, max_ts))
         pos += 12 + bl
+    return out
+
+
+def delivered(seg):
+    """the records a consumer delivers from a segment (bytes, or read_segment's batches): control batches (attributes bit 5)
+    and batches without records are not delivered, and a LogAppendTime batch (bit 3) stamps every record with its
+    maxTimestamp"""
+    batches = read_segment(seg) if isinstance(seg, (bytes, bytearray, memoryview)) else seg
+    out = []
+    for b in batches:
+        if b.attributes & 0x20 or not b.records:
+            continue
+        out += [(off, b.max_ts, key, vl) for off, _, key, vl in b.records] if b.attributes & 0x08 else b.records
     return out

@@ -1,0 +1,173 @@
+// TEST INFRASTRUCTURE: the record stage of the RecordBatch decoder on the GPU, with its output made visible.  It launches what
+// scan_log_batches (csrc/kta_api.cu) launches up to the scan — log_header_kernel, its record-count scan, the size and copy passes
+// when there are compressed batches, the record decode, the key-length tile bases and the key gather — through the same launch
+// functions (csrc/kta_logdecode_launch.cuh), and writes out every decoded column, so that tests/test_logdecode_records.py can
+// compare them record by record with the records a case was built from.
+// stdin, per case (little-endian): u32 nbytes, the bytes; u32 nbatches, u64 batch offsets; u32 with_partitions, then i32 per
+// batch partitions when it is 1 (else every batch is partition 0); u32 slack: the bytes behind nbytes that may be read (0 as
+// the device entry points pass, 48 as kta_push_log_segments_host passes).  The device buffer is exactly nbytes + slack long.
+// stdout: u32 SM count and u32 opt-in shared memory per block of the device; then per case: u32 header flags, u32 longest
+// batch, u32 size-pass flags, u32 decode flags, u64 records, u32 staged, u32 stage, u32 grid, u32 ran (the decode was launched: the header and size passes accepted the call and it has records);
+// when ran: per record i32 partition, i64 ts_ms, i32 key_len, i32 value_len (column by column); when ran and the decode flags
+// are 0: u64 tile base[ntiles + 1], then the key buffer (tile base[ntiles] packed key bytes and the 64 bytes behind them).
+// The decoded columns and the key buffer are filled with 0xA5 first: an entry the decoder does not write shows up.
+#include <cuda_runtime.h>
+
+#include <cstdint>
+#include <cstdio>
+#include <cstdlib>
+#include <vector>
+
+#include "../../kafka_topic_analyzer_b200/csrc/kta_logdecode_launch.cuh"
+
+using namespace kta;
+
+#define CK(call)                                                                                           \
+    do {                                                                                                   \
+        cudaError_t e_ = (call);                                                                           \
+        if (e_ != cudaSuccess) {                                                                           \
+            fprintf(stderr, "%s: %s (%s:%d)\n", #call, cudaGetErrorString(e_), __FILE__, __LINE__);        \
+            exit(3);                                                                                       \
+        }                                                                                                  \
+    } while (0)
+
+static void put(const void *p, size_t n) {
+    if (n && fwrite(p, 1, n, stdout) != n) exit(4);
+}
+
+static void get(void *p, size_t n) {
+    if (n && fread(p, 1, n, stdin) != n) exit(2);
+}
+
+template <typename T>
+static T *dev_alloc(size_t count, int fill, cudaStream_t s) {
+    T *p = nullptr;
+    CK(cudaMalloc(&p, std::max<size_t>(count, 1) * sizeof(T)));
+    CK(cudaMemsetAsync(p, fill, std::max<size_t>(count, 1) * sizeof(T), s));
+    return p;
+}
+
+template <typename T>
+static void put_dev(const T *d, size_t count) {
+    std::vector<T> h(count);
+    if (count) CK(cudaMemcpy(h.data(), d, count * sizeof(T), cudaMemcpyDeviceToHost));
+    put(h.data(), count * sizeof(T));
+}
+
+int main() {
+    int sm_count = 0, optin = 0;
+    CK(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, 0));
+    CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, 0));
+    // as create_impl does: the staged decoder may take the device's opt-in shared memory
+    CK(cudaFuncSetAttribute(log_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    const uint32_t device[2] = {(uint32_t)sm_count, (uint32_t)optin};
+    put(device, 8);
+    cudaStream_t s;
+    CK(cudaStreamCreate(&s));
+    uint32_t n;
+    while (fread(&n, 4, 1, stdin) == 1) {
+        std::vector<uint8_t> seg(n);
+        get(seg.data(), n);
+        uint32_t nb32 = 0, with_part = 0, slack = 0;
+        get(&nb32, 4);
+        const int64_t nb = nb32;
+        std::vector<uint64_t> offs((size_t)nb);
+        get(offs.data(), (size_t)nb * 8);
+        get(&with_part, 4);
+        std::vector<int32_t> parts(with_part ? (size_t)nb : 0);
+        get(parts.data(), parts.size() * 4);
+        get(&slack, 4);
+        const uint64_t readable = (uint64_t)n + slack;
+
+        uint8_t *d_bytes = dev_alloc<uint8_t>(readable, 0, s);
+        uint64_t *d_off = dev_alloc<uint64_t>((size_t)nb, 0, s), *d_cnt = dev_alloc<uint64_t>((size_t)nb + 1, 0, s);
+        int32_t *d_part = with_part ? dev_alloc<int32_t>((size_t)nb, 0, s) : nullptr;
+        LogBatchInfo *d_info = dev_alloc<LogBatchInfo>((size_t)nb, 0, s);
+        uint32_t *d_err = dev_alloc<uint32_t>(2, 0, s);
+        CK(cudaMemcpyAsync(d_bytes, seg.data(), n, cudaMemcpyHostToDevice, s));
+        CK(cudaMemcpyAsync(d_off, offs.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s));
+        if (d_part) CK(cudaMemcpyAsync(d_part, parts.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, s));
+        if (nb) {
+            log_header_kernel<<<log_thread_grid(nb, sm_count), 128, 0, s>>>(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info, d_cnt, d_err);
+            tile_base_scan_kernel<<<1, 1024, 0, s>>>(d_cnt, nb);
+            CK(cudaGetLastError());
+        }
+        uint32_t hdr[2] = {0, 0}, unc_err = 0, dec_err = 0;
+        uint64_t nrec = 0;
+        CK(cudaMemcpyAsync(hdr, d_err, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(&nrec, d_cnt + nb, 8, cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        bool ran = nb > 0 && !(hdr[0] & (LOGB_BAD | LOGB_COMPRESSED)) && nrec > 0;
+        uint8_t *d_unc = nullptr, *d_lit = nullptr;
+        uint64_t *d_slot = nullptr;
+        const uint32_t codecs = hdr[0] & LOGB_CODECS;
+        if (ran && codecs) {
+            const bool zstd = (codecs & LOGB_ZSTD) != 0;
+            d_slot = dev_alloc<uint64_t>((size_t)nb + 2, 0, s);
+            CK(cudaMemsetAsync(d_err, 0, 4, s));
+            CK(log_launch_size_pass(d_bytes, d_info, nb, d_slot, d_err, zstd, sm_count, s));
+            uint64_t unc_total = 0;
+            CK(cudaMemcpyAsync(&unc_total, d_slot + nb, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(&unc_err, d_err, 4, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            if (unc_err) ran = false;
+            else {
+                d_unc = dev_alloc<uint8_t>(unc_total + 64, 0, s);
+                if (zstd) d_lit = dev_alloc<uint8_t>(unc_total + 64, 0, s);
+                CK(log_launch_copy_pass(d_bytes, d_info, nb, d_slot, d_unc, d_lit, d_err, codecs, sm_count, s));
+            }
+        }
+        const LogDecodeShape shape = log_decode_shape(hdr[1], nb, sm_count, (size_t)optin);
+        int32_t *d_dpart = nullptr, *d_klen = nullptr, *d_vlen = nullptr;
+        int64_t *d_ts = nullptr;
+        uint64_t *d_ksrc = nullptr, *d_tb = nullptr;
+        uint8_t *d_keys = nullptr;
+        const int64_t ntiles = ((int64_t)nrec + TILE - 1) / TILE;
+        uint64_t nkey = 0;
+        if (ran) {
+            d_dpart = dev_alloc<int32_t>(nrec, 0xA5, s);
+            d_ts = dev_alloc<int64_t>(nrec, 0xA5, s);
+            d_klen = dev_alloc<int32_t>(nrec, 0xA5, s);
+            d_vlen = dev_alloc<int32_t>(nrec, 0xA5, s);
+            d_ksrc = dev_alloc<uint64_t>(nrec, 0xA5, s);
+            d_tb = dev_alloc<uint64_t>((size_t)ntiles + 1, 0xA5, s);
+            // (d_err[0] is 0 here, or holds what the copy pass found, as in scan_log_batches)
+            CK(log_launch_decode(shape, d_bytes, readable, d_info, nb, d_cnt, d_dpart, d_ts, d_klen, d_vlen, d_ksrc, d_err, s));
+            CK(log_launch_tile_base(d_klen, (int64_t)nrec, d_tb, sm_count, s));
+            CK(cudaMemcpyAsync(&dec_err, d_err, 4, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(&nkey, d_tb + ntiles, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+            if (!dec_err) {
+                d_keys = dev_alloc<uint8_t>(nkey + 64, 0xA5, s);
+                CK(log_launch_gather_keys(d_bytes, d_ksrc, d_klen, (int64_t)nrec, d_tb, d_keys, sm_count, s));
+            }
+            CK(cudaStreamSynchronize(s));
+        }
+        const uint32_t staged = shape.staged ? 1u : 0u, stage = shape.stage, grid = (uint32_t)shape.grid, ran32 = ran ? 1u : 0u;
+        put(hdr, 8);
+        put(&unc_err, 4);
+        put(&dec_err, 4);
+        put(&nrec, 8);
+        put(&staged, 4);
+        put(&stage, 4);
+        put(&grid, 4);
+        put(&ran32, 4);
+        if (ran) {
+            put_dev(d_dpart, nrec);
+            put_dev(d_ts, nrec);
+            put_dev(d_klen, nrec);
+            put_dev(d_vlen, nrec);
+            if (!dec_err) {
+                put_dev(d_tb, (size_t)ntiles + 1);
+                put_dev(d_keys, nkey + 64);
+            }
+        }
+        for (void *p : {(void *)d_bytes, (void *)d_off, (void *)d_cnt, (void *)d_part, (void *)d_info, (void *)d_err, (void *)d_unc,
+                        (void *)d_lit, (void *)d_slot, (void *)d_dpart, (void *)d_ts, (void *)d_klen, (void *)d_vlen, (void *)d_ksrc,
+                        (void *)d_tb, (void *)d_keys})
+            if (p) CK(cudaFree(p));
+    }
+    CK(cudaStreamDestroy(s));
+    fflush(stdout);
+    return 0;
+}

@@ -2,6 +2,8 @@
 
   logdecomp_probe  tests/native/logdecomp_probe.cu: the product's decompression stage on the GPU, output made visible
                    (sm_90a, the library's nvcc flags without -shared / -fPIC)
+  logdecode_probe  tests/native/logdecode_probe.cu: the product's record stage (decode, tile bases, key gather) on the GPU,
+                   every decoded column made visible (built like logdecomp_probe)
   codec_harness    tests/native/codec_harness.cu: the same codec walks as plain host code, one "lane" (codec_harness.py runs it)
 
 build() makes the plain programs in tests/native/build/ (git-ignored).  __graft_entry__.build() builds them, because the machine
@@ -16,7 +18,8 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(ROOT, "kafka_topic_analyzer_b200", "csrc")
 NATIVE = os.path.join(HERE, "native")
 OUT = os.path.join(NATIVE, "build")
-PROGRAMS = ("logdecomp_probe", "codec_harness")
+PROGRAMS = ("logdecomp_probe", "logdecode_probe", "codec_harness")
+GPU_PROGRAMS = ("logdecomp_probe", "logdecode_probe")
 SANITIZE = ["-g", "-Xcompiler", "-fsanitize=address,-fno-omit-frame-pointer"]
 
 
@@ -27,7 +30,7 @@ def nvcc():
 
 def _command(nvcc, name, exe, flags=()):
     src = os.path.join(NATIVE, name + ".cu")
-    if name == "logdecomp_probe":
+    if name in GPU_PROGRAMS:
         from kafka_topic_analyzer_b200 import _native
         lib_flags = " ".join(_native.NVCC_FLAGS).replace("-Xcompiler -fPIC", "").replace("-shared", "").split()
         return [nvcc, *lib_flags, "-o", exe, src]

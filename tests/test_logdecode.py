@@ -142,9 +142,11 @@ def test_cli_log_dir(tmp_path):
 
 
 def test_cpp_segment_encoder_matches_the_topic():
-    """kta_synth_encode_segment_host (the broker-format face of the synthetic topic) against fill_host."""
+    """kta_synth_encode_segment_host (the broker-format face of the synthetic topic) against fill_host.  Records without a
+    timestamp, alone and inside batches that have one, read back as -1 (baseTimestamp + timestampDelta = -1)."""
     P = 8
-    spec = synth.make_spec(P * 700, P, key_mode=2, distinct_keys=400, tombstone_per_10k=1500, null_key_per_10k=500)
+    spec = synth.make_spec(P * 700, P, key_mode=2, distinct_keys=400, tombstone_per_10k=1500, null_key_per_10k=500,
+                           ts_missing_per_10k=800)
     for p in (0, 5):
         got = [r for b in kc.read_segment(synth.encode_segment(spec, p, batch_records=33)) for r in b.records]
         t = synth.fill_host(spec, rank=p, world=P)              # partition p's records in offset order
@@ -154,6 +156,25 @@ def test_cpp_segment_encoder_matches_the_topic():
             assert off == t.offset[i] and ts == t.ts_ms[i]
             assert key == (None if t.key_len[i] < 0 else t.key_bytes[koff[i]:koff[i] + t.key_len[i]].tobytes())
             assert vl == (None if t.value_len[i] < 0 else t.value_len[i])
+        assert 0 < int((t.ts_ms == -1).sum()) < t.n
+
+
+@pytest.mark.gpu
+def test_synthetic_topic_with_missing_timestamps_as_log_segments():
+    """A topic whose records lack timestamps here and there, encoded broker-style by kta_synth_encode_segment_host: the
+    decoded log gives the oracle's answer over fill_host, its earliest message (-1 ms: a record without a timestamp)
+    included."""
+    P = 3
+    spec = synth.make_spec(P * 3000, P, key_mode=2, distinct_keys=500, tombstone_per_10k=1500, ts_missing_per_10k=30)
+    o = Oracle(count_alive_keys=True, now=NOW)
+    with KtaEngine(P, count_alive_keys=True, now=NOW) as e:
+        for p in range(P):
+            t = synth.fill_host(spec, rank=p, world=P)
+            o.handle_batch(t.partition, t.ts_ms, t.key_len, t.value_len, t.key_bytes)
+            assert e.push_log_segment(p, synth.encode_segment(spec, p, batch_records=100)) == t.n
+        e.finalize()
+        assert e.message_metrics.earliest_message() == o.earliest()
+        assert_parity(e, o, P, check_alive=True)
 
 
 @pytest.mark.gpu
