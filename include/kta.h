@@ -283,6 +283,31 @@ int kta_log_crc_stats(kta_handle *h, uint64_t *checked_batches, uint64_t *failed
  * batch order: min(cap, kept) of them are copied to out; *count (may be NULL) = the number kept.  kta_reset clears them. */
 int kta_log_crc_failures(kta_handle *h, kta_log_crc_failure *out, int64_t cap, int64_t *count);
 
+/* Offsets: read only what a consumer would fetch, from a partition's log start offset S up to its high watermark H.
+ * A broker keeps both in its data directory (log-start-offset-checkpoint, replication-offset-checkpoint); records below S
+ * (DeleteRecords, purged repartition topics) and at or above H (appends not yet committed) stay in the .log files, and a
+ * consumer that starts at S (auto.offset.reset=earliest) and reads up to H never sees them.
+ * Unset (the default): nothing changes.  Set for partition p: with last = baseOffset + lastOffsetDelta (the stored field,
+ * which can lie past the last record of a compacted batch), a batch is served only when S <= last < H: a fetch from S
+ * starts at the first batch whose last offset is >= S, and a fetch bounded by H stops before the batch that holds H.  A
+ * batch that is not served is skipped unread: it is not CRC-checked, decompressed, decoded, or classified as transactional
+ * data or as a marker; it delivers no records, takes no sequence numbers and raises no error, so damage inside it does
+ * not refuse the call.  Within a served batch a record with baseOffset + offsetDelta < S is dropped, as librdkafka's
+ * reader drops messages older than the fetch offset; offsets are read from the decompressed records, so a compressed
+ * batch may be cut.  With check.crcs only served batches are checked and counted; a served batch that fails is skipped
+ * and listed as before, cut or not.  Under read_committed a marker outside the window is not seen (its transaction is
+ * decided by the registered ranges, or is undecided), and the producers' baseOffset order is checked over served batches
+ * only.  The fields that frame a batch still refuse the call as before: it must fit the buffer, batchLength >= 49, magic 2.
+ * Windows apply to the log entry points only; kta_push and the batch entry points ignore them.
+ * log_start_offset, high_watermark: -1 = no bound on that side.  KTA_ERR_INVALID when the partition lies outside
+ * [0, num_partitions), when a value is below -1, or when both are set and log_start_offset > high_watermark.  A later
+ * call replaces the partition's window; it applies to every later log call; kta_reset clears every window. */
+int kta_log_set_offsets(kta_handle *h, int32_t partition, int64_t log_start_offset, int64_t high_watermark);
+/* totals over the successful log calls since create / reset: the batches that were not served, and the records left out
+ * (the recordsCount of the data batches not served, plus the records dropped below the log start offset).  Either pointer
+ * may be NULL. */
+int kta_log_offset_stats(kta_handle *h, uint64_t *batches_not_served, uint64_t *records_left_out);
+
 /* ---- introspection for benchmarks ---- */
 /* kernels launched by this handle since create/reset, and device time of the scan kernels (ms,
  * CUDA events on the handle's stream; only collected when enabled) */

@@ -152,6 +152,8 @@ SYMBOLS = {
     "kta_log_set_check_crcs": (C.c_int, [_P, C.c_int]),
     "kta_log_crc_stats": (C.c_int, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "kta_log_crc_failures": (C.c_int, [_P, C.POINTER(CrcFailure), C.c_int64, C.POINTER(C.c_int64)]),
+    "kta_log_set_offsets": (C.c_int, [_P, C.c_int32, C.c_int64, C.c_int64]),
+    "kta_log_offset_stats": (C.c_int, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "kta_stats": (C.c_int, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "kta_set_timing": (C.c_int, [_P, C.c_int]),
     "kta_scan_time_ms": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),

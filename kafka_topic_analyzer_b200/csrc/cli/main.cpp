@@ -18,6 +18,11 @@
 //                              CRC-32C on the GPU: a batch that fails it is skipped, and reported on stderr in librdkafka's
 //                              words ("... failed CRC32C check ..."); the report covers the rest and the exit status stays
 //                              0, as the reference logs a failed poll and goes on (src/kafka.rs:95-97).
+//                              DIR/log-start-offset-checkpoint and DIR/replication-offset-checkpoint, when present, give each
+//                              partition they list the offsets a consumer reads: from the log start offset (raised to the
+//                              first segment's base offset) up to the high watermark (clamped into [start, log end offset]),
+//                              as the reference reads from the earliest offset up to the high watermark (src/kafka.rs:28-31,
+//                              60-72).  Records outside are left out, and the two offsets are the report's < OS and > OS.
 //   --feed push|batch|device   how records reach the handlers: kta_push per record (the reference's call shape),
 //                              kta_push_batch_host, or generated and scanned in HBM
 //
@@ -87,10 +92,45 @@ static void warn_crc_failures(kta_handle *h) {
         fprintf(stderr, "warning: %llu more record batch(es) failed CRC32C check and were skipped\n", (unsigned long long)(failed - (uint64_t)kept));
 }
 
+// A broker's offset checkpoint file (log-start-offset-checkpoint, replication-offset-checkpoint): a version line "0", a
+// count line, then `count` lines "topic partition offset".  The entries of `topic` go to out[partition].  false (and a
+// message naming the file) when it does not parse; true without entries when the file does not exist.
+static bool read_checkpoint(const std::string &path, const std::string &topic, std::map<int, int64_t> &out) {
+    std::ifstream f(path);
+    if (!f) return true;
+    auto bad = [&](const char *why) { fprintf(stderr, "error: %s: %s\n", path.c_str(), why); return false; };
+    auto number = [](const std::string &t, int64_t &v) {
+        if (t.empty() || t.size() > 19 || t.find_first_not_of("0123456789", t[0] == '-' ? 1 : 0) != std::string::npos || t == "-") return false;
+        v = strtoll(t.c_str(), nullptr, 10);
+        return true;
+    };
+    std::string line;
+    int64_t version = -1, count = -1;
+    if (!std::getline(f, line) || !number(line, version) || version != 0) return bad("not version 0");
+    if (!std::getline(f, line) || !number(line, count) || count < 0) return bad("no entry count");
+    for (int64_t i = 0; i < count; i++) {
+        if (!std::getline(f, line)) return bad("fewer entries than its count");
+        const size_t a = line.find(' '), b = a == std::string::npos ? a : line.find(' ', a + 1);
+        int64_t part = -1, off = 0;
+        if (b == std::string::npos || line.find(' ', b + 1) != std::string::npos || !number(line.substr(a + 1, b - a - 1), part) ||
+            part < 0 || part > INT32_MAX || !number(line.substr(b + 1), off))
+            return bad("an entry is not \"topic partition offset\"");
+        if (line.compare(0, a, topic) == 0 && a == topic.size()) out[(int)part] = off;
+    }
+    while (std::getline(f, line))
+        if (!line.empty()) return bad("more entries than its count");
+    return true;
+}
+
 static int analyze_log_dir(const std::string &topic, const std::string &dir, bool alive, int hll, bool read_committed, bool check_crcs,
                            std::chrono::steady_clock::time_point start_time) {
     // get_topic_offsets (src/kafka.rs:60-72) from the files: partitions = <topic>-<n> directories, low watermark =
-    // first batch's baseOffset, high watermark = last batch's baseOffset + lastOffsetDelta + 1
+    // first batch's baseOffset, high watermark = last batch's baseOffset + lastOffsetDelta + 1; for the partitions the
+    // broker's checkpoint files list, its log start offset and high watermark instead (and only what lies between is read)
+    std::map<int, int64_t> log_start, high_watermark;
+    if (!read_checkpoint(dir + "/log-start-offset-checkpoint", topic, log_start) ||
+        !read_checkpoint(dir + "/replication-offset-checkpoint", topic, high_watermark))
+        return 1;
     std::map<int, std::vector<std::string>> segs, txn_indexes;
     DIR *d = opendir(dir.c_str());
     if (!d) { fprintf(stderr, "Error fetching metadata: cannot open %s\n", dir.c_str()); return 101; }
@@ -127,6 +167,27 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
     kta_handle *h = nullptr;
     KTA(kta_create(&cfg, &h));
     if (check_crcs) KTA(kta_log_set_check_crcs(h, 1));
+    // the window of every partition the checkpoints list: the log start offset raised to the first segment's base offset
+    // (its 20-digit file name, as the broker loads a log), the high watermark no lower than that (it is clamped to the log
+    // end offset once the files are read: no batch lies beyond it, so the window reads the same either way)
+    std::map<int, int64_t> win_start;
+    for (auto &kv : segs) {
+        const int p = kv.first;
+        if (!log_start.count(p) && !high_watermark.count(p)) continue;
+        int64_t s = -1;
+        if (log_start.count(p)) {
+            s = std::max<int64_t>(log_start[p], 0);
+            if (!kv.second.empty()) {
+                const std::string &f = kv.second.front();
+                const std::string base = f.substr(f.rfind('/') + 1, f.size() - 4 - (f.rfind('/') + 1));
+                if (base.size() == 20 && base.find_first_not_of("0123456789") == std::string::npos)
+                    s = std::max<int64_t>(s, strtoll(base.c_str(), nullptr, 10));
+            }
+        }
+        const int64_t hw = high_watermark.count(p) ? std::max<int64_t>(std::max<int64_t>(high_watermark[p], 0), s) : -1;
+        KTA(kta_log_set_offsets(h, p, s, hw));
+        win_start[p] = s;
+    }
     // read_committed: every partition's aborted transactions are known before any segment is decoded, so a transaction
     // whose marker lies in a later group of segments is decided exactly
     if (read_committed)
@@ -177,6 +238,12 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
         }
     }
     flush();
+    for (auto &kv : win_start) {   // < OS and > OS of the partitions with a window
+        const int p = kv.first;
+        if (kv.second >= 0) start_offsets[p] = kv.second;
+        if (high_watermark.count(p))   // clamped into [start, log end offset]
+            end_offsets[p] = std::max(start_offsets[p], std::min(std::max<int64_t>(high_watermark[p], 0), end_offsets[p]));
+    }
     if (check_crcs) warn_crc_failures(h);
     if (std::all_of(end_offsets.begin(), end_offsets.end(), [](int64_t v) { return v == 0; })) {
         fprintf(stderr, "Given topic has no content, no analysis possible. Exiting.\n");  // main.rs:98-101
@@ -227,7 +294,10 @@ int main(int argc, char **argv) {
                  "                                                 librdkafka's): true verifies every batch's CRC-32C, skips and\n"
                  "                                                 reports the batches that fail it, and reports the rest\n"
                  "        --log-dir <DIR>                          read <DIR>/<TOPIC>-<partition>/*.log (and, read_committed,\n"
-                 "                                                 *.txnindex) instead of a broker\n"
+                 "                                                 *.txnindex) instead of a broker; for the partitions that\n"
+                 "                                                 <DIR>/log-start-offset-checkpoint and\n"
+                 "                                                 <DIR>/replication-offset-checkpoint list, only the records\n"
+                 "                                                 from the log start offset up to the high watermark\n"
                  "    -t, --topic <TOPIC>                          The topic to analyze\n"
                  "        --synthetic <k=v,...>                    in-memory synthetic topic (this build has no Kafka client)\n"
                  "        --feed <push|batch|device>               how records are handed to the metric handlers");

@@ -25,6 +25,7 @@
 #include "kta_logcrc.cuh"
 #include "kta_logdecode.cuh"
 #include "kta_logdecode_launch.cuh"
+#include "kta_logoffsets.cuh"
 #include "kta_logtxn.cuh"
 #include "kta_synth.h"
 
@@ -175,6 +176,19 @@ struct CrcState {
     std::vector<kta_log_crc_failure> kept;           // the first KTA_LOG_CRC_KEEP failures
 };
 
+// The log start offset and high watermark of each partition (kta_log_set_offsets, kta_logoffsets.cuh): the table, the
+// passes' buffers, and what successful calls left out
+struct OffsetState {
+    std::vector<int64_t> win;                        // [2p] log start offset, [2p + 1] high watermark (-1: unbounded);
+                                                     // empty until a window is set
+    int64_t set = 0;                                 // partitions with a bound: the window passes run only while > 0
+    bool dirty = false;                              // win changed since it was last copied to d_win
+    DevBuf<int64_t> d_win;                           // win on the device, one longlong2 per partition
+    DevBuf<uint32_t> d_cut;                          // the call's cut batches (served, with records below the start)
+    DevBuf<uint64_t> d_drop;                         // per batch: records the count pass drops, then their scan
+    uint64_t totals[2] = {0, 0};                     // batches not served, records left out
+};
+
 // State of the log entry points (Kafka RecordBatch v2 segments → SoA → scan), reused from call to call
 struct LogScan {
     DevBuf<uint8_t> bytes;                   // segments staged from the host (kta_push_log_segments_host)
@@ -182,7 +196,8 @@ struct LogScan {
     DevBuf<int32_t> part;                    // and each batch's partition
     DevBuf<LogBatchInfo> info;               // per batch, from the header pass
     DevBuf<uint64_t> cnt;                    // records per batch, then their inclusive scan
-    DevBuf<uint32_t> err;                    // [0] error flags, [1] longest batch; check.crcs: [2] failures, [4..5] their bytes
+    DevBuf<uint32_t> err;                    // [0] error flags, [1] longest batch; check.crcs: [2] failures, [4..5] their bytes;
+                                             // windows: [6] cut batches, [7] batches not served, [8..9] their records
     DevBuf<int32_t> dec_part, dec_klen, dec_vlen;   // the decoded columns
     DevBuf<int64_t> dec_ts;
     DevBuf<uint64_t> dec_ksrc;               // per decoded record: where its key bytes lie in the segment buffer
@@ -193,6 +208,7 @@ struct LogScan {
     bool read_committed = false;
     TxnState txn;
     CrcState crc;
+    OffsetState offsets;
 };
 
 struct kta_handle {
@@ -654,6 +670,7 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
                 if (f) CU(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
     // the record decoder stages a batch of up to 48 KiB per warp (log_decode); attributes belong to the device
     CU(cudaFuncSetAttribute(log_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+    CU(cudaFuncSetAttribute(log_decode_window_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
     if ((rc = state_reset_device(h))) return rc;
     CU(cudaStreamSynchronize(h->stream));
     return KTA_OK;
@@ -896,15 +913,17 @@ static int txn_passes(kta_handle *h, int32_t partition, const uint8_t *dev_bytes
 // What the header pass (and read_committed's passes and the CRC check) found in one call's batches
 struct LogHeaders {
     uint64_t nrec = 0;                               // records in all
-    uint32_t err[6] = {0, 0, 0, 0, 0, 0};            // the header pass's error word: [0] LOGB_* flags, [1] longest batch;
-                                                     // check.crcs: [2] failed batches, [4..5] their bytes (u64)
+    uint32_t err[LOG_WIN_WORDS] = {};                // the header pass's error word: [0] LOGB_* flags, [1] longest batch;
+                                                     // check.crcs: [2] failed batches, [4..5] their bytes (u64); windows:
+                                                     // [6] cut batches, [7] batches not served, [8..9] their records (u64)
     unsigned long long txn_stats[3] = {0, 0, 0};     // this call's aborted batches, aborted records, undecided records
     std::vector<kta_log_crc_failure> crc_fails;      // check.crcs: this call's failures, in batch order, as many as are kept
 };
 
 // check.crcs: the passes of kta_logcrc.cuh that precede the header pass (span counts, their scan, the spans' CRCs).  No
 // host round trip: the span kernel reads the total from the scan, and its grid is bounded by the call's bytes.
-static int log_crc_spans(kta_handle *h, const uint8_t *dev_bytes, int64_t len, const uint64_t *dev_batch_off, int64_t nbatches) {
+static int log_crc_spans(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes, int64_t len,
+                         const uint64_t *dev_batch_off, int64_t nbatches, bool window) {
     CrcState &c = h->log.crc;
     cudaStream_t s = h->stream;
     int rc;
@@ -917,7 +936,12 @@ static int log_crc_spans(kta_handle *h, const uint8_t *dev_bytes, int64_t len, c
         CU(cudaFuncSetAttribute(log_crc_span_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LOG_CRC_SMEM));
     }
     if ((rc = c.d_spans.grow(s, nbatches + 1)) || (rc = c.d_acc.grow(s, nbatches)) || (rc = c.d_fails.grow(s, nbatches))) return rc;
-    log_crc_count_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, c.d_spans, c.d_acc);
+    if (window)   // batches that are not served are not checked
+        log_window_crc_count_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(
+            dev_bytes, len, dev_batch_off, nbatches, c.d_spans, c.d_acc, partition, dev_batch_partition,
+            reinterpret_cast<const longlong2 *>(h->log.offsets.d_win.get()), h->cfg.num_partitions);
+    else
+        log_crc_count_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, c.d_spans, c.d_acc);
     tile_base_scan_kernel<<<1, 1024, 0, s>>>(c.d_spans, nbatches);
     // at most len / S + nbatches spans, one per thread at least: a small call gets a small grid
     const int64_t max_spans = len / LOG_CRC_SPAN + nbatches;
@@ -928,24 +952,48 @@ static int log_crc_spans(kta_handle *h, const uint8_t *dev_bytes, int64_t len, c
     return KTA_OK;
 }
 
+// windows: the window table goes to the device when it changed since the last call (two host synchronisations, only then)
+static int log_offsets_upload(kta_handle *h) {
+    OffsetState &o = h->log.offsets;
+    if (!o.dirty) return KTA_OK;
+    int rc;
+    if (!o.d_win && (rc = o.d_win.alloc((int64_t)o.win.size()))) return rc;
+    CU(cudaStreamSynchronize(h->stream));   // no queued pass reads the table while it is replaced
+    CU(cudaMemcpyAsync(o.d_win, o.win.data(), o.win.size() * sizeof(int64_t), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    o.dirty = false;
+    return KTA_OK;
+}
+
 // The header pass, read_committed's passes and the scan of the record counts.  One host round trip (two under
 // read_committed); refuses the call for its headers and for the order of a producer's batches.  With check.crcs the CRC
 // passes come first and the failures are counted in the same round trip; only a call with failures makes one more, for
-// their list.
+// their list.  With windows the header pass also skips the batches that are not served and lists the cut ones; their
+// counts come back in the same round trip.
 static int log_headers(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes, int64_t len,
                        const uint64_t *dev_batch_off, int64_t nbatches, LogHeaders &out) {
     LogScan &L = h->log;
     cudaStream_t s = h->stream;
     int rc;
     if ((rc = L.info.grow(s, nbatches + 1)) || (rc = L.cnt.grow(s, nbatches + 1))) return rc;
-    if (!L.err && (rc = L.err.alloc(6))) return rc;
-    const bool crc = L.crc.on;
-    const size_t err_bytes = crc ? 24 : 8;
-    if (crc && (rc = log_crc_spans(h, dev_bytes, len, dev_batch_off, nbatches))) return rc;
+    if (!L.err && (rc = L.err.alloc(LOG_WIN_WORDS))) return rc;
+    const bool crc = L.crc.on, win = L.offsets.set > 0;
+    if (win && ((rc = log_offsets_upload(h)) || (rc = L.offsets.d_cut.grow(s, nbatches)))) return rc;
+    const size_t err_bytes = win ? LOG_WIN_WORDS * sizeof(uint32_t) : crc ? 24 : 8;
+    if (crc && (rc = log_crc_spans(h, partition, dev_batch_partition, dev_bytes, len, dev_batch_off, nbatches, win))) return rc;
     CU(cudaMemsetAsync(L.err, 0, err_bytes, s));
-    if (crc)
+    const longlong2 *d_win = reinterpret_cast<const longlong2 *>(L.offsets.d_win.get());
+    const int32_t P = h->cfg.num_partitions;
+    if (crc && win)
+        log_window_crc_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(
+            dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, L.info, L.cnt, L.err, L.crc.d_acc, L.crc.d_fails,
+            d_win, P, L.offsets.d_cut);
+    else if (crc)
         log_crc_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(
             dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, L.info, L.cnt, L.err, L.crc.d_acc, L.crc.d_fails);
+    else if (win)
+        log_window_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(
+            dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, L.info, L.cnt, L.err, d_win, P, L.offsets.d_cut);
     else
         log_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, partition,
                                                                                 dev_batch_partition, L.info, L.cnt, L.err);
@@ -1010,8 +1058,9 @@ static int log_decompress(kta_handle *h, int32_t partition, const uint8_t *dev_b
 
 // The records of every batch into the decoded columns, which b then names; with keys, where each record's key bytes lie.
 // One warp per batch; the batch is staged in shared memory when the longest one fits a stage of <= 48 KiB.
+// window: the call has cut batches, whose records below the log start offset are left out (log_decode_window_kernel).
 static int log_decode(kta_handle *h, const uint8_t *dev_bytes, int64_t readable, int64_t nbatches, uint64_t nrec,
-                      uint32_t longest, bool keys, kta_batch &b) {
+                      uint32_t longest, bool keys, bool window, kta_batch &b) {
     LogScan &L = h->log;
     cudaStream_t s = h->stream;
     if ((int64_t)nrec >= ((int64_t)1 << 31) - 2) return fail(KTA_ERR_INVALID, "%llu records in one call: split the segments", (unsigned long long)nrec);
@@ -1020,8 +1069,13 @@ static int log_decode(kta_handle *h, const uint8_t *dev_bytes, int64_t readable,
         (rc = L.dec_ts.grow(s, (int64_t)nrec)) || (rc = L.dec_ksrc.grow(s, (int64_t)nrec)))
         return rc;
     const LogDecodeShape shape = log_decode_shape(longest, nbatches, h->sm_count, h->smem_optin);
-    CU(log_launch_decode(shape, dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, L.dec_ts, L.dec_klen, L.dec_vlen,
-                         keys ? L.dec_ksrc.get() : nullptr, L.err, s));
+    if (window)
+        CU(log_launch_decode_window(shape, dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, L.dec_ts, L.dec_klen,
+                                    L.dec_vlen, keys ? L.dec_ksrc.get() : nullptr, L.err,
+                                    reinterpret_cast<const longlong2 *>(L.offsets.d_win.get()), h->cfg.num_partitions, s));
+    else
+        CU(log_launch_decode(shape, dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, L.dec_ts, L.dec_klen, L.dec_vlen,
+                             keys ? L.dec_ksrc.get() : nullptr, L.err, s));
     h->launches++;
     b = kta_batch{};
     b.n = (int64_t)nrec;
@@ -1059,6 +1113,23 @@ static int log_gather_keys(kta_handle *h, int32_t partition, const uint8_t *dev_
     return KTA_OK;
 }
 
+// windows: the call's cut batches (ncut of them, after the decompression) are walked and their records below the log
+// start offset counted; the record-count scan is corrected for them.  One host round trip: *nrec = the records kept,
+// *dropped = the records dropped.
+static int log_cut_count(kta_handle *h, const uint8_t *dev_bytes, int64_t nbatches, int64_t ncut, uint64_t *nrec, uint64_t *dropped) {
+    LogScan &L = h->log;
+    cudaStream_t s = h->stream;
+    int rc;
+    if ((rc = L.offsets.d_drop.grow(s, nbatches + 1))) return rc;
+    CU(log_launch_cut_count(dev_bytes, L.info, nbatches, L.offsets.d_cut, ncut, reinterpret_cast<const longlong2 *>(L.offsets.d_win.get()),
+                            h->cfg.num_partitions, L.cnt, L.offsets.d_drop, h->sm_count, s));
+    h->launches += 3;
+    CU(cudaMemcpyAsync(nrec, L.cnt + nbatches, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(dropped, L.offsets.d_drop + nbatches, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    return KTA_OK;
+}
+
 static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes,
                             int64_t len, int64_t readable /* bytes of dev_bytes that may be READ (>= len when the buffer has slack) */,
                             const uint64_t *dev_batch_off, int64_t nbatches, int64_t *records_out) {
@@ -1071,25 +1142,33 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     if ((rc = alive_settle_if_any(h))) return rc;   // the decode scratch of an earlier call is about to be reused
     LogHeaders hd;
     if ((rc = log_headers(h, partition, dev_batch_partition, dev_bytes, len, dev_batch_off, nbatches, hd))) return rc;
+    const int64_t ncut = hd.err[6];
+    uint64_t nrec = hd.nrec, dropped = 0;
     if (hd.nrec > 0) {
         const uint32_t codecs = hd.err[0] & LOGB_CODECS;
         if (codecs && (rc = log_decompress(h, partition, dev_bytes, nbatches, codecs))) return rc;
-        const bool keys = keys_travel(h);
+        if (ncut && (rc = log_cut_count(h, dev_bytes, nbatches, ncut, &nrec, &dropped))) return rc;
+        // (cut batches that keep no record are still decoded, so damage in them refuses the call as elsewhere)
+        const bool keys = nrec > 0 && keys_travel(h);
         kta_batch b;
-        if ((rc = log_decode(h, dev_bytes, readable, nbatches, hd.nrec, hd.err[1], keys, b))) return rc;
+        if ((rc = log_decode(h, dev_bytes, readable, nbatches, nrec, hd.err[1], keys, ncut > 0, b))) return rc;
         if ((rc = log_gather_keys(h, partition, dev_bytes, keys, b))) return rc;
-        if ((rc = scan_device_batch(h, &b))) return rc;
+        if (nrec > 0 && (rc = scan_device_batch(h, &b))) return rc;
     }
-    // the call succeeded: its transaction counters and CRC results join the handle's totals
+    // the call succeeded: its transaction counters, CRC results and what its windows left out join the handle's totals
     for (int i = 0; i < 3; i++) h->log.txn.totals[i] += hd.txn_stats[i];
+    const uint32_t not_served = hd.err[7];
+    OffsetState &o = h->log.offsets;
+    o.totals[0] += not_served;
+    o.totals[1] += ((uint64_t)hd.err[8] | ((uint64_t)hd.err[9] << 32)) + dropped;
     CrcState &c = h->log.crc;
     if (c.on) {
-        c.totals[0] += (uint64_t)nbatches;
+        c.totals[0] += (uint64_t)nbatches - not_served;
         c.totals[1] += hd.err[2];
         c.totals[2] += (uint64_t)hd.err[4] | ((uint64_t)hd.err[5] << 32);
         c.kept.insert(c.kept.end(), hd.crc_fails.begin(), hd.crc_fails.end());
     }
-    if (records_out) *records_out = (int64_t)hd.nrec;
+    if (records_out) *records_out = (int64_t)nrec;
     return KTA_OK;
 }
 
@@ -1219,6 +1298,34 @@ extern "C" int kta_log_crc_stats(kta_handle *h, uint64_t *checked_batches, uint6
     if (checked_batches) *checked_batches = h->log.crc.totals[0];
     if (failed_batches) *failed_batches = h->log.crc.totals[1];
     if (failed_bytes) *failed_bytes = h->log.crc.totals[2];
+    return KTA_OK;
+}
+
+extern "C" int kta_log_set_offsets(kta_handle *h, int32_t partition, int64_t log_start_offset, int64_t high_watermark) {
+    if (!h) return fail(KTA_ERR_INVALID, "null handle");
+    if (partition < 0 || partition >= h->cfg.num_partitions)
+        return fail(KTA_ERR_INVALID, "partition %d outside [0, %d)", partition, h->cfg.num_partitions);
+    if (log_start_offset < -1 || high_watermark < -1)
+        return fail(KTA_ERR_INVALID, "log start offset %lld / high watermark %lld below -1", (long long)log_start_offset,
+                    (long long)high_watermark);
+    if (log_start_offset >= 0 && high_watermark >= 0 && log_start_offset > high_watermark)
+        return fail(KTA_ERR_INVALID, "log start offset %lld above the high watermark %lld", (long long)log_start_offset,
+                    (long long)high_watermark);
+    OffsetState &o = h->log.offsets;
+    if (o.win.empty()) o.win.assign(2 * (size_t)h->cfg.num_partitions, -1);
+    int64_t *w = o.win.data() + 2 * (size_t)partition;
+    o.set -= (w[0] != -1 || w[1] != -1);
+    w[0] = log_start_offset;
+    w[1] = high_watermark;
+    o.set += (w[0] != -1 || w[1] != -1);
+    o.dirty = true;
+    return KTA_OK;
+}
+
+extern "C" int kta_log_offset_stats(kta_handle *h, uint64_t *batches_not_served, uint64_t *records_left_out) {
+    if (!h) return fail(KTA_ERR_INVALID, "null handle");
+    if (batches_not_served) *batches_not_served = h->log.offsets.totals[0];
+    if (records_left_out) *records_left_out = h->log.offsets.totals[1];
     return KTA_OK;
 }
 
@@ -1469,6 +1576,11 @@ extern "C" int kta_reset(kta_handle *h) {
     for (uint64_t &v : h->log.txn.totals) v = 0;
     for (uint64_t &v : h->log.crc.totals) v = 0;   // (the check.crcs switch itself stays as it is)
     h->log.crc.kept.clear();
+    OffsetState &o = h->log.offsets;   // windows and their totals
+    std::fill(o.win.begin(), o.win.end(), -1);
+    o.set = 0;
+    o.dirty = !o.win.empty();
+    for (uint64_t &v : o.totals) v = 0;
     return state_reset_device(h);
 }
 

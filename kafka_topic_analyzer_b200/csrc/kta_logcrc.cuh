@@ -93,16 +93,24 @@ __device__ __forceinline__ bool log_framed(const uint8_t *bytes, int64_t nbytes,
 }
 
 // thread per batch: spans[b + 1] = spans of batch b's CRC region (0 when it is not framed: the header pass refuses the
-// call), acc[b] = 0
-__global__ void log_crc_count_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches, uint64_t *spans,
-                                     uint32_t *acc) {
+// call; with a Window, also 0 when the batch is not served, kta_logoffsets.cuh), acc[b] = 0
+template <typename Window>
+__device__ __forceinline__ void log_crc_count_pass(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches,
+                                                   uint64_t *spans, uint32_t *acc, int32_t partition, const int32_t *batch_partition,
+                                                   const Window &window) {
     for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nbatches; b += (int64_t)gridDim.x * blockDim.x) {
         uint32_t len = 0;
-        const bool framed = log_framed(bytes, nbytes, batch_off[b], &len);
+        bool framed = log_framed(bytes, nbytes, batch_off[b], &len);
+        if constexpr (Window::on)
+            framed = framed && window.test(bytes + batch_off[b], batch_partition ? batch_partition[b] : partition) != LOG_WIN_SKIP;
         spans[b + 1] = framed ? (len - LOG_CRC_FROM + LOG_CRC_SPAN - 1) / LOG_CRC_SPAN : 0;
         acc[b] = 0;
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) spans[0] = 0;
+}
+__global__ void log_crc_count_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches, uint64_t *spans,
+                                     uint32_t *acc) {
+    log_crc_count_pass(bytes, nbytes, batch_off, nbatches, spans, acc, 0, nullptr, NoWindow{});
 }
 
 // table k, entry i, in the lane's replica (tl = table base + lane): word (k * 256 + i) * 32 sits in the lane's own bank

@@ -40,8 +40,10 @@ constexpr int LOG_HEADER_BYTES = 61;
 // turn such a batch into LOGB_OK).  LOGB_SKIP_ABORTED: a batch of an aborted transaction (read_committed only,
 // kta_logtxn.cuh); it replaces any codec flag, so no later pass touches the batch.  LOGB_SKIP_CRC: a batch whose CRC-32C
 // failed (check.crcs only, kta_logcrc.cuh); nothing CRC-covered of it is read, by the header pass or any later one.
+// LOGB_SKIP_OFFSET: a batch a consumer is not served, wholly outside its partition's [log start offset, high watermark)
+// window (kta_logoffsets.cuh); like LOGB_SKIP_CRC it is neither checked nor read further.
 enum LogBatchFlags { LOGB_OK = 0, LOGB_SKIP_CONTROL = 1, LOGB_BAD = 2, LOGB_COMPRESSED = 4, LOGB_LZ4 = 8, LOGB_SNAPPY = 16, LOGB_GZIP = 32,
-                     LOGB_ZSTD = 64, LOGB_SKIP_ABORTED = 128, LOGB_SKIP_CRC = 256 };
+                     LOGB_ZSTD = 64, LOGB_SKIP_ABORTED = 128, LOGB_SKIP_CRC = 256, LOGB_SKIP_OFFSET = 512 };
 constexpr uint32_t LOGB_CODECS = LOGB_LZ4 | LOGB_SNAPPY | LOGB_GZIP | LOGB_ZSTD;   // batches log_decompress_kernel turns into LOGB_OK
 
 // the flag of Kafka's compression codec id 0-4 (attributes & 7: none, gzip, Snappy, LZ4, zstd)
@@ -76,13 +78,24 @@ struct LogBatchInfo {      // one per record batch, filled by log_header_kernel
 // The header pass, thread per batch: validate + read the header.  crc_failed(p, len, b, partition) is asked first for a
 // framed batch (magic 2, batchLength >= 49, inside the buffer); when it says so, the batch is LOGB_SKIP_CRC and none of
 // its CRC-covered fields is read (check.crcs, kta_logcrc.cuh).  log_header_kernel asks NoCrcCheck, which never says so.
+// Before that, a Window with `on` set is asked whether the framed batch is served at all (window.test(p, partition):
+// LOG_WIN_SKIP makes it LOGB_SKIP_OFFSET, counted by window.skipped; LOG_WIN_CUT puts a data batch with records on the
+// window's cut list, kta_logoffsets.cuh).  NoWindow is off: the pass compiles to what it was without the question.
 struct NoCrcCheck {
     __device__ __forceinline__ bool operator()(const uint8_t *, uint32_t, int64_t, int32_t) const { return false; }
 };
-template <typename CrcCheck>
+enum LogWinVerdict { LOG_WIN_SERVED = 0, LOG_WIN_CUT = 1, LOG_WIN_SKIP = 2 };
+struct NoWindow {
+    static constexpr bool on = false;
+    __device__ __forceinline__ int test(const uint8_t *, int32_t) const { return LOG_WIN_SERVED; }
+    __device__ __forceinline__ void skipped(uint32_t, int32_t) const {}
+    __device__ __forceinline__ void cut(int64_t) const {}
+};
+template <typename CrcCheck, typename Window = NoWindow>
 __device__ __forceinline__ void log_header_pass(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches,
                                                 int32_t partition, const int32_t *batch_partition, LogBatchInfo *info,
-                                                uint64_t *rec_count, uint32_t *error_flags, const CrcCheck &crc_failed) {
+                                                uint64_t *rec_count, uint32_t *error_flags, const CrcCheck &crc_failed,
+                                                const Window &window = Window{}) {
     for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nbatches; b += (int64_t)gridDim.x * blockDim.x) {
         LogBatchInfo bi{};
         bi.off = batch_off[b];
@@ -98,7 +111,14 @@ __device__ __forceinline__ void log_header_pass(const uint8_t *bytes, int64_t nb
             // smallest record is 7 bytes (length, attributes, two deltas, key length, value length, header count)
             const uint32_t codec = attrs & 0x7u;
             const bool framed = magic == 2 && batch_len >= LOG_HEADER_BYTES - 12 && bi.off + 12 + (uint64_t)batch_len <= (uint64_t)nbytes;
-            if (framed && crc_failed(p, 12u + (uint32_t)batch_len, b, bi.partition)) {
+            int verdict = LOG_WIN_SERVED;
+            if constexpr (Window::on) verdict = framed ? window.test(p, bi.partition) : LOG_WIN_SERVED;
+            if (Window::on && verdict == LOG_WIN_SKIP) {
+                bi.flags = LOGB_SKIP_OFFSET;
+                bi.len = 12u + (uint32_t)batch_len;
+                bi.base_offset = (int64_t)be_u64(p);
+                window.skipped(attrs, count);
+            } else if (framed && crc_failed(p, 12u + (uint32_t)batch_len, b, bi.partition)) {
                 bi.flags = LOGB_SKIP_CRC;
                 bi.len = 12u + (uint32_t)batch_len;
                 bi.base_offset = (int64_t)be_u64(p);
@@ -113,6 +133,7 @@ __device__ __forceinline__ void log_header_pass(const uint8_t *bytes, int64_t nb
                 else if (codec <= 4) {
                     bi.flags = log_codec_flag(codec);
                     bi.records = count;
+                    if (Window::on && verdict == LOG_WIN_CUT && count > 0) window.cut(b);
                 } else bi.flags = LOGB_COMPRESSED;   // unassigned codes
             }
         }
@@ -242,11 +263,15 @@ __global__ void __launch_bounds__(128) log_decompress_kernel(const uint8_t *byte
 constexpr int LOG_DECODE_THREADS = 128;
 constexpr int LOG_WARP_HEADER = 192;   // per warp: mbarrier (8 B) + 33 record starts (132 B), padded
 
-template <bool STAGED>
-__global__ void __launch_bounds__(LOG_DECODE_THREADS) log_decode_kernel(
-    const uint8_t *bytes, uint64_t readable /* bytes that may be read from `bytes` */, const LogBatchInfo *info, int64_t nbatches,
-    const uint64_t *rec_base, int32_t *partition, int64_t *offset, int64_t *ts_ms, int32_t *key_len, int32_t *value_len,
-    uint64_t *key_src, uint32_t stage_bytes /* per warp, multiple of 16 */, uint32_t *error_flags) {
+// WINDOW (log_decode_window_kernel, kta_logoffsets.cuh; launched only for a call with cut batches): a record whose offset
+// lies below its partition's log start offset (window[p].x, -1 = none) is walked but not written.  The kept records of a
+// batch are written densely from rec_base[b]: each one's rank is the popcount of the lanes below it that keep theirs, plus
+// the records the batch kept in the rounds before (rec_base already counts only the kept records, log_cut_count_kernel).
+template <bool STAGED, bool WINDOW>
+__device__ __forceinline__ void log_decode_pass(
+    const uint8_t *bytes, uint64_t readable, const LogBatchInfo *info, int64_t nbatches, const uint64_t *rec_base, int32_t *partition,
+    int64_t *offset, int64_t *ts_ms, int32_t *key_len, int32_t *value_len, uint64_t *key_src, uint32_t stage_bytes,
+    uint32_t *error_flags, const longlong2 *window, int32_t num_partitions) {
     extern __shared__ __align__(128) unsigned char log_smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const unsigned full = 0xffffffffu;
@@ -289,6 +314,13 @@ __global__ void __launch_bounds__(LOG_DECODE_THREADS) log_decode_kernel(
             uint32_t pos = LOG_HEADER_BYTES;          // offset of the next record inside the batch
             const uint64_t r0 = rec_base[b];
             bool ok = true;
+            int64_t lo = -1;      // WINDOW: the partition's log start offset
+            uint64_t room = 0;    // WINDOW: the records rec_base gives the batch
+            uint32_t kept = 0;    // WINDOW: the records it kept in the rounds before
+            if constexpr (WINDOW) {
+                lo = (uint32_t)bi.partition < (uint32_t)num_partitions ? window[bi.partition].x : -1;
+                room = rec_base[b + 1] - r0;
+            }
             for (int32_t i0 = 0; i0 < bi.records && ok; i0 += 32) {
                 const int cnt = min(32, bi.records - i0);
                 if (lane == 0) {
@@ -331,7 +363,20 @@ __global__ void __launch_bounds__(LOG_DECODE_THREADS) log_decode_kernel(
                 __syncwarp();   // every lane has read its start before lane 0 overwrites them
                 ok = __all_sync(full, lane_ok);
                 if (!ok) break;
-                if (lane < cnt) {
+                if constexpr (WINDOW) {
+                    const bool below = lo >= 0 && (int64_t)((uint64_t)bi.base_offset + (uint64_t)off_delta) < lo;
+                    const unsigned mask = __ballot_sync(full, lane < cnt && !below);
+                    const uint32_t rank = kept + (uint32_t)__popc(mask & ((1u << lane) - 1u));
+                    kept += (uint32_t)__popc(mask);
+                    if (lane < cnt && !below && rank < room) {
+                        const uint64_t r = r0 + rank;
+                        partition[r] = bi.partition;
+                        ts_ms[r] = bi.log_append_time ? bi.max_ts : bi.base_ts + ts_delta;
+                        key_len[r] = (int32_t)klen;
+                        value_len[r] = (int32_t)vlen;
+                        if (key_src) key_src[r] = bi.off + key_at;
+                    }
+                } else if (lane < cnt) {
                     const uint64_t r = r0 + (uint64_t)i0 + lane;
                     partition[r] = bi.partition;
                     if (offset) offset[r] = bi.base_offset + off_delta;
@@ -345,6 +390,15 @@ __global__ void __launch_bounds__(LOG_DECODE_THREADS) log_decode_kernel(
             __syncwarp();   // the stage is free for the next batch's copy
         }
     }
+}
+
+template <bool STAGED>
+__global__ void __launch_bounds__(LOG_DECODE_THREADS) log_decode_kernel(
+    const uint8_t *bytes, uint64_t readable /* bytes that may be read from `bytes` */, const LogBatchInfo *info, int64_t nbatches,
+    const uint64_t *rec_base, int32_t *partition, int64_t *offset, int64_t *ts_ms, int32_t *key_len, int32_t *value_len,
+    uint64_t *key_src, uint32_t stage_bytes /* per warp, multiple of 16 */, uint32_t *error_flags) {
+    log_decode_pass<STAGED, false>(bytes, readable, info, nbatches, rec_base, partition, offset, ts_ms, key_len, value_len, key_src,
+                                   stage_bytes, error_flags, nullptr, 0);
 }
 
 // Packs the key bytes in record order (what the scan kernel hashes): one warp per 128-record tile, a lane owns four

@@ -86,7 +86,7 @@ __global__ void txn_classify_kernel(const uint8_t *bytes, const LogBatchInfo *in
     for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nbatches; b += (int64_t)gridDim.x * blockDim.x) {
         const LogBatchInfo bi = info[b];
         if (bi.flags & (LOGB_BAD | LOGB_COMPRESSED)) continue;   // refused by the header pass: the call fails
-        if (bi.flags == LOGB_SKIP_CRC) continue;                 // failed its CRC: not read (check.crcs)
+        if (bi.flags & (LOGB_SKIP_CRC | LOGB_SKIP_OFFSET)) continue;   // failed its CRC (check.crcs) or not served: not read
         const uint8_t *p = bytes + bi.off;
         uint32_t k;
         if (bi.flags == LOGB_SKIP_CONTROL) {

@@ -216,6 +216,21 @@ class KtaEngine:
         check(lib().kta_log_crc_failures(self._h, buf, n.value, C.byref(n)))
         return [(f.partition, f.batch_bytes, f.base_offset, f.stored_crc, f.computed_crc) for f in buf[:n.value]]
 
+    def set_log_offsets(self, partition: int, log_start_offset: Optional[int] = None,
+                        high_watermark: Optional[int] = None) -> None:
+        """The offsets a consumer of `partition` fetches, for every later log call: from its log start offset up to its
+        high watermark (None = no bound on that side).  Batches outside are skipped unread, and records below the log
+        start offset inside a served batch are dropped (include/kta.h).  A later call replaces the window; reset()
+        clears every window."""
+        check(lib().kta_log_set_offsets(self._h, partition, -1 if log_start_offset is None else log_start_offset,
+                                        -1 if high_watermark is None else high_watermark))
+
+    def log_offset_stats(self):
+        """(batches not served, records left out) over the successful log calls since create / reset."""
+        v = [C.c_uint64() for _ in range(2)]
+        check(lib().kta_log_offset_stats(self._h, *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
+
     def sync(self) -> None:
         check(lib().kta_sync(self._h))
         self._keep = []

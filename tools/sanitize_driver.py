@@ -1,17 +1,18 @@
 """Small end-to-end runs of every scan-kernel mode for compute-sanitizer (tools/sanitize.sh): counters, in-stream HLL,
 exact alive keys (table starting far too small, so growth + stamps-only re-runs happen too), ragged keys, a tail tile,
-the host ring path, the log-segment decoder and its read_committed passes.  Each run is checked against the oracle so a 'clean' sanitizer log is the
+the host ring path, the log-segment decoder, its read_committed passes and its offset windows.  Each run is checked against the oracle so a 'clean' sanitizer log is the
 log of a run that also computed the right answer."""
 import itertools, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import kafka_codec as kc
+import offsets_codec as oc
 import kafka_topic_analyzer_b200 as kta
 from kafka_topic_analyzer_b200 import synth
 from parity import assert_parity, oracle_for
 
 NOW = (4102444800, 1)
-which = sys.argv[1:] or ["counters", "hll", "exact", "ragged", "ring", "log", "logz", "logzstd", "logtxn", "logcrc"]
+which = sys.argv[1:] or ["counters", "hll", "exact", "ragged", "ring", "log", "logz", "logzstd", "logtxn", "logcrc", "logoffsets"]
 
 
 def rotate(seg, codecs, first):
@@ -55,6 +56,24 @@ for name in which:
             e.finalize()
             assert e.log_crc_stats()[:2] == (nb, bad), (e.log_crc_stats(), nb, bad)
         print(name, "ok", nb, bad)
+        continue
+    if name == "logoffsets":   # windows: cut compressed and plain batches, batches not served, check.crcs on, two calls
+        segs, want, nb_out = [], 0, 0
+        for p in range(P):
+            s = kc.set_crcs(rotate(synth.encode_segment(synth.make_spec(n, P), p, 0, n // P, batch_records=7 + 60 * p),
+                                   ("gzip", "zstd", None, "lz4"), p))
+            lo, hi = 13 * p + 5, n // P - 40 * p - 3
+            segs.append((p, s, lo, hi))
+            want += len(oc.fetched(s, lo, hi))
+            nb_out += oc.fetch_stats(s, lo, hi)[0]
+        with kta.KtaEngine(P, count_alive_keys=True, device=0, now=NOW, check_crcs=True) as e:
+            for p, _, lo, hi in segs:
+                e.set_log_offsets(p, lo, hi)
+            got = e.push_log_segments([(p, s) for p, s, _, _ in segs[:P // 2]])
+            got += e.push_log_segments([(p, s) for p, s, _, _ in segs[P // 2:]])
+            e.finalize()
+            assert got == want == e.message_metrics.overall_count() and e.log_offset_stats()[0] == nb_out, (got, want)
+        print(name, "ok", got, nb_out)
         continue
     key_mode = 2 if name in ("ragged", "ring") else 0
     spec = synth.make_spec(n, P, key_mode=key_mode, distinct_keys=3000, tombstone_per_10k=2500, ts_missing_per_10k=20,
