@@ -292,10 +292,12 @@ int kta_log_crc_failures(kta_handle *h, kta_log_crc_failure *out, int64_t cap, i
  * starts at the first batch whose last offset is >= S, and a fetch bounded by H stops before the batch that holds H.  A
  * batch that is not served is skipped unread: it is not CRC-checked, decompressed, decoded, or classified as transactional
  * data or as a marker; it delivers no records, takes no sequence numbers and raises no error, so damage inside it does
- * not refuse the call.  Within a served batch a record with baseOffset + offsetDelta < S is dropped, as librdkafka's
- * reader drops messages older than the fetch offset; offsets are read from the decompressed records, so a compressed
- * batch may be cut.  With check.crcs only served batches are checked and counted; a served batch that fails is skipped
- * and listed as before, cut or not.  Under read_committed a marker outside the window is not seen (its transaction is
+ * not refuse the call.  Within a served batch with baseOffset < S (a cut batch) a record with baseOffset + offsetDelta < S
+ * is dropped, as librdkafka's reader drops messages older than the fetch offset; offsets are read from the decompressed
+ * records, so a compressed batch may be cut.  A served batch with baseOffset >= S keeps all its records, so a forged
+ * negative offsetDelta cannot drop one: a batch's records depend only on its bytes and its partition's window.  On every
+ * log a broker writes this equals librdkafka's rule, because stored offset deltas are never negative.  With check.crcs
+ * only served batches are checked and counted; a served batch that fails is skipped and listed as before, cut or not.  Under read_committed a marker outside the window is not seen (its transaction is
  * decided by the registered ranges, or is undecided), and the producers' baseOffset order is checked over served batches
  * only.  The fields that frame a batch still refuse the call as before: it must fit the buffer, batchLength >= 49, magic 2.
  * Windows apply to the log entry points only; kta_push and the batch entry points ignore them.

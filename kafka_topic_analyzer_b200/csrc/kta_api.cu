@@ -1058,9 +1058,9 @@ static int log_decompress(kta_handle *h, int32_t partition, const uint8_t *dev_b
 
 // The records of every batch into the decoded columns, which b then names; with keys, where each record's key bytes lie.
 // One warp per batch; the batch is staged in shared memory when the longest one fits a stage of <= 48 KiB.
-// window: the call has cut batches, whose records below the log start offset are left out (log_decode_window_kernel).
+// ncut: the call's cut batches, whose records below the log start offset are left out (log_launch_decode_call).
 static int log_decode(kta_handle *h, const uint8_t *dev_bytes, int64_t readable, int64_t nbatches, uint64_t nrec,
-                      uint32_t longest, bool keys, bool window, kta_batch &b) {
+                      uint32_t longest, bool keys, int64_t ncut, kta_batch &b) {
     LogScan &L = h->log;
     cudaStream_t s = h->stream;
     if ((int64_t)nrec >= ((int64_t)1 << 31) - 2) return fail(KTA_ERR_INVALID, "%llu records in one call: split the segments", (unsigned long long)nrec);
@@ -1069,13 +1069,9 @@ static int log_decode(kta_handle *h, const uint8_t *dev_bytes, int64_t readable,
         (rc = L.dec_ts.grow(s, (int64_t)nrec)) || (rc = L.dec_ksrc.grow(s, (int64_t)nrec)))
         return rc;
     const LogDecodeShape shape = log_decode_shape(longest, nbatches, h->sm_count, h->smem_optin);
-    if (window)
-        CU(log_launch_decode_window(shape, dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, L.dec_ts, L.dec_klen,
-                                    L.dec_vlen, keys ? L.dec_ksrc.get() : nullptr, L.err,
-                                    reinterpret_cast<const longlong2 *>(L.offsets.d_win.get()), h->cfg.num_partitions, s));
-    else
-        CU(log_launch_decode(shape, dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, L.dec_ts, L.dec_klen, L.dec_vlen,
-                             keys ? L.dec_ksrc.get() : nullptr, L.err, s));
+    CU(log_launch_decode_call(shape, dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, L.dec_ts, L.dec_klen, L.dec_vlen,
+                              keys ? L.dec_ksrc.get() : nullptr, L.err, ncut, reinterpret_cast<const longlong2 *>(L.offsets.d_win.get()),
+                              h->cfg.num_partitions, s));
     h->launches++;
     b = kta_batch{};
     b.n = (int64_t)nrec;
@@ -1151,7 +1147,7 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
         // (cut batches that keep no record are still decoded, so damage in them refuses the call as elsewhere)
         const bool keys = nrec > 0 && keys_travel(h);
         kta_batch b;
-        if ((rc = log_decode(h, dev_bytes, readable, nbatches, nrec, hd.err[1], keys, ncut > 0, b))) return rc;
+        if ((rc = log_decode(h, dev_bytes, readable, nbatches, nrec, hd.err[1], keys, ncut, b))) return rc;
         if ((rc = log_gather_keys(h, partition, dev_bytes, keys, b))) return rc;
         if (nrec > 0 && (rc = scan_device_batch(h, &b))) return rc;
     }

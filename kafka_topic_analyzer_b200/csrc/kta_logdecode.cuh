@@ -263,8 +263,9 @@ __global__ void __launch_bounds__(128) log_decompress_kernel(const uint8_t *byte
 constexpr int LOG_DECODE_THREADS = 128;
 constexpr int LOG_WARP_HEADER = 192;   // per warp: mbarrier (8 B) + 33 record starts (132 B), padded
 
-// WINDOW (log_decode_window_kernel, kta_logoffsets.cuh; launched only for a call with cut batches): a record whose offset
-// lies below its partition's log start offset (window[p].x, -1 = none) is walked but not written.  The kept records of a
+// WINDOW (log_decode_window_kernel, kta_logoffsets.cuh; launched only for a call with cut batches): a record of a cut batch
+// (baseOffset below its partition's log start offset window[p].x, -1 = none) whose own offset lies below that start is
+// walked but not written; every other batch keeps all its records, whatever their offset deltas.  The kept records of a
 // batch are written densely from rec_base[b]: each one's rank is the popcount of the lanes below it that keep theirs, plus
 // the records the batch kept in the rounds before (rec_base already counts only the kept records, log_cut_count_kernel).
 template <bool STAGED, bool WINDOW>
@@ -364,7 +365,8 @@ __device__ __forceinline__ void log_decode_pass(
                 ok = __all_sync(full, lane_ok);
                 if (!ok) break;
                 if constexpr (WINDOW) {
-                    const bool below = lo >= 0 && (int64_t)((uint64_t)bi.base_offset + (uint64_t)off_delta) < lo;
+                    // only a cut batch (baseOffset < S, the header pass's test) drops records, as the count pass counts
+                    const bool below = lo >= 0 && bi.base_offset < lo && (int64_t)((uint64_t)bi.base_offset + (uint64_t)off_delta) < lo;
                     const unsigned mask = __ballot_sync(full, lane < cnt && !below);
                     const uint32_t rank = kept + (uint32_t)__popc(mask & ((1u << lane) - 1u));
                     kept += (uint32_t)__popc(mask);

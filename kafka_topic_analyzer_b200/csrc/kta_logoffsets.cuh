@@ -8,7 +8,10 @@
 //      that is not served is LOGB_SKIP_OFFSET: not CRC-checked, decompressed, decoded or classified, and no error.
 //   2. the records librdkafka keeps: inside a served batch, a record with baseOffset + offsetDelta < S is dropped (the
 //      v2 reader skips messages older than the fetch offset).  Only a served batch with baseOffset < S can hold such
-//      records; the header pass lists these CUT batches.
+//      records in a log a broker writes; the header pass lists these CUT batches, and records are dropped from cut batches
+//      only (the count pass and the window decode both apply this rule).  A served batch with baseOffset >= S keeps every
+//      record even when a forged negative offsetDelta puts one below S: its rows then depend on its own bytes and its
+//      partition's window alone, not on whether another batch of the call is cut.
 //
 // The passes, on a handle with at least one window (a handle without one launches none of this):
 //   header   (log_window_header_kernel / log_window_crc_header_kernel)  the header pass with LogOffsetWindow: one 16-byte
@@ -175,6 +178,21 @@ inline cudaError_t log_launch_decode_window(const LogDecodeShape &d, const uint8
     decode<<<d.grid, LOG_DECODE_THREADS, d.smem, s>>>(bytes, readable, info, nbatches, rec_base, partition, ts_ms, key_len, value_len,
                                                       key_src, d.stage, error_flags, window, num_partitions);
     return cudaGetLastError();
+}
+
+// which decode a call with ncut cut batches runs: the window decode only when some batch is cut; a call whose windows cut
+// nothing keeps every record of its served batches, which is what log_decode_kernel writes
+inline bool log_decode_windowed(int64_t ncut) { return ncut > 0; }
+
+// the record decode of a call with windows (ncut: the header pass's cut batches), in the shape log_decode_shape chose
+inline cudaError_t log_launch_decode_call(const LogDecodeShape &d, const uint8_t *bytes, uint64_t readable, const LogBatchInfo *info,
+                                          int64_t nbatches, const uint64_t *rec_base, int32_t *partition, int64_t *ts_ms,
+                                          int32_t *key_len, int32_t *value_len, uint64_t *key_src, uint32_t *error_flags, int64_t ncut,
+                                          const longlong2 *window, int32_t num_partitions, cudaStream_t s) {
+    if (log_decode_windowed(ncut))
+        return log_launch_decode_window(d, bytes, readable, info, nbatches, rec_base, partition, ts_ms, key_len, value_len, key_src,
+                                        error_flags, window, num_partitions, s);
+    return log_launch_decode(d, bytes, readable, info, nbatches, rec_base, partition, ts_ms, key_len, value_len, key_src, error_flags, s);
 }
 
 }  // namespace kta

@@ -3,14 +3,25 @@
 // when there are compressed batches, the record decode, the key-length tile bases and the key gather — through the same launch
 // functions (csrc/kta_logdecode_launch.cuh), and writes out every decoded column, so that tests/test_logdecode_records.py can
 // compare them record by record with the records a case was built from.
+// With a window table (tests/test_logoffsets_records.py) it launches what scan_log_batches launches for a handle with offset
+// windows (kta_logoffsets.cuh): log_window_header_kernel and the record-count scan, the size and copy passes, the count pass
+// and its correction of the scan when the header pass cut batches, the record decode that log_launch_decode_call picks (the
+// window decode when some batch is cut), the tile bases and the gather.
 // stdin, per case (little-endian): u32 nbytes, the bytes; u32 nbatches, u64 batch offsets; u32 with_partitions, then i32 per
 // batch partitions when it is 1 (else every batch is partition 0); u32 slack: the bytes behind nbytes that may be read (0 as
-// the device entry points pass, 48 as kta_push_log_segments_host passes).  The device buffer is exactly nbytes + slack long.
+// the device entry points pass, 48 as kta_push_log_segments_host passes); u32 nwin, then nwin x (i64 S, i64 H): the window
+// table of partitions [0, nwin) (-1: that side unbounded; nwin 0: no windows, the plain header pass and decode).  The device
+// buffer is exactly nbytes + slack long.
 // stdout: u32 SM count and u32 opt-in shared memory per block of the device; then per case: u32 header flags, u32 longest
-// batch, u32 size-pass flags, u32 decode flags, u64 records, u32 staged, u32 stage, u32 grid, u32 ran (the decode was launched: the header and size passes accepted the call and it has records);
-// when ran: per record i32 partition, i64 ts_ms, i32 key_len, i32 value_len (column by column); when ran and the decode flags
-// are 0: u64 tile base[ntiles + 1], then the key buffer (tile base[ntiles] packed key bytes and the 64 bytes behind them).
-// The decoded columns and the key buffer are filled with 0xA5 first: an entry the decoder does not write shows up.
+// batch, u32 size-pass flags, u32 decode flags, u64 records (with windows: after the count pass), u32 staged, u32 stage,
+// u32 grid, u32 ran (the decode was launched: the header and size passes accepted the call and the header pass found
+// records); with windows then u32 header words [6..9] (cut batches, batches not served, their records as u64), u32 windowed
+// (the window decode ran), u32 flags of every batch after the header pass, u64 drop[nbatches + 1] (the count pass's drops,
+// scanned: [b] = the records dropped before batch b; zeros when it did not run); when ran: per record i32 partition, i64
+// ts_ms, i32 key_len, i32 value_len (column by column); when ran, the decode flags are 0 and there are records: u64 tile
+// base[ntiles + 1], then the key buffer (tile base[ntiles] packed key bytes and the 64 bytes behind them).
+// The decoded columns and the key buffer are filled with 0xA5 first: an entry the decoder does not write shows up (its
+// key_len is then negative, so the gather skips it).
 #include <cuda_runtime.h>
 
 #include <cstdint>
@@ -19,6 +30,7 @@
 #include <vector>
 
 #include "../../kafka_topic_analyzer_b200/csrc/kta_logdecode_launch.cuh"
+#include "../../kafka_topic_analyzer_b200/csrc/kta_logoffsets.cuh"
 
 using namespace kta;
 
@@ -60,6 +72,7 @@ int main() {
     CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, 0));
     // as create_impl does: the staged decoder may take the device's opt-in shared memory
     CK(cudaFuncSetAttribute(log_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    CK(cudaFuncSetAttribute(log_decode_window_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
     const uint32_t device[2] = {(uint32_t)sm_count, (uint32_t)optin};
     put(device, 8);
     cudaStream_t s;
@@ -77,26 +90,41 @@ int main() {
         std::vector<int32_t> parts(with_part ? (size_t)nb : 0);
         get(parts.data(), parts.size() * 4);
         get(&slack, 4);
+        uint32_t nwin = 0;
+        get(&nwin, 4);
+        std::vector<longlong2> win(nwin);
+        get(win.data(), (size_t)nwin * sizeof(longlong2));
         const uint64_t readable = (uint64_t)n + slack;
 
         uint8_t *d_bytes = dev_alloc<uint8_t>(readable, 0, s);
         uint64_t *d_off = dev_alloc<uint64_t>((size_t)nb, 0, s), *d_cnt = dev_alloc<uint64_t>((size_t)nb + 1, 0, s);
         int32_t *d_part = with_part ? dev_alloc<int32_t>((size_t)nb, 0, s) : nullptr;
         LogBatchInfo *d_info = dev_alloc<LogBatchInfo>((size_t)nb, 0, s);
-        uint32_t *d_err = dev_alloc<uint32_t>(2, 0, s);
+        uint32_t *d_err = dev_alloc<uint32_t>(LOG_WIN_WORDS, 0, s);
+        longlong2 *d_win = nwin ? dev_alloc<longlong2>(nwin, 0, s) : nullptr;
+        uint32_t *d_cut = nwin ? dev_alloc<uint32_t>((size_t)nb, 0, s) : nullptr;
+        uint64_t *d_drop = nwin ? dev_alloc<uint64_t>((size_t)nb + 1, 0, s) : nullptr;
         CK(cudaMemcpyAsync(d_bytes, seg.data(), n, cudaMemcpyHostToDevice, s));
         CK(cudaMemcpyAsync(d_off, offs.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s));
         if (d_part) CK(cudaMemcpyAsync(d_part, parts.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, s));
+        if (d_win) CK(cudaMemcpyAsync(d_win, win.data(), (size_t)nwin * sizeof(longlong2), cudaMemcpyHostToDevice, s));
         if (nb) {
-            log_header_kernel<<<log_thread_grid(nb, sm_count), 128, 0, s>>>(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info, d_cnt, d_err);
+            if (nwin)
+                log_window_header_kernel<<<log_thread_grid(nb, sm_count), 128, 0, s>>>(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info,
+                                                                                       d_cnt, d_err, d_win, (int32_t)nwin, d_cut);
+            else
+                log_header_kernel<<<log_thread_grid(nb, sm_count), 128, 0, s>>>(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info, d_cnt, d_err);
             tile_base_scan_kernel<<<1, 1024, 0, s>>>(d_cnt, nb);
             CK(cudaGetLastError());
         }
-        uint32_t hdr[2] = {0, 0}, unc_err = 0, dec_err = 0;
+        uint32_t hdr[LOG_WIN_WORDS] = {}, unc_err = 0, dec_err = 0;
         uint64_t nrec = 0;
-        CK(cudaMemcpyAsync(hdr, d_err, 8, cudaMemcpyDeviceToHost, s));
+        std::vector<LogBatchInfo> info(nwin ? (size_t)nb : 0);
+        CK(cudaMemcpyAsync(hdr, d_err, sizeof hdr, cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(&nrec, d_cnt + nb, 8, cudaMemcpyDeviceToHost, s));
+        if (nwin && nb) CK(cudaMemcpyAsync(info.data(), d_info, (size_t)nb * sizeof(LogBatchInfo), cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
+        const int64_t ncut = nwin ? hdr[6] : 0;
         bool ran = nb > 0 && !(hdr[0] & (LOGB_BAD | LOGB_COMPRESSED)) && nrec > 0;
         uint8_t *d_unc = nullptr, *d_lit = nullptr;
         uint64_t *d_slot = nullptr;
@@ -117,6 +145,11 @@ int main() {
                 CK(log_launch_copy_pass(d_bytes, d_info, nb, d_slot, d_unc, d_lit, d_err, codecs, sm_count, s));
             }
         }
+        if (ran && ncut) {   // as log_cut_count: the records kept, after the count pass's correction of the scan
+            CK(log_launch_cut_count(d_bytes, d_info, nb, d_cut, ncut, d_win, (int32_t)nwin, d_cnt, d_drop, sm_count, s));
+            CK(cudaMemcpyAsync(&nrec, d_cnt + nb, 8, cudaMemcpyDeviceToHost, s));
+            CK(cudaStreamSynchronize(s));
+        }
         const LogDecodeShape shape = log_decode_shape(hdr[1], nb, sm_count, (size_t)optin);
         int32_t *d_dpart = nullptr, *d_klen = nullptr, *d_vlen = nullptr;
         int64_t *d_ts = nullptr;
@@ -132,12 +165,16 @@ int main() {
             d_ksrc = dev_alloc<uint64_t>(nrec, 0xA5, s);
             d_tb = dev_alloc<uint64_t>((size_t)ntiles + 1, 0xA5, s);
             // (d_err[0] is 0 here, or holds what the copy pass found, as in scan_log_batches)
-            CK(log_launch_decode(shape, d_bytes, readable, d_info, nb, d_cnt, d_dpart, d_ts, d_klen, d_vlen, d_ksrc, d_err, s));
-            CK(log_launch_tile_base(d_klen, (int64_t)nrec, d_tb, sm_count, s));
+            // (a call whose cut batches keep no record is still decoded, so damage in them refuses it, as in scan_log_batches)
+            CK(log_launch_decode_call(shape, d_bytes, readable, d_info, nb, d_cnt, d_dpart, d_ts, d_klen, d_vlen, d_ksrc, d_err, ncut,
+                                      d_win, (int32_t)nwin, s));
+            if (nrec) {
+                CK(log_launch_tile_base(d_klen, (int64_t)nrec, d_tb, sm_count, s));
+                CK(cudaMemcpyAsync(&nkey, d_tb + ntiles, 8, cudaMemcpyDeviceToHost, s));
+            }
             CK(cudaMemcpyAsync(&dec_err, d_err, 4, cudaMemcpyDeviceToHost, s));
-            CK(cudaMemcpyAsync(&nkey, d_tb + ntiles, 8, cudaMemcpyDeviceToHost, s));
             CK(cudaStreamSynchronize(s));
-            if (!dec_err) {
+            if (!dec_err && nrec) {
                 d_keys = dev_alloc<uint8_t>(nkey + 64, 0xA5, s);
                 CK(log_launch_gather_keys(d_bytes, d_ksrc, d_klen, (int64_t)nrec, d_tb, d_keys, sm_count, s));
             }
@@ -152,19 +189,26 @@ int main() {
         put(&stage, 4);
         put(&grid, 4);
         put(&ran32, 4);
+        if (nwin) {
+            const uint32_t windowed = ran && log_decode_windowed(ncut) ? 1u : 0u;
+            put(hdr + 6, 16);
+            put(&windowed, 4);
+            for (const LogBatchInfo &bi : info) put(&bi.flags, 4);
+            put_dev(d_drop, (size_t)nb + 1);
+        }
         if (ran) {
             put_dev(d_dpart, nrec);
             put_dev(d_ts, nrec);
             put_dev(d_klen, nrec);
             put_dev(d_vlen, nrec);
-            if (!dec_err) {
+            if (!dec_err && nrec) {
                 put_dev(d_tb, (size_t)ntiles + 1);
                 put_dev(d_keys, nkey + 64);
             }
         }
         for (void *p : {(void *)d_bytes, (void *)d_off, (void *)d_cnt, (void *)d_part, (void *)d_info, (void *)d_err, (void *)d_unc,
                         (void *)d_lit, (void *)d_slot, (void *)d_dpart, (void *)d_ts, (void *)d_klen, (void *)d_vlen, (void *)d_ksrc,
-                        (void *)d_tb, (void *)d_keys})
+                        (void *)d_tb, (void *)d_keys, (void *)d_win, (void *)d_cut, (void *)d_drop})
             if (p) CK(cudaFree(p));
     }
     CK(cudaStreamDestroy(s));

@@ -4,7 +4,8 @@ independent of the decoder's code.
 
 A consumer that starts at a partition's log start offset S and reads up to its high watermark H is served only the
 batches with S <= last < H, last being baseOffset + the lastOffsetDelta stored in the batch (which can lie past the last
-record of a compacted batch), and drops the records whose offset is below S inside them.  A batch that is not served is
+record of a compacted batch), and drops the records whose offset is below S inside the served batches that start below S
+(the cut ones).  A batch that is not served is
 known by its header alone: its records section is never read, as a consumer never receives it."""
 import struct
 
@@ -27,8 +28,8 @@ def _bound(x):
 def fetched(seg, log_start=None, high_watermark=None):
     """the records a consumer delivers when it fetches from log_start up to high_watermark (None or -1: no bound), on top
     of kafka_codec.delivered(): a batch is served only when log_start <= last < high_watermark, last being baseOffset +
-    the lastOffsetDelta stored in the batch's bytes; inside a served batch a record whose offset is below log_start is
-    dropped"""
+    the lastOffsetDelta stored in the batch's bytes; inside a served batch with baseOffset < log_start a record whose
+    offset is below log_start is dropped"""
     return kc.delivered(_served(seg, _bound(log_start), _bound(high_watermark))[0])
 
 
@@ -40,7 +41,9 @@ def fetch_stats(seg, log_start=None, high_watermark=None):
 
 
 def _served(seg, lo, hi):
-    """(the served batches with their records below lo removed, the batches not served, the data records removed)"""
+    """(the served batches with their records below lo removed, the batches not served, the data records removed).  Records
+    are removed only from cut batches, those with baseOffset < lo: a served batch at or past lo keeps every record, even one
+    that a negative offset delta (which no broker writes) puts below lo"""
     served, skipped, dropped = [], [], 0
     for raw in kc.split_batches(bytes(seg)):
         base, = struct.unpack(">q", raw[:8])
@@ -50,7 +53,7 @@ def _served(seg, lo, hi):
             skipped.append(kc.Batch(base, attrs, None, None, struct.unpack(">i", raw[57:61])[0], None, None))
             continue
         b = kc.read_segment(raw)[0]
-        if lo is not None:
+        if lo is not None and base < lo:
             kept = [r for r in b.records if r[0] >= lo]
             if not b.attributes & 0x20:
                 dropped += len(b.records) - len(kept)

@@ -321,6 +321,23 @@ def test_many_partitions_each_cut(in_place):
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("entry", ["segments_host", "batches_device"])
+@pytest.mark.parametrize("with_cut", [False, True], ids=["alone", "beside-a-cut-batch"])
+def test_negative_offset_delta_at_the_log_start(entry, with_cut):
+    """partition 1: S = 10 and a batch at baseOffset 10 with offset deltas [0, -3, 1] (no broker writes a negative delta).
+    It is served and not cut, so it keeps all three records, whether or not partition 0 has a cut batch in the same call
+    (records are dropped only from cut batches, kta_log_set_offsets)"""
+    rng = np.random.default_rng(13)
+    parts = {0: [mk(0, 0, recs_at(range(0, 10), rng))], 1: [mk(1, 10, recs_at([10, 7, 11], rng))]}
+    win = {0: (5 if with_cut else 0, None), 1: (10, None)}
+    with engine(2) as e:
+        set_windows(e, win)
+        n, order = scan_log(e, entry, parts)
+        recs = check(e, order, win, 2, n)
+        assert sum(r[0] == 1 for r in recs) == 3 and n == (8 if with_cut else 13)
+
+
+@pytest.mark.gpu
 def test_compaction_below_the_log_start():
     """-c: a key whose only live write lies below S is not alive; a tombstone inside the window over a live write below
     S leaves its key dead"""

@@ -21,7 +21,10 @@ import native_build
 TS0 = 1_700_000_000_000
 LOGB_BAD = 2
 M64 = (1 << 64) - 1
-Result = namedtuple("Result", "hdr longest unc_err dec_err nrec staged stage grid ran part ts klen vlen tile_base keys")
+FILL32, FILL64 = np.int32(-0x5A5A5A5B), np.int64(-0x5A5A5A5A5A5A5A5B)   # 0xA5 bytes: what the probe fills the columns with
+# words, windowed, flags, drop: the window mode's outputs (cases with a window table, tests/test_logoffsets_records.py)
+Result = namedtuple("Result", "hdr longest unc_err dec_err nrec staged stage grid ran part ts klen vlen tile_base keys "
+                              "words windowed flags drop", defaults=(None,) * 4)
 
 
 @pytest.fixture(scope="module")
@@ -53,7 +56,9 @@ def batch(records, base_ts=TS0, attributes=0, max_ts=None, compression=None, bas
 
 
 class Case:
-    """batches laid out in one buffer: leads[i] filler bytes before batch i; parts: per-batch partitions or None (all 0)"""
+    """batches laid out in one buffer: leads[i] filler bytes before batch i; parts: per-batch partitions or None (all 0);
+    win: the window table [(S, H)] of partitions [0, len(win)), or None (no windows)"""
+    win = None
 
     def __init__(self, name, batches, leads=None, parts=None, slack=0, check_reader=True):
         self.name, self.slack, self.parts = name, slack, parts
@@ -77,7 +82,9 @@ class Case:
         nb = len(self.offs)
         out = struct.pack("<I", len(self.data)) + self.data + struct.pack("<I", nb) + np.array(self.offs, "<u8").tobytes()
         out += struct.pack("<I", 1) + np.array(self.parts, "<i4").tobytes() if self.parts else struct.pack("<I", 0)
-        return out + struct.pack("<I", self.slack)
+        out += struct.pack("<I", self.slack)
+        win = np.zeros((0, 2)) if self.win is None else self.win
+        return out + struct.pack("<I", len(win)) + np.asarray(win, "<i8").reshape(-1).tobytes()
 
 
 Cols = namedtuple("Cols", "part ts klen vlen keys")
@@ -102,21 +109,26 @@ def run_probe(exe, cases):
     out = r.stdout
     sm, optin = struct.unpack_from("<II", out, 0)
     at, res = 8, []
-    for _ in cases:
+    def take(dt, n):
+        nonlocal at
+        a = np.frombuffer(out, dt, n, at)
+        at += a.nbytes
+        return a
+    for c in cases:
         hdr0, longest, unc, dec, nrec, staged, stage, grid, ran = struct.unpack_from("<IIIIQIIII", out, at)
         at += 40
-        part = ts = klen = vlen = tb = keys = None
+        part = ts = klen = vlen = tb = keys = words = windowed = flags = drop = None
+        if c.win is not None and len(c.win):
+            w = take("<u4", 5)
+            words, windowed = (int(w[0]), int(w[1]), int(w[2]) | int(w[3]) << 32), int(w[4])
+            flags, drop = take("<u4", len(c.offs)), take("<u8", len(c.offs) + 1)
         if ran:
-            def take(dt, n):
-                nonlocal at
-                a = np.frombuffer(out, dt, n, at)
-                at += a.nbytes
-                return a
             part, ts, klen, vlen = take("<i4", nrec), take("<i8", nrec), take("<i4", nrec), take("<i4", nrec)
-            if not dec:
+            if not dec and nrec:
                 tb = take("<u8", (nrec + 127) // 128 + 1)
                 keys = take("u1", int(tb[-1]) + 64).tobytes()
-        res.append(Result(hdr0, longest, unc, dec, nrec, staged, stage, grid, ran, part, ts, klen, vlen, tb, keys))
+        res.append(Result(hdr0, longest, unc, dec, nrec, staged, stage, grid, ran, part, ts, klen, vlen, tb, keys, words, windowed,
+                          flags, drop))
     assert at == len(out)
     return (sm, optin), res
 
@@ -148,10 +160,13 @@ def check(case, r, cols=None, counts=None):
         starts = np.concatenate([[0], np.cumsum(counts)])
         b = int(np.searchsorted(starts, i, "right") - 1)
         j = i - int(starts[b])
-        pytest.fail("%s: record %d (batch %d, record %d of it, lane %d, warp %d of %d; %d bad records): got (%d, %d, %d, %d), "
-                    "want (%d, %d, %d, %d)" % (case.name, i, b, j, j % 32, b % (4 * r.grid), 4 * r.grid, int(bad.sum()),
-                                               r.part[i], r.ts[i], r.klen[i], r.vlen[i], cols.part[i], cols.ts[i],
-                                               cols.klen[i], cols.vlen[i]))
+        # rows the decoder never wrote still hold the 0xA5 fill in every column
+        unwritten = np.flatnonzero((r.part == FILL32) & (r.ts == FILL64) & (r.klen == FILL32) & (r.vlen == FILL32))
+        pytest.fail("%s: record %d (batch %d, record %d of it, lane %d, warp %d of %d; %d bad records, %d rows unwritten%s): "
+                    "got (%d, %d, %d, %d), want (%d, %d, %d, %d)"
+                    % (case.name, i, b, j, j % 32, b % (4 * r.grid), 4 * r.grid, int(bad.sum()), len(unwritten),
+                       ", the first row %d" % unwritten[0] if len(unwritten) else "", r.part[i], r.ts[i], r.klen[i], r.vlen[i],
+                       cols.part[i], cols.ts[i], cols.klen[i], cols.vlen[i]))
     want_tb = tile_base(cols.klen)
     assert np.array_equal(r.tile_base, want_tb), (case.name, "tile base", int(np.argmax(r.tile_base != want_tb)))
     n = len(cols.keys)
@@ -379,9 +394,10 @@ def test_every_warp_decodes_many_batches(probe, shape):
 
 
 # ---- damaged record sections --------------------------------------------------------------------------------------------------
-def contract(data, offs, n):
+def contract(data, offs, n, with_offsets=False):
     """A plain restatement of what the header pass and the decoder accept (kta_logdecode.cuh), for uncompressed batches of
-    partition 0: None when the call is refused, else the delivered records [(0, ts, key|None, value_len)].
+    partition 0: None when the call is refused, else the delivered records [(0, ts, key|None, value_len)], with_offsets: each
+    with its offset baseOffset + offsetDelta (64-bit two's complement) behind.
     Framing: magic 2, batchLength >= 49 and inside the buffer, 7 * recordsCount + 49 <= batchLength.  Per record: a length
     varint of <= 10 bytes, >= 0 and inside the batch; the attributes byte; the timestamp, offset and key-length varints
     inside the record; key and value lengths in [-1, 2^31 - 1] with their bytes inside the record.  Headers, the bytes after
@@ -406,7 +422,7 @@ def contract(data, offs, n):
     for off in offs:
         if off + 61 > n:
             return None
-        bl, = struct.unpack_from(">i", data, off + 8)
+        base, bl = struct.unpack_from(">qi", data, off)
         magic, = struct.unpack_from(">b", data, off + 16)
         attrs, = struct.unpack_from(">H", data, off + 21)
         base_ts, max_ts = struct.unpack_from(">qq", data, off + 27)
@@ -430,7 +446,7 @@ def contract(data, offs, n):
                     return None
                 fields.append(unzz(u))
                 q += k
-            ts_delta, _, kl = fields
+            ts_delta, off_delta, kl = fields
             if not (-1 <= kl <= 2 ** 31 - 1) or (kl > 0 and q + kl > rec_end):
                 return None
             key = None if kl < 0 else bytes(data[q:q + kl])
@@ -439,7 +455,8 @@ def contract(data, offs, n):
             vl = unzz(u)
             if not k or not (-1 <= vl <= 2 ** 31 - 1) or (vl > 0 and q + k + vl > rec_end):
                 return None
-            out.append((0, max_ts if attrs & 0x08 else i64(base_ts + ts_delta), key, vl))
+            rec = (0, max_ts if attrs & 0x08 else i64(base_ts + ts_delta), key, vl)
+            out.append(rec + (i64(base + off_delta),) if with_offsets else rec)
     return out
 
 
