@@ -19,8 +19,6 @@
 #include <new>
 #include <vector>
 
-#include <cub/device/device_radix_sort.cuh>
-
 #include "kta_kernels.cuh"
 #include "kta_logcrc.cuh"
 #include "kta_logdecode.cuh"
@@ -878,8 +876,7 @@ static int txn_passes(kta_handle *h, int32_t partition, const uint8_t *dev_bytes
         (rc = t.d_res.grow(s, nbatches)))
         return rc;
     CU(cudaMemsetAsync(t.d_word, 0, 8, s));
-    txn_classify_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, L.info, nbatches, t.d_keys, t.d_kind, t.d_word);
-    CU(cudaGetLastError());
+    CU(log_launch_txn_classify(dev_bytes, L.info, nbatches, t.d_keys, t.d_kind, t.d_word, h->sm_count, s));
     h->launches++;
     uint32_t w[3] = {0, 0, 0};   // keys, TxnErr bits, header flags
     CU(cudaMemcpyAsync(w, t.d_word, 8, cudaMemcpyDeviceToHost, s));
@@ -891,20 +888,14 @@ static int txn_passes(kta_handle *h, int32_t partition, const uint8_t *dev_bytes
                     "truncated, or with a key that is not version 0 | type)", partition);
     const int64_t m = w[0];
     if (m == 0) return KTA_OK;
-    size_t tmp = 0;
-    CU(cub::DeviceRadixSort::SortKeys(nullptr, tmp, t.d_keys.get(), t.d_sorted.get(), m, TxnKeyDecomposer{}, s));
-    if ((rc = t.d_sort_tmp.grow(s, (int64_t)tmp))) return rc;
+    const int64_t nranges = (int64_t)t.ranges.size();
+    size_t tmp = 0;   // first the sort's scratch size, then the passes
+    CU(log_launch_txn_passes(t.d_keys, t.d_sorted, m, t.d_kind, L.info, t.d_res, nullptr, nullptr, tmp, t.d_ranges, nranges, L.cnt,
+                             t.d_word, t.d_stats, h->sm_count, s));
+    if ((rc = t.d_sort_tmp.grow(s, (int64_t)tmp)) || (rc = t.d_tile.grow(s, 2 * log_txn_tiles(m)))) return rc;
     tmp = (size_t)t.d_sort_tmp.cap;
-    CU(cub::DeviceRadixSort::SortKeys(t.d_sort_tmp.get(), tmp, t.d_keys.get(), t.d_sorted.get(), m, TxnKeyDecomposer{}, s));
-    const int64_t tiles = (m + TXN_TILE - 1) / TXN_TILE;
-    if ((rc = t.d_tile.grow(s, 2 * tiles))) return rc;
-    CU(cudaMemsetAsync(t.d_stats, 0, 24, s));
-    txn_resolve_kernel<<<(unsigned)tiles, TXN_TILE, 0, s>>>(t.d_sorted, m, t.d_kind, L.info, t.d_res, t.d_tile, t.d_word);
-    txn_carry_kernel<<<1, 1024, 0, s>>>(t.d_tile, tiles, t.d_tile + tiles);
-    txn_apply_kernel<<<(int)std::min<int64_t>((m + 255) / 256, (int64_t)h->sm_count * 16), 256, 0, s>>>(
-        t.d_sorted, m, t.d_kind, t.d_res, t.d_tile + tiles, t.d_ranges, (int64_t)t.ranges.size(), L.info, L.cnt, t.d_word,
-        t.d_stats);
-    CU(cudaGetLastError());
+    CU(log_launch_txn_passes(t.d_keys, t.d_sorted, m, t.d_kind, L.info, t.d_res, t.d_tile, t.d_sort_tmp.get(), tmp, t.d_ranges, nranges,
+                             L.cnt, t.d_word, t.d_stats, h->sm_count, s));
     h->launches += 4;   // (the sort counted as one)
     *ran = true;
     return KTA_OK;

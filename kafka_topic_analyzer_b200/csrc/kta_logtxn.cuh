@@ -21,10 +21,14 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
+
+#include <cub/device/device_radix_sort.cuh>
 #include <cuda/std/tuple>
 
 #include "kta_codec.cuh"
 #include "kta_logdecode.cuh"
+#include "kta_logdecode_launch.cuh"
 
 namespace kta {
 
@@ -206,6 +210,37 @@ __global__ void txn_apply_kernel(const TxnKey *keys, int64_t m, const uint8_t *k
             if (records) atomicAdd(stats + 1, (unsigned long long)records);
         } else if (s == TXN_UNDECIDED && records) atomicAdd(stats + 2, (unsigned long long)records);
     }
+}
+
+// The launch groups of the passes.  log_headers (kta_api.cu) and tests/native/logtxn_probe.cu both launch through these, so
+// the probe runs what the product runs.  Allocation, the host round trip, error reporting and launch counting stay with the
+// caller.  (They live here and not in kta_logdecode_launch.cuh: a translation unit that includes them compiles the radix
+// sort's kernels, which the other probes have no use for.)
+
+// the classify pass over the batches log_header_kernel has read; word[0..1] zeroed by the caller
+inline cudaError_t log_launch_txn_classify(const uint8_t *bytes, const LogBatchInfo *info, int64_t nbatches, TxnKey *keys, uint8_t *kind,
+                                           uint32_t *word, int sm_count, cudaStream_t s) {
+    txn_classify_kernel<<<log_thread_grid(nbatches, sm_count), 128, 0, s>>>(bytes, info, nbatches, keys, kind, word);
+    return cudaGetLastError();
+}
+
+inline int64_t log_txn_tiles(int64_t m) { return (m + TXN_TILE - 1) / TXN_TILE; }
+
+// sort, resolve, carry and apply over the m > 0 keys the classify pass wrote.  tile: 2 * log_txn_tiles(m) bytes, the tile
+// heads, then the carries.  With sort_tmp == nullptr nothing is launched and tmp_bytes becomes the sort's scratch size, as
+// with CUB; else tmp_bytes is the size of sort_tmp.  stats[0..2] are zeroed here.
+inline cudaError_t log_launch_txn_passes(TxnKey *keys, TxnKey *sorted, int64_t m, const uint8_t *kind, LogBatchInfo *info, uint8_t *res,
+                                         uint8_t *tile, void *sort_tmp, size_t &tmp_bytes, const TxnRange *ranges, int64_t nranges,
+                                         uint64_t *rec_count, uint32_t *word, unsigned long long *stats, int sm_count, cudaStream_t s) {
+    cudaError_t e = cub::DeviceRadixSort::SortKeys(sort_tmp, tmp_bytes, keys, sorted, m, TxnKeyDecomposer{}, s);
+    if (e != cudaSuccess || !sort_tmp) return e;
+    const int64_t tiles = log_txn_tiles(m);
+    if ((e = cudaMemsetAsync(stats, 0, 24, s)) != cudaSuccess) return e;
+    txn_resolve_kernel<<<(unsigned)tiles, TXN_TILE, 0, s>>>(sorted, m, kind, info, res, tile, word);
+    txn_carry_kernel<<<1, 1024, 0, s>>>(tile, tiles, tile + tiles);
+    txn_apply_kernel<<<(int)std::min<int64_t>((m + 255) / 256, (int64_t)sm_count * 16), 256, 0, s>>>(
+        sorted, m, kind, res, tile + tiles, ranges, nranges, info, rec_count, word, stats);
+    return cudaGetLastError();
 }
 
 }  // namespace kta

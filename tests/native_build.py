@@ -4,6 +4,8 @@
                    (sm_90a, the library's nvcc flags without -shared / -fPIC)
   logdecode_probe  tests/native/logdecode_probe.cu: the product's record stage (decode, tile bases, key gather) on the GPU,
                    every decoded column made visible (built like logdecomp_probe)
+  logtxn_probe     tests/native/logtxn_probe.cu: the product's read_committed passes (classify, sort, resolve, carry, apply) on
+                   the GPU, every array they produce made visible (built like logdecomp_probe)
   codec_harness    tests/native/codec_harness.cu: the same codec walks as plain host code, one "lane" (codec_harness.py runs it)
 
 build() makes the plain programs in tests/native/build/ (git-ignored).  __graft_entry__.build() builds them, because the machine
@@ -18,8 +20,8 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(ROOT, "kafka_topic_analyzer_b200", "csrc")
 NATIVE = os.path.join(HERE, "native")
 OUT = os.path.join(NATIVE, "build")
-PROGRAMS = ("logdecomp_probe", "logdecode_probe", "codec_harness")
-GPU_PROGRAMS = ("logdecomp_probe", "logdecode_probe")
+PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe", "codec_harness")
+GPU_PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe")
 SANITIZE = ["-g", "-Xcompiler", "-fsanitize=address,-fno-omit-frame-pointer"]
 
 

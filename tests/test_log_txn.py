@@ -365,7 +365,9 @@ def test_reset_clears_ranges_and_counters():
 def test_many_transactional_batches_in_one_call():
     """16 partitions x 256 producers, 8 transactions each of 4 single-record batches + marker, interleaved across producers
     (every producer has a transaction open at once): 2^17 transactional batches in one call, 1 in 10 transactions aborted;
-    the sort, resolve and carry passes run over hundreds of tiles"""
+    the sort, resolve and carry passes run over hundreds of tiles.  Its chains are at most 4 keys long and it stays inside
+    one carry chunk; long transactions, chains across warps, tiles and carry chunks, and every array of the passes key by key
+    are in tests/test_logtxn_passes.py"""
     P, PR, T = 16, 256, 8
     rng = np.random.default_rng(5)
     keys = [b"key-%d" % i for i in range(5000)]
