@@ -911,8 +911,8 @@ struct LogHeaders {
     std::vector<kta_log_crc_failure> crc_fails;      // check.crcs: this call's failures, in batch order, as many as are kept
 };
 
-// check.crcs: the passes of kta_logcrc.cuh that precede the header pass (span counts, their scan, the spans' CRCs).  No
-// host round trip: the span kernel reads the total from the scan, and its grid is bounded by the call's bytes.
+// check.crcs: the passes of kta_logcrc.cuh that precede the header pass (span counts, their scan, the spans' CRCs), through
+// log_launch_crc_spans.  No host round trip; the span kernel's grid is bounded by the call's bytes.
 static int log_crc_spans(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes, int64_t len,
                          const uint64_t *dev_batch_off, int64_t nbatches, bool window) {
     CrcState &c = h->log.crc;
@@ -927,18 +927,10 @@ static int log_crc_spans(kta_handle *h, int32_t partition, const int32_t *dev_ba
         CU(cudaFuncSetAttribute(log_crc_span_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LOG_CRC_SMEM));
     }
     if ((rc = c.d_spans.grow(s, nbatches + 1)) || (rc = c.d_acc.grow(s, nbatches)) || (rc = c.d_fails.grow(s, nbatches))) return rc;
-    if (window)   // batches that are not served are not checked
-        log_window_crc_count_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(
-            dev_bytes, len, dev_batch_off, nbatches, c.d_spans, c.d_acc, partition, dev_batch_partition,
-            reinterpret_cast<const longlong2 *>(h->log.offsets.d_win.get()), h->cfg.num_partitions);
-    else
-        log_crc_count_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, c.d_spans, c.d_acc);
-    tile_base_scan_kernel<<<1, 1024, 0, s>>>(c.d_spans, nbatches);
-    // at most len / S + nbatches spans, one per thread at least: a small call gets a small grid
-    const int64_t max_spans = len / LOG_CRC_SPAN + nbatches;
-    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((max_spans + LOG_CRC_THREADS - 1) / LOG_CRC_THREADS, h->sm_count));
-    log_crc_span_kernel<<<grid, LOG_CRC_THREADS, LOG_CRC_SMEM, s>>>(dev_bytes, dev_batch_off, nbatches, c.d_spans, c.d_tables, c.d_acc);
-    CU(cudaGetLastError());
+    // batches that are not served are not checked
+    const longlong2 *d_win = window ? reinterpret_cast<const longlong2 *>(h->log.offsets.d_win.get()) : nullptr;
+    CU(log_launch_crc_spans(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, d_win, h->cfg.num_partitions,
+                            c.d_tables, c.d_spans, c.d_acc, log_crc_span_grid(len, nbatches, h->sm_count), h->sm_count, s));
     h->launches += 3;
     return KTA_OK;
 }
@@ -973,22 +965,9 @@ static int log_headers(kta_handle *h, int32_t partition, const int32_t *dev_batc
     const size_t err_bytes = win ? LOG_WIN_WORDS * sizeof(uint32_t) : crc ? 24 : 8;
     if (crc && (rc = log_crc_spans(h, partition, dev_batch_partition, dev_bytes, len, dev_batch_off, nbatches, win))) return rc;
     CU(cudaMemsetAsync(L.err, 0, err_bytes, s));
-    const longlong2 *d_win = reinterpret_cast<const longlong2 *>(L.offsets.d_win.get());
-    const int32_t P = h->cfg.num_partitions;
-    if (crc && win)
-        log_window_crc_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(
-            dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, L.info, L.cnt, L.err, L.crc.d_acc, L.crc.d_fails,
-            d_win, P, L.offsets.d_cut);
-    else if (crc)
-        log_crc_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(
-            dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, L.info, L.cnt, L.err, L.crc.d_acc, L.crc.d_fails);
-    else if (win)
-        log_window_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(
-            dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, L.info, L.cnt, L.err, d_win, P, L.offsets.d_cut);
-    else
-        log_header_kernel<<<log_thread_grid(nbatches, h->sm_count), 128, 0, s>>>(dev_bytes, len, dev_batch_off, nbatches, partition,
-                                                                                dev_batch_partition, L.info, L.cnt, L.err);
-    CU(cudaGetLastError());
+    const longlong2 *d_win = win ? reinterpret_cast<const longlong2 *>(L.offsets.d_win.get()) : nullptr;
+    CU(log_launch_header(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, L.info, L.cnt, L.err,
+                         crc ? L.crc.d_acc.get() : nullptr, L.crc.d_fails, d_win, h->cfg.num_partitions, L.offsets.d_cut, h->sm_count, s));
     bool txn = false;   // read_committed and the call has transactional batches
     if (L.read_committed && (rc = txn_passes(h, partition, dev_bytes, nbatches, &txn))) return rc;
     tile_base_scan_kernel<<<1, 1024, 0, s>>>(L.cnt, nbatches);   // inclusive scan of [1..nbatches] in place

@@ -152,9 +152,11 @@ __device__ __forceinline__ uint32_t crc_span(const uint8_t *a, const uint8_t *e,
 #undef LOG_CRC_T
 
 // Each warp takes one contiguous run of the call's spans (spans[nbatches] in all, so the grid needs no host round trip),
-// 32 at a time, lane j span g0 + j.  The batch of a span is found among the 32 batch ends behind the warp's current batch
-// (every framed batch has a span, so 32 spans lie in at most 32 batches); lanes of one batch xor their shares together
-// before one of them adds the result to acc[b].
+// 32 at a time, lane j span g0 + j.  The batch of a span is looked for among the 32 batch ends behind the warp's current
+// batch b0 (the batch of the previous round's last span, or of `start`): when every batch has a span, the 32 spans of a
+// round lie in batches b0 .. b0 + 32.  Under offset windows a batch that is not served has no span, so a round can reach
+// further; a lane whose span lies past batch b0 + 32 finds its batch by a binary search of the rest of the scan.  Lanes of
+// one batch xor their shares together before one of them adds the result to acc[b].
 __global__ void __launch_bounds__(LOG_CRC_THREADS) log_crc_span_kernel(const uint8_t *bytes, const uint64_t *batch_off, int64_t nbatches,
                                                                        const uint64_t *spans, const LogCrcTables *tables, uint32_t *acc) {
     extern __shared__ uint32_t crc_smem[];
@@ -186,8 +188,21 @@ __global__ void __launch_bounds__(LOG_CRC_THREADS) log_crc_span_kernel(const uin
 #pragma unroll
         for (int step = 16; step >= 1; step >>= 1)
             if (__shfl_sync(0xffffffffu, bound, c + step - 1) <= gc) c += step;
-        if (c == 31 && __shfl_sync(0xffffffffu, bound, 31) <= gc) c = 32;
-        const int64_t b = b0 + c;
+        // (every lane takes part in the shuffle: a full-mask shuffle that only some lanes reach is undefined)
+        const uint64_t bound31 = __shfl_sync(0xffffffffu, bound, 31);
+        if (c == 31 && bound31 <= gc) c = 32;
+        int64_t b = b0 + c;
+        // past the lookahead: batch b0 + 32 ends at or before gc, so batches without spans lie behind b0 and gc's batch is
+        // the last one in [b0 + 33, nbatches - 1] whose first span is <= gc (spans[b0 + 33] <= gc < total, so b0 + 33 <
+        // nbatches); without batches that lack spans this is never taken
+        if (c == 32 && spans[b + 1] <= gc) {
+            int64_t hi_b = nbatches - 1;
+            for (b = b + 1; b < hi_b;) {
+                const int64_t mid = (b + hi_b + 1) >> 1;
+                if (spans[mid] <= gc) b = mid;
+                else hi_b = mid - 1;
+            }
+        }
         uint32_t share = 0;
         if (active) {
             const uint64_t first = spans[b], n = spans[b + 1] - first, i = g - first;

@@ -195,4 +195,50 @@ inline cudaError_t log_launch_decode_call(const LogDecodeShape &d, const uint8_t
     return log_launch_decode(d, bytes, readable, info, nbatches, rec_base, partition, ts_ms, key_len, value_len, key_src, error_flags, s);
 }
 
+// check.crcs: the span pass's grid.  A call has at most nbytes / S + nbatches spans, one per thread at least, so a small
+// call gets a small grid; at most one block per SM (the pass's 128 KiB of tables leave room for one).
+inline int log_crc_span_grid(int64_t nbytes, int64_t nbatches, int sm_count) {
+    const int64_t max_spans = nbytes / LOG_CRC_SPAN + nbatches;
+    return (int)std::max<int64_t>(1, std::min<int64_t>((max_spans + LOG_CRC_THREADS - 1) / LOG_CRC_THREADS, sm_count));
+}
+
+// check.crcs: the passes of kta_logcrc.cuh that precede the header pass: the span counts (with a window table, batches that
+// are not served get none), their scan into spans[0, nbatches], and the span pass on `grid` blocks (log_crc_span_grid; the
+// span pass needs LOG_CRC_SMEM of dynamic shared memory allowed).  No host round trip: the span pass reads the total from
+// the scan.
+inline cudaError_t log_launch_crc_spans(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches, int32_t partition,
+                                        const int32_t *batch_partition, const longlong2 *window, int32_t num_partitions,
+                                        const LogCrcTables *tables, uint64_t *spans, uint32_t *acc, int grid, int sm_count, cudaStream_t s) {
+    if (window)
+        log_window_crc_count_kernel<<<log_thread_grid(nbatches, sm_count), 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, spans, acc, partition,
+                                                                                        batch_partition, window, num_partitions);
+    else
+        log_crc_count_kernel<<<log_thread_grid(nbatches, sm_count), 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, spans, acc);
+    tile_base_scan_kernel<<<1, 1024, 0, s>>>(spans, nbatches);
+    log_crc_span_kernel<<<grid, LOG_CRC_THREADS, LOG_CRC_SMEM, s>>>(bytes, batch_off, nbatches, spans, tables, acc);
+    return cudaGetLastError();
+}
+
+// The header pass of a call: with check.crcs (acc: the span pass's registers, fails: room for the call's batches) and with a
+// window table (cut_list: room for the call's batches), either, both or neither.  error_flags: LOG_WIN_WORDS words with a
+// window table, else 6 with check.crcs, else 2.
+inline cudaError_t log_launch_header(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches, int32_t partition,
+                                     const int32_t *batch_partition, LogBatchInfo *info, uint64_t *rec_count, uint32_t *error_flags,
+                                     const uint32_t *acc, LogCrcFail *fails, const longlong2 *window, int32_t num_partitions,
+                                     uint32_t *cut_list, int sm_count, cudaStream_t s) {
+    const int grid = log_thread_grid(nbatches, sm_count);
+    if (acc && window)
+        log_window_crc_header_kernel<<<grid, 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count,
+                                                          error_flags, acc, fails, window, num_partitions, cut_list);
+    else if (acc)
+        log_crc_header_kernel<<<grid, 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count,
+                                                   error_flags, acc, fails);
+    else if (window)
+        log_window_header_kernel<<<grid, 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count,
+                                                      error_flags, window, num_partitions, cut_list);
+    else
+        log_header_kernel<<<grid, 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count, error_flags);
+    return cudaGetLastError();
+}
+
 }  // namespace kta

@@ -6,6 +6,9 @@
                    every decoded column made visible (built like logdecomp_probe)
   logtxn_probe     tests/native/logtxn_probe.cu: the product's read_committed passes (classify, sort, resolve, carry, apply) on
                    the GPU, every array they produce made visible (built like logdecomp_probe)
+  logcrc_probe     tests/native/logcrc_probe.cu: the product's check.crcs passes (span counts, span pass, header verdict) on
+                   the GPU, every array they produce made visible, and a plain host CRC-32C that needs no GPU (built like
+                   logdecomp_probe)
   codec_harness    tests/native/codec_harness.cu: the same codec walks as plain host code, one "lane" (codec_harness.py runs it)
 
 build() makes the plain programs in tests/native/build/ (git-ignored).  __graft_entry__.build() builds them, because the machine
@@ -20,8 +23,8 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(ROOT, "kafka_topic_analyzer_b200", "csrc")
 NATIVE = os.path.join(HERE, "native")
 OUT = os.path.join(NATIVE, "build")
-PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe", "codec_harness")
-GPU_PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe")
+PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe", "logcrc_probe", "codec_harness")
+GPU_PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe", "logcrc_probe")
 SANITIZE = ["-g", "-Xcompiler", "-fsanitize=address,-fno-omit-frame-pointer"]
 
 

@@ -249,6 +249,27 @@ def test_batches_at_odd_byte_offsets():
         assert [f[4] for f in e.log_crc_failures()] == [kc.batch_crc(b.raw, 0) for b in bad]
 
 
+@pytest.mark.gpu
+def test_failed_bytes_carry_past_2_32():
+    """260 copies of one 16 MiB batch whose stored CRC is wrong, repeated on the device into one call of
+    kta_scan_log_batches_device (4.4 GB on the device, nothing that size on the host): the failed bytes sum past 2^32, so the
+    header pass's u64 carries into its high word.  baseOffset lies outside the CRC, so one reference serves every copy."""
+    import torch
+    from test_logcrc_passes import host_crcs
+    rng = np.random.default_rng(30)
+    b = flip_crc(sized_batch(0, 0, 16 << 20, rng))
+    copies, size = 260, len(b.raw)
+    assert copies * size > 1 << 32
+    computed = int(host_crcs([np.frombuffer(b.raw, np.uint8)[21:]])[0])
+    buf = torch.from_numpy(np.frombuffer(b.raw, np.uint8).copy()).cuda().repeat(copies)
+    offs = torch.arange(copies, dtype=torch.int64, device="cuda") * size
+    parts = torch.zeros(copies, dtype=torch.int32, device="cuda")
+    with engine(1) as e:
+        assert scan_log_batches(e, (buf, buf.numel(), offs, parts, copies)) == 0
+        assert e.log_crc_stats() == (copies, copies, copies * size)
+        assert e.log_crc_failures() == [failure(b, computed)] * copies
+
+
 def _damaged(kind, rng):
     """a call of good batches with one batch damaged by a single bit inside its CRC region, and the refusal that damage
     causes without the check"""

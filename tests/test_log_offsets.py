@@ -420,6 +420,51 @@ def test_check_crcs_counts_served_batches_only(entry):
         assert e.log_crc_stats()[:2] == (4, 2)                          # cut, ok, and partition 1's two
 
 
+def _one_call(e, entry, order):
+    """the batches in the given order in one call: every partition's segment to kta_push_log_segments_host, or every batch
+    (not interleaved) to kta_scan_log_batches_device"""
+    from feed import scan_log_batches, stage_batches
+    if entry == "segments_host":
+        segs = {}
+        for b in order:
+            segs[b.p] = segs.get(b.p, b"") + b.raw
+        return e.push_log_segments(list(segs.items()))
+    return scan_log_batches(e, stage_batches([(b.p, b.raw) for b in order]))
+
+
+def _check_crcs_call(entry, P, order, win):
+    with engine(P, check_crcs=True) as e:
+        set_windows(e, win)
+        n = _one_call(e, entry, order)
+        check(e, order, win, P, n)
+        assert e.log_crc_failures() == []
+        assert e.log_crc_stats() == (len(order) - e.log_offset_stats()[0], 0, 0)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("entry", ["segments_host", "batches_device"])
+def test_check_crcs_across_a_partition_seam(entry):
+    """check.crcs, one call: partition 0's 100 batches, then partition 1's 40 below its log start offset (no CRC spans) and
+    its 100 served ones.  The span pass's warps each take 7 spans; the warp over the seam looks past the 32 batch ends behind
+    its current batch (partition 1's first, empty ones) for the first five served batches of partition 1."""
+    rng = np.random.default_rng(40)
+    order = [mk(0, i, recs_at([i], rng)) for i in range(100)] + [mk(1, i, recs_at([i], rng)) for i in range(140)]
+    _check_crcs_call(entry, 2, order, {1: (40, None)})
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("entry", ["segments_host", "batches_device"])
+def test_check_crcs_on_a_saturated_grid(entry):
+    """check.crcs, one call of ~150 000 one-record batches in 1024 partitions, each partition's first two below its log start
+    offset: the span pass's grid is capped at the SM count (more than 32 spans per warp), and gaps of two batches without
+    spans sit at every partition seam.  The batches are tiled from 64 templates: baseOffset lies outside the CRC."""
+    rng = np.random.default_rng(41)
+    tmpl = [mk(0, 0, recs_at([0], rng)).raw for _ in range(64)]
+    P, per_part = 1024, 150
+    order = [B(p, struct.pack(">q", i) + tmpl[(p * 7 + i) % 64][8:]) for p in range(P) for i in range(per_part)]
+    _check_crcs_call(entry, P, order, {p: (2, None) for p in range(P)})
+
+
 @pytest.mark.gpu
 def test_damage_inside_a_batch_that_is_not_served():
     rng = np.random.default_rng(4)
@@ -568,3 +613,24 @@ def test_cli_watermarks_all_zero_is_no_content(tmp_path):
     _checkpoint(tmp_path / "replication-offset-checkpoint", [("orders", 0, 0), ("orders", 1, 0)])
     r = _run(_cli(), tmp_path)
     assert r.returncode == 254 and "no content" in r.stderr
+
+
+@pytest.mark.gpu
+def test_cli_check_crcs_across_a_partition_seam(tmp_path):
+    """--log-dir with check.crcs=true: partition 0's 100 batches and partition 1's 140, the first 40 below the log start
+    offset its checkpoint gives; every segment goes to the library in one call.  No batch fails its check."""
+    rng = np.random.default_rng(19)
+    parts = {0: [mk(0, i, recs_at([i], rng)) for i in range(100)], 1: [mk(1, i, recs_at([i], rng)) for i in range(140)]}
+    _write_topic(tmp_path, parts)
+    _checkpoint(tmp_path / "log-start-offset-checkpoint", [("orders", 1, 40)])
+    r = _run(_cli(), tmp_path, "--librdkafka", "check.crcs=true")
+    assert r.returncode == 0, r.stderr
+    assert not [l for l in r.stderr.splitlines() if "CRC32C" in l]
+    order = [b for p in sorted(parts) for b in parts[p]]
+    recs, _ = expect(order, {1: (40, None)})
+    assert len(recs) == 200
+    o = oracle_in_order(recs)
+    rows = _rows(r.stdout)
+    for p, c in rows.items():
+        assert [int(c[3]), int(c[4]), int(c[5])] == [o.counter("total", p), o.counter("alive", p), o.counter("tombstones", p)]
+    assert "Alive keys: %d" % o.scalar("sum_all_alive") in r.stdout.splitlines()
