@@ -177,11 +177,11 @@ struct CrcState {
 // The log start offset and high watermark of each partition (kta_log_set_offsets, kta_logoffsets.cuh): the table, the
 // passes' buffers, and what successful calls left out
 struct OffsetState {
-    std::vector<int64_t> win;                        // [2p] log start offset, [2p + 1] high watermark (-1: unbounded);
+    std::vector<longlong2> win;                      // per partition: x log start offset, y high watermark (-1: unbounded);
                                                      // empty until a window is set
     int64_t set = 0;                                 // partitions with a bound: the window passes run only while > 0
     bool dirty = false;                              // win changed since it was last copied to d_win
-    DevBuf<int64_t> d_win;                           // win on the device, one longlong2 per partition
+    DevBuf<longlong2> d_win;                         // win on the device
     DevBuf<uint32_t> d_cut;                          // the call's cut batches (served, with records below the start)
     DevBuf<uint64_t> d_drop;                         // per batch: records the count pass drops, then their scan
     uint64_t totals[2] = {0, 0};                     // batches not served, records left out
@@ -194,8 +194,7 @@ struct LogScan {
     DevBuf<int32_t> part;                    // and each batch's partition
     DevBuf<LogBatchInfo> info;               // per batch, from the header pass
     DevBuf<uint64_t> cnt;                    // records per batch, then their inclusive scan
-    DevBuf<uint32_t> err;                    // [0] error flags, [1] longest batch; check.crcs: [2] failures, [4..5] their bytes;
-                                             // windows: [6] cut batches, [7] batches not served, [8..9] their records
+    DevBuf<LogHeaderWord> err;               // the header pass's error word; its flags, the later passes' flag word
     DevBuf<int32_t> dec_part, dec_klen, dec_vlen;   // the decoded columns
     DevBuf<int64_t> dec_ts;
     DevBuf<uint64_t> dec_ksrc;               // per decoded record: where its key bytes lie in the segment buffer
@@ -667,8 +666,8 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
             for (const ScanFn f : by_capture)
                 if (f) CU(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
     // the record decoder stages a batch of up to 48 KiB per warp (log_decode); attributes belong to the device
-    CU(cudaFuncSetAttribute(log_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
-    CU(cudaFuncSetAttribute(log_decode_window_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+    CU(cudaFuncSetAttribute(log_decode_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+    CU(cudaFuncSetAttribute(log_decode_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
     if ((rc = state_reset_device(h))) return rc;
     CU(cudaStreamSynchronize(h->stream));
     return KTA_OK;
@@ -880,7 +879,7 @@ static int txn_passes(kta_handle *h, int32_t partition, const uint8_t *dev_bytes
     h->launches++;
     uint32_t w[3] = {0, 0, 0};   // keys, TxnErr bits, header flags
     CU(cudaMemcpyAsync(w, t.d_word, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(w + 2, L.err, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(w + 2, &L.err.get()->flags, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     if (w[2] & (LOGB_BAD | LOGB_COMPRESSED)) return KTA_OK;   // the call is refused for its headers (log_headers says so)
     if (w[1] & TXN_ERR_MARKER)
@@ -904,17 +903,21 @@ static int txn_passes(kta_handle *h, int32_t partition, const uint8_t *dev_bytes
 // What the header pass (and read_committed's passes and the CRC check) found in one call's batches
 struct LogHeaders {
     uint64_t nrec = 0;                               // records in all
-    uint32_t err[LOG_WIN_WORDS] = {};                // the header pass's error word: [0] LOGB_* flags, [1] longest batch;
-                                                     // check.crcs: [2] failed batches, [4..5] their bytes (u64); windows:
-                                                     // [6] cut batches, [7] batches not served, [8..9] their records (u64)
+    LogHeaderWord word{};                            // the header pass's error word
     unsigned long long txn_stats[3] = {0, 0, 0};     // this call's aborted batches, aborted records, undecided records
     std::vector<kta_log_crc_failure> crc_fails;      // check.crcs: this call's failures, in batch order, as many as are kept
 };
 
+// windows: the table the window passes read (on the device once log_offsets_upload ran), or null while the handle has none
+static const longlong2 *log_window_table(const kta_handle *h) {
+    return h->log.offsets.set > 0 ? h->log.offsets.d_win.get() : nullptr;
+}
+
 // check.crcs: the passes of kta_logcrc.cuh that precede the header pass (span counts, their scan, the spans' CRCs), through
-// log_launch_crc_spans.  No host round trip; the span kernel's grid is bounded by the call's bytes.
+// log_launch_crc_spans.  No host round trip; the span kernel's grid is bounded by the call's bytes.  Batches that are not
+// served are not checked (the window table goes to the device first, log_offsets_upload).
 static int log_crc_spans(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes, int64_t len,
-                         const uint64_t *dev_batch_off, int64_t nbatches, bool window) {
+                         const uint64_t *dev_batch_off, int64_t nbatches) {
     CrcState &c = h->log.crc;
     cudaStream_t s = h->stream;
     int rc;
@@ -927,9 +930,7 @@ static int log_crc_spans(kta_handle *h, int32_t partition, const int32_t *dev_ba
         CU(cudaFuncSetAttribute(log_crc_span_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LOG_CRC_SMEM));
     }
     if ((rc = c.d_spans.grow(s, nbatches + 1)) || (rc = c.d_acc.grow(s, nbatches)) || (rc = c.d_fails.grow(s, nbatches))) return rc;
-    // batches that are not served are not checked
-    const longlong2 *d_win = window ? reinterpret_cast<const longlong2 *>(h->log.offsets.d_win.get()) : nullptr;
-    CU(log_launch_crc_spans(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, d_win, h->cfg.num_partitions,
+    CU(log_launch_crc_spans(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, log_window_table(h), h->cfg.num_partitions,
                             c.d_tables, c.d_spans, c.d_acc, log_crc_span_grid(len, nbatches, h->sm_count), h->sm_count, s));
     h->launches += 3;
     return KTA_OK;
@@ -942,7 +943,7 @@ static int log_offsets_upload(kta_handle *h) {
     int rc;
     if (!o.d_win && (rc = o.d_win.alloc((int64_t)o.win.size()))) return rc;
     CU(cudaStreamSynchronize(h->stream));   // no queued pass reads the table while it is replaced
-    CU(cudaMemcpyAsync(o.d_win, o.win.data(), o.win.size() * sizeof(int64_t), cudaMemcpyHostToDevice, h->stream));
+    CU(cudaMemcpyAsync(o.d_win, o.win.data(), o.win.size() * sizeof(longlong2), cudaMemcpyHostToDevice, h->stream));
     CU(cudaStreamSynchronize(h->stream));
     o.dirty = false;
     return KTA_OK;
@@ -959,15 +960,14 @@ static int log_headers(kta_handle *h, int32_t partition, const int32_t *dev_batc
     cudaStream_t s = h->stream;
     int rc;
     if ((rc = L.info.grow(s, nbatches + 1)) || (rc = L.cnt.grow(s, nbatches + 1))) return rc;
-    if (!L.err && (rc = L.err.alloc(LOG_WIN_WORDS))) return rc;
-    const bool crc = L.crc.on, win = L.offsets.set > 0;
-    if (win && ((rc = log_offsets_upload(h)) || (rc = L.offsets.d_cut.grow(s, nbatches)))) return rc;
-    const size_t err_bytes = win ? LOG_WIN_WORDS * sizeof(uint32_t) : crc ? 24 : 8;
-    if (crc && (rc = log_crc_spans(h, partition, dev_batch_partition, dev_bytes, len, dev_batch_off, nbatches, win))) return rc;
-    CU(cudaMemsetAsync(L.err, 0, err_bytes, s));
-    const longlong2 *d_win = win ? reinterpret_cast<const longlong2 *>(L.offsets.d_win.get()) : nullptr;
+    if (!L.err && (rc = L.err.alloc(1))) return rc;
+    const bool crc = L.crc.on;
+    if (L.offsets.set > 0 && ((rc = log_offsets_upload(h)) || (rc = L.offsets.d_cut.grow(s, nbatches)))) return rc;
+    if (crc && (rc = log_crc_spans(h, partition, dev_batch_partition, dev_bytes, len, dev_batch_off, nbatches))) return rc;
+    CU(cudaMemsetAsync(L.err, 0, sizeof(LogHeaderWord), s));
     CU(log_launch_header(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, L.info, L.cnt, L.err,
-                         crc ? L.crc.d_acc.get() : nullptr, L.crc.d_fails, d_win, h->cfg.num_partitions, L.offsets.d_cut, h->sm_count, s));
+                         crc ? L.crc.d_acc.get() : nullptr, L.crc.d_fails, log_window_table(h), h->cfg.num_partitions, L.offsets.d_cut,
+                         h->sm_count, s));
     bool txn = false;   // read_committed and the call has transactional batches
     if (L.read_committed && (rc = txn_passes(h, partition, dev_bytes, nbatches, &txn))) return rc;
     tile_base_scan_kernel<<<1, 1024, 0, s>>>(L.cnt, nbatches);   // inclusive scan of [1..nbatches] in place
@@ -975,19 +975,19 @@ static int log_headers(kta_handle *h, int32_t partition, const int32_t *dev_batc
     h->launches += 2;
     uint32_t txn_word[2] = {0, 0};
     CU(cudaMemcpyAsync(&out.nrec, L.cnt + nbatches, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(out.err, L.err, err_bytes, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&out.word, L.err, sizeof(LogHeaderWord), cudaMemcpyDeviceToHost, s));
     if (txn) {
         CU(cudaMemcpyAsync(txn_word, L.txn.d_word, 8, cudaMemcpyDeviceToHost, s));
         CU(cudaMemcpyAsync(out.txn_stats, L.txn.d_stats, 24, cudaMemcpyDeviceToHost, s));
     }
     CU(cudaStreamSynchronize(s));
-    if (out.err[0] & LOGB_COMPRESSED)
+    if (out.word.flags & LOGB_COMPRESSED)
         return fail(KTA_ERR_INVALID, "unknown compression codec (attributes bits 0-2 = 5..7) in partition %d", partition);
-    if (out.err[0] & LOGB_BAD) return fail(KTA_ERR_INVALID, "malformed record batch header in partition %d", partition);
+    if (out.word.flags & LOGB_BAD) return fail(KTA_ERR_INVALID, "malformed record batch header in partition %d", partition);
     if (txn_word[1] & TXN_ERR_ORDER)
         return fail(KTA_ERR_INVALID, "the batches of one producer in partition %d are not in increasing baseOffset order", partition);
     // the failures to keep: the first ones in batch order, as many as the handle's list still has room for
-    const uint32_t nfail = out.err[2];
+    const uint32_t nfail = out.word.crc_failed;
     const size_t room = KTA_LOG_CRC_KEEP - L.crc.kept.size();
     if (nfail && room) {
         std::vector<LogCrcFail> f(nfail);
@@ -1007,30 +1007,31 @@ static int log_decompress(kta_handle *h, int32_t partition, const uint8_t *dev_b
     cudaStream_t s = h->stream;
     int rc;
     if ((rc = L.unc_slot.grow(s, nbatches + 2))) return rc;
-    CU(cudaMemsetAsync(L.err, 0, 4, s));
+    uint32_t *flags = &L.err.get()->flags;
+    CU(cudaMemsetAsync(flags, 0, 4, s));
     const bool zstd = (codecs & LOGB_ZSTD) != 0;
-    CU(log_launch_size_pass(dev_bytes, L.info, nbatches, L.unc_slot, L.err, zstd, h->sm_count, s));
+    CU(log_launch_size_pass(dev_bytes, L.info, nbatches, L.unc_slot, flags, zstd, h->sm_count, s));
     h->launches += zstd ? 3 : 2;
     uint64_t unc_total = 0;
     uint32_t bad = 0;
     CU(cudaMemcpyAsync(&unc_total, L.unc_slot + nbatches, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&bad, L.err, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&bad, flags, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     if (bad) return fail(KTA_ERR_INVALID, "malformed compressed record batch in partition %d", partition);
     if ((rc = L.unc.grow(s, (int64_t)unc_total + 64))) return rc;
     // zstd's literal buffer has the size of the scratch buffer (a block's literals go at its output's offset); it is
     // only allocated once zstd batches are seen
     if (zstd && (rc = L.unc_lit.grow(s, (int64_t)unc_total + 64))) return rc;
-    CU(log_launch_copy_pass(dev_bytes, L.info, nbatches, L.unc_slot, L.unc, L.unc_lit, L.err, codecs, h->sm_count, s));
+    CU(log_launch_copy_pass(dev_bytes, L.info, nbatches, L.unc_slot, L.unc, L.unc_lit, flags, codecs, h->sm_count, s));
     h->launches += ((codecs & ~(uint32_t)LOGB_ZSTD) ? 1 : 0) + (zstd ? 1 : 0);
     return KTA_OK;
 }
 
 // The records of every batch into the decoded columns, which b then names; with keys, where each record's key bytes lie.
 // One warp per batch; the batch is staged in shared memory when the longest one fits a stage of <= 48 KiB.
-// ncut: the call's cut batches, whose records below the log start offset are left out (log_launch_decode_call).
+// window: the window table when the call has cut batches, whose records below the log start offset are left out, else null.
 static int log_decode(kta_handle *h, const uint8_t *dev_bytes, int64_t readable, int64_t nbatches, uint64_t nrec,
-                      uint32_t longest, bool keys, int64_t ncut, kta_batch &b) {
+                      uint32_t longest, bool keys, const longlong2 *window, kta_batch &b) {
     LogScan &L = h->log;
     cudaStream_t s = h->stream;
     if ((int64_t)nrec >= ((int64_t)1 << 31) - 2) return fail(KTA_ERR_INVALID, "%llu records in one call: split the segments", (unsigned long long)nrec);
@@ -1039,9 +1040,8 @@ static int log_decode(kta_handle *h, const uint8_t *dev_bytes, int64_t readable,
         (rc = L.dec_ts.grow(s, (int64_t)nrec)) || (rc = L.dec_ksrc.grow(s, (int64_t)nrec)))
         return rc;
     const LogDecodeShape shape = log_decode_shape(longest, nbatches, h->sm_count, h->smem_optin);
-    CU(log_launch_decode_call(shape, dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, L.dec_ts, L.dec_klen, L.dec_vlen,
-                              keys ? L.dec_ksrc.get() : nullptr, L.err, ncut, reinterpret_cast<const longlong2 *>(L.offsets.d_win.get()),
-                              h->cfg.num_partitions, s));
+    CU(log_launch_decode(shape, dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, L.dec_ts, L.dec_klen, L.dec_vlen,
+                         keys ? L.dec_ksrc.get() : nullptr, &L.err.get()->flags, window, h->cfg.num_partitions, s));
     h->launches++;
     b = kta_batch{};
     b.n = (int64_t)nrec;
@@ -1059,16 +1059,16 @@ static int log_gather_keys(kta_handle *h, int32_t partition, const uint8_t *dev_
     LogScan &L = h->log;
     cudaStream_t s = h->stream;
     int rc;
-    uint32_t err[2] = {0, 0};
+    uint32_t flags = 0;
     uint64_t nkey = 0;
     const int64_t ntiles = (b.n + TILE - 1) / TILE;
     if (keys) {
         if ((rc = derive_tile_base(h, b.key_len, b.n))) return rc;
         CU(cudaMemcpyAsync(&nkey, h->d_tb_scratch + ntiles, 8, cudaMemcpyDeviceToHost, s));
     }
-    CU(cudaMemcpyAsync(err, L.err, 8, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&flags, &L.err.get()->flags, 4, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
-    if (err[0]) return fail(KTA_ERR_INVALID, "malformed record inside a batch of partition %d", partition);
+    if (flags) return fail(KTA_ERR_INVALID, "malformed record inside a batch of partition %d", partition);
     if (!keys) return KTA_OK;
     if ((rc = L.dec_keys.grow(s, (int64_t)nkey + 64))) return rc;
     CU(log_launch_gather_keys(dev_bytes, L.dec_ksrc, L.dec_klen, b.n, h->d_tb_scratch, L.dec_keys, h->sm_count, s));
@@ -1087,8 +1087,8 @@ static int log_cut_count(kta_handle *h, const uint8_t *dev_bytes, int64_t nbatch
     cudaStream_t s = h->stream;
     int rc;
     if ((rc = L.offsets.d_drop.grow(s, nbatches + 1))) return rc;
-    CU(log_launch_cut_count(dev_bytes, L.info, nbatches, L.offsets.d_cut, ncut, reinterpret_cast<const longlong2 *>(L.offsets.d_win.get()),
-                            h->cfg.num_partitions, L.cnt, L.offsets.d_drop, h->sm_count, s));
+    CU(log_launch_cut_count(dev_bytes, L.info, nbatches, L.offsets.d_cut, ncut, log_window_table(h), h->cfg.num_partitions, L.cnt,
+                            L.offsets.d_drop, h->sm_count, s));
     h->launches += 3;
     CU(cudaMemcpyAsync(nrec, L.cnt + nbatches, 8, cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(dropped, L.offsets.d_drop + nbatches, 8, cudaMemcpyDeviceToHost, s));
@@ -1108,30 +1108,31 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     if ((rc = alive_settle_if_any(h))) return rc;   // the decode scratch of an earlier call is about to be reused
     LogHeaders hd;
     if ((rc = log_headers(h, partition, dev_batch_partition, dev_bytes, len, dev_batch_off, nbatches, hd))) return rc;
-    const int64_t ncut = hd.err[6];
+    const int64_t ncut = hd.word.cut;
     uint64_t nrec = hd.nrec, dropped = 0;
     if (hd.nrec > 0) {
-        const uint32_t codecs = hd.err[0] & LOGB_CODECS;
+        const uint32_t codecs = hd.word.flags & LOGB_CODECS;
         if (codecs && (rc = log_decompress(h, partition, dev_bytes, nbatches, codecs))) return rc;
         if (ncut && (rc = log_cut_count(h, dev_bytes, nbatches, ncut, &nrec, &dropped))) return rc;
         // (cut batches that keep no record are still decoded, so damage in them refuses the call as elsewhere)
         const bool keys = nrec > 0 && keys_travel(h);
         kta_batch b;
-        if ((rc = log_decode(h, dev_bytes, readable, nbatches, nrec, hd.err[1], keys, ncut, b))) return rc;
+        if ((rc = log_decode(h, dev_bytes, readable, nbatches, nrec, hd.word.longest, keys, ncut ? log_window_table(h) : nullptr, b)))
+            return rc;
         if ((rc = log_gather_keys(h, partition, dev_bytes, keys, b))) return rc;
         if (nrec > 0 && (rc = scan_device_batch(h, &b))) return rc;
     }
     // the call succeeded: its transaction counters, CRC results and what its windows left out join the handle's totals
     for (int i = 0; i < 3; i++) h->log.txn.totals[i] += hd.txn_stats[i];
-    const uint32_t not_served = hd.err[7];
+    const uint32_t not_served = hd.word.not_served;
     OffsetState &o = h->log.offsets;
     o.totals[0] += not_served;
-    o.totals[1] += ((uint64_t)hd.err[8] | ((uint64_t)hd.err[9] << 32)) + dropped;
+    o.totals[1] += hd.word.not_served_records + dropped;
     CrcState &c = h->log.crc;
     if (c.on) {
         c.totals[0] += (uint64_t)nbatches - not_served;
-        c.totals[1] += hd.err[2];
-        c.totals[2] += (uint64_t)hd.err[4] | ((uint64_t)hd.err[5] << 32);
+        c.totals[1] += hd.word.crc_failed;
+        c.totals[2] += hd.word.crc_failed_bytes;
         c.kept.insert(c.kept.end(), hd.crc_fails.begin(), hd.crc_fails.end());
     }
     if (records_out) *records_out = (int64_t)nrec;
@@ -1153,9 +1154,8 @@ extern "C" int kta_push_log_segments_host(kta_handle *h, int32_t nsegs, const in
                                           const int64_t *lens, int64_t *records_out) {
     if (!h || nsegs < 0 || (nsegs && (!partitions || !bytes || !lens))) return fail(KTA_ERR_INVALID, "bad argument");
     if (records_out) *records_out = 0;
-    // hop from batch header to batch header on the host (12 + batchLength bytes each); a truncated tail is ignored,
-    // as a consumer would ignore a partially fetched batch.  All segments go to ONE staging buffer and are decoded
-    // and scanned together (one decode, one scan, two host round trips in total).
+    // the batches of each segment, found on the host (log_walk_batches: a truncated tail is ignored).  All segments go to
+    // ONE staging buffer and are decoded and scanned together (one decode, one scan, two host round trips in total).
     std::vector<uint64_t> offs;
     std::vector<int32_t> parts;
     std::vector<int64_t> used((size_t)nsegs, 0), base((size_t)nsegs, 0);
@@ -1163,15 +1163,8 @@ extern "C" int kta_push_log_segments_host(kta_handle *h, int32_t nsegs, const in
     for (int32_t sgi = 0; sgi < nsegs; sgi++) {
         if (lens[sgi] < 0 || (lens[sgi] && !bytes[sgi])) return fail(KTA_ERR_INVALID, "bad segment %d", sgi);
         base[(size_t)sgi] = total;
-        int64_t pos = 0;
-        while (pos + LOG_HEADER_BYTES <= lens[sgi]) {
-            const uint8_t *p = bytes[sgi] + pos;
-            const int64_t bl = (int64_t)(int32_t)(((uint32_t)p[8] << 24) | ((uint32_t)p[9] << 16) | ((uint32_t)p[10] << 8) | p[11]);
-            if (bl < LOG_HEADER_BYTES - 12 || pos + 12 + bl > lens[sgi]) break;
-            offs.push_back((uint64_t)(total + pos));
-            parts.push_back(partitions[sgi]);
-            pos += 12 + bl;
-        }
+        const int64_t pos = log_walk_batches(bytes[sgi], lens[sgi], total, offs);
+        parts.resize(offs.size(), partitions[sgi]);
         used[(size_t)sgi] = pos;
         total += (pos + 15) & ~(int64_t)15;
     }
@@ -1278,12 +1271,11 @@ extern "C" int kta_log_set_offsets(kta_handle *h, int32_t partition, int64_t log
         return fail(KTA_ERR_INVALID, "log start offset %lld above the high watermark %lld", (long long)log_start_offset,
                     (long long)high_watermark);
     OffsetState &o = h->log.offsets;
-    if (o.win.empty()) o.win.assign(2 * (size_t)h->cfg.num_partitions, -1);
-    int64_t *w = o.win.data() + 2 * (size_t)partition;
-    o.set -= (w[0] != -1 || w[1] != -1);
-    w[0] = log_start_offset;
-    w[1] = high_watermark;
-    o.set += (w[0] != -1 || w[1] != -1);
+    if (o.win.empty()) o.win.assign((size_t)h->cfg.num_partitions, make_longlong2(-1, -1));
+    longlong2 &w = o.win[(size_t)partition];
+    o.set -= (w.x != -1 || w.y != -1);
+    w = make_longlong2(log_start_offset, high_watermark);
+    o.set += (w.x != -1 || w.y != -1);
     o.dirty = true;
     return KTA_OK;
 }
@@ -1543,7 +1535,7 @@ extern "C" int kta_reset(kta_handle *h) {
     for (uint64_t &v : h->log.crc.totals) v = 0;   // (the check.crcs switch itself stays as it is)
     h->log.crc.kept.clear();
     OffsetState &o = h->log.offsets;   // windows and their totals
-    std::fill(o.win.begin(), o.win.end(), -1);
+    std::fill(o.win.begin(), o.win.end(), make_longlong2(-1, -1));
     o.set = 0;
     o.dirty = !o.win.empty();
     for (uint64_t &v : o.totals) v = 0;

@@ -7,12 +7,14 @@
 // value is the big-endian u32 at bytes 17-20.  baseOffset, batchLength, partitionLeaderEpoch and magic lie outside it: they
 // frame the batch, and the header pass keeps refusing a call for them.
 //
-// The passes, run before log_header_kernel's checks of any CRC-covered field (only while the switch is on):
-//   count   (thread per batch)  framed batches: the number of LOG_CRC_SPAN-byte spans of the CRC region; acc[b] = 0
+// The passes, run before the header pass checks any CRC-covered field (only while the switch is on; the kernels and their
+// launches are in kta_logoffsets.cuh, next to the window switch's):
+//   count   (log_crc_count_kernel, thread per batch)  framed batches: the number of LOG_CRC_SPAN-byte spans of the CRC
+//                                     region; acc[b] = 0
 //   scan    (tile_base_scan_kernel)  span counts → the first span of every batch
 //   spans   (warp per run of spans)  each lane one span: its CRC from shared-memory tables, moved to the end of its batch
 //                                     by a multiplication mod P, xor-combined per batch into acc[b]
-//   header  (log_crc_header_kernel)  the header pass, which compares acc[b] ^ 0xFFFFFFFF with the stored CRC first: a
+//   header  (log_header_kernel<true, W>)  the header pass, which compares acc[b] ^ 0xFFFFFFFF with the stored CRC first: a
 //                                     batch that fails is LOGB_SKIP_CRC with records = 0, raises no error bit, and is listed
 // Spans are aligned to the region's END, so every span but a batch's first is exactly LOG_CRC_SPAN bytes long and span i of
 // n is moved by x^(8 * LOG_CRC_SPAN * (n - 1 - i)): the register is linear, R(init, A | B) = R(init, A) * x^(8|B|) ^
@@ -107,10 +109,6 @@ __device__ __forceinline__ void log_crc_count_pass(const uint8_t *bytes, int64_t
         acc[b] = 0;
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) spans[0] = 0;
-}
-__global__ void log_crc_count_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches, uint64_t *spans,
-                                     uint32_t *acc) {
-    log_crc_count_pass(bytes, nbytes, batch_off, nbatches, spans, acc, 0, nullptr, NoWindow{});
 }
 
 // table k, entry i, in the lane's replica (tl = table base + lane): word (k * 256 + i) * 32 sits in the lane's own bank
@@ -236,29 +234,20 @@ __global__ void __launch_bounds__(LOG_CRC_THREADS) log_crc_span_kernel(const uin
 }
 
 // The header pass's question for a framed batch: does the CRC that the span pass computed differ from the stored one?  A
-// failure is listed in fails[] (capacity: the call's batches) and counted in error_flags[2] (failures) and, as one u64,
-// error_flags[4..5] (their bytes).
+// failure is listed in fails[] (capacity: the call's batches) and counted in the header word's crc_failed and
+// crc_failed_bytes.
 struct CrcAccCheck {
     const uint32_t *acc;
     LogCrcFail *fails;
-    uint32_t *error_flags;
+    LogHeaderWord *word;
     __device__ __forceinline__ bool operator()(const uint8_t *p, uint32_t len, int64_t b, int32_t partition) const {
         const uint32_t stored = be_u32(p + 17), computed = acc[b] ^ 0xffffffffu;
         if (stored == computed) return false;
-        const uint32_t slot = atomicAdd(error_flags + 2, 1u);
+        const uint32_t slot = atomicAdd(&word->crc_failed, 1u);
         fails[slot] = LogCrcFail{(uint32_t)b, len, (int64_t)be_u64(p), partition, stored, computed, 0u};
-        atomicAdd(reinterpret_cast<unsigned long long *>(error_flags + 4), (unsigned long long)len);
+        atomicAdd(&word->crc_failed_bytes, (unsigned long long)len);
         return true;
     }
 };
-
-// log_header_kernel with the check: the same pass, but a batch whose CRC failed is skipped before its CRC-covered fields
-// are checked (error_flags: 6 words)
-__global__ void log_crc_header_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches, int32_t partition,
-                                      const int32_t *batch_partition, LogBatchInfo *info, uint64_t *rec_count, uint32_t *error_flags,
-                                      const uint32_t *acc, LogCrcFail *fails) {
-    log_header_pass(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count, error_flags,
-                    CrcAccCheck{acc, fails, error_flags});
-}
 
 }  // namespace kta

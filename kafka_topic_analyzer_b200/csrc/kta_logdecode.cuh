@@ -25,6 +25,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cstddef>
 #include <type_traits>
 
 #include "kta_codec.cuh"
@@ -75,12 +76,30 @@ struct LogBatchInfo {      // one per record batch, filled by log_header_kernel
     uint32_t pad;
 };
 
+// The header pass's error word: zeroed before the pass and read back whole.  The decompression and decode passes that
+// follow use `flags` as their own flag word.
+struct LogHeaderWord {
+    uint32_t flags;                            // LOGB_* bits of batches that refuse the call or are to be decompressed
+    uint32_t longest;                          // the longest LOGB_OK batch (sizes the decode stage)
+    uint32_t crc_failed;                       // check.crcs: batches whose CRC failed
+    uint32_t pad;
+    unsigned long long crc_failed_bytes;       // check.crcs: their bytes
+    uint32_t cut;                              // windows: cut batches (on the cut list)
+    uint32_t not_served;                       // windows: batches not served
+    unsigned long long not_served_records;     // windows: their data records
+};
+static_assert(sizeof(LogHeaderWord) == 40 && offsetof(LogHeaderWord, longest) == 4 && offsetof(LogHeaderWord, crc_failed) == 8 &&
+                  offsetof(LogHeaderWord, crc_failed_bytes) == 16 && offsetof(LogHeaderWord, cut) == 24 &&
+                  offsetof(LogHeaderWord, not_served) == 28 && offsetof(LogHeaderWord, not_served_records) == 32,
+              "the probes write the header word out as ten u32 words");
+
 // The header pass, thread per batch: validate + read the header.  crc_failed(p, len, b, partition) is asked first for a
 // framed batch (magic 2, batchLength >= 49, inside the buffer); when it says so, the batch is LOGB_SKIP_CRC and none of
-// its CRC-covered fields is read (check.crcs, kta_logcrc.cuh).  log_header_kernel asks NoCrcCheck, which never says so.
+// its CRC-covered fields is read (check.crcs, kta_logcrc.cuh).  Without the check it is NoCrcCheck, which never says so.
 // Before that, a Window with `on` set is asked whether the framed batch is served at all (window.test(p, partition):
 // LOG_WIN_SKIP makes it LOGB_SKIP_OFFSET, counted by window.skipped; LOG_WIN_CUT puts a data batch with records on the
 // window's cut list, kta_logoffsets.cuh).  NoWindow is off: the pass compiles to what it was without the question.
+// log_header_kernel (kta_logoffsets.cuh) runs the pass with either switch.
 struct NoCrcCheck {
     __device__ __forceinline__ bool operator()(const uint8_t *, uint32_t, int64_t, int32_t) const { return false; }
 };
@@ -91,11 +110,11 @@ struct NoWindow {
     __device__ __forceinline__ void skipped(uint32_t, int32_t) const {}
     __device__ __forceinline__ void cut(int64_t) const {}
 };
-template <typename CrcCheck, typename Window = NoWindow>
+template <typename CrcCheck, typename Window>
 __device__ __forceinline__ void log_header_pass(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches,
                                                 int32_t partition, const int32_t *batch_partition, LogBatchInfo *info,
-                                                uint64_t *rec_count, uint32_t *error_flags, const CrcCheck &crc_failed,
-                                                const Window &window = Window{}) {
+                                                uint64_t *rec_count, LogHeaderWord *word, const CrcCheck &crc_failed,
+                                                const Window &window) {
     for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < nbatches; b += (int64_t)gridDim.x * blockDim.x) {
         LogBatchInfo bi{};
         bi.off = batch_off[b];
@@ -137,18 +156,12 @@ __device__ __forceinline__ void log_header_pass(const uint8_t *bytes, int64_t nb
                 } else bi.flags = LOGB_COMPRESSED;   // unassigned codes
             }
         }
-        if (bi.flags & (LOGB_BAD | LOGB_COMPRESSED | LOGB_CODECS)) atomicOr(error_flags, bi.flags);
-        else if (bi.flags == LOGB_OK) atomicMax(error_flags + 1, bi.len);   // [1]: the longest batch (sizes the decode stage)
+        if (bi.flags & (LOGB_BAD | LOGB_COMPRESSED | LOGB_CODECS)) atomicOr(&word->flags, bi.flags);
+        else if (bi.flags == LOGB_OK) atomicMax(&word->longest, bi.len);
         info[b] = bi;
         rec_count[b + 1] = (uint64_t)bi.records;
     }
     if (blockIdx.x == 0 && threadIdx.x == 0) rec_count[0] = 0;
-}
-
-__global__ void log_header_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches,
-                                  int32_t partition, const int32_t *batch_partition /* per batch, or NULL = `partition` */,
-                                  LogBatchInfo *info, uint64_t *rec_count /*[nbatches+1], [b+1]*/, uint32_t *error_flags) {
-    log_header_pass(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count, error_flags, NoCrcCheck{});
 }
 
 // The records section in[0, n) of a gzip, LZ4 or Snappy batch (flags: its LOGB_GZIP / LOGB_LZ4 / LOGB_SNAPPY): its uncompressed
@@ -263,16 +276,17 @@ __global__ void __launch_bounds__(128) log_decompress_kernel(const uint8_t *byte
 constexpr int LOG_DECODE_THREADS = 128;
 constexpr int LOG_WARP_HEADER = 192;   // per warp: mbarrier (8 B) + 33 record starts (132 B), padded
 
-// WINDOW (log_decode_window_kernel, kta_logoffsets.cuh; launched only for a call with cut batches): a record of a cut batch
-// (baseOffset below its partition's log start offset window[p].x, -1 = none) whose own offset lies below that start is
-// walked but not written; every other batch keeps all its records, whatever their offset deltas.  The kept records of a
-// batch are written densely from rec_base[b]: each one's rank is the popcount of the lanes below it that keep theirs, plus
-// the records the batch kept in the rounds before (rec_base already counts only the kept records, log_cut_count_kernel).
+// WINDOW (launched only for a call with cut batches, kta_logoffsets.cuh): a record of a cut batch (baseOffset below its
+// partition's log start offset window[p].x, -1 = none) whose own offset lies below that start is walked but not written;
+// every other batch keeps all its records, whatever their offset deltas.  The kept records of a batch are written densely
+// from rec_base[b]: each one's rank is the popcount of the lanes below it that keep theirs, plus the records the batch kept
+// in the rounds before (rec_base already counts only the kept records, log_cut_count_kernel).  Without WINDOW, window and
+// num_partitions are not read.
 template <bool STAGED, bool WINDOW>
-__device__ __forceinline__ void log_decode_pass(
-    const uint8_t *bytes, uint64_t readable, const LogBatchInfo *info, int64_t nbatches, const uint64_t *rec_base, int32_t *partition,
-    int64_t *offset, int64_t *ts_ms, int32_t *key_len, int32_t *value_len, uint64_t *key_src, uint32_t stage_bytes,
-    uint32_t *error_flags, const longlong2 *window, int32_t num_partitions) {
+__global__ void __launch_bounds__(LOG_DECODE_THREADS) log_decode_kernel(
+    const uint8_t *bytes, uint64_t readable /* bytes that may be read from `bytes` */, const LogBatchInfo *info, int64_t nbatches,
+    const uint64_t *rec_base, int32_t *partition, int64_t *ts_ms, int32_t *key_len, int32_t *value_len, uint64_t *key_src,
+    uint32_t stage_bytes /* per warp, multiple of 16 */, uint32_t *error_flags, const longlong2 *window, int32_t num_partitions) {
     extern __shared__ __align__(128) unsigned char log_smem[];
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const unsigned full = 0xffffffffu;
@@ -381,7 +395,6 @@ __device__ __forceinline__ void log_decode_pass(
                 } else if (lane < cnt) {
                     const uint64_t r = r0 + (uint64_t)i0 + lane;
                     partition[r] = bi.partition;
-                    if (offset) offset[r] = bi.base_offset + off_delta;
                     ts_ms[r] = bi.log_append_time ? bi.max_ts : bi.base_ts + ts_delta;
                     key_len[r] = (int32_t)klen;
                     value_len[r] = (int32_t)vlen;
@@ -392,15 +405,6 @@ __device__ __forceinline__ void log_decode_pass(
             __syncwarp();   // the stage is free for the next batch's copy
         }
     }
-}
-
-template <bool STAGED>
-__global__ void __launch_bounds__(LOG_DECODE_THREADS) log_decode_kernel(
-    const uint8_t *bytes, uint64_t readable /* bytes that may be read from `bytes` */, const LogBatchInfo *info, int64_t nbatches,
-    const uint64_t *rec_base, int32_t *partition, int64_t *offset, int64_t *ts_ms, int32_t *key_len, int32_t *value_len,
-    uint64_t *key_src, uint32_t stage_bytes /* per warp, multiple of 16 */, uint32_t *error_flags) {
-    log_decode_pass<STAGED, false>(bytes, readable, info, nbatches, rec_base, partition, offset, ts_ms, key_len, value_len, key_src,
-                                   stage_bytes, error_flags, nullptr, 0);
 }
 
 // Packs the key bytes in record order (what the scan kernel hashes): one warp per 128-record tile, a lane owns four

@@ -1,20 +1,37 @@
 // kta_logdecode_launch.cuh — the launch groups of the RecordBatch decoder (kta_logdecode.cuh): the ones that turn compressed
 // record batches into ordinary ones (the size pass, then, once the caller has sized the scratch buffers from its result, the
-// copy pass), the record decode with its shape, the key-length tile bases and the key gather.  scan_log_batches (kta_api.cu)
-// and the probes under tests/native/ (logdecomp_probe.cu, logdecode_probe.cu) all launch through these, so the probes run
-// what the product runs.  Allocation, error reporting and launch counting stay with the caller.
+// copy pass), the record decode with its shape (plain, or with offset windows), the key-length tile bases and the key
+// gather; and the host walk that finds a segment's batches.  The header pass is launched by log_launch_header
+// (kta_logoffsets.cuh).  scan_log_batches (kta_api.cu) and the probes under tests/native/ all launch through these, so the
+// probes run what the product runs.  Allocation, error reporting and launch counting stay with the caller.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <algorithm>
+#include <vector>
 
 #include "kta_kernels.cuh"
 #include "kta_logdecode.cuh"
 
 namespace kta {
 
-// thread per batch (log_header_kernel, log_unc_size_kernel) and warp per batch (the zstd size pass, the copies), 128 threads
+// The record batches of a segment of n bytes, found on the host: hops from batch header to batch header (12 + batchLength
+// bytes each) and appends base + each batch's offset to offs.  A truncated tail is ignored, as a consumer ignores a
+// partially fetched batch.  Returns the bytes the whole batches take.
+inline int64_t log_walk_batches(const uint8_t *seg, int64_t n, int64_t base, std::vector<uint64_t> &offs) {
+    int64_t pos = 0;
+    while (pos + LOG_HEADER_BYTES <= n) {
+        const uint8_t *p = seg + pos;
+        const int64_t bl = (int64_t)(int32_t)(((uint32_t)p[8] << 24) | ((uint32_t)p[9] << 16) | ((uint32_t)p[10] << 8) | p[11]);
+        if (bl < LOG_HEADER_BYTES - 12 || pos + 12 + bl > n) break;
+        offs.push_back((uint64_t)(base + pos));
+        pos += 12 + bl;
+    }
+    return pos;
+}
+
+// thread per batch (the header pass, log_unc_size_kernel) and warp per batch (the zstd size pass, the copies), 128 threads
 inline int log_thread_grid(int64_t nbatches, int sm_count) { return (int)std::min<int64_t>((nbatches + 127) / 128, (int64_t)sm_count * 16); }
 inline int log_warp_grid(int64_t nbatches, int sm_count) { return (int)std::min<int64_t>((nbatches + 3) / 4, (int64_t)sm_count * 16); }
 
@@ -61,13 +78,18 @@ inline LogDecodeShape log_decode_shape(uint32_t longest, int64_t nbatches, int s
     return d;
 }
 
-// the record decode in that shape: the columns of record rec_base[b] + i of batch b; key_src only when keys are gathered
+// the record decode in that shape: the columns of record rec_base[b] + i of batch b; key_src only when keys are gathered.
+// With a window table (given only for a call with cut batches) the window decode runs, which leaves out the records of cut
+// batches below their partition's log start offset; a call whose windows cut nothing keeps every record of its served
+// batches, which is what the plain decode writes.
 inline cudaError_t log_launch_decode(const LogDecodeShape &d, const uint8_t *bytes, uint64_t readable, const LogBatchInfo *info,
                                      int64_t nbatches, const uint64_t *rec_base, int32_t *partition, int64_t *ts_ms, int32_t *key_len,
-                                     int32_t *value_len, uint64_t *key_src, uint32_t *error_flags, cudaStream_t s) {
-    const auto decode = d.staged ? log_decode_kernel<true> : log_decode_kernel<false>;
-    decode<<<d.grid, LOG_DECODE_THREADS, d.smem, s>>>(bytes, readable, info, nbatches, rec_base, partition, nullptr, ts_ms, key_len,
-                                                      value_len, key_src, d.stage, error_flags);
+                                     int32_t *value_len, uint64_t *key_src, uint32_t *error_flags, const longlong2 *window,
+                                     int32_t num_partitions, cudaStream_t s) {
+    const auto decode = window ? (d.staged ? log_decode_kernel<true, true> : log_decode_kernel<false, true>)
+                               : (d.staged ? log_decode_kernel<true, false> : log_decode_kernel<false, false>);
+    decode<<<d.grid, LOG_DECODE_THREADS, d.smem, s>>>(bytes, readable, info, nbatches, rec_base, partition, ts_ms, key_len, value_len,
+                                                      key_src, d.stage, error_flags, window, num_partitions);
     return cudaGetLastError();
 }
 

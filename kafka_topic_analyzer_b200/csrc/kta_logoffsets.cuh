@@ -14,14 +14,16 @@
 //      partition's window alone, not on whether another batch of the call is cut.
 //
 // The passes, on a handle with at least one window (a handle without one launches none of this):
-//   header   (log_window_header_kernel / log_window_crc_header_kernel)  the header pass with LogOffsetWindow: one 16-byte
-//            load of [S, H) per batch; not served → LOGB_SKIP_OFFSET, counted; cut data batches with records → cut list
-//   crc      (log_window_crc_count_kernel)  check.crcs: batches that are not served get no spans
+//   header   (log_header_kernel<C, true>)  the header pass with LogOffsetWindow: one 16-byte load of [S, H) per batch; not
+//            served → LOGB_SKIP_OFFSET, counted in the header word's not_served and not_served_records; cut data batches
+//            with records → cut list, counted in its cut
+//   crc      (log_crc_count_kernel<true>)  check.crcs: batches that are not served get no spans
 //   count    (log_cut_count_kernel, warp per cut batch, after decompression)  walks the batch's records as the decode does
 //            and stores how many it drops at drop[b + 1]; then the drops are scanned (tile_base_scan_kernel) and taken off
 //            the record-count scan (log_cut_fix_kernel), so rec_base counts kept records only
-//   decode   (log_decode_window_kernel, only when the call has cut batches)  writes the kept records densely
-// error_flags, the header pass's word: [6] cut batches, [7] batches not served, [8..9] their data records (u64).
+//   decode   (log_decode_kernel<S, true>, only when the call has cut batches)  writes the kept records densely
+// The header pass and the CRC span count are one kernel each, with check.crcs and the window as template switches; their
+// launches (log_launch_header, log_launch_crc_spans) are at the end of this file.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -31,8 +33,6 @@
 #include "kta_logdecode_launch.cuh"
 
 namespace kta {
-
-constexpr int LOG_WIN_WORDS = 10;   // the header pass's error word with a window (see above)
 
 // [S, H) of a partition inside [0, num_partitions) (-1: that side unbounded); any other partition has no window
 __device__ __forceinline__ longlong2 log_window(const longlong2 *window, int32_t num_partitions, int32_t p) {
@@ -45,7 +45,7 @@ struct LogOffsetWindow {
     const longlong2 *window;
     int32_t num_partitions;
     uint32_t *cut_list;        // the cut batches, in the order the pass met them (capacity: the call's batches)
-    uint32_t *error_flags;
+    LogHeaderWord *word;
     __device__ __forceinline__ int test(const uint8_t *p, int32_t partition) const {
         const longlong2 w = log_window(window, num_partitions, partition);
         const int64_t base = (int64_t)be_u64(p);
@@ -55,33 +55,43 @@ struct LogOffsetWindow {
     }
     // a batch that is not served: its records count as left out when it is a data batch
     __device__ __forceinline__ void skipped(uint32_t attrs, int32_t count) const {
-        atomicAdd(error_flags + 7, 1u);
-        if (!(attrs & 0x20u) && count > 0)
-            atomicAdd(reinterpret_cast<unsigned long long *>(error_flags + 8), (unsigned long long)count);
+        atomicAdd(&word->not_served, 1u);
+        if (!(attrs & 0x20u) && count > 0) atomicAdd(&word->not_served_records, (unsigned long long)count);
     }
-    __device__ __forceinline__ void cut(int64_t b) const { cut_list[atomicAdd(error_flags + 6, 1u)] = (uint32_t)b; }
+    __device__ __forceinline__ void cut(int64_t b) const { cut_list[atomicAdd(&word->cut, 1u)] = (uint32_t)b; }
 };
 
-__global__ void log_window_header_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches,
-                                         int32_t partition, const int32_t *batch_partition, LogBatchInfo *info, uint64_t *rec_count,
-                                         uint32_t *error_flags, const longlong2 *window, int32_t num_partitions, uint32_t *cut_list) {
-    log_header_pass(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count, error_flags, NoCrcCheck{},
-                    LogOffsetWindow{window, num_partitions, cut_list, error_flags});
+// the header pass's questions with a switch on (the CRC check, the window) or off (NoCrcCheck, NoWindow)
+template <bool CRC>
+__device__ __forceinline__ auto log_crc_check(const uint32_t *acc, LogCrcFail *fails, LogHeaderWord *word) {
+    if constexpr (CRC) return CrcAccCheck{acc, fails, word};
+    else return NoCrcCheck{};
+}
+template <bool WIN>
+__device__ __forceinline__ auto log_offset_window(const longlong2 *window, int32_t num_partitions, uint32_t *cut_list, LogHeaderWord *word) {
+    if constexpr (WIN) return LogOffsetWindow{window, num_partitions, cut_list, word};
+    else return NoWindow{};
 }
 
-__global__ void log_window_crc_header_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches,
-                                             int32_t partition, const int32_t *batch_partition, LogBatchInfo *info, uint64_t *rec_count,
-                                             uint32_t *error_flags, const uint32_t *acc, LogCrcFail *fails, const longlong2 *window,
-                                             int32_t num_partitions, uint32_t *cut_list) {
-    log_header_pass(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count, error_flags,
-                    CrcAccCheck{acc, fails, error_flags}, LogOffsetWindow{window, num_partitions, cut_list, error_flags});
+// The header pass, with check.crcs (CRC: acc, the span pass's registers; fails, room for the call's batches) and with a
+// window table (WIN: window of num_partitions; cut_list, room for the call's batches); a switch that is off leaves its
+// parameters unread.
+template <bool CRC, bool WIN>
+__global__ void log_header_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches, int32_t partition,
+                                  const int32_t *batch_partition /* per batch, or NULL = `partition` */, LogBatchInfo *info,
+                                  uint64_t *rec_count /*[nbatches+1], [b+1]*/, LogHeaderWord *word, const uint32_t *acc,
+                                  LogCrcFail *fails, const longlong2 *window, int32_t num_partitions, uint32_t *cut_list) {
+    log_header_pass(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count, word,
+                    log_crc_check<CRC>(acc, fails, word), log_offset_window<WIN>(window, num_partitions, cut_list, word));
 }
 
-__global__ void log_window_crc_count_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches,
-                                            uint64_t *spans, uint32_t *acc, int32_t partition, const int32_t *batch_partition,
-                                            const longlong2 *window, int32_t num_partitions) {
+// check.crcs: the span count (kta_logcrc.cuh), with a window table (WIN) for batches that are not served
+template <bool WIN>
+__global__ void log_crc_count_kernel(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches, uint64_t *spans,
+                                     uint32_t *acc, int32_t partition, const int32_t *batch_partition, const longlong2 *window,
+                                     int32_t num_partitions) {
     log_crc_count_pass(bytes, nbytes, batch_off, nbatches, spans, acc, partition, batch_partition,
-                       LogOffsetWindow{window, num_partitions, nullptr, nullptr});
+                       log_offset_window<WIN>(window, num_partitions, nullptr, nullptr));
 }
 
 // Warp per cut batch (cut[0, ncut)), after the decompression, so a compressed batch is walked in its uncompressed image.
@@ -147,15 +157,6 @@ __global__ void log_cut_fix_kernel(uint64_t *rec_count, const uint64_t *drop, in
         rec_count[b] -= drop[b];
 }
 
-template <bool STAGED>
-__global__ void __launch_bounds__(LOG_DECODE_THREADS) log_decode_window_kernel(
-    const uint8_t *bytes, uint64_t readable, const LogBatchInfo *info, int64_t nbatches, const uint64_t *rec_base, int32_t *partition,
-    int64_t *ts_ms, int32_t *key_len, int32_t *value_len, uint64_t *key_src, uint32_t stage_bytes, uint32_t *error_flags,
-    const longlong2 *window, int32_t num_partitions) {
-    log_decode_pass<STAGED, true>(bytes, readable, info, nbatches, rec_base, partition, nullptr, ts_ms, key_len, value_len, key_src,
-                                  stage_bytes, error_flags, window, num_partitions);
-}
-
 // the count pass and the scan correction of a call with ncut cut batches (drop: nbatches + 1 words, zeroed here).  After
 // it rec_count[nbatches] is the call's record count and drop[nbatches] the records dropped.
 inline cudaError_t log_launch_cut_count(const uint8_t *bytes, const LogBatchInfo *info, int64_t nbatches, const uint32_t *cut, int64_t ncut,
@@ -167,32 +168,6 @@ inline cudaError_t log_launch_cut_count(const uint8_t *bytes, const LogBatchInfo
     tile_base_scan_kernel<<<1, 1024, 0, s>>>(drop, nbatches);
     log_cut_fix_kernel<<<log_thread_grid(nbatches + 1, sm_count), 128, 0, s>>>(rec_count, drop, nbatches);
     return cudaGetLastError();
-}
-
-// the record decode of a call with cut batches, in the shape log_decode_shape chose (staged or in place)
-inline cudaError_t log_launch_decode_window(const LogDecodeShape &d, const uint8_t *bytes, uint64_t readable, const LogBatchInfo *info,
-                                            int64_t nbatches, const uint64_t *rec_base, int32_t *partition, int64_t *ts_ms,
-                                            int32_t *key_len, int32_t *value_len, uint64_t *key_src, uint32_t *error_flags,
-                                            const longlong2 *window, int32_t num_partitions, cudaStream_t s) {
-    const auto decode = d.staged ? log_decode_window_kernel<true> : log_decode_window_kernel<false>;
-    decode<<<d.grid, LOG_DECODE_THREADS, d.smem, s>>>(bytes, readable, info, nbatches, rec_base, partition, ts_ms, key_len, value_len,
-                                                      key_src, d.stage, error_flags, window, num_partitions);
-    return cudaGetLastError();
-}
-
-// which decode a call with ncut cut batches runs: the window decode only when some batch is cut; a call whose windows cut
-// nothing keeps every record of its served batches, which is what log_decode_kernel writes
-inline bool log_decode_windowed(int64_t ncut) { return ncut > 0; }
-
-// the record decode of a call with windows (ncut: the header pass's cut batches), in the shape log_decode_shape chose
-inline cudaError_t log_launch_decode_call(const LogDecodeShape &d, const uint8_t *bytes, uint64_t readable, const LogBatchInfo *info,
-                                          int64_t nbatches, const uint64_t *rec_base, int32_t *partition, int64_t *ts_ms,
-                                          int32_t *key_len, int32_t *value_len, uint64_t *key_src, uint32_t *error_flags, int64_t ncut,
-                                          const longlong2 *window, int32_t num_partitions, cudaStream_t s) {
-    if (log_decode_windowed(ncut))
-        return log_launch_decode_window(d, bytes, readable, info, nbatches, rec_base, partition, ts_ms, key_len, value_len, key_src,
-                                        error_flags, window, num_partitions, s);
-    return log_launch_decode(d, bytes, readable, info, nbatches, rec_base, partition, ts_ms, key_len, value_len, key_src, error_flags, s);
 }
 
 // check.crcs: the span pass's grid.  A call has at most nbytes / S + nbatches spans, one per thread at least, so a small
@@ -209,35 +184,25 @@ inline int log_crc_span_grid(int64_t nbytes, int64_t nbatches, int sm_count) {
 inline cudaError_t log_launch_crc_spans(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches, int32_t partition,
                                         const int32_t *batch_partition, const longlong2 *window, int32_t num_partitions,
                                         const LogCrcTables *tables, uint64_t *spans, uint32_t *acc, int grid, int sm_count, cudaStream_t s) {
-    if (window)
-        log_window_crc_count_kernel<<<log_thread_grid(nbatches, sm_count), 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, spans, acc, partition,
-                                                                                        batch_partition, window, num_partitions);
-    else
-        log_crc_count_kernel<<<log_thread_grid(nbatches, sm_count), 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, spans, acc);
+    const auto count = window ? log_crc_count_kernel<true> : log_crc_count_kernel<false>;
+    count<<<log_thread_grid(nbatches, sm_count), 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, spans, acc, partition, batch_partition,
+                                                              window, num_partitions);
     tile_base_scan_kernel<<<1, 1024, 0, s>>>(spans, nbatches);
     log_crc_span_kernel<<<grid, LOG_CRC_THREADS, LOG_CRC_SMEM, s>>>(bytes, batch_off, nbatches, spans, tables, acc);
     return cudaGetLastError();
 }
 
-// The header pass of a call: with check.crcs (acc: the span pass's registers, fails: room for the call's batches) and with a
-// window table (cut_list: room for the call's batches), either, both or neither.  error_flags: LOG_WIN_WORDS words with a
-// window table, else 6 with check.crcs, else 2.
+// The header pass of a call: with check.crcs when acc is given (the span pass's registers; fails: room for the call's
+// batches) and with windows when the window table is (cut_list: room for the call's batches), either, both or neither.
+// word: zeroed by the caller.
 inline cudaError_t log_launch_header(const uint8_t *bytes, int64_t nbytes, const uint64_t *batch_off, int64_t nbatches, int32_t partition,
-                                     const int32_t *batch_partition, LogBatchInfo *info, uint64_t *rec_count, uint32_t *error_flags,
+                                     const int32_t *batch_partition, LogBatchInfo *info, uint64_t *rec_count, LogHeaderWord *word,
                                      const uint32_t *acc, LogCrcFail *fails, const longlong2 *window, int32_t num_partitions,
                                      uint32_t *cut_list, int sm_count, cudaStream_t s) {
-    const int grid = log_thread_grid(nbatches, sm_count);
-    if (acc && window)
-        log_window_crc_header_kernel<<<grid, 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count,
-                                                          error_flags, acc, fails, window, num_partitions, cut_list);
-    else if (acc)
-        log_crc_header_kernel<<<grid, 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count,
-                                                   error_flags, acc, fails);
-    else if (window)
-        log_window_header_kernel<<<grid, 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count,
-                                                      error_flags, window, num_partitions, cut_list);
-    else
-        log_header_kernel<<<grid, 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info, rec_count, error_flags);
+    const auto header = acc ? (window ? log_header_kernel<true, true> : log_header_kernel<true, false>)
+                            : (window ? log_header_kernel<false, true> : log_header_kernel<false, false>);
+    header<<<log_thread_grid(nbatches, sm_count), 128, 0, s>>>(bytes, nbytes, batch_off, nbatches, partition, batch_partition, info,
+                                                               rec_count, word, acc, fails, window, num_partitions, cut_list);
     return cudaGetLastError();
 }
 

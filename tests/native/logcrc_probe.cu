@@ -9,56 +9,19 @@
 // blocks, 0 for the library's rule (log_crc_span_grid).  The span pass's body does not depend on its grid, so a small grid
 // gives every warp many rounds with few spans.
 // stdout: u32 SM count of the device; then per case: u32 the span pass's grid, u64 spans[nbatches + 1] after the scan, u32
-// acc[nbatches], u32 flags[nbatches] after the header pass, u32 error word [0..9], then error word [2] LogCrcFail records
-// (u32 batch, u32 batch bytes, i64 baseOffset, i32 partition, u32 stored, u32 computed, u32 0), sorted by batch.
+// acc[nbatches], u32 flags[nbatches] after the header pass, the header pass's error word (LogHeaderWord: ten u32 words), then
+// its crc_failed LogCrcFail records (u32 batch, u32 batch bytes, i64 baseOffset, i32 partition, u32 stored, u32 computed,
+// u32 0), sorted by batch.
 // acc is filled with 0xA5 first: an entry the count pass does not write shows up.
 //
 // `logcrc_probe host` is a plain reference instead, which touches no CUDA: stdin, per region, u64 n and n bytes; stdout the
 // u32 CRC-32C of each, one byte at a time with a table of its own.
-#include <cuda_runtime.h>
-
-#include <algorithm>
-#include <cstdint>
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
-#include <vector>
 
 #include "../../kafka_topic_analyzer_b200/csrc/kta_logoffsets.cuh"
+#include "probe.h"
 
 using namespace kta;
-
-#define CK(call)                                                                                           \
-    do {                                                                                                   \
-        cudaError_t e_ = (call);                                                                           \
-        if (e_ != cudaSuccess) {                                                                           \
-            fprintf(stderr, "%s: %s (%s:%d)\n", #call, cudaGetErrorString(e_), __FILE__, __LINE__);        \
-            exit(3);                                                                                       \
-        }                                                                                                  \
-    } while (0)
-
-static void put(const void *p, size_t n) {
-    if (n && fwrite(p, 1, n, stdout) != n) exit(4);
-}
-
-static void get(void *p, size_t n) {
-    if (n && fread(p, 1, n, stdin) != n) exit(2);
-}
-
-template <typename T>
-static T *dev_alloc(size_t count, int fill, cudaStream_t s) {
-    T *p = nullptr;
-    CK(cudaMalloc(&p, std::max<size_t>(count, 1) * sizeof(T)));
-    CK(cudaMemsetAsync(p, fill, std::max<size_t>(count, 1) * sizeof(T), s));
-    return p;
-}
-
-template <typename T>
-static std::vector<T> from_dev(const T *d, size_t count) {
-    std::vector<T> h(count);
-    if (count) CK(cudaMemcpy(h.data(), d, count * sizeof(T), cudaMemcpyDeviceToHost));
-    return h;
-}
 
 // CRC-32C (reflected 0x82F63B78, init and xorout 0xFFFFFFFF), one byte at a time
 static int host_mode() {
@@ -121,7 +84,7 @@ int main(int argc, char **argv) {
         LogCrcFail *d_fails = dev_alloc<LogCrcFail>((size_t)nb, 0, s);
         int32_t *d_part = with_part ? dev_alloc<int32_t>((size_t)nb, 0, s) : nullptr;
         LogBatchInfo *d_info = dev_alloc<LogBatchInfo>((size_t)nb, 0, s);
-        uint32_t *d_err = dev_alloc<uint32_t>(LOG_WIN_WORDS, 0, s);
+        LogHeaderWord *d_word = dev_alloc<LogHeaderWord>(1, 0, s);
         longlong2 *d_win = nwin ? dev_alloc<longlong2>(nwin, 0, s) : nullptr;
         uint32_t *d_cut = nwin ? dev_alloc<uint32_t>((size_t)nb, 0, s) : nullptr;
         CK(cudaMemcpyAsync(d_bytes, seg.data(), n, cudaMemcpyHostToDevice, s));
@@ -132,7 +95,7 @@ int main(int argc, char **argv) {
         if (nb) {
             CK(log_launch_crc_spans(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_win, (int32_t)nwin, d_tables, d_spans, d_acc, grid,
                                     sm_count, s));
-            CK(log_launch_header(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info, d_cnt, d_err, d_acc, d_fails, d_win, (int32_t)nwin,
+            CK(log_launch_header(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info, d_cnt, d_word, d_acc, d_fails, d_win, (int32_t)nwin,
                                  d_cut, sm_count, s));
         }
         CK(cudaStreamSynchronize(s));
@@ -144,13 +107,13 @@ int main(int argc, char **argv) {
         std::vector<uint32_t> flags((size_t)nb);
         for (size_t b = 0; b < (size_t)nb; b++) flags[b] = info[b].flags;
         put(flags.data(), (size_t)nb * 4);
-        const std::vector<uint32_t> err = from_dev(d_err, LOG_WIN_WORDS);
-        put(err.data(), LOG_WIN_WORDS * 4);
-        std::vector<LogCrcFail> fails = from_dev(d_fails, std::min<size_t>(err[2], (size_t)nb));
+        const LogHeaderWord word = from_dev(d_word, 1)[0];
+        put(&word, sizeof word);
+        std::vector<LogCrcFail> fails = from_dev(d_fails, std::min<size_t>(word.crc_failed, (size_t)nb));
         std::sort(fails.begin(), fails.end(), [](const LogCrcFail &a, const LogCrcFail &b) { return a.batch < b.batch; });
         put(fails.data(), fails.size() * sizeof(LogCrcFail));
         for (void *p : {(void *)d_bytes, (void *)d_off, (void *)d_cnt, (void *)d_spans, (void *)d_acc, (void *)d_fails, (void *)d_part,
-                        (void *)d_info, (void *)d_err, (void *)d_win, (void *)d_cut})
+                        (void *)d_info, (void *)d_word, (void *)d_win, (void *)d_cut})
             if (p) CK(cudaFree(p));
     }
     CK(cudaFree(d_tables));

@@ -1,12 +1,13 @@
 // TEST INFRASTRUCTURE: the record stage of the RecordBatch decoder on the GPU, with its output made visible.  It launches what
-// scan_log_batches (csrc/kta_api.cu) launches up to the scan — log_header_kernel, its record-count scan, the size and copy passes
+// scan_log_batches (csrc/kta_api.cu) launches up to the scan — the header pass, its record-count scan, the size and copy passes
 // when there are compressed batches, the record decode, the key-length tile bases and the key gather — through the same launch
-// functions (csrc/kta_logdecode_launch.cuh), and writes out every decoded column, so that tests/test_logdecode_records.py can
-// compare them record by record with the records a case was built from.
+// functions (log_launch_header in csrc/kta_logoffsets.cuh, the others in csrc/kta_logdecode_launch.cuh), and writes out every
+// decoded column, so that tests/test_logdecode_records.py can compare them record by record with the records a case was built
+// from.
 // With a window table (tests/test_logoffsets_records.py) it launches what scan_log_batches launches for a handle with offset
-// windows (kta_logoffsets.cuh): log_window_header_kernel and the record-count scan, the size and copy passes, the count pass
-// and its correction of the scan when the header pass cut batches, the record decode that log_launch_decode_call picks (the
-// window decode when some batch is cut), the tile bases and the gather.
+// windows (kta_logoffsets.cuh): the header pass with the window and the record-count scan, the size and copy passes, the count
+// pass and its correction of the scan when the header pass cut batches, the record decode (given the window table, so the
+// window decode runs, only when some batch is cut), the tile bases and the gather.
 // stdin, per case (little-endian): u32 nbytes, the bytes; u32 nbatches, u64 batch offsets; u32 with_partitions, then i32 per
 // batch partitions when it is 1 (else every batch is partition 0); u32 slack: the bytes behind nbytes that may be read (0 as
 // the device entry points pass, 48 as kta_push_log_segments_host passes); u32 nwin, then nwin x (i64 S, i64 H): the window
@@ -22,57 +23,18 @@
 // base[ntiles + 1], then the key buffer (tile base[ntiles] packed key bytes and the 64 bytes behind them).
 // The decoded columns and the key buffer are filled with 0xA5 first: an entry the decoder does not write shows up (its
 // key_len is then negative, so the gather skips it).
-#include <cuda_runtime.h>
-
-#include <cstdint>
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-
-#include "../../kafka_topic_analyzer_b200/csrc/kta_logdecode_launch.cuh"
 #include "../../kafka_topic_analyzer_b200/csrc/kta_logoffsets.cuh"
+#include "probe.h"
 
 using namespace kta;
-
-#define CK(call)                                                                                           \
-    do {                                                                                                   \
-        cudaError_t e_ = (call);                                                                           \
-        if (e_ != cudaSuccess) {                                                                           \
-            fprintf(stderr, "%s: %s (%s:%d)\n", #call, cudaGetErrorString(e_), __FILE__, __LINE__);        \
-            exit(3);                                                                                       \
-        }                                                                                                  \
-    } while (0)
-
-static void put(const void *p, size_t n) {
-    if (n && fwrite(p, 1, n, stdout) != n) exit(4);
-}
-
-static void get(void *p, size_t n) {
-    if (n && fread(p, 1, n, stdin) != n) exit(2);
-}
-
-template <typename T>
-static T *dev_alloc(size_t count, int fill, cudaStream_t s) {
-    T *p = nullptr;
-    CK(cudaMalloc(&p, std::max<size_t>(count, 1) * sizeof(T)));
-    CK(cudaMemsetAsync(p, fill, std::max<size_t>(count, 1) * sizeof(T), s));
-    return p;
-}
-
-template <typename T>
-static void put_dev(const T *d, size_t count) {
-    std::vector<T> h(count);
-    if (count) CK(cudaMemcpy(h.data(), d, count * sizeof(T), cudaMemcpyDeviceToHost));
-    put(h.data(), count * sizeof(T));
-}
 
 int main() {
     int sm_count = 0, optin = 0;
     CK(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, 0));
     CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, 0));
     // as create_impl does: the staged decoder may take the device's opt-in shared memory
-    CK(cudaFuncSetAttribute(log_decode_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
-    CK(cudaFuncSetAttribute(log_decode_window_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    CK(cudaFuncSetAttribute(log_decode_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
+    CK(cudaFuncSetAttribute(log_decode_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin));
     const uint32_t device[2] = {(uint32_t)sm_count, (uint32_t)optin};
     put(device, 8);
     cudaStream_t s;
@@ -100,7 +62,8 @@ int main() {
         uint64_t *d_off = dev_alloc<uint64_t>((size_t)nb, 0, s), *d_cnt = dev_alloc<uint64_t>((size_t)nb + 1, 0, s);
         int32_t *d_part = with_part ? dev_alloc<int32_t>((size_t)nb, 0, s) : nullptr;
         LogBatchInfo *d_info = dev_alloc<LogBatchInfo>((size_t)nb, 0, s);
-        uint32_t *d_err = dev_alloc<uint32_t>(LOG_WIN_WORDS, 0, s);
+        LogHeaderWord *d_word = dev_alloc<LogHeaderWord>(1, 0, s);
+        uint32_t *d_flags = &d_word->flags;
         longlong2 *d_win = nwin ? dev_alloc<longlong2>(nwin, 0, s) : nullptr;
         uint32_t *d_cut = nwin ? dev_alloc<uint32_t>((size_t)nb, 0, s) : nullptr;
         uint64_t *d_drop = nwin ? dev_alloc<uint64_t>((size_t)nb + 1, 0, s) : nullptr;
@@ -109,40 +72,38 @@ int main() {
         if (d_part) CK(cudaMemcpyAsync(d_part, parts.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, s));
         if (d_win) CK(cudaMemcpyAsync(d_win, win.data(), (size_t)nwin * sizeof(longlong2), cudaMemcpyHostToDevice, s));
         if (nb) {
-            if (nwin)
-                log_window_header_kernel<<<log_thread_grid(nb, sm_count), 128, 0, s>>>(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info,
-                                                                                       d_cnt, d_err, d_win, (int32_t)nwin, d_cut);
-            else
-                log_header_kernel<<<log_thread_grid(nb, sm_count), 128, 0, s>>>(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info, d_cnt, d_err);
+            CK(log_launch_header(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info, d_cnt, d_word, nullptr, nullptr, d_win, (int32_t)nwin,
+                                 d_cut, sm_count, s));
             tile_base_scan_kernel<<<1, 1024, 0, s>>>(d_cnt, nb);
             CK(cudaGetLastError());
         }
-        uint32_t hdr[LOG_WIN_WORDS] = {}, unc_err = 0, dec_err = 0;
+        LogHeaderWord hdr{};
+        uint32_t unc_err = 0, dec_err = 0;
         uint64_t nrec = 0;
         std::vector<LogBatchInfo> info(nwin ? (size_t)nb : 0);
-        CK(cudaMemcpyAsync(hdr, d_err, sizeof hdr, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(&hdr, d_word, sizeof hdr, cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(&nrec, d_cnt + nb, 8, cudaMemcpyDeviceToHost, s));
         if (nwin && nb) CK(cudaMemcpyAsync(info.data(), d_info, (size_t)nb * sizeof(LogBatchInfo), cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
-        const int64_t ncut = nwin ? hdr[6] : 0;
-        bool ran = nb > 0 && !(hdr[0] & (LOGB_BAD | LOGB_COMPRESSED)) && nrec > 0;
+        const int64_t ncut = nwin ? hdr.cut : 0;
+        bool ran = nb > 0 && !(hdr.flags & (LOGB_BAD | LOGB_COMPRESSED)) && nrec > 0;
         uint8_t *d_unc = nullptr, *d_lit = nullptr;
         uint64_t *d_slot = nullptr;
-        const uint32_t codecs = hdr[0] & LOGB_CODECS;
+        const uint32_t codecs = hdr.flags & LOGB_CODECS;
         if (ran && codecs) {
             const bool zstd = (codecs & LOGB_ZSTD) != 0;
             d_slot = dev_alloc<uint64_t>((size_t)nb + 2, 0, s);
-            CK(cudaMemsetAsync(d_err, 0, 4, s));
-            CK(log_launch_size_pass(d_bytes, d_info, nb, d_slot, d_err, zstd, sm_count, s));
+            CK(cudaMemsetAsync(d_flags, 0, 4, s));
+            CK(log_launch_size_pass(d_bytes, d_info, nb, d_slot, d_flags, zstd, sm_count, s));
             uint64_t unc_total = 0;
             CK(cudaMemcpyAsync(&unc_total, d_slot + nb, 8, cudaMemcpyDeviceToHost, s));
-            CK(cudaMemcpyAsync(&unc_err, d_err, 4, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(&unc_err, d_flags, 4, cudaMemcpyDeviceToHost, s));
             CK(cudaStreamSynchronize(s));
             if (unc_err) ran = false;
             else {
                 d_unc = dev_alloc<uint8_t>(unc_total + 64, 0, s);
                 if (zstd) d_lit = dev_alloc<uint8_t>(unc_total + 64, 0, s);
-                CK(log_launch_copy_pass(d_bytes, d_info, nb, d_slot, d_unc, d_lit, d_err, codecs, sm_count, s));
+                CK(log_launch_copy_pass(d_bytes, d_info, nb, d_slot, d_unc, d_lit, d_flags, codecs, sm_count, s));
             }
         }
         if (ran && ncut) {   // as log_cut_count: the records kept, after the count pass's correction of the scan
@@ -150,7 +111,7 @@ int main() {
             CK(cudaMemcpyAsync(&nrec, d_cnt + nb, 8, cudaMemcpyDeviceToHost, s));
             CK(cudaStreamSynchronize(s));
         }
-        const LogDecodeShape shape = log_decode_shape(hdr[1], nb, sm_count, (size_t)optin);
+        const LogDecodeShape shape = log_decode_shape(hdr.longest, nb, sm_count, (size_t)optin);
         int32_t *d_dpart = nullptr, *d_klen = nullptr, *d_vlen = nullptr;
         int64_t *d_ts = nullptr;
         uint64_t *d_ksrc = nullptr, *d_tb = nullptr;
@@ -164,15 +125,15 @@ int main() {
             d_vlen = dev_alloc<int32_t>(nrec, 0xA5, s);
             d_ksrc = dev_alloc<uint64_t>(nrec, 0xA5, s);
             d_tb = dev_alloc<uint64_t>((size_t)ntiles + 1, 0xA5, s);
-            // (d_err[0] is 0 here, or holds what the copy pass found, as in scan_log_batches)
+            // (*d_flags is 0 here, or holds what the copy pass found, as in scan_log_batches)
             // (a call whose cut batches keep no record is still decoded, so damage in them refuses it, as in scan_log_batches)
-            CK(log_launch_decode_call(shape, d_bytes, readable, d_info, nb, d_cnt, d_dpart, d_ts, d_klen, d_vlen, d_ksrc, d_err, ncut,
-                                      d_win, (int32_t)nwin, s));
+            CK(log_launch_decode(shape, d_bytes, readable, d_info, nb, d_cnt, d_dpart, d_ts, d_klen, d_vlen, d_ksrc, d_flags,
+                                 ncut ? d_win : nullptr, (int32_t)nwin, s));
             if (nrec) {
                 CK(log_launch_tile_base(d_klen, (int64_t)nrec, d_tb, sm_count, s));
                 CK(cudaMemcpyAsync(&nkey, d_tb + ntiles, 8, cudaMemcpyDeviceToHost, s));
             }
-            CK(cudaMemcpyAsync(&dec_err, d_err, 4, cudaMemcpyDeviceToHost, s));
+            CK(cudaMemcpyAsync(&dec_err, d_flags, 4, cudaMemcpyDeviceToHost, s));
             CK(cudaStreamSynchronize(s));
             if (!dec_err && nrec) {
                 d_keys = dev_alloc<uint8_t>(nkey + 64, 0xA5, s);
@@ -181,7 +142,8 @@ int main() {
             CK(cudaStreamSynchronize(s));
         }
         const uint32_t staged = shape.staged ? 1u : 0u, stage = shape.stage, grid = (uint32_t)shape.grid, ran32 = ran ? 1u : 0u;
-        put(hdr, 8);
+        put(&hdr.flags, 4);
+        put(&hdr.longest, 4);
         put(&unc_err, 4);
         put(&dec_err, 4);
         put(&nrec, 8);
@@ -190,8 +152,10 @@ int main() {
         put(&grid, 4);
         put(&ran32, 4);
         if (nwin) {
-            const uint32_t windowed = ran && log_decode_windowed(ncut) ? 1u : 0u;
-            put(hdr + 6, 16);
+            const uint32_t windowed = ran && ncut ? 1u : 0u;
+            put(&hdr.cut, 4);
+            put(&hdr.not_served, 4);
+            put(&hdr.not_served_records, 8);
             put(&windowed, 4);
             for (const LogBatchInfo &bi : info) put(&bi.flags, 4);
             put_dev(d_drop, (size_t)nb + 1);
@@ -206,7 +170,7 @@ int main() {
                 put_dev(d_keys, nkey + 64);
             }
         }
-        for (void *p : {(void *)d_bytes, (void *)d_off, (void *)d_cnt, (void *)d_part, (void *)d_info, (void *)d_err, (void *)d_unc,
+        for (void *p : {(void *)d_bytes, (void *)d_off, (void *)d_cnt, (void *)d_part, (void *)d_info, (void *)d_word, (void *)d_unc,
                         (void *)d_lit, (void *)d_slot, (void *)d_dpart, (void *)d_ts, (void *)d_klen, (void *)d_vlen, (void *)d_ksrc,
                         (void *)d_tb, (void *)d_keys, (void *)d_win, (void *)d_cut, (void *)d_drop})
             if (p) CK(cudaFree(p));

@@ -1,8 +1,9 @@
 // TEST INFRASTRUCTURE: the read_committed passes of the RecordBatch decoder (csrc/kta_logtxn.cuh) on the GPU, with everything
 // they produce made visible.  It launches what log_headers (csrc/kta_api.cu) launches for a read_committed handle —
-// log_header_kernel, the classify pass, the host round trip for the key count, the sort, resolve, carry and apply passes, then
-// the record-count scan — through the same launch functions (log_launch_txn_classify, log_launch_txn_passes), and writes out
-// every array, so that tests/test_logtxn_passes.py can compare them key by key with a plain restatement of the rule.
+// the header pass, the classify pass, the host round trip for the key count, the sort, resolve, carry and apply passes, then
+// the record-count scan — through the same launch functions (log_launch_header, log_launch_txn_classify,
+// log_launch_txn_passes), and writes out every array, so that tests/test_logtxn_passes.py can compare them key by key with a
+// plain restatement of the rule.
 // stdin, per case (little-endian): u32 nbytes, the bytes; u32 nbatches, u64 batch offsets, i32 batch partitions; u32 nranges,
 // then nranges TxnRange images (i32 partition, u32 0, u64 producerId, i64 first, i64 last), sorted by (partition, producerId,
 // first) and disjoint within a (partition, producerId): the table as the handle keeps it (the host's sort and merge are not run
@@ -14,53 +15,11 @@
 // [b + 1] = the rows of batch b); when ran: TxnKey sorted[m] (u64 producerId, u32 partition, u32 batch), u8 res[m], u8
 // tile_head[ntiles], u8 carry[ntiles].
 // kind, res, tile_head and carry are filled with 0xA5 first: an entry the passes do not write shows up.
-#include <cuda_runtime.h>
-
-#include <cstdint>
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
-
+#include "../../kafka_topic_analyzer_b200/csrc/kta_logoffsets.cuh"
 #include "../../kafka_topic_analyzer_b200/csrc/kta_logtxn.cuh"
+#include "probe.h"
 
 using namespace kta;
-
-#define CK(call)                                                                                           \
-    do {                                                                                                   \
-        cudaError_t e_ = (call);                                                                           \
-        if (e_ != cudaSuccess) {                                                                           \
-            fprintf(stderr, "%s: %s (%s:%d)\n", #call, cudaGetErrorString(e_), __FILE__, __LINE__);        \
-            exit(3);                                                                                       \
-        }                                                                                                  \
-    } while (0)
-
-static void put(const void *p, size_t n) {
-    if (n && fwrite(p, 1, n, stdout) != n) exit(4);
-}
-
-static void get(void *p, size_t n) {
-    if (n && fread(p, 1, n, stdin) != n) exit(2);
-}
-
-template <typename T>
-static T *dev_alloc(size_t count, int fill, cudaStream_t s) {
-    T *p = nullptr;
-    CK(cudaMalloc(&p, std::max<size_t>(count, 1) * sizeof(T)));
-    CK(cudaMemsetAsync(p, fill, std::max<size_t>(count, 1) * sizeof(T), s));
-    return p;
-}
-
-template <typename T>
-static std::vector<T> from_dev(const T *d, size_t count) {
-    std::vector<T> h(count);
-    if (count) CK(cudaMemcpy(h.data(), d, count * sizeof(T), cudaMemcpyDeviceToHost));
-    return h;
-}
-
-template <typename T>
-static void put_dev(const T *d, size_t count) {
-    put(from_dev(d, count).data(), count * sizeof(T));
-}
 
 int main() {
     int sm_count = 0;
@@ -88,7 +47,8 @@ int main() {
         uint64_t *d_off = dev_alloc<uint64_t>((size_t)nb, 0, s), *d_cnt = dev_alloc<uint64_t>((size_t)nb + 1, 0, s);
         int32_t *d_part = dev_alloc<int32_t>((size_t)nb, 0, s);
         LogBatchInfo *d_info = dev_alloc<LogBatchInfo>((size_t)nb + 1, 0, s);
-        uint32_t *d_err = dev_alloc<uint32_t>(2, 0, s), *d_word = dev_alloc<uint32_t>(2, 0, s);
+        LogHeaderWord *d_hdr = dev_alloc<LogHeaderWord>(1, 0, s);
+        uint32_t *d_word = dev_alloc<uint32_t>(2, 0, s);
         TxnKey *d_keys = dev_alloc<TxnKey>((size_t)nb, 0, s), *d_sorted = dev_alloc<TxnKey>((size_t)nb, 0, s);
         uint8_t *d_kind = dev_alloc<uint8_t>((size_t)nb, 0xA5, s), *d_res = dev_alloc<uint8_t>((size_t)nb, 0xA5, s);
         unsigned long long *d_stats = dev_alloc<unsigned long long>(3, 0, s);
@@ -99,12 +59,12 @@ int main() {
         if (nranges) CK(cudaMemcpyAsync(d_ranges, ranges.data(), (size_t)nranges * sizeof(TxnRange), cudaMemcpyHostToDevice, s));
         uint32_t w[3] = {0, 0, 0};   // keys, TxnErr bits, header flags (as txn_passes reads them back)
         if (nb) {
-            log_header_kernel<<<log_thread_grid(nb, sm_count), 128, 0, s>>>(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info, d_cnt, d_err);
-            CK(cudaGetLastError());
+            CK(log_launch_header(d_bytes, (int64_t)n, d_off, nb, 0, d_part, d_info, d_cnt, d_hdr, nullptr, nullptr, nullptr, 0, nullptr,
+                                 sm_count, s));
             CK(log_launch_txn_classify(d_bytes, d_info, nb, d_keys, d_kind, d_word, sm_count, s));
         }
         CK(cudaMemcpyAsync(w, d_word, 8, cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(w + 2, d_err, 4, cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(w + 2, &d_hdr->flags, 4, cudaMemcpyDeviceToHost, s));
         CK(cudaStreamSynchronize(s));
         const bool ran = !(w[2] & (LOGB_BAD | LOGB_COMPRESSED)) && !(w[1] & TXN_ERR_MARKER) && w[0] > 0;
         const int64_t m = ran ? w[0] : 0, tiles = log_txn_tiles(m);
@@ -145,7 +105,7 @@ int main() {
             put_dev(d_res, (size_t)m);
             put_dev(d_tile, (size_t)(2 * tiles));
         }
-        for (void *p : {(void *)d_bytes, (void *)d_off, (void *)d_cnt, (void *)d_part, (void *)d_info, (void *)d_err, (void *)d_word,
+        for (void *p : {(void *)d_bytes, (void *)d_off, (void *)d_cnt, (void *)d_part, (void *)d_info, (void *)d_hdr, (void *)d_word,
                         (void *)d_keys, (void *)d_sorted, (void *)d_kind, (void *)d_res, (void *)d_stats, (void *)d_ranges, (void *)d_tile,
                         (void *)d_tmp})
             if (p) CK(cudaFree(p));

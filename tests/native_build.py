@@ -45,7 +45,7 @@ def _command(nvcc, name, exe, flags=()):
 def _stale(name, exe):
     if not os.path.exists(exe):
         return True
-    srcs = [os.path.join(NATIVE, name + ".cu")] + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if os.path.isfile(os.path.join(CSRC, f))]
+    srcs = [os.path.join(NATIVE, name + ".cu"), os.path.join(NATIVE, "probe.h")] + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if os.path.isfile(os.path.join(CSRC, f))]
     return os.path.getmtime(exe) < max(os.path.getmtime(p) for p in srcs)
 
 

@@ -87,7 +87,7 @@ def main():
             us = ev.device_time if hasattr(ev, "device_time") else ev.cuda_time
             tot[ev.name] = tot.get(ev.name, 0.0) + us / 3
         span = sum(v for k, v in tot.items() if "log_crc_span" in k)
-        crc = sum(v for k, v in tot.items() if "log_crc_" in k)
+        crc = sum(v for k, v in tot.items() if "log_crc_" in k or "log_header_kernel<true" in k)
         dec = sum(v for k, v in tot.items() if "log_decode_kernel" in k)
         all_us = sum(v for k, v in tot.items() if "Memcpy" not in k and "Memset" not in k)
         nbytes = work[w][1]
