@@ -10,14 +10,19 @@ import numpy as np
 import torch
 
 import kafka_codec as kc
+import native_build
+import np_oracle
 import scan_ref as R
 from kafka_topic_analyzer_b200 import KtaEngine, lib
 from kafka_topic_analyzer_b200 import _native as N
 from kafka_topic_analyzer_b200.synth import HostTopic, tile_base_from_key_len
+from parity import last_writer
 
 NOW = (4102444800, 123456789)   # 2100-01-01: later than every synthetic record
 T = N.KTA_KEY_TILE
 MASK32 = 0xFFFFFFFF
+FNV = 0x811C9DC5                # basis and multiplier of the reference hash (src/fnv32.rs)
+FNV_INV = pow(FNV, -1, 1 << 32)
 
 
 def settle():
@@ -200,6 +205,51 @@ def unmix32(x):
     return x ^ (x >> 16)
 
 
+_forward = None
+
+
+def _fnv_forward3():
+    """The 2^24 FNV states after three bytes, sorted, with the prefix that reaches each (built once per process)."""
+    global _forward
+    if _forward is None:
+        h = np.full(1, FNV, dtype=np.uint32)
+        for _ in range(3):
+            h = ((h[:, None] ^ np.arange(256, dtype=np.uint32)[None, :]) * np.uint32(FNV)).reshape(-1)
+        order = np.argsort(h, kind="stable").astype(np.uint32)
+        _forward = (h[order], order)   # prefix index = b0 << 16 | b1 << 8 | b2
+    return _forward
+
+
+def keys_for_mixed(xs):
+    """One 5-byte key per target: fmix32(fnv32(key)) == x.  Meet in the middle: two backward FNV steps from the target
+    (2^16 candidates) looked up among the forward states after three bytes (2^24): about 256 hits per target."""
+    states, prefix = _fnv_forward3()
+    b = np.arange(1 << 16, dtype=np.uint32)
+    b3, b4 = b >> 8, b & 0xFF
+    keys = []
+    for x in xs:
+        h4 = np.uint32((unmix32(int(x)) * FNV_INV) & MASK32) ^ b4     # undo the last step for every last byte
+        h3 = (h4 * np.uint32(FNV_INV)) ^ b3
+        pos = np.searchsorted(states, h3)
+        pos = np.minimum(pos, states.size - 1)
+        hit = np.nonzero(states[pos] == h3)[0]
+        assert hit.size, "no 5-byte preimage for x = %#x" % int(x)
+        j = int(hit[0])
+        pre = int(prefix[pos[j]])
+        keys.append(bytes([pre >> 16, (pre >> 8) & 0xFF, pre & 0xFF, int(b3[j]), int(b4[j])]))
+    return keys
+
+
+def last_writer_map(t, seq, keep=None, parts=8):
+    """Independent statement of the alive-key table: for every hash of a keyed record of a partition in [0, parts) that
+    is kept, the largest (seq + 1) << 1 | alive.  Sorted (hash u32, stamp u64) arrays."""
+    h = np_oracle.fnv32_many(t.key_len, t.key_bytes)
+    m = (t.key_len >= 0) & (t.partition >= 0) & (t.partition < parts)
+    if keep is not None:
+        m &= keep
+    return last_writer(h[m], np.asarray(seq, dtype=np.uint64)[m], t.value_len[m] >= 0)
+
+
 def engine(P=8, **kw):
     """an engine counting alive keys exactly (-c), with 2^12 HLL registers"""
     return KtaEngine(P, count_alive_keys=True, hll_precision=12, now=NOW, **kw)
@@ -231,14 +281,34 @@ def push_host(e, t, *, tile_base=True, seq=None, seq_base=None):
                       seq=None if seq is None else np.ascontiguousarray(seq, dtype=np.uint64), seq_base=seq_base)
 
 
-def push_records(e, t, count=None):
-    """the first `count` records of a HostTopic (all when None), one kta_push each"""
-    off = 0
-    for i in range(t.n if count is None else count):
-        kl = int(t.key_len[i])
-        key = None if kl < 0 else t.key_bytes[off:off + kl].tobytes()
-        off += max(kl, 0)
-        e.push(int(t.partition[i]), int(t.offset[i]), int(t.ts_ms[i]), key, int(t.value_len[i]))
+_push_loop = None
+
+
+def push_loop():
+    """tests/native/push_loop.cu, loaded once"""
+    global _push_loop
+    if _push_loop is None:
+        f = C.CDLL(native_build.build("push_loop")).push_loop
+        f.restype = C.c_int
+        f.argtypes = [C.c_void_p] * 2 + [C.c_int64] + [C.c_void_p] * 8
+        _push_loop = f
+    return _push_loop
+
+
+def push_records(e, t, count=None, start=0):
+    """records [start, start + count) of a HostTopic (to its end when count is None), one kta_push each, called from C.
+    A refused record raises KtaError, with the records before it taken."""
+    kl = np.ascontiguousarray(t.key_len, dtype=np.int32)
+    off = np.cumsum(np.maximum(kl, 0), dtype=np.int64) - np.maximum(kl, 0)
+    stop = t.n if count is None else start + count
+    cols = [np.ascontiguousarray(c[start:stop], dtype=d) for c, d in ((t.partition, np.int32), (t.offset, np.int64),
+                                                                       (t.ts_ms, np.int64), (kl, np.int32),
+                                                                       (t.value_len, np.int32), (off, np.int64))]
+    keys = np.ascontiguousarray(t.key_bytes, dtype=np.uint8) if t.key_bytes.size else np.zeros(1, dtype=np.uint8)
+    failed = C.c_int64(-1)
+    rc = push_loop()(C.cast(lib().kta_push, C.c_void_p), e.handle, stop - start, *(c.ctypes.data for c in cols[:5]),
+                     keys.ctypes.data, cols[5].ctypes.data, C.addressof(failed))
+    N.check(rc)
 
 
 def feed(e, t, entry):

@@ -10,6 +10,8 @@
                    the GPU, every array they produce made visible, and a plain host CRC-32C that needs no GPU (built like
                    logdecomp_probe)
   codec_harness    tests/native/codec_harness.cu: the same codec walks as plain host code, one "lane" (codec_harness.py runs it)
+  push_loop        tests/native/push_loop.cu: a shared library (host code only) that calls kta_push record by record over
+                   numpy columns (feed.push_records)
 
 build() makes the plain programs in tests/native/build/ (git-ignored).  __graft_entry__.build() builds them, because the machine
 that runs the GPU tests may have no nvcc; build() rebuilds one when it is older than the sources, and fails when it is missing
@@ -23,7 +25,8 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(ROOT, "kafka_topic_analyzer_b200", "csrc")
 NATIVE = os.path.join(HERE, "native")
 OUT = os.path.join(NATIVE, "build")
-PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe", "logcrc_probe", "codec_harness")
+PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe", "logcrc_probe", "codec_harness", "push_loop")
+LIBRARIES = ("push_loop",)
 GPU_PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe", "logcrc_probe")
 SANITIZE = ["-g", "-Xcompiler", "-fsanitize=address,-fno-omit-frame-pointer"]
 
@@ -39,6 +42,8 @@ def _command(nvcc, name, exe, flags=()):
         from kafka_topic_analyzer_b200 import _native
         lib_flags = " ".join(_native.NVCC_FLAGS).replace("-Xcompiler -fPIC", "").replace("-shared", "").split()
         return [nvcc, *lib_flags, "-o", exe, src]
+    if name in LIBRARIES:
+        return [nvcc, "-O2", "-std=c++17", "-shared", "-Xcompiler", "-fPIC", *flags, "-o", exe, src]
     return [nvcc, "-O1", "-std=c++17", *flags, "-o", exe, src]
 
 

@@ -12,54 +12,15 @@ import pytest
 
 from kafka_topic_analyzer_b200 import KtaError, synth
 from kafka_topic_analyzer_b200.synth import HostTopic, tile_base_from_key_len
-from feed import MASK32, NOW, alive_import, engine, fmix32, gather, push_host, scan, settle, take, unmix32
+from feed import (MASK32, NOW, alive_import, engine, fmix32, gather, keys_for_mixed, last_writer_map, push_host, scan, settle,
+                  take, unmix32)
 from oracle_lib import Oracle, fnv32, olib
-from parity import assert_parity, assert_same_map, exported, last_writer
+from parity import assert_parity, assert_same_map, exported
 import np_oracle
 
 HLL_P = 12                      # feed.engine's
 P = 8                           # feed.engine's default
 M20 = 1 << 20
-FNV = 0x811C9DC5                # basis and multiplier of the reference hash (src/fnv32.rs)
-FNV_INV = pow(FNV, -1, 1 << 32)
-
-
-# ------------------------------------------------------------------------------------------------
-# crafted keys
-# ------------------------------------------------------------------------------------------------
-_forward = None
-
-
-def _fnv_forward3():
-    """The 2^24 FNV states after three bytes, sorted, with the prefix that reaches each (built once per module)."""
-    global _forward
-    if _forward is None:
-        h = np.full(1, FNV, dtype=np.uint32)
-        for _ in range(3):
-            h = ((h[:, None] ^ np.arange(256, dtype=np.uint32)[None, :]) * np.uint32(FNV)).reshape(-1)
-        order = np.argsort(h, kind="stable").astype(np.uint32)
-        _forward = (h[order], order)   # prefix index = b0 << 16 | b1 << 8 | b2
-    return _forward
-
-
-def keys_for_mixed(xs):
-    """One 5-byte key per target: fmix32(fnv32(key)) == x.  Meet in the middle: two backward FNV steps from the target
-    (2^16 candidates) looked up among the forward states after three bytes (2^24): about 256 hits per target."""
-    states, prefix = _fnv_forward3()
-    b = np.arange(1 << 16, dtype=np.uint32)
-    b3, b4 = b >> 8, b & 0xFF
-    keys = []
-    for x in xs:
-        h4 = np.uint32((unmix32(int(x)) * FNV_INV) & MASK32) ^ b4     # undo the last step for every last byte
-        h3 = (h4 * np.uint32(FNV_INV)) ^ b3
-        pos = np.searchsorted(states, h3)
-        pos = np.minimum(pos, states.size - 1)
-        hit = np.nonzero(states[pos] == h3)[0]
-        assert hit.size, "no 5-byte preimage for x = %#x" % int(x)
-        j = int(hit[0])
-        pre = int(prefix[pos[j]])
-        keys.append(bytes([pre >> 16, (pre >> 8) & 0xFF, pre & 0xFF, int(b3[j]), int(b4[j])]))
-    return keys
 
 
 # ------------------------------------------------------------------------------------------------
@@ -87,16 +48,6 @@ def filler_pool(rng, count, length=8):
 # ------------------------------------------------------------------------------------------------
 # expected and observed tables
 # ------------------------------------------------------------------------------------------------
-def last_writer_map(t, seq, keep=None, parts=P):
-    """Independent statement of the table: for every hash of a keyed record of a partition in [0, parts) that is kept,
-    the largest (seq + 1) << 1 | alive.  Sorted (hash u32, stamp u64) arrays."""
-    h = np_oracle.fnv32_many(t.key_len, t.key_bytes)
-    m = (t.key_len >= 0) & (t.partition >= 0) & (t.partition < parts)
-    if keep is not None:
-        m &= keep
-    return last_writer(h[m], np.asarray(seq, dtype=np.uint64)[m], t.value_len[m] >= 0)
-
-
 def oracle_of(*topics):
     o = Oracle(count_alive_keys=True, now=NOW)
     for t in topics:
