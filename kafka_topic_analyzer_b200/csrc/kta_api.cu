@@ -19,12 +19,9 @@
 #include <new>
 #include <vector>
 
+#include "kta_host.cuh"
 #include "kta_kernels.cuh"
-#include "kta_logcrc.cuh"
-#include "kta_logdecode.cuh"
-#include "kta_logdecode_launch.cuh"
-#include "kta_logoffsets.cuh"
-#include "kta_logtxn.cuh"
+#include "kta_logscan.cuh"
 #include "kta_synth.h"
 
 using namespace kta;
@@ -32,24 +29,6 @@ using namespace kta;
 // ------------------------------------------------------------------------------------------------
 // errors
 // ------------------------------------------------------------------------------------------------
-static thread_local char g_err[512] = "";
-
-static int fail(int code, const char *fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
-    va_end(ap);
-    return code;
-}
-
-#define CU(call)                                                                                     \
-    do {                                                                                             \
-        cudaError_t e_ = (call);                                                                     \
-        if (e_ != cudaSuccess)                                                                       \
-            return fail(e_ == cudaErrorMemoryAllocation ? KTA_ERR_NOMEM : KTA_ERR_CUDA, "%s: %s (%s:%d)", #call, \
-                        cudaGetErrorString(e_), __FILE__, __LINE__);                                 \
-    } while (0)
-
 extern "C" const char *kta_last_error(void) { return g_err; }
 extern "C" int kta_abi_version(void) { return KTA_ABI_VERSION; }
 extern "C" int kta_device_count(void) {
@@ -69,44 +48,6 @@ static constexpr int32_t ALIVE_DEFAULT_KIB = 256 * 1024;       // initial alive-
 static constexpr int32_t ALIVE_MAX_KIB = 32 * 1024 * 1024;     // 32 GiB = one slot per possible 32-bit hash
 static constexpr int64_t ALIVE_CACHE_MIN_RECORDS = 1 << 20;    // smaller batches go straight to the table
 static constexpr int64_t DEFAULT_RING_RECORDS = 1 << 22;  // 4 Mi records per chunk
-
-// Owner of `cap` elements of device (DevBuf) or pinned host (PinnedBuf) memory: move-only, freed by its destructor.
-template <typename T, bool PINNED>
-class Buf {
-    T *p_ = nullptr;
-    void release() {
-        if (p_) PINNED ? cudaFreeHost(p_) : cudaFree(p_);
-        p_ = nullptr;
-        cap = 0;
-    }
-
-  public:
-    int64_t cap = 0;
-    Buf() = default;
-    Buf(Buf &&o) noexcept : p_(o.p_), cap(o.cap) { o.p_ = nullptr; o.cap = 0; }
-    Buf &operator=(Buf &&o) noexcept { std::swap(p_, o.p_); std::swap(cap, o.cap); return *this; }   // o frees the old memory
-    ~Buf() { release(); }
-    T *get() const { return p_; }
-    operator T *() const { return p_; }
-    // n elements, for a buffer of fixed size
-    int alloc(int64_t n) {
-        release();
-        void *p = nullptr;
-        const size_t bytes = (size_t)n * sizeof(T);
-        CU(PINNED ? cudaHostAlloc(&p, bytes, cudaHostAllocDefault) : cudaMalloc(&p, bytes));
-        p_ = static_cast<T *>(p);
-        cap = n;
-        return KTA_OK;
-    }
-    // at least `need` elements (contents not kept): null with cap 0 if the allocation fails
-    int grow(cudaStream_t s, int64_t need) {
-        if (need <= cap) return KTA_OK;
-        CU(cudaStreamSynchronize(s));   // queued work may still read the old buffer
-        return alloc(need + need / 4 + 64);
-    }
-};
-template <typename T> using DevBuf = Buf<T, false>;
-template <typename T> using PinnedBuf = Buf<T, true>;
 
 struct Chunk {
     // device staging (shared by kta_push and kta_push_batch_host)
@@ -147,65 +88,6 @@ struct AliveKeys {
     uint64_t grows = 0, reruns = 0;
     uint64_t now = 0, occupied = 0;          // counted by the last alive_settle
     std::vector<AlivePending> pending;
-};
-
-// read_committed isolation of the log entry points (kta_logtxn.cuh); allocated only on a read_committed handle
-struct TxnState {
-    DevBuf<TxnKey> d_keys, d_sorted;                 // classify's keys / sorted by (partition, producerId, batch)
-    DevBuf<uint8_t> d_kind;                          // per batch: TxnKind of transactional data batches and markers
-    DevBuf<uint8_t> d_res;                           // per sorted key: next marker within its resolve tile
-    DevBuf<uint8_t> d_tile;                          // tile heads, then the carries behind each tile
-    DevBuf<uint8_t> d_sort_tmp;
-    DevBuf<uint32_t> d_word;                         // [0] keys classified, [1] TxnErr bits
-    DevBuf<unsigned long long> d_stats;              // this call: aborted batches, aborted records, undecided records
-    std::vector<TxnRange> ranges;                    // registered aborted ranges, sorted and merged; mirrored in d_ranges
-    DevBuf<TxnRange> d_ranges;
-    uint64_t totals[3] = {0, 0, 0};                  // the stats of every successful call since create / reset
-};
-
-// check.crcs of the log entry points (kta_logcrc.cuh): the switch, the passes' buffers, and what successful calls found
-struct CrcState {
-    bool on = false;
-    DevBuf<uint64_t> d_spans;                        // per batch: spans of its CRC region, then their inclusive scan
-    DevBuf<uint32_t> d_acc;                          // per batch: the xor of its spans' shares of the register
-    DevBuf<LogCrcFail> d_fails;                      // the call's failures, in the order the header pass met them
-    DevBuf<LogCrcTables> d_tables;                   // built on the first call with the switch on
-    uint64_t totals[3] = {0, 0, 0};                  // checked batches, failed batches, failed bytes
-    std::vector<kta_log_crc_failure> kept;           // the first KTA_LOG_CRC_KEEP failures
-};
-
-// The log start offset and high watermark of each partition (kta_log_set_offsets, kta_logoffsets.cuh): the table, the
-// passes' buffers, and what successful calls left out
-struct OffsetState {
-    std::vector<longlong2> win;                      // per partition: x log start offset, y high watermark (-1: unbounded);
-                                                     // empty until a window is set
-    int64_t set = 0;                                 // partitions with a bound: the window passes run only while > 0
-    bool dirty = false;                              // win changed since it was last copied to d_win
-    DevBuf<longlong2> d_win;                         // win on the device
-    DevBuf<uint32_t> d_cut;                          // the call's cut batches (served, with records below the start)
-    DevBuf<uint64_t> d_drop;                         // per batch: records the count pass drops, then their scan
-    uint64_t totals[2] = {0, 0};                     // batches not served, records left out
-};
-
-// State of the log entry points (Kafka RecordBatch v2 segments → SoA → scan), reused from call to call
-struct LogScan {
-    DevBuf<uint8_t> bytes;                   // segments staged from the host (kta_push_log_segments_host)
-    DevBuf<uint64_t> off;                    // their batch offsets
-    DevBuf<int32_t> part;                    // and each batch's partition
-    DevBuf<LogBatchInfo> info;               // per batch, from the header pass
-    DevBuf<uint64_t> cnt;                    // records per batch, then their inclusive scan
-    DevBuf<LogHeaderWord> err;               // the header pass's error word; its flags, the later passes' flag word
-    DevBuf<int32_t> dec_part, dec_klen, dec_vlen;   // the decoded columns
-    DevBuf<int64_t> dec_ts;
-    DevBuf<uint64_t> dec_ksrc;               // per decoded record: where its key bytes lie in the segment buffer
-    DevBuf<uint8_t> dec_keys;                // the keys gathered in record order
-    DevBuf<uint8_t> unc;                     // uncompressed images of compressed batches
-    DevBuf<uint8_t> unc_lit;                 // zstd: Huffman-decoded literals, at the offsets of unc
-    DevBuf<uint64_t> unc_slot;               // per compressed batch: offset of its image in unc
-    bool read_committed = false;
-    TxnState txn;
-    CrcState crc;
-    OffsetState offsets;
 };
 
 struct kta_handle {
@@ -616,7 +498,6 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
         return fail(KTA_ERR_INVALID, "hll_precision %d not 0 or 4..18", cfg->hll_precision);
     if (cfg->isolation_level != KTA_READ_UNCOMMITTED && cfg->isolation_level != KTA_READ_COMMITTED)
         return fail(KTA_ERR_INVALID, "isolation_level %d is neither KTA_READ_UNCOMMITTED (0) nor KTA_READ_COMMITTED (1)", cfg->isolation_level);
-    h->log.read_committed = cfg->isolation_level == KTA_READ_COMMITTED;
     int ndev = 0;
     CU(cudaGetDeviceCount(&ndev));
     if (ndev < 1) return fail(KTA_ERR_CUDA, "no CUDA device (this library has no CPU fallback)");
@@ -650,7 +531,6 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
         return rc;
     if (h->nhll && (rc = h->d_hll.alloc((int64_t)h->nhll))) return rc;
     if (cfg->count_alive_keys == 1 && (rc = alive_create(h))) return rc;
-    if (h->log.read_committed && ((rc = h->log.txn.d_word.alloc(2)) || (rc = h->log.txn.d_stats.alloc(3)))) return rc;
     h->smem_optin = prop.sharedMemPerBlockOptin;
     if (cfg->shard_world > 1) {
         if (cfg->shard_rank < 0 || cfg->shard_rank >= cfg->shard_world || cfg->shard_world > P)
@@ -665,9 +545,7 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
         for (const auto &by_capture : by_mode)
             for (const ScanFn f : by_capture)
                 if (f) CU(cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
-    // the record decoder stages a batch of up to 48 KiB per warp (log_decode); attributes belong to the device
-    CU(cudaFuncSetAttribute(log_decode_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
-    CU(cudaFuncSetAttribute(log_decode_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+    if ((rc = log_scan_create(h->log, cfg->isolation_level == KTA_READ_COMMITTED, h->smem_optin))) return rc;
     if ((rc = state_reset_device(h))) return rc;
     CU(cudaStreamSynchronize(h->stream));
     return KTA_OK;
@@ -793,15 +671,13 @@ static int collect_timing(kta_handle *h) {
     return KTA_OK;
 }
 
-// the key_tile_base column of n records' key lengths, into h->d_tb_scratch ([ntiles] = the key bytes in all)
-static int derive_tile_base(kta_handle *h, const int32_t *d_klen, int64_t n) {
-    const int64_t ntiles = (n + TILE - 1) / TILE;
-    int rc;
-    if ((rc = h->d_tb_scratch.grow(h->stream, ntiles + 1))) return rc;
-    CU(log_launch_tile_base(d_klen, n, h->d_tb_scratch, h->sm_count, h->stream));
-    h->launches += 2;
-    return KTA_OK;
+// what the log path's steps (kta_logscan.cuh) need of the handle
+static LogEnv log_env(kta_handle *h) {
+    return LogEnv{h->stream, h->sm_count, h->smem_optin, h->cfg.num_partitions, h->d_tb_scratch, h->launches};
 }
+
+// the key_tile_base column of n records' key lengths, into h->d_tb_scratch ([ntiles] = the key bytes in all)
+static int derive_tile_base(kta_handle *h, const int32_t *d_klen, int64_t n) { return log_tile_base(log_env(h), d_klen, n); }
 
 // a scan's params over the columns of n records from seq_base on (ScanParams' leading fields, in their order; the rest zero)
 static ScanParams scan_params(int64_t n, uint64_t seq_base, const int32_t *partition, const int64_t *ts_ms, const int32_t *key_len,
@@ -861,241 +737,6 @@ extern "C" int kta_scan_batch_device(kta_handle *h, const kta_batch *b) {
 // Kafka RecordBatch v2 segments → SoA → scan (SURVEY.md §8 f2; kernels in kta_logdecode.cuh)
 // ------------------------------------------------------------------------------------------------
 
-// read_committed: the passes of kta_logtxn.cuh over the batches log_header_kernel has read, before the record count is
-// scanned.  Classify always; sort, resolve, carry and apply only when the call has transactional batches.  One host round
-// trip (the classify count).  *ran: the apply pass was launched, so its error word and counters are to be read back.
-static int txn_passes(kta_handle *h, int32_t partition, const uint8_t *dev_bytes, int64_t nbatches, bool *ran) {
-    LogScan &L = h->log;
-    TxnState &t = L.txn;
-    cudaStream_t s = h->stream;
-    *ran = false;
-    if (nbatches > (int64_t)UINT32_MAX) return fail(KTA_ERR_INVALID, "%lld batches in one read_committed call: split them", (long long)nbatches);
-    int rc;
-    if ((rc = t.d_keys.grow(s, nbatches)) || (rc = t.d_sorted.grow(s, nbatches)) || (rc = t.d_kind.grow(s, nbatches)) ||
-        (rc = t.d_res.grow(s, nbatches)))
-        return rc;
-    CU(cudaMemsetAsync(t.d_word, 0, 8, s));
-    CU(log_launch_txn_classify(dev_bytes, L.info, nbatches, t.d_keys, t.d_kind, t.d_word, h->sm_count, s));
-    h->launches++;
-    uint32_t w[3] = {0, 0, 0};   // keys, TxnErr bits, header flags
-    CU(cudaMemcpyAsync(w, t.d_word, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(w + 2, &L.err.get()->flags, 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    if (w[2] & (LOGB_BAD | LOGB_COMPRESSED)) return KTA_OK;   // the call is refused for its headers (log_headers says so)
-    if (w[1] & TXN_ERR_MARKER)
-        return fail(KTA_ERR_INVALID, "unreadable transaction marker in partition %d (control batch compressed, without a record, "
-                    "truncated, or with a key that is not version 0 | type)", partition);
-    const int64_t m = w[0];
-    if (m == 0) return KTA_OK;
-    const int64_t nranges = (int64_t)t.ranges.size();
-    size_t tmp = 0;   // first the sort's scratch size, then the passes
-    CU(log_launch_txn_passes(t.d_keys, t.d_sorted, m, t.d_kind, L.info, t.d_res, nullptr, nullptr, tmp, t.d_ranges, nranges, L.cnt,
-                             t.d_word, t.d_stats, h->sm_count, s));
-    if ((rc = t.d_sort_tmp.grow(s, (int64_t)tmp)) || (rc = t.d_tile.grow(s, 2 * log_txn_tiles(m)))) return rc;
-    tmp = (size_t)t.d_sort_tmp.cap;
-    CU(log_launch_txn_passes(t.d_keys, t.d_sorted, m, t.d_kind, L.info, t.d_res, t.d_tile, t.d_sort_tmp.get(), tmp, t.d_ranges, nranges,
-                             L.cnt, t.d_word, t.d_stats, h->sm_count, s));
-    h->launches += 4;   // (the sort counted as one)
-    *ran = true;
-    return KTA_OK;
-}
-
-// What the header pass (and read_committed's passes and the CRC check) found in one call's batches
-struct LogHeaders {
-    uint64_t nrec = 0;                               // records in all
-    LogHeaderWord word{};                            // the header pass's error word
-    unsigned long long txn_stats[3] = {0, 0, 0};     // this call's aborted batches, aborted records, undecided records
-    std::vector<kta_log_crc_failure> crc_fails;      // check.crcs: this call's failures, in batch order, as many as are kept
-};
-
-// windows: the table the window passes read (on the device once log_offsets_upload ran), or null while the handle has none
-static const longlong2 *log_window_table(const kta_handle *h) {
-    return h->log.offsets.set > 0 ? h->log.offsets.d_win.get() : nullptr;
-}
-
-// check.crcs: the passes of kta_logcrc.cuh that precede the header pass (span counts, their scan, the spans' CRCs), through
-// log_launch_crc_spans.  No host round trip; the span kernel's grid is bounded by the call's bytes.  Batches that are not
-// served are not checked (the window table goes to the device first, log_offsets_upload).
-static int log_crc_spans(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes, int64_t len,
-                         const uint64_t *dev_batch_off, int64_t nbatches) {
-    CrcState &c = h->log.crc;
-    cudaStream_t s = h->stream;
-    int rc;
-    if (!c.d_tables) {
-        LogCrcTables t;
-        log_crc_tables_host(t);
-        if ((rc = c.d_tables.alloc(1))) return rc;
-        CU(cudaMemcpyAsync(c.d_tables, &t, sizeof t, cudaMemcpyHostToDevice, s));
-        CU(cudaStreamSynchronize(s));   // `t` lives on this stack frame
-        CU(cudaFuncSetAttribute(log_crc_span_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)LOG_CRC_SMEM));
-    }
-    if ((rc = c.d_spans.grow(s, nbatches + 1)) || (rc = c.d_acc.grow(s, nbatches)) || (rc = c.d_fails.grow(s, nbatches))) return rc;
-    CU(log_launch_crc_spans(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, log_window_table(h), h->cfg.num_partitions,
-                            c.d_tables, c.d_spans, c.d_acc, log_crc_span_grid(len, nbatches, h->sm_count), h->sm_count, s));
-    h->launches += 3;
-    return KTA_OK;
-}
-
-// windows: the window table goes to the device when it changed since the last call (two host synchronisations, only then)
-static int log_offsets_upload(kta_handle *h) {
-    OffsetState &o = h->log.offsets;
-    if (!o.dirty) return KTA_OK;
-    int rc;
-    if (!o.d_win && (rc = o.d_win.alloc((int64_t)o.win.size()))) return rc;
-    CU(cudaStreamSynchronize(h->stream));   // no queued pass reads the table while it is replaced
-    CU(cudaMemcpyAsync(o.d_win, o.win.data(), o.win.size() * sizeof(longlong2), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaStreamSynchronize(h->stream));
-    o.dirty = false;
-    return KTA_OK;
-}
-
-// The header pass, read_committed's passes and the scan of the record counts.  One host round trip (two under
-// read_committed); refuses the call for its headers and for the order of a producer's batches.  With check.crcs the CRC
-// passes come first and the failures are counted in the same round trip; only a call with failures makes one more, for
-// their list.  With windows the header pass also skips the batches that are not served and lists the cut ones; their
-// counts come back in the same round trip.
-static int log_headers(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes, int64_t len,
-                       const uint64_t *dev_batch_off, int64_t nbatches, LogHeaders &out) {
-    LogScan &L = h->log;
-    cudaStream_t s = h->stream;
-    int rc;
-    if ((rc = L.info.grow(s, nbatches + 1)) || (rc = L.cnt.grow(s, nbatches + 1))) return rc;
-    if (!L.err && (rc = L.err.alloc(1))) return rc;
-    const bool crc = L.crc.on;
-    if (L.offsets.set > 0 && ((rc = log_offsets_upload(h)) || (rc = L.offsets.d_cut.grow(s, nbatches)))) return rc;
-    if (crc && (rc = log_crc_spans(h, partition, dev_batch_partition, dev_bytes, len, dev_batch_off, nbatches))) return rc;
-    CU(cudaMemsetAsync(L.err, 0, sizeof(LogHeaderWord), s));
-    CU(log_launch_header(dev_bytes, len, dev_batch_off, nbatches, partition, dev_batch_partition, L.info, L.cnt, L.err,
-                         crc ? L.crc.d_acc.get() : nullptr, L.crc.d_fails, log_window_table(h), h->cfg.num_partitions, L.offsets.d_cut,
-                         h->sm_count, s));
-    bool txn = false;   // read_committed and the call has transactional batches
-    if (L.read_committed && (rc = txn_passes(h, partition, dev_bytes, nbatches, &txn))) return rc;
-    tile_base_scan_kernel<<<1, 1024, 0, s>>>(L.cnt, nbatches);   // inclusive scan of [1..nbatches] in place
-    CU(cudaGetLastError());
-    h->launches += 2;
-    uint32_t txn_word[2] = {0, 0};
-    CU(cudaMemcpyAsync(&out.nrec, L.cnt + nbatches, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&out.word, L.err, sizeof(LogHeaderWord), cudaMemcpyDeviceToHost, s));
-    if (txn) {
-        CU(cudaMemcpyAsync(txn_word, L.txn.d_word, 8, cudaMemcpyDeviceToHost, s));
-        CU(cudaMemcpyAsync(out.txn_stats, L.txn.d_stats, 24, cudaMemcpyDeviceToHost, s));
-    }
-    CU(cudaStreamSynchronize(s));
-    if (out.word.flags & LOGB_COMPRESSED)
-        return fail(KTA_ERR_INVALID, "unknown compression codec (attributes bits 0-2 = 5..7) in partition %d", partition);
-    if (out.word.flags & LOGB_BAD) return fail(KTA_ERR_INVALID, "malformed record batch header in partition %d", partition);
-    if (txn_word[1] & TXN_ERR_ORDER)
-        return fail(KTA_ERR_INVALID, "the batches of one producer in partition %d are not in increasing baseOffset order", partition);
-    // the failures to keep: the first ones in batch order, as many as the handle's list still has room for
-    const uint32_t nfail = out.word.crc_failed;
-    const size_t room = KTA_LOG_CRC_KEEP - L.crc.kept.size();
-    if (nfail && room) {
-        std::vector<LogCrcFail> f(nfail);
-        CU(cudaMemcpyAsync(f.data(), L.crc.d_fails, (size_t)nfail * sizeof(LogCrcFail), cudaMemcpyDeviceToHost, s));
-        CU(cudaStreamSynchronize(s));
-        std::sort(f.begin(), f.end(), [](const LogCrcFail &a, const LogCrcFail &b) { return a.batch < b.batch; });
-        for (size_t i = 0; i < std::min<size_t>(room, f.size()); i++)
-            out.crc_fails.push_back(kta_log_crc_failure{f[i].partition, f[i].batch_bytes, f[i].base_offset, f[i].stored, f[i].computed});
-    }
-    return KTA_OK;
-}
-
-// Compressed batches (codecs: the LOGB_CODECS bits the header pass saw): size pass, scratch allocation, decompression.
-// Afterwards they are ordinary batches that happen to lie in the scratch buffer.  One host round trip.
-static int log_decompress(kta_handle *h, int32_t partition, const uint8_t *dev_bytes, int64_t nbatches, uint32_t codecs) {
-    LogScan &L = h->log;
-    cudaStream_t s = h->stream;
-    int rc;
-    if ((rc = L.unc_slot.grow(s, nbatches + 2))) return rc;
-    uint32_t *flags = &L.err.get()->flags;
-    CU(cudaMemsetAsync(flags, 0, 4, s));
-    const bool zstd = (codecs & LOGB_ZSTD) != 0;
-    CU(log_launch_size_pass(dev_bytes, L.info, nbatches, L.unc_slot, flags, zstd, h->sm_count, s));
-    h->launches += zstd ? 3 : 2;
-    uint64_t unc_total = 0;
-    uint32_t bad = 0;
-    CU(cudaMemcpyAsync(&unc_total, L.unc_slot + nbatches, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(&bad, flags, 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    if (bad) return fail(KTA_ERR_INVALID, "malformed compressed record batch in partition %d", partition);
-    if ((rc = L.unc.grow(s, (int64_t)unc_total + 64))) return rc;
-    // zstd's literal buffer has the size of the scratch buffer (a block's literals go at its output's offset); it is
-    // only allocated once zstd batches are seen
-    if (zstd && (rc = L.unc_lit.grow(s, (int64_t)unc_total + 64))) return rc;
-    CU(log_launch_copy_pass(dev_bytes, L.info, nbatches, L.unc_slot, L.unc, L.unc_lit, flags, codecs, h->sm_count, s));
-    h->launches += ((codecs & ~(uint32_t)LOGB_ZSTD) ? 1 : 0) + (zstd ? 1 : 0);
-    return KTA_OK;
-}
-
-// The records of every batch into the decoded columns, which b then names; with keys, where each record's key bytes lie.
-// One warp per batch; the batch is staged in shared memory when the longest one fits a stage of <= 48 KiB.
-// window: the window table when the call has cut batches, whose records below the log start offset are left out, else null.
-static int log_decode(kta_handle *h, const uint8_t *dev_bytes, int64_t readable, int64_t nbatches, uint64_t nrec,
-                      uint32_t longest, bool keys, const longlong2 *window, kta_batch &b) {
-    LogScan &L = h->log;
-    cudaStream_t s = h->stream;
-    if ((int64_t)nrec >= ((int64_t)1 << 31) - 2) return fail(KTA_ERR_INVALID, "%llu records in one call: split the segments", (unsigned long long)nrec);
-    int rc;
-    if ((rc = L.dec_part.grow(s, (int64_t)nrec)) || (rc = L.dec_klen.grow(s, (int64_t)nrec)) || (rc = L.dec_vlen.grow(s, (int64_t)nrec)) ||
-        (rc = L.dec_ts.grow(s, (int64_t)nrec)) || (rc = L.dec_ksrc.grow(s, (int64_t)nrec)))
-        return rc;
-    const LogDecodeShape shape = log_decode_shape(longest, nbatches, h->sm_count, h->smem_optin);
-    CU(log_launch_decode(shape, dev_bytes, (uint64_t)readable, L.info, nbatches, L.cnt, L.dec_part, L.dec_ts, L.dec_klen, L.dec_vlen,
-                         keys ? L.dec_ksrc.get() : nullptr, &L.err.get()->flags, window, h->cfg.num_partitions, s));
-    h->launches++;
-    b = kta_batch{};
-    b.n = (int64_t)nrec;
-    b.seq_base = KTA_SEQ_AUTO;
-    b.partition = L.dec_part;
-    b.ts_ms = L.dec_ts;
-    b.key_len = L.dec_klen;
-    b.value_len = L.dec_vlen;
-    return KTA_OK;
-}
-
-// Reads the decode's error word back (one host round trip).  With keys, first packs them in record order into b's key
-// columns: tile bases from the key_len column, then one gather pass (no second walk of the log).
-static int log_gather_keys(kta_handle *h, int32_t partition, const uint8_t *dev_bytes, bool keys, kta_batch &b) {
-    LogScan &L = h->log;
-    cudaStream_t s = h->stream;
-    int rc;
-    uint32_t flags = 0;
-    uint64_t nkey = 0;
-    const int64_t ntiles = (b.n + TILE - 1) / TILE;
-    if (keys) {
-        if ((rc = derive_tile_base(h, b.key_len, b.n))) return rc;
-        CU(cudaMemcpyAsync(&nkey, h->d_tb_scratch + ntiles, 8, cudaMemcpyDeviceToHost, s));
-    }
-    CU(cudaMemcpyAsync(&flags, &L.err.get()->flags, 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    if (flags) return fail(KTA_ERR_INVALID, "malformed record inside a batch of partition %d", partition);
-    if (!keys) return KTA_OK;
-    if ((rc = L.dec_keys.grow(s, (int64_t)nkey + 64))) return rc;
-    CU(log_launch_gather_keys(dev_bytes, L.dec_ksrc, L.dec_klen, b.n, h->d_tb_scratch, L.dec_keys, h->sm_count, s));
-    h->launches++;
-    b.key_bytes = L.dec_keys;
-    b.key_bytes_len = (int64_t)nkey;
-    b.key_tile_base = h->d_tb_scratch;
-    return KTA_OK;
-}
-
-// windows: the call's cut batches (ncut of them, after the decompression) are walked and their records below the log
-// start offset counted; the record-count scan is corrected for them.  One host round trip: *nrec = the records kept,
-// *dropped = the records dropped.
-static int log_cut_count(kta_handle *h, const uint8_t *dev_bytes, int64_t nbatches, int64_t ncut, uint64_t *nrec, uint64_t *dropped) {
-    LogScan &L = h->log;
-    cudaStream_t s = h->stream;
-    int rc;
-    if ((rc = L.offsets.d_drop.grow(s, nbatches + 1))) return rc;
-    CU(log_launch_cut_count(dev_bytes, L.info, nbatches, L.offsets.d_cut, ncut, log_window_table(h), h->cfg.num_partitions, L.cnt,
-                            L.offsets.d_drop, h->sm_count, s));
-    h->launches += 3;
-    CU(cudaMemcpyAsync(nrec, L.cnt + nbatches, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(dropped, L.offsets.d_drop + nbatches, 8, cudaMemcpyDeviceToHost, s));
-    CU(cudaStreamSynchronize(s));
-    return KTA_OK;
-}
-
 static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev_batch_partition, const uint8_t *dev_bytes,
                             int64_t len, int64_t readable /* bytes of dev_bytes that may be READ (>= len when the buffer has slack) */,
                             const uint64_t *dev_batch_off, int64_t nbatches, int64_t *records_out) {
@@ -1106,29 +747,36 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;   // keep seq order with records pushed earlier
     if ((rc = alive_settle_if_any(h))) return rc;   // the decode scratch of an earlier call is about to be reused
+    LogScan &L = h->log;
+    const LogEnv e = log_env(h);
     LogHeaders hd;
-    if ((rc = log_headers(h, partition, dev_batch_partition, dev_bytes, len, dev_batch_off, nbatches, hd))) return rc;
+    if ((rc = log_headers(L, e, partition, dev_batch_partition, dev_bytes, len, dev_batch_off, nbatches, hd))) return rc;
     const int64_t ncut = hd.word.cut;
     uint64_t nrec = hd.nrec, dropped = 0;
     if (hd.nrec > 0) {
         const uint32_t codecs = hd.word.flags & LOGB_CODECS;
-        if (codecs && (rc = log_decompress(h, partition, dev_bytes, nbatches, codecs))) return rc;
-        if (ncut && (rc = log_cut_count(h, dev_bytes, nbatches, ncut, &nrec, &dropped))) return rc;
+        if (codecs) {
+            uint64_t unc_total = 0;
+            uint32_t bad = 0;
+            if ((rc = log_unc_size(L, e, dev_bytes, nbatches, codecs, &unc_total, &bad))) return rc;
+            if (bad) return fail(KTA_ERR_INVALID, "malformed compressed record batch in partition %d", partition);
+            if ((rc = log_unc_copy(L, e, dev_bytes, nbatches, codecs, unc_total))) return rc;
+        }
+        if (ncut && (rc = log_cut_count(L, e, dev_bytes, nbatches, ncut, &nrec, &dropped))) return rc;
         // (cut batches that keep no record are still decoded, so damage in them refuses the call as elsewhere)
         const bool keys = nrec > 0 && keys_travel(h);
         kta_batch b;
-        if ((rc = log_decode(h, dev_bytes, readable, nbatches, nrec, hd.word.longest, keys, ncut ? log_window_table(h) : nullptr, b)))
-            return rc;
-        if ((rc = log_gather_keys(h, partition, dev_bytes, keys, b))) return rc;
+        if ((rc = log_decode(L, e, dev_bytes, readable, nbatches, nrec, hd.word.longest, keys, ncut, b))) return rc;
+        if ((rc = log_gather_keys(L, e, partition, dev_bytes, keys, b))) return rc;
         if (nrec > 0 && (rc = scan_device_batch(h, &b))) return rc;
     }
     // the call succeeded: its transaction counters, CRC results and what its windows left out join the handle's totals
-    for (int i = 0; i < 3; i++) h->log.txn.totals[i] += hd.txn_stats[i];
+    for (int i = 0; i < 3; i++) L.txn.totals[i] += hd.txn_stats[i];
     const uint32_t not_served = hd.word.not_served;
-    OffsetState &o = h->log.offsets;
+    OffsetState &o = L.offsets;
     o.totals[0] += not_served;
     o.totals[1] += hd.word.not_served_records + dropped;
-    CrcState &c = h->log.crc;
+    CrcState &c = L.crc;
     if (c.on) {
         c.totals[0] += (uint64_t)nbatches - not_served;
         c.totals[1] += hd.word.crc_failed;
@@ -1212,28 +860,9 @@ extern "C" int kta_log_add_txn_index_host(kta_handle *h, int32_t partition, cons
         add.push_back(r);
     }
     if (add.empty()) return KTA_OK;
-    // sorted by (partition, producerId, firstOffset), overlapping ranges of one producer merged: the apply pass's binary
-    // search then has one candidate per offset
-    TxnState &t = h->log.txn;
-    std::vector<TxnRange> &v = t.ranges;
-    v.insert(v.end(), add.begin(), add.end());
-    std::sort(v.begin(), v.end(), [](const TxnRange &a, const TxnRange &b) {
-        return a.part != b.part ? a.part < b.part : a.pid != b.pid ? a.pid < b.pid : a.first < b.first;
-    });
-    size_t out = 0;
-    for (size_t i = 0; i < v.size(); i++) {
-        if (out && v[out - 1].part == v[i].part && v[out - 1].pid == v[i].pid && v[i].first <= v[out - 1].last)
-            v[out - 1].last = std::max(v[out - 1].last, v[i].last);
-        else v[out++] = v[i];
-    }
-    v.resize(out);
     int rc;
     if ((rc = set_device(h))) return rc;
-    if ((rc = t.d_ranges.grow(h->stream, (int64_t)v.size()))) return rc;
-    CU(cudaStreamSynchronize(h->stream));   // no queued pass reads the ranges while they are replaced
-    CU(cudaMemcpyAsync(t.d_ranges, v.data(), v.size() * sizeof(TxnRange), cudaMemcpyHostToDevice, h->stream));
-    CU(cudaStreamSynchronize(h->stream));
-    return KTA_OK;
+    return log_add_txn_ranges(h->log, log_env(h), add);
 }
 
 extern "C" int kta_log_txn_stats(kta_handle *h, uint64_t *aborted_batches, uint64_t *aborted_records, uint64_t *undecided_records) {
@@ -1270,13 +899,7 @@ extern "C" int kta_log_set_offsets(kta_handle *h, int32_t partition, int64_t log
     if (log_start_offset >= 0 && high_watermark >= 0 && log_start_offset > high_watermark)
         return fail(KTA_ERR_INVALID, "log start offset %lld above the high watermark %lld", (long long)log_start_offset,
                     (long long)high_watermark);
-    OffsetState &o = h->log.offsets;
-    if (o.win.empty()) o.win.assign((size_t)h->cfg.num_partitions, make_longlong2(-1, -1));
-    longlong2 &w = o.win[(size_t)partition];
-    o.set -= (w.x != -1 || w.y != -1);
-    w = make_longlong2(log_start_offset, high_watermark);
-    o.set += (w.x != -1 || w.y != -1);
-    o.dirty = true;
+    log_set_window(h->log, h->cfg.num_partitions, partition, log_start_offset, high_watermark);
     return KTA_OK;
 }
 

@@ -2,8 +2,8 @@
 // record batches into ordinary ones (the size pass, then, once the caller has sized the scratch buffers from its result, the
 // copy pass), the record decode with its shape (plain, or with offset windows), the key-length tile bases and the key
 // gather; and the host walk that finds a segment's batches.  The header pass is launched by log_launch_header
-// (kta_logoffsets.cuh).  scan_log_batches (kta_api.cu) and the probes under tests/native/ all launch through these, so the
-// probes run what the product runs.  Allocation, error reporting and launch counting stay with the caller.
+// (kta_logoffsets.cuh).  The steps of kta_logscan.cuh launch through these; allocation, the host round trips, error reporting
+// and launch counting are theirs.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

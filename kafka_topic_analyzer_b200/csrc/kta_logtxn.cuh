@@ -212,10 +212,9 @@ __global__ void txn_apply_kernel(const TxnKey *keys, int64_t m, const uint8_t *k
     }
 }
 
-// The launch groups of the passes.  log_headers (kta_api.cu) and tests/native/logtxn_probe.cu both launch through these, so
-// the probe runs what the product runs.  Allocation, the host round trip, error reporting and launch counting stay with the
-// caller.  (They live here and not in kta_logdecode_launch.cuh: a translation unit that includes them compiles the radix
-// sort's kernels, which the other probes have no use for.)
+// The launch groups of the passes, launched by txn_passes (kta_logscan.cuh), which does the allocation, the host round trip,
+// error reporting and launch counting.  (They live here and not in kta_logdecode_launch.cuh: a translation unit that includes
+// them compiles the radix sort's kernels.)
 
 // the classify pass over the batches log_header_kernel has read; word[0..1] zeroed by the caller
 inline cudaError_t log_launch_txn_classify(const uint8_t *bytes, const LogBatchInfo *info, int64_t nbatches, TxnKey *keys, uint8_t *kind,

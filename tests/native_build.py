@@ -1,14 +1,8 @@
 """Build recipe of the native test programs — TEST INFRASTRUCTURE.
 
-  logdecomp_probe  tests/native/logdecomp_probe.cu: the product's decompression stage on the GPU, output made visible
-                   (sm_90a, the library's nvcc flags without -shared / -fPIC)
-  logdecode_probe  tests/native/logdecode_probe.cu: the product's record stage (decode, tile bases, key gather) on the GPU,
-                   every decoded column made visible (built like logdecomp_probe)
-  logtxn_probe     tests/native/logtxn_probe.cu: the product's read_committed passes (classify, sort, resolve, carry, apply) on
-                   the GPU, every array they produce made visible (built like logdecomp_probe)
-  logcrc_probe     tests/native/logcrc_probe.cu: the product's check.crcs passes (span counts, span pass, header verdict) on
-                   the GPU, every array they produce made visible, and a plain host CRC-32C that needs no GPU (built like
-                   logdecomp_probe)
+  log_probe        tests/native/log_probe.cu: the log entry points' steps (csrc/kta_logscan.cuh) on the GPU in the library's
+                   order, everything they produce made visible, and a plain host CRC-32C that needs no GPU (sm_90a, the
+                   library's nvcc flags without -shared / -fPIC; log_probe.py runs it)
   codec_harness    tests/native/codec_harness.cu: the same codec walks as plain host code, one "lane" (codec_harness.py runs it)
   push_loop        tests/native/push_loop.cu: a shared library (host code only) that calls kta_push record by record over
                    numpy columns (feed.push_records)
@@ -25,9 +19,9 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(ROOT, "kafka_topic_analyzer_b200", "csrc")
 NATIVE = os.path.join(HERE, "native")
 OUT = os.path.join(NATIVE, "build")
-PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe", "logcrc_probe", "codec_harness", "push_loop")
+PROGRAMS = ("log_probe", "codec_harness", "push_loop")
 LIBRARIES = ("push_loop",)
-GPU_PROGRAMS = ("logdecomp_probe", "logdecode_probe", "logtxn_probe", "logcrc_probe")
+GPU_PROGRAMS = ("log_probe",)
 SANITIZE = ["-g", "-Xcompiler", "-fsanitize=address,-fno-omit-frame-pointer"]
 
 
@@ -50,7 +44,7 @@ def _command(nvcc, name, exe, flags=()):
 def _stale(name, exe):
     if not os.path.exists(exe):
         return True
-    srcs = [os.path.join(NATIVE, name + ".cu"), os.path.join(NATIVE, "probe.h")] + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if os.path.isfile(os.path.join(CSRC, f))]
+    srcs = [os.path.join(NATIVE, name + ".cu")] + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if os.path.isfile(os.path.join(CSRC, f))]
     return os.path.getmtime(exe) < max(os.path.getmtime(p) for p in srcs)
 
 

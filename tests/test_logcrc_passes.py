@@ -3,24 +3,21 @@ their scan, log_crc_span_kernel (each warp a contiguous run of the call's spans,
 from the batch ends behind the warp's current batch, computes its span's register and moves it to the batch's end; the lanes
 of one batch xor-combine their shares before one atomic) and the header pass's verdict.
 
-tests/native/logcrc_probe.cu launches what log_headers launches for a handle with check.crcs on, through the same launch
-functions, and returns spans[0..nbatches], acc[b] for every batch, every batch's flags, the failure list and the header pass's
-error words.  Each case compares all of them with crc_contract(), a numpy restatement of the stage's contract: a framed batch
+tests/native/log_probe.cu runs scan_log_batches' steps (kta_logscan.cuh) for a handle with check.crcs on and returns
+spans[0..nbatches], acc[b] for every batch, every batch's flags, the failure list and the header pass's error words.  Each case compares all of them with crc_contract(), a numpy restatement of the stage's contract: a framed batch
 that is served has ceil((12 + batchLength - 21) / 1024) spans and acc = its plain CRC-32C ^ 0xFFFFFFFF, every other batch 0
 spans and acc 0.  The plain CRC is kafka_codec's byte loop, run in lockstep over many regions with numpy, or the probe's host
 mode for large regions; test_plain_crcs_agree pins them to each other.  The probe can also run the span pass on a grid of
 one block (32 warps): the pass's body does not depend on its grid, so every warp then reaches many rounds with few spans.
 A case built to reach an edge (a gap of unserved batches at lane j of round r of warp w) asserts from the spans that it does."""
 import struct
-import subprocess
-import threading
 from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
 import kafka_codec as kc
-import native_build
+import log_probe
 
 SPAN, FROM, THREADS = 1024, 21, 1024                          # LOG_CRC_SPAN, LOG_CRC_FROM, LOG_CRC_THREADS
 LOGB_SKIP_CONTROL, LOGB_BAD, LOGB_COMPRESSED, LOGB_CODECS = 1, 2, 4, 8 | 16 | 32 | 64
@@ -34,11 +31,6 @@ NEVER = 1 << 40                                                # a log start off
 KS = (1, 2, 3, 31, 32, 33, 64, 1000)                           # gap sizes (unserved batches in a row)
 PERS = (1, 2, 31, 32, 33, 2048)                                # spans per warp with the one-block grid (2048: 64 rounds)
 _T = np.array(kc._CRC32C, np.uint32)
-
-
-@pytest.fixture(scope="module")
-def probe():
-    return native_build.build("logcrc_probe")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -67,19 +59,7 @@ def crc32c_lockstep(regions):
 
 def host_crcs(regions):
     """the probe's host mode (plain C++, no CUDA): the CRC-32C of every region"""
-    p = subprocess.Popen([native_build.build("logcrc_probe"), "host"], stdin=subprocess.PIPE, stdout=subprocess.PIPE)
-
-    def feed():
-        for r in regions:
-            p.stdin.write(struct.pack("<Q", len(r)))
-            p.stdin.write(memoryview(np.ascontiguousarray(r, np.uint8)))
-        p.stdin.close()
-    t = threading.Thread(target=feed)
-    t.start()
-    out = p.stdout.read()
-    t.join()
-    assert p.wait() == 0
-    return np.frombuffer(out, "<u4").astype(np.uint32)
+    return log_probe.crc32c(regions)
 
 
 def plain_crcs(regions, large=1 << 16):
@@ -247,54 +227,12 @@ def regrid(c, grid):
 # ------------------------------------------------------------------------------------------------
 # the probe
 # ------------------------------------------------------------------------------------------------
-def _pieces(c):
-    nb = c.offs.size
-    yield struct.pack("<Q", c.data.size)
-    yield c.data
-    yield struct.pack("<I", nb)
-    yield c.offs.astype("<u8")
-    yield struct.pack("<I", c.parts is not None)
-    if c.parts is not None:
-        yield c.parts.astype("<i4")
-    yield struct.pack("<II", c.slack, len(c.win))
-    yield np.array(c.win, "<i8").reshape(-1)
-    yield struct.pack("<I", c.grid)
-
-
-def run_probe(exe, cases):
-    p = subprocess.Popen([exe], stdin=subprocess.PIPE, stdout=subprocess.PIPE, stderr=subprocess.PIPE)
-
-    def feed():
-        try:
-            for c in cases:
-                for x in _pieces(c):
-                    p.stdin.write(memoryview(np.ascontiguousarray(x)) if isinstance(x, np.ndarray) else x)
-            p.stdin.close()
-        except BrokenPipeError:
-            pass
-    t = threading.Thread(target=feed)
-    t.start()
-    out = p.stdout.read()
-    t.join()
-    err = p.stderr.read()
-    assert p.wait() == 0, err.decode("utf-8", "replace")[-3000:]
-    at = 4
-    sm_count = struct.unpack_from("<I", out)[0]
-
-    def take(dt, n):
-        nonlocal at
-        a = np.frombuffer(out, dt, n, at)
-        at += a.nbytes
-        return a
-    res = []
-    for c in cases:
-        nb = c.offs.size
-        g = SimpleNamespace(sm_count=sm_count, grid=int(take("<u4", 1)[0]))
-        g.spans, g.acc, g.flags, g.err = take("<u8", nb + 1), take("<u4", nb), take("<u4", nb), take("<u4", 10)
-        g.fails = take(FAIL, int(g.err[2]))
-        res.append(g)
-    assert at == len(out)
-    return res
+def spans(cases):
+    """the cases through the library's steps with check.crcs on (log_probe) → per case the passes' arrays"""
+    sm_count = log_probe.device()[0]
+    ins = [log_probe.inputs(c.data, c.offs, c.parts, c.slack, c.win, check_crcs=True, span_grid=c.grid) for c in cases]
+    return [SimpleNamespace(sm_count=sm_count, grid=int(r.crc_grid[0]), spans=r.spans, acc=r.acc, flags=r.flags, err=r.word,
+                            fails=np.sort(r.crc_fails, order="batch").astype(FAIL)) for r in log_probe.run(ins)]
 
 
 def check(c, g, want=None):
@@ -317,9 +255,9 @@ def check(c, g, want=None):
     return w
 
 
-def probe_all(probe, cases):
+def probe_all(cases):
     out = []
-    for c, g in zip(cases, run_probe(probe, cases)):
+    for c, g in zip(cases, spans(cases)):
         out.append((c, g, check(c, g)))
     return out
 
@@ -504,22 +442,22 @@ def test_gap_layouts_reach_their_edges():
 # ------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 @pytest.mark.parametrize("P", PERS)
-def test_gaps_at_lookahead_and_run_edges(probe, P):
+def test_gaps_at_lookahead_and_run_edges(P):
     """gaps of 1 to 1000 unserved batches at every lane, at the ends of every warp's run, and at the call's ends, with
     one-span batches (a round of one-span batches covers 32 batches, 33 with one empty batch in it), through the one-block
     grid and the library's grid"""
     cases = [c for k in KS for c in gap_cases(P, k)]
-    for c, g, w in probe_all(probe, cases + [regrid(c, 0) for c in cases]):
+    for c, g, w in probe_all(cases + [regrid(c, 0) for c in cases]):
         assert int(g.err[7]) == int(w.skip.sum()) > 0
 
 
 @pytest.mark.gpu
-def test_gap_layouts_on_the_library_grid(probe):
+def test_gap_layouts_on_the_library_grid():
     """the partition seam (100 batches of partition 0, then 40 of partition 1 below its log start offset, then 100 served),
     the library's grid capped at the SM count with gaps of two, several warps per batch, every batch unserved"""
     cases = [seam_case(), saturated_case(), multi_span_case(), all_unserved_case()]
     cases.append(regrid(cases[2], 0))
-    res = probe_all(probe, cases)
+    res = probe_all(cases)
     c, g, w = res[0]
     assert g.grid == 1 and -(-int(w.spans[-1]) // 32) == 7
     assert [where[1:3] for n, where, _ in gaps(w, 32) if where] == [(0, 2)]     # the seam at lane 2 of warp 14's round
@@ -538,7 +476,7 @@ def test_gap_layouts_on_the_library_grid(probe):
 
 
 @pytest.mark.gpu
-def test_region_lengths(probe):
+def test_region_lengths():
     """every CRC region of 40 to 2 * 1024 + 64 bytes; k * 1024 - 1, k * 1024 and k * 1024 + 1 bytes for k around 4096 (where a
     span's power of x starts to take a pow_hi factor) and around 8192 (pow_hi[2]); both grids"""
     rng = np.random.default_rng(11)
@@ -548,13 +486,13 @@ def test_region_lengths(probe):
     cases = [case("lengths 40..2112", pool, rng.permutation(small), bases=np.arange(small.size)),
              case("lengths around 4096 and 8192 spans", pool, np.concatenate([big, small[:50]]), bases=np.arange(big.size + 50))]
     cases += [regrid(c, 1) for c in cases]
-    res = probe_all(probe, cases)
+    res = probe_all(cases)
     w = res[1][2]
     assert int(w.nspans.max()) == 8194 and {4095, 4096, 4097, 8192, 8193}.issubset(set(w.nspans.tolist()))
 
 
 @pytest.mark.gpu
-def test_largest_batch(probe):
+def test_largest_batch():
     """one batch with batchLength = 2^31 - 1 (2^21 spans: the last pow_hi entry), a batch without records followed by
     unread bytes, between two small ones.  The file's largest cost: on an H100 the test process peaked at 4.3 GiB of host
     memory and the device at 2.5 GiB."""
@@ -572,12 +510,12 @@ def test_largest_batch(probe):
     pool.crc = np.concatenate([pool.crc, [crc]]).astype(np.uint32)
     c = case("batchLength 2^31 - 1", pool, [small[0], len(pool.raw) - 1, small[1]], bases=[0, 1, 2])
     del raw
-    (c2, g, w), = probe_all(probe, [c])
+    (c2, g, w), = probe_all([c])
     assert int(w.nspans[1]) == 1 << 21 and int(g.err[2]) == 0
 
 
 @pytest.mark.gpu
-def test_alignment(probe):
+def test_alignment():
     """batch offsets at every residue mod 16 times CRC regions at every residue mod 64, of one span and of three: every
     head, 64-byte, 16-byte and tail path of crc_span, for the first span of a batch and the later ones; both grids"""
     rng = np.random.default_rng(13)
@@ -596,11 +534,11 @@ def test_alignment(probe):
     for one in (True, False):
         sel = (lens - FROM <= SPAN) == one
         assert len(set(zip((c.offs[sel] % 16).tolist(), ((lens[sel] - FROM) % 64).tolist()))) == 16 * 64
-    probe_all(probe, [c, regrid(c, 1)])
+    probe_all([c, regrid(c, 1)])
 
 
 @pytest.mark.gpu
-def test_verdicts(probe):
+def test_verdicts():
     """stored CRC equal and one bit off; a failed batch that is not served (not reported); a cut batch (checked whole);
     compressed batches of every codec (checked over their stored bytes); control batches"""
     rng = np.random.default_rng(14)
@@ -622,14 +560,14 @@ def test_verdicts(probe):
                 bad.append(len(tidx))
             tidx.append(x)
     c = case("verdicts", pool, tidx, bases=bases, parts=parts, win=win, bad=bad)
-    (c, g, w), = probe_all(probe, [c])
+    (c, g, w), = probe_all([c])
     n = len(t)
     assert w.fail.tolist() == [k == 1 for _ in t for k in range(4)]
     assert int(g.err[6]) == n - 1 and int(g.err[7]) == n + 1  # every data batch cut once; the marker's last is below S
 
 
 @pytest.mark.gpu
-def test_single_bit_damage(probe):
+def test_single_bit_damage():
     """3000 single-bit flips, each in its own batch, at random positions of the CRC region or the stored CRC field: exactly
     the damaged batches fail, each with the plain CRC of its damaged bytes as computed"""
     rng = np.random.default_rng(15)
@@ -641,12 +579,12 @@ def test_single_bit_damage(probe):
     pos = c.offs[hit].astype(np.int64) + 17 + (rng.random(hit.size) * (lens[hit] - 17)).astype(np.int64)
     c.data[pos] ^= (1 << rng.integers(0, 8, hit.size)).astype(np.uint8)
     c.crcs = None                                              # the contract computes the CRC of the damaged bytes
-    (c, g, w), = probe_all(probe, [c])
+    (c, g, w), = probe_all([c])
     assert np.array_equal(np.flatnonzero(w.fail), hit)
 
 
 @pytest.mark.gpu
-def test_at_depth(probe):
+def test_at_depth():
     """the library's grid at its cap with every warp at least 64 rounds of 32 spans: ~9 million one-span batches (about
     0.5 GB, tiled from 64 templates), in partitions of 1000 to 3000 batches whose log start offsets leave out their first 1
     to 40 batches, so gaps sit at every partition seam"""
@@ -676,7 +614,7 @@ def test_at_depth(probe):
     data[at[unserved] + 20] ^= 0x40                            # (and their stored CRCs are wrong)
     c = SimpleNamespace(name="depth", data=data, offs=offs, parts=parts, slack=0, win=[(int(s), -1) for s in skipped], grid=0,
                         crcs=np.tile(pool.crc[tmpl[block]], reps))
-    (c, g, w), = probe_all(probe, [c])
+    (c, g, w), = probe_all([c])
     per = -(-int(w.spans[-1]) // (32 * g.grid))
     assert g.grid == g.sm_count and per >= 64 * 32, (g.grid, per)
     assert int(g.err[7]) == int(unserved.sum()) and int(g.err[2]) == 0

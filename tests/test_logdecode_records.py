@@ -2,21 +2,20 @@
 lane 0 hops 32 record-length varints, then 32 lanes parse), the key-length tile bases and log_gather_keys_kernel — checked
 record by record.
 
-tests/native/logdecode_probe.cu launches what scan_log_batches launches up to the scan, through the same launch functions
-(kta_logdecode_launch.cuh), and returns every decoded column.  Every case compares partition, ts_ms, key_len and value_len of
-every record, the tile-base column (the running sum of max(key_len, 0) per 128-record tile) and the packed key bytes with the
-records the case was built from, after the consumer's rules (control and empty batches are not delivered; LogAppendTime
-stamps maxTimestamp; a timestamp is baseTimestamp + timestampDelta).  The metrics behind the scan would hide most of these
+tests/native/log_probe.cu runs scan_log_batches' steps up to the scan (kta_logscan.cuh) and returns every decoded column.
+Every case compares partition, ts_ms, key_len and value_len of every record, the tile-base column (the running sum of
+max(key_len, 0) per 128-record tile) and the packed key bytes with the records the case was built from, after the
+consumer's rules (control and empty batches are not delivered; LogAppendTime stamps maxTimestamp; a timestamp is
+baseTimestamp + timestampDelta).  The metrics behind the scan would hide most of these
 errors (a timestamp that is not an extreme, value lengths shifted inside one partition)."""
 import struct
-import subprocess
 from collections import namedtuple
 
 import numpy as np
 import pytest
 
 import kafka_codec as kc
-import native_build
+import log_probe
 
 TS0 = 1_700_000_000_000
 LOGB_BAD = 2
@@ -25,11 +24,6 @@ FILL32, FILL64 = np.int32(-0x5A5A5A5B), np.int64(-0x5A5A5A5A5A5A5A5B)   # 0xA5 b
 # words, windowed, flags, drop: the window mode's outputs (cases with a window table, tests/test_logoffsets_records.py)
 Result = namedtuple("Result", "hdr longest unc_err dec_err nrec staged stage grid ran part ts klen vlen tile_base keys "
                               "words windowed flags drop", defaults=(None,) * 4)
-
-
-@pytest.fixture(scope="module")
-def probe():
-    return native_build.build("logdecode_probe")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -78,14 +72,6 @@ class Case:
             got = [r for b, _ in batches for r in kc.delivered(b)]
             assert [(ts, key, -1 if vl is None else vl) for _, ts, key, vl in got] == [r[1:] for r in want], name
 
-    def blob(self):
-        nb = len(self.offs)
-        out = struct.pack("<I", len(self.data)) + self.data + struct.pack("<I", nb) + np.array(self.offs, "<u8").tobytes()
-        out += struct.pack("<I", 1) + np.array(self.parts, "<i4").tobytes() if self.parts else struct.pack("<I", 0)
-        out += struct.pack("<I", self.slack)
-        win = np.zeros((0, 2)) if self.win is None else self.win
-        return out + struct.pack("<I", len(win)) + np.asarray(win, "<i8").reshape(-1).tobytes()
-
 
 Cols = namedtuple("Cols", "part ts klen vlen keys")
 
@@ -102,35 +88,23 @@ def tile_base(klen):
     return np.concatenate([[0], np.cumsum(t)]).astype(np.uint64)
 
 
-def run_probe(exe, cases):
-    blob = b"".join(c.blob() for c in cases)
-    r = subprocess.run([exe], input=blob, capture_output=True)
-    assert r.returncode == 0, r.stderr.decode("utf-8", "replace")[-3000:]
-    out = r.stdout
-    sm, optin = struct.unpack_from("<II", out, 0)
-    at, res = 8, []
-    def take(dt, n):
-        nonlocal at
-        a = np.frombuffer(out, dt, n, at)
-        at += a.nbytes
-        return a
-    for c in cases:
-        hdr0, longest, unc, dec, nrec, staged, stage, grid, ran = struct.unpack_from("<IIIIQIIII", out, at)
-        at += 40
-        part = ts = klen = vlen = tb = keys = words = windowed = flags = drop = None
+def decode(cases):
+    """the cases through the library's steps (log_probe) → ((SM count, opt-in shared memory), a Result per case)"""
+    res = []
+    for c, r in zip(cases, log_probe.run([log_probe.inputs(c.data, c.offs, c.parts or None, c.slack, () if c.win is None else c.win) for c in cases])):
+        w, nb = r.word, len(c.offs)
+        ran = r.get("part") is not None
+        nrec = len(r.part) if ran else int(r.cnt[-1])
+        keys = r.get("keys")
+        extra = ()
         if c.win is not None and len(c.win):
-            w = take("<u4", 5)
-            words, windowed = (int(w[0]), int(w[1]), int(w[2]) | int(w[3]) << 32), int(w[4])
-            flags, drop = take("<u4", len(c.offs)), take("<u8", len(c.offs) + 1)
-        if ran:
-            part, ts, klen, vlen = take("<i4", nrec), take("<i8", nrec), take("<i4", nrec), take("<i4", nrec)
-            if not dec and nrec:
-                tb = take("<u8", (nrec + 127) // 128 + 1)
-                keys = take("u1", int(tb[-1]) + 64).tobytes()
-        res.append(Result(hdr0, longest, unc, dec, nrec, staged, stage, grid, ran, part, ts, klen, vlen, tb, keys, words, windowed,
-                          flags, drop))
-    assert at == len(out)
-    return (sm, optin), res
+            drop = r.get("drop")
+            extra = ((int(w[6]), int(w[7]), int(w[8]) | int(w[9]) << 32), int(r.get("windowed", [0])[0]), r.flags,
+                     np.zeros(nb + 1, np.uint64) if drop is None else drop)
+        res.append(Result(int(w[0]), int(w[1]), int(r.get("size_flags", [0])[0]), int(r.get("dec_flags", [0])[0]), nrec,
+                          *(int(x) for x in r.shape), int(ran), r.get("part"), r.get("ts"), r.get("klen"), r.get("vlen"),
+                          r.get("tile_base"), None if keys is None else keys.tobytes(), *extra))
+    return log_probe.device(), res
 
 
 def decode_shape(longest, nbatches, sm_count, optin):
@@ -307,9 +281,9 @@ def hand_built():
 
 
 @pytest.mark.gpu
-def test_hand_built_cases_decode_record_by_record(probe):
+def test_hand_built_cases_decode_record_by_record():
     cases = hand_built()
-    (sm, optin), res = run_probe(probe, cases)
+    (sm, optin), res = decode(cases)
     for c, r in zip(cases, res):
         staged, stage, _, grid = decode_shape(r.longest, len(c.offs), sm, optin)
         assert (r.staged, r.stage, r.grid) == (staged, stage, grid), c.name
@@ -370,13 +344,13 @@ def tiled(pool, nbatches, rng):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", ["small-batches", "stage-48k"])
-def test_every_warp_decodes_many_batches(probe, shape):
+def test_every_warp_decodes_many_batches(shape):
     """Every warp of the decode grid decodes >= 64 batches, so each one's mbarrier phase flips many times, stages are reused
     after __syncwarp, and staged and in-place batches alternate within one warp."""
     rng = np.random.default_rng(71 if shape == "small-batches" else 73)
     big = 49136 if shape == "stage-48k" else None
     pool = pool_batches(rng, big)
-    (sm, optin), _ = run_probe(probe, [])
+    sm, optin = log_probe.device()
     longest = max(len(b) for kind, (b, _) in pool if kind == "S")
     staged, stage, per_sm, grid = decode_shape(longest, 1 << 40, sm, optin)
     assert staged and per_sm == (16 if shape == "small-batches" else 1)
@@ -387,7 +361,7 @@ def test_every_warp_decodes_many_batches(probe, shape):
     kinds = [pool[(w + j * warps) % len(pool)][0] for w in range(warps) for j in range(64)]
     seqs = ["".join(k for k in kinds[w * 64:(w + 1) * 64] if k != "-") for w in range(warps)]
     assert sum("SPS" in s for s in seqs) > warps // 4
-    _, (r,) = run_probe(probe, [case])
+    _, (r,) = decode([case])
     assert (r.staged, r.stage, r.grid) == (staged, stage, grid)
     print("%s: %d batches, %d records, %d warps, %.1f batches per warp" % (shape, nb, r.nrec, warps, nb / warps))
     check(case, r)
@@ -501,11 +475,11 @@ def damaged_cases():
 
 
 @pytest.mark.gpu
-def test_damaged_record_sections_agree_with_the_contract(probe):
+def test_damaged_record_sections_agree_with_the_contract():
     """Each mutated batch is refused exactly when the plain restatement of the decoder's contract refuses it, and otherwise
     decodes to that restatement's columns.  One probe run carries every case."""
     cases = damaged_cases()
-    _, res = run_probe(probe, cases)
+    _, res = decode(cases)
     disagree = []
     for c, r in zip(cases, res):
         refused = bool(r.hdr & LOGB_BAD or r.unc_err or r.dec_err)

@@ -1,16 +1,14 @@
 """The GPU decompression stage of the RecordBatch decoder (log_decompress_kernel: gzip, LZ4, Snappy, zstd; one warp per batch,
 32 lanes sharing the copies, the Huffman table fill and the Huffman streams) against the reference codecs, byte for byte.
 
-tests/native/logdecomp_probe.cu launches what scan_log_batches launches up to the record decode, through the same launch
-functions, and returns every batch's rewritten image.  For every batch that image must equal the same batch encoded
+tests/native/log_probe.cu runs scan_log_batches' steps (kta_logscan.cuh) through the size and copy steps, and returns every
+batch's rewritten image.  For every batch that image must equal the same batch encoded
 uncompressed (kafka_codec: byte-identical apart from batchLength and the codec bits), and its scratch slot must be that
 length rounded up to 16.  The host tests run the same walks with one lane; the scan afterwards never reads value bytes,
 header bytes or offset deltas, so this is where the lane-split output is checked.  Damaged sections must be accepted or
 rejected as the host walks (one lane) accept or reject them, with the same bytes.  One more test sends batches whose every
 decompressed byte the scan sees is a key byte through the product's entry points and compares the per-record key hashes."""
 import gzip
-import struct
-import subprocess
 import zlib
 
 import numpy as np
@@ -18,6 +16,7 @@ import pytest
 
 import codec_harness as ch
 import kafka_codec as kc
+import log_probe
 import native_build
 import np_oracle
 import test_inflate_host as ih
@@ -32,29 +31,20 @@ LOGB_OK, LOGB_BAD = 0, 2
 STRATEGIES = (zlib.Z_DEFAULT_STRATEGY, zlib.Z_FIXED, zlib.Z_HUFFMAN_ONLY, zlib.Z_RLE, zlib.Z_FILTERED)
 
 
-@pytest.fixture(scope="module")
-def probe():
-    return native_build.build("logdecomp_probe")
-
-
-def run_probe(exe, segments):
-    """segments: list of bytes (whole record batches each, one launch group per segment) → per segment, per batch
-    (flags, slot size, image)"""
-    blob = b"".join(struct.pack("<I", len(s)) + s for s in segments)
-    r = subprocess.run([exe], input=blob, capture_output=True)
-    assert r.returncode == 0, r.stderr.decode("utf-8", "replace")[-3000:]
-    out, at, res = r.stdout, 0, []
-    for _ in segments:
-        nb, = struct.unpack_from("<I", out, at)
-        at += 4
+def decompress(segments):
+    """segments: list of bytes (whole record batches each, found by the host walk; one call per segment, in a buffer with 64
+    bytes of slack), the size and copy steps run even where the library stops before or between them → per segment, per
+    batch (flags, slot size, image)"""
+    res = []
+    for seg, r in zip(segments, log_probe.run([log_probe.inputs(s, slack=64, decompress=True) for s in segments])):
+        assert r.get("info") is not None, (r.rc, r.msg)
+        slot, unc_at = np.diff(r.slot.astype(np.int64)), int(r.unc_at[0])
         batches = []
-        for _ in range(nb):
-            flags, slot, n = struct.unpack_from("<IQI", out, at)
-            at += 16
-            batches.append((flags, slot, out[at:at + n]))
-            at += n
+        for bi, size in zip(r.info, slot):
+            n = int(bi["len"]) if bi["flags"] == LOGB_OK else 0
+            at = (int(bi["off"]) - unc_at) % (1 << 64) if size else int(bi["off"])   # (a decompressed image lies in the scratch)
+            batches.append((int(bi["flags"]), int(size), bytes((r.unc if size else np.frombuffer(seg, np.uint8))[at:at + n])))
         res.append(batches)
-    assert at == len(out)
     return res
 
 
@@ -203,15 +193,15 @@ def check_images(items, got):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("corpus", sorted(CORPORA))
-def test_decompressed_images_match_the_reference_codecs(probe, corpus):
+def test_decompressed_images_match_the_reference_codecs(corpus):
     items = CORPORA[corpus]()
     assert all(c[22] & 7 for _, c, _ in items)
-    got = run_probe(probe, [b"".join(c for _, c, _ in items)])[0]   # every batch of the corpus in one launch group
+    got = decompress([b"".join(c for _, c, _ in items)])[0]   # every batch of the corpus in one launch group
     check_images(items, got)
 
 
 @pytest.mark.gpu
-def test_many_batches_per_launch(probe):
+def test_many_batches_per_launch():
     """more small batches than the warps of the decompression grid (132 SMs x 16 CTAs x 4 warps), every codec interleaved
     (uncompressed ones too): the grid-stride loop wraps, and the warps of one CTA run different codecs side by side"""
     rng = np.random.default_rng(53)
@@ -224,7 +214,7 @@ def test_many_batches_per_launch(probe):
         codec = codecs[b % len(codecs)]
         comp = kc.recompress(unc, lambda: codec)
         items.append(("batch-%d/%s" % (b, codec), comp, unc, codec))
-    got = run_probe(probe, [b"".join(c for _, c, _, _ in items)])[0]
+    got = decompress([b"".join(c for _, c, _, _ in items)])[0]
     assert len(got) == len(items)
     bad = [name for (name, _, unc, codec), (flags, slot, img) in zip(items, got)
            if flags != LOGB_OK or img != unc or slot != (0 if codec is None else (len(unc) + 15) & ~15)]
@@ -232,13 +222,13 @@ def test_many_batches_per_launch(probe):
 
 
 @pytest.mark.gpu
-def test_damaged_sections_agree_with_the_host_walks(probe):
+def test_damaged_sections_agree_with_the_host_walks():
     """The damaged sections of the host tests (900 zstd frames, 1200 gzip / LZ4 / Snappy sections), once, in one launch: the
     GPU accepts exactly the ones the host walk accepts, with the same bytes.  recordsCount is 0, so that only the walks decide."""
     cases = [(kc.CODEC_BITS["zstd"], f) for f in zh.damaged_frames()] + lh.damaged_sections()
     host = ch.run_cases(native_build.build("codec_harness"), cases)
     base = payload_batch(b"")
-    got = run_probe(probe, [b"".join(with_section(base, s, c) for c, s in cases)])[0]
+    got = decompress([b"".join(with_section(base, s, c) for c, s in cases)])[0]
     assert len(got) == len(cases)
     disagree = []
     for i, ((ok, _, out), (flags, slot, img)) in enumerate(zip(host, got)):

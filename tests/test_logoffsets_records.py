@@ -2,8 +2,8 @@
 pass, log_cut_count_kernel (warp per cut batch: how many rows each cut batch gets) and log_decode_window_kernel (the kept
 records ranked by a ballot and a popcount, plus a carry across lane rounds).
 
-tests/native/logdecode_probe.cu, given a window table, launches what scan_log_batches launches for a handle with windows,
-through the same launch functions, and returns every decoded column, every batch's flags after the header pass, the count
+tests/native/log_probe.cu, given a window table, runs scan_log_batches' steps (kta_logscan.cuh) for a handle with windows
+and returns every decoded column, every batch's flags after the header pass, the count
 pass's drops and the header pass's window words.  Each case compares them with window_contract(), a plain restatement on top
 of test_logdecode_records.contract(): a batch's verdict (not served / served / cut) comes from baseOffset and the stored
 lastOffsetDelta alone; records below the log start offset S are dropped only from cut batches (baseOffset < S); offsets are
@@ -16,10 +16,10 @@ import numpy as np
 import pytest
 
 import kafka_codec as kc
-import native_build
+import log_probe
 import offsets_codec as oc
-from test_logdecode_records import (TS0, Case, Cols, batch_of_length, check, columns, contract, decode_shape, i64, key,
-                                    run_probe)
+from test_logdecode_records import (TS0, Case, Cols, batch_of_length, check, columns, contract, decode, decode_shape, i64,
+                                    key)
 
 LOGB_BAD, LOGB_SKIP_OFFSET = 2, 512
 CODECS = (None, "gzip", "snappy", "snappy-xerial", "lz4", "zstd", "zstd-stream")   # test_log_offsets.CODECS
@@ -27,11 +27,6 @@ CODECS = (None, "gzip", "snappy", "snappy-xerial", "lz4", "zstd", "zstd-stream")
 # rows it gets, whether it is not served, whether it is cut and how many records it drops; the header pass's words [6..9]
 # as (cut batches, batches not served, their data records)
 WinWant = namedtuple("WinWant", "recs counts skip cut drops words")
-
-
-@pytest.fixture(scope="module")
-def probe():
-    return native_build.build("logdecode_probe")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -343,9 +338,9 @@ def test_negative_delta_rule():
 
 # ---- GPU: the hand-built cases -------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_hand_built_window_cases_decode_record_by_record(probe):
+def test_hand_built_window_cases_decode_record_by_record():
     cases = hand_built()
-    (sm, optin), res = run_probe(probe, cases)
+    (sm, optin), res = decode(cases)
     for c, r in zip(cases, res):
         staged, stage, _, grid = decode_shape(r.longest, len(c.offs), sm, optin)
         assert (r.staged, r.stage, r.grid) == (staged, stage, grid), c.name
@@ -424,12 +419,12 @@ def depth_case(pool, idx, name):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", ["small-batches", "stage-48k"])
-def test_every_warp_counts_and_decodes_many_cut_batches(probe, shape):
+def test_every_warp_counts_and_decodes_many_cut_batches(shape):
     """Every warp of the count pass takes >= 64 cut batches (one per partition, next to batches not served and batches
     served whole), and every warp of the window decode >= 64 batches, going staged -> in place -> staged."""
     rng = np.random.default_rng(103 if shape == "small-batches" else 107)
     pool = depth_pool(rng, 49136 if shape == "stage-48k" else None)
-    (sm, optin), _ = run_probe(probe, [])
+    sm, optin = log_probe.device()
     k = len(pool) - (1 if shape == "stage-48k" else 0)
     cut_per = sum(p[0] in "CZ" for p in pool[:k])
     count_warps = 4 * sm * 16
@@ -445,7 +440,7 @@ def test_every_warp_counts_and_decodes_many_cut_batches(probe, shape):
     kinds = np.array([{"C": "S", "W": "S", "B": "S", "Z": "P"}.get(pool[t][0], "-") for t in range(len(pool))])[idx]
     seqs = ["".join(k for k in kinds[w::warps][:64] if k != "-") for w in range(warps)]
     assert sum("SPS" in s for s in seqs) > warps // 4
-    _, (r,) = run_probe(probe, [case])
+    _, (r,) = decode([case])
     assert (r.staged, r.stage, r.grid) == (staged, stage, grid)
     ncut = r.words[0]
     cgrid = min((ncut + 3) // 4, sm * 16)
@@ -518,11 +513,11 @@ def damaged_cases():
 
 
 @pytest.mark.gpu
-def test_damaged_cut_batches_agree_with_the_contract(probe):
+def test_damaged_cut_batches_agree_with_the_contract():
     """Each mutated cut batch is refused exactly when window_contract refuses it, and otherwise decodes to its columns,
     flags, drops and words.  One probe run carries every case."""
     cases = damaged_cases()
-    _, res = run_probe(probe, cases)
+    _, res = decode(cases)
     disagree = []
     for c, r in zip(cases, res):
         if refused(r) != (c.want is None):

@@ -2,22 +2,21 @@
 txn_resolve_kernel (a warp-shuffle scan from the right, then across the warps of a 256-key tile), txn_carry_kernel (one block
 over chunks of 1024 tiles, from the last chunk down) and txn_apply_kernel with its binary search of the aborted ranges.
 
-tests/native/logtxn_probe.cu launches what log_headers launches for a read_committed handle, through the same launch functions,
-and returns every array the passes produce: the error word, the sorted keys, kind per batch, res per key, tile_head and carry
+tests/native/log_probe.cu runs scan_log_batches' steps (kta_logscan.cuh) for a read_committed handle and returns every array
+the passes produce: the error word, the sorted keys, kind per batch, res per key, tile_head and carry
 per tile, every batch's flags, records and row count, and the three counters.  Each case compares them with txn_contract(), a
 plain restatement of the rule of include/kta.h over (partition, producerId, baseOffset, kind) per batch; it knows nothing of
 warps, and of tiles only where res is cut at a tile's end.  A case that is built to reach an edge (a chain behind six all-PASS
 warps, a group that ends on the last key of a carry chunk) asserts from the sorted keys that it does.  The scan's metrics
 behind these passes say that some verdict was wrong; these arrays say which key, in which pass."""
 import struct
-import subprocess
 from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
 import kafka_codec as kc
-import native_build
+import log_probe
 from feed import LOG_ENTRIES, scan_log
 from kafka_topic_analyzer_b200 import KtaEngine
 from parity import assert_parity, oracle_in_order
@@ -33,11 +32,6 @@ NOPID = (1 << 64) - 1                                              # producerId 
 D, A, C, N, X, B = DATA, ABORT, COMMIT, 10, 11, 12
 RANGE = np.dtype([("part", "<i4"), ("pad", "<u4"), ("pid", "<u8"), ("first", "<i8"), ("last", "<i8")])   # TxnRange
 KEY = np.dtype([("pid", "<u8"), ("part", "<u4"), ("batch", "<u4")])                                        # TxnKey
-
-
-@pytest.fixture(scope="module")
-def probe():
-    return native_build.build("logtxn_probe")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -234,34 +228,19 @@ def finish(c):
     return c
 
 
-def blob(c):
-    buf = build_batches(c.code, c.pid, c.off, c.keyid)
-    n = len(c.code)
-    return b"".join([struct.pack("<I", buf.size), buf.tobytes(), struct.pack("<I", n), (np.arange(n, dtype="<u8") * BL).tobytes(),
-                     c.part.astype("<i4").tobytes(), struct.pack("<I", len(c.ranges)), c.ranges.tobytes()])
-
-
-def run_probe(exe, cases):
-    r = subprocess.run([exe], input=b"".join(blob(c) for c in cases), capture_output=True)
-    assert r.returncode == 0, r.stderr.decode("utf-8", "replace")[-3000:]
-    out, at, res = r.stdout, 4, []
-
-    def take(dt, n):
-        nonlocal at
-        a = np.frombuffer(out, dt, n, at)
-        at += a.nbytes
-        return a
-    for c in cases:
-        nb = len(c.code)
-        g = SimpleNamespace()
-        g.hdr, g.keys, g.err, g.ran = (int(x) for x in take("<u4", 4))
-        g.stats, g.nrec = tuple(int(x) for x in take("<u8", 3)), int(take("<u8", 1)[0])
-        g.kind, g.flags, g.records, g.cnt = take("u1", nb), take("<u4", nb), take("<i4", nb), take("<u8", nb + 1)
+def passes(cases):
+    """the cases through the library's steps on a read_committed handle (log_probe) → per case the passes' arrays"""
+    res = []
+    ins = [log_probe.inputs(build_batches(c.code, c.pid, c.off, c.keyid).reshape(-1), np.arange(len(c.code)) * BL, c.part,
+                            ranges=c.ranges, read_committed=True) for c in cases]
+    for c, r in zip(cases, log_probe.run(ins)):
+        g = SimpleNamespace(rc=r.rc, msg=r.msg, hdr=int(r.word[0]), keys=int(r.txn_word[0]), err=int(r.txn_word[1]),
+                            ran=int(r.txn_ran[0]), stats=tuple(int(x) for x in r.txn_stats), nrec=int(r.nrec[0]), kind=r.kind,
+                            flags=r.flags, records=r.records, cnt=r.cnt)
         if g.ran:
             nt = -(-g.keys // TILE)
-            g.sorted, g.res, g.tile_head, g.carry = take(KEY, g.keys), take("u1", g.keys), take("u1", nt), take("u1", nt)
+            g.sorted, g.res, g.tile_head, g.carry = r.sorted, r.res, r.tile[:nt], r.tile[nt:]
         res.append(g)
-    assert at == len(out)
     return res
 
 
@@ -303,12 +282,20 @@ def check(c, g):
         first_bad(c, "tile_head", g.tile_head, w.tile_head, None)
         first_bad(c, "carry", g.carry, w.carry, None)
         assert g.err == w.err, (c.name, "error word", g.err, w.err)
+        if w.err:
+            assert g.rc == log_probe.KTA_ERR_INVALID and "increasing baseOffset order" in g.msg, (c.name, g.rc, g.msg)
     refused = c.bad_marker or w.err
     first_bad(c, "flags", g.flags, np.where(w.aborted & (not refused), LOGB_SKIP_ABORTED, flags0), False)
     first_bad(c, "records", g.records, c.records0 if refused else w.records, False)
-    first_bad(c, "rec_count", g.cnt, np.append(0, c.records0 if refused else w.records).astype(np.uint64), False)
+    if c.bad_marker:
+        # refused before the record-count scan: the counts are the header pass's rows, unscanned
+        assert g.rc == log_probe.KTA_ERR_INVALID and "unreadable transaction marker" in g.msg, (c.name, g.rc, g.msg)
+        rows = g.cnt[1:]
+    else:
+        rows = np.diff(g.cnt)
+        assert int(g.cnt[-1]) == g.nrec == int((c.records0 if refused else w.records).sum()), c.name
+    first_bad(c, "rec_count", rows, (c.records0 if refused else w.records).astype(np.uint64), False)
     assert g.stats == ((0, 0, 0) if refused else w.stats), (c.name, g.stats, w.stats)
-    assert g.nrec == int((c.records0 if refused else w.records).sum()), c.name
 
 
 # ------------------------------------------------------------------------------------------------
@@ -671,42 +658,42 @@ def test_range_case_covers_its_edges():
 
 # ---- GPU tests --------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
-def test_chains_edges_ids_and_refusals(probe):
+def test_chains_edges_ids_and_refusals():
     """a, b, d, f"""
     cases = flat(SMALL)
-    for c, g in zip(cases, run_probe(probe, cases)):
+    for c, g in zip(cases, passes(cases)):
         if g.ran:
             placed(c, g.sorted["batch"].astype(np.int64))
         check(c, g)
 
 
 @pytest.mark.gpu
-def test_carry_chunks(probe):
+def test_carry_chunks():
     """c"""
     cases = carry_cases()
-    for c, g in zip(cases, run_probe(probe, cases)):
+    for c, g in zip(cases, passes(cases)):
         placed(c, g.sorted["batch"].astype(np.int64))
         check(c, g)
 
 
 @pytest.mark.gpu
-def test_range_search(probe):
+def test_range_search():
     """e, the device's search: a table deep enough for 17 steps"""
     c = range_case()
     assert len(c.ranges) > 1 << 16
-    g, = run_probe(probe, [c])
+    g, = passes([c])
     check(c, g)
     assert c.want.stats[0] > 100_000
 
 
 @pytest.mark.gpu
-def test_at_depth(probe):
+def test_at_depth():
     """g"""
     c = depth_case()
     d = depth(c.want)
     assert c.want.m > 8 * CHUNK and len(c.ranges) > 1000
     assert d.cross_warp > 500_000 and d.cross_tile > 100_000 and d.cross_chunk > 1000, (d.cross_warp, d.cross_tile, d.cross_chunk)
-    g, = run_probe(probe, [c])
+    g, = passes([c])
     check(c, g)
     assert c.want.stats[0] > 0 and c.want.stats[2] > 0
 
