@@ -189,11 +189,39 @@ int kta_hll_registers(const kta_handle *h, uint8_t *out, size_t cap);
 int kta_fnv32_host(kta_handle *h, int64_t n, const int32_t *key_len, const uint8_t *key_bytes,
                    int64_t key_bytes_len, uint32_t *out);
 
+/* Timeline: per partition, the records, tombstones and bytes written in each time bucket (when a partition's data was
+ * written: how much of it is older than retention.ms, which tombstones are older than delete.retention.ms, whether a
+ * partition has stopped receiving data, whether the topic was filled in bursts).  Off by default.
+ *   Records counted: exactly the records the counters count.  A record whose partition lies outside [0, P), a record of
+ *   a foreign partition on a sharded handle, and log records never delivered (aborted, CRC-failed, outside a window,
+ *   dropped below the log start) are left out; stamps-only re-runs of the alive-key table are not counted again.
+ *   Second of a record: t = (ts_ms == -1 ? 0 : ts_ms) / 1000, truncating toward zero, as earliest / latest
+ *   (src/metric.rs:209-211).  A record without a timestamp lands at 1970-01-01; other negative ms are real times:
+ *   -999 gives 0, -1000 gives -1, -1001 gives -1.
+ *   Buckets: origin O (s), width W >= 1 (s), B buckets.  Index 0 counts t < O; index 1 + (t - O) / W counts
+ *   O <= t < O + B*W; index B + 1 counts everything later.
+ *   Counters per (partition, index): KTA_TIMELINE_RECORDS (sums to KTA_TOTAL over the B + 2 indices),
+ *   KTA_TIMELINE_TOMBSTONES (value_len < 0; sums to KTA_TOMBSTONES), KTA_TIMELINE_BYTES (max(key_len, 0) +
+ *   max(value_len, 0); sums to KTA_KEY_SIZE_SUM + KTA_VALUE_SIZE_SUM).
+ * kta_set_timeline: buckets == 0 turns the timeline off.  KTA_ERR_INVALID when a record has been pushed or scanned since
+ * create or the last kta_reset (records still in the landing ring included), when width_s < 1, buckets lies outside
+ * [0, 65536], origin_s + buckets * width_s overflows int64, or num_partitions * (buckets + 2) > 2^24.  The arrays take
+ * 3 * num_partitions * (buckets + 2) u64 of device memory; kta_reset zeroes them and keeps the configuration.  Every
+ * counted scan is followed by one more kernel (kta_stats counts it) that reads the four header columns again.
+ * kta_timeline: valid after kta_finalize; copies min(cap, buckets + 2) words of one partition's row.
+ * KTA_ERR_NOT_ENABLED when the timeline is off, KTA_ERR_NOT_FINALIZED before kta_finalize; a partition outside [0, P)
+ * reads as zeros (like kta_counter).  A sharded handle keeps all P rows; foreign rows stay zero. */
+enum { KTA_TIMELINE_RECORDS = 0, KTA_TIMELINE_TOMBSTONES = 1, KTA_TIMELINE_BYTES = 2 };
+int kta_set_timeline(kta_handle *h, int64_t origin_s, int64_t width_s, int32_t buckets);
+int kta_timeline(const kta_handle *h, int which, int32_t partition, uint64_t *out, int64_t cap);
+
 /* ---- multi-GPU merge (one process per GPU; the collective itself is the caller's: NCCL via
  * torch.distributed, or ncclAllReduce directly) ----
  * The mergeable state is exported as ONE array of u64 laid out so that a single SUM all-reduce
  * merges everything: sums as they are; min/max scalars and HLL registers in per-rank slots
- * (zero elsewhere) that the import folds with min/max.  words = kta_merge_words(h, world). */
+ * (zero elsewhere) that the import folds with min/max.  words = kta_merge_words(h, world).
+ * With the timeline on, its 3 * P * (B + 2) words follow at the end, summed as they are: every rank must use the same
+ * timeline configuration (origin, width, buckets). */
 int64_t kta_merge_words(const kta_handle *h, int32_t world);
 int kta_merge_export_device(kta_handle *h, int32_t rank, int32_t world, uint64_t *dev_buf);
 int kta_merge_import_device(kta_handle *h, int32_t world, const uint64_t *dev_buf);

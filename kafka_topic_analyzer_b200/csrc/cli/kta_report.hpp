@@ -108,4 +108,26 @@ inline std::string render(const Summary &s, const std::vector<PartitionRow> &par
     return o;
 }
 
+// extension (--timeline): one table row per non-empty index of the summed timeline (include/kta.h kta_timeline)
+struct TimelineRow {
+    int64_t index;       // 0 = before the range, 1..B = bucket index - 1, B + 1 = after it
+    int64_t start_s;     // start of the bucket (index 1..B)
+    uint64_t records, tombstones, bytes;
+};
+
+inline std::string render_timeline(int64_t origin, int64_t width, int64_t buckets, const std::vector<TimelineRow> &rows) {
+    auto u = [](uint64_t v) { return std::to_string(v); };
+    std::string o = "| extension: timeline, " + std::to_string(buckets) + " buckets of " + std::to_string(width) + " s from " +
+                    format_utc(origin, 0) + "\n";
+    std::vector<std::vector<std::string>> t;
+    t.push_back({"Bucket start", "Records", "Tmb", "Bytes"});
+    for (const auto &r : rows) {
+        const std::string start = r.index == 0 ? "before " + format_utc(origin, 0)
+                                  : r.index == buckets + 1 ? format_utc(origin + buckets * width, 0) + " and later"
+                                                           : format_utc(r.start_s, 0);
+        t.push_back({start, u(r.records), u(r.tombstones), u(r.bytes)});
+    }
+    return o + render_table(t);
+}
+
 }  // namespace kta_report

@@ -25,6 +25,12 @@
 //                              60-72).  Records outside are left out, and the two offsets are the report's < OS and > OS.
 //   --feed push|batch|device   how records reach the handlers: kta_push per record (the reference's call shape),
 //                              kta_push_batch_host, or generated and scanned in HBM
+//   --timeline W[,ORIGIN,BUCKETS]  extension: after the report, one row per non-empty W-second bucket (start time in UTC,
+//                              records, tombstones, bytes, summed over the report's partitions), plus "before" and "after"
+//                              rows when records fall outside.  Without ORIGIN and BUCKETS the range is what can be seen
+//                              before the first record: under --log-dir every batch's baseTimestamp and maxTimestamp (a
+//                              header-only walk of the segments), under --synthetic the timestamps of the first and last
+//                              record; the origin is rounded down to a multiple of W.  More than 10 000 buckets are refused.
 //
 // There is no librdkafka and no broker in this build (SURVEY.md D9): without --synthetic the program explains
 // that and exits, like the reference does when it cannot fetch metadata.  Everything numeric comes from the
@@ -35,6 +41,7 @@
 #include <sys/stat.h>
 
 #include <algorithm>
+#include <cerrno>
 #include <chrono>
 #include <fstream>
 #include <cstdio>
@@ -73,8 +80,99 @@ static bool read_file(const std::string &path, std::vector<uint8_t> &out) {
     return n == 0 || (bool)f.read(reinterpret_cast<char *>(out.data()), n);
 }
 
+// --timeline: the bucket width and, once known, the range (kta_set_timeline)
+struct TimelineOpt {
+    bool on = false, ranged = false;   // ranged: ORIGIN and BUCKETS were given (or have been derived)
+    int64_t width = 0, origin = 0, buckets = 0;
+};
+static constexpr int64_t TIMELINE_MAX_BUCKETS = 10000;
+
+static bool parse_i64(const std::string &t, int64_t &v) {
+    if (t.empty() || t.size() > 20 || t.find_first_not_of("0123456789", t[0] == '-' ? 1 : 0) != std::string::npos || t == "-") return false;
+    errno = 0;
+    v = strtoll(t.c_str(), nullptr, 10);
+    return errno == 0;
+}
+
+// "W" or "W,ORIGIN,BUCKETS"; false (with a message) when it does not parse
+static bool parse_timeline(const std::string &arg, TimelineOpt &t) {
+    std::vector<std::string> f;
+    for (size_t p = 0;;) {
+        const size_t e = arg.find(',', p);
+        f.push_back(arg.substr(p, e == std::string::npos ? std::string::npos : e - p));
+        if (e == std::string::npos) break;
+        p = e + 1;
+    }
+    if ((f.size() != 1 && f.size() != 3) || !parse_i64(f[0], t.width) || t.width < 1) {
+        fprintf(stderr, "error: --timeline takes W[,ORIGIN,BUCKETS]: a bucket width of at least 1 second, optionally the first "
+                "bucket's start (UTC seconds) and the number of buckets, not '%s'\n", arg.c_str());
+        return false;
+    }
+    t.on = true;
+    if (f.size() == 3) {
+        if (!parse_i64(f[1], t.origin) || !parse_i64(f[2], t.buckets) || t.buckets < 1) {
+            fprintf(stderr, "error: --timeline: ORIGIN must be an integer and BUCKETS at least 1, not '%s'\n", arg.c_str());
+            return false;
+        }
+        if (t.buckets > TIMELINE_MAX_BUCKETS) {
+            fprintf(stderr, "error: --timeline: %lld buckets is more than %lld: use a wider W or fewer buckets\n",
+                    (long long)t.buckets, (long long)TIMELINE_MAX_BUCKETS);
+            return false;
+        }
+        t.ranged = true;
+    }
+    return true;
+}
+
+// the second a record's timestamp counts in (include/kta.h): -1 = not available = 0, truncating toward zero
+static int64_t ts_second(int64_t ts_ms) { return (ts_ms == -1 ? 0 : ts_ms) / 1000; }
+
+// the range from the earliest and latest second seen: origin rounded down to a multiple of W, enough buckets to reach the
+// latest second; false (with a message) beyond TIMELINE_MAX_BUCKETS
+static bool timeline_range(TimelineOpt &t, int64_t lo_s, int64_t hi_s) {
+    if (t.ranged) return true;
+    if (lo_s > hi_s) lo_s = hi_s = 0;   // nothing seen
+    const int64_t W = t.width;
+    t.origin = lo_s / W * W - ((lo_s % W) < 0 ? W : 0);   // floor
+    const __int128 n = ((__int128)hi_s - t.origin) / W + 1;
+    if (n > TIMELINE_MAX_BUCKETS) {
+        fprintf(stderr, "error: --timeline: the records span %s to %s, %lld buckets of %lld s, more than %lld: use a wider W\n",
+                kta_report::format_utc(lo_s, 0).c_str(), kta_report::format_utc(hi_s, 0).c_str(), (long long)n, (long long)W,
+                (long long)TIMELINE_MAX_BUCKETS);
+        return false;
+    }
+    t.buckets = (int64_t)n;
+    t.ranged = true;
+    return true;
+}
+
+// one row per non-empty bucket, summed over the report's partitions, with "before" and "after" rows when nonzero
+static void print_timeline(kta_handle *h, const std::vector<int> &partitions, const TimelineOpt &t) {
+    const size_t row = (size_t)t.buckets + 2;
+    std::vector<uint64_t> sum[3], one(row);
+    for (int w = 0; w < 3; w++) {
+        sum[w].assign(row, 0);
+        for (int p : partitions) {
+            KTA(kta_timeline(h, w, p, one.data(), (int64_t)row));
+            for (size_t i = 0; i < row; i++) sum[w][i] += one[i];
+        }
+    }
+    std::vector<kta_report::TimelineRow> rows;
+    for (size_t i = 0; i < row; i++) {
+        if (!sum[KTA_TIMELINE_RECORDS][i]) continue;
+        kta_report::TimelineRow r{};
+        r.index = (int64_t)i;
+        r.start_s = t.origin + ((int64_t)i - 1) * t.width;
+        r.records = sum[KTA_TIMELINE_RECORDS][i];
+        r.tombstones = sum[KTA_TIMELINE_TOMBSTONES][i];
+        r.bytes = sum[KTA_TIMELINE_BYTES][i];
+        rows.push_back(r);
+    }
+    fputs(kta_report::render_timeline(t.origin, t.width, t.buckets, rows).c_str(), stdout);
+}
+
 static int print_report(kta_handle *h, const std::string &topic, const std::vector<int> &partitions, const std::vector<int64_t> &start_offsets,
-                        const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs);
+                        const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs, const TimelineOpt &tl);
 
 // check.crcs: every kept failure as librdkafka words the consumer error it raises (RD_KAFKA_RESP_ERR__BAD_MSG), logged as
 // the reference logs a failed poll; the failures beyond those kept in one line
@@ -122,8 +220,38 @@ static bool read_checkpoint(const std::string &path, const std::string &topic, s
     return true;
 }
 
+// --timeline under --log-dir: the earliest and latest second of every batch's baseTimestamp (bytes 27-34) and maxTimestamp
+// (bytes 35-42), read from the batch headers alone
+static bool log_dir_seconds(const std::map<int, std::vector<std::string>> &segs, int64_t &lo_s, int64_t &hi_s) {
+    lo_s = INT64_MAX; hi_s = INT64_MIN;
+    uint8_t hdr[43];
+    for (const auto &kv : segs)
+        for (const auto &path : kv.second) {
+            std::ifstream f(path, std::ios::binary);
+            if (!f) { fprintf(stderr, "cannot read %s\n", path.c_str()); return false; }
+            f.seekg(0, std::ios::end);
+            const int64_t size = (int64_t)f.tellg();
+            for (int64_t pos = 0; pos + 61 <= size;) {
+                f.seekg(pos);
+                if (!f.read(reinterpret_cast<char *>(hdr), sizeof hdr)) break;
+                int64_t bl = 0, base = 0, mx = 0;
+                for (int i = 8; i < 12; i++) bl = (bl << 8) | hdr[i];
+                bl = (int32_t)bl;
+                for (int i = 27; i < 35; i++) base = (int64_t)(((uint64_t)base << 8) | hdr[i]);
+                for (int i = 35; i < 43; i++) mx = (int64_t)(((uint64_t)mx << 8) | hdr[i]);
+                if (bl < 49 || pos + 12 + bl > size) break;
+                for (int64_t ts : {base, mx}) {
+                    lo_s = std::min(lo_s, ts_second(ts));
+                    hi_s = std::max(hi_s, ts_second(ts));
+                }
+                pos += 12 + bl;
+            }
+        }
+    return true;
+}
+
 static int analyze_log_dir(const std::string &topic, const std::string &dir, bool alive, int hll, bool read_committed, bool check_crcs,
-                           std::chrono::steady_clock::time_point start_time) {
+                           std::chrono::steady_clock::time_point start_time, TimelineOpt tl) {
     // get_topic_offsets (src/kafka.rs:60-72) from the files: partitions = <topic>-<n> directories, low watermark =
     // first batch's baseOffset, high watermark = last batch's baseOffset + lastOffsetDelta + 1; for the partitions the
     // broker's checkpoint files list, its log start offset and high watermark instead (and only what lies between is read)
@@ -164,9 +292,15 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
     cfg.hll_precision = hll;
     cfg.now_s = INT64_MIN;
     cfg.isolation_level = read_committed ? KTA_READ_COMMITTED : KTA_READ_UNCOMMITTED;
+    if (tl.on && !tl.ranged) {
+        int64_t lo = 0, hi = 0;
+        if (!log_dir_seconds(segs, lo, hi)) return 1;
+        if (!timeline_range(tl, lo, hi)) return 2;
+    }
     kta_handle *h = nullptr;
     KTA(kta_create(&cfg, &h));
     if (check_crcs) KTA(kta_log_set_check_crcs(h, 1));
+    if (tl.on) KTA(kta_set_timeline(h, tl.origin, tl.width, (int32_t)tl.buckets));
     // the window of every partition the checkpoints list: the log start offset raised to the first segment's base offset
     // (its 20-digit file name, as the broker loads a log), the high watermark no lower than that (it is clamped to the log
     // end offset once the files are read: no batch lies beyond it, so the window reads the same either way)
@@ -261,7 +395,7 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
     // the report has one row per partition of the topic's metadata (main.rs:103-106): the <topic>-<n> directories found
     std::vector<int> present;
     for (auto &kv : segs) present.push_back(kv.first);
-    const int rc = print_report(h, topic, present, start_offsets, end_offsets, alive, hll, secs);
+    const int rc = print_report(h, topic, present, start_offsets, end_offsets, alive, hll, secs, tl);
     kta_destroy(h);
     return rc;
 }
@@ -269,6 +403,7 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
 int main(int argc, char **argv) {
     std::string topic, bootstrap, librdkafka, synthetic, log_dir, feed = "batch";
     int count_alive_occurrences = 0, hll = 0;
+    TimelineOpt tl;
     for (int i = 1; i < argc; i++) {
         const std::string a = argv[i];
         auto val = [&]() -> std::string { if (i + 1 >= argc) { fprintf(stderr, "error: %s needs a value\n", a.c_str()); exit(2); } return argv[++i]; };
@@ -281,6 +416,7 @@ int main(int argc, char **argv) {
         else if (a == "--log-dir") log_dir = val();
         else if (a == "--feed") feed = val();
         else if (a == "--hll") hll = atoi(val().c_str());
+        else if (a == "--timeline") { if (!parse_timeline(val(), tl)) return 2; }
         else if (a == "-V" || a == "--version") { puts("Kafka Topic Analyzer 0.4.1"); return 0; }  // main.rs:35
         else if (a == "-h" || a == "--help") {
             puts("Kafka Topic Analyzer 0.4.1\n\nUSAGE:\n    kafka-topic-analyzer [FLAGS] [OPTIONS] --bootstrap-server <BOOTSTRAP_SERVER> --topic <TOPIC>\n\n"
@@ -300,7 +436,11 @@ int main(int argc, char **argv) {
                  "                                                 from the log start offset up to the high watermark\n"
                  "    -t, --topic <TOPIC>                          The topic to analyze\n"
                  "        --synthetic <k=v,...>                    in-memory synthetic topic (this build has no Kafka client)\n"
-                 "        --feed <push|batch|device>               how records are handed to the metric handlers");
+                 "        --feed <push|batch|device>               how records are handed to the metric handlers\n"
+                 "        --timeline <W[,ORIGIN,BUCKETS]>          extension: records, tombstones and bytes per W-second bucket\n"
+                 "                                                 (UTC), printed after the report; without ORIGIN and BUCKETS\n"
+                 "                                                 the range covers the records' timestamps (at most 10000\n"
+                 "                                                 buckets)");
             return 0;
         } else { fprintf(stderr, "error: Found argument '%s' which wasn't expected\n", a.c_str()); return 2; }
     }
@@ -339,7 +479,7 @@ int main(int argc, char **argv) {
     }
     const auto start_time = std::chrono::steady_clock::now();  // main.rs:69
     if (!log_dir.empty())
-        return analyze_log_dir(topic, log_dir, count_alive_occurrences == 1, hll, read_committed, check_crcs, start_time);
+        return analyze_log_dir(topic, log_dir, count_alive_occurrences == 1, hll, read_committed, check_crcs, start_time, tl);
 
     std::map<std::string, std::string> kv;
     for (size_t p = 0; p < synthetic.size();) {
@@ -371,6 +511,15 @@ int main(int argc, char **argv) {
     // get_topic_offsets (src/kafka.rs:60-72): synthetic watermarks
     std::vector<int64_t> start_offsets(P, 0), end_offsets(P, n / P);
     if (n == 0) { fprintf(stderr, "Given topic has no content, no analysis possible. Exiting.\n"); return 254; }  // main.rs:98-101
+    if (tl.on && !tl.ranged) {   // the range from the first and the last record of the topic
+        int64_t ts0 = 0, ts1 = 0;
+        if (kta_synth_fill_host(&spec, 0, 1, 0, 1, nullptr, nullptr, &ts0, nullptr, nullptr, nullptr, nullptr, 0, nullptr) ||
+            kta_synth_fill_host(&spec, 0, 1, n - 1, 1, nullptr, nullptr, &ts1, nullptr, nullptr, nullptr, nullptr, 0, nullptr)) {
+            fprintf(stderr, "synthetic fill failed\n");
+            return 1;
+        }
+        if (!timeline_range(tl, std::min(ts_second(ts0), ts_second(ts1)), std::max(ts_second(ts0), ts_second(ts1)))) return 2;
+    }
 
     kta_config cfg{};
     cfg.struct_size = sizeof cfg;
@@ -381,6 +530,7 @@ int main(int argc, char **argv) {
     cfg.now_s = INT64_MIN;
     kta_handle *h = nullptr;
     KTA(kta_create(&cfg, &h));
+    if (tl.on) KTA(kta_set_timeline(h, tl.origin, tl.width, (int32_t)tl.buckets));
 
     printf("Subscribing to %s\n", topic.c_str());          // src/kafka.rs:88
     printf("Starting message consumption...\n");            // src/kafka.rs:91
@@ -407,7 +557,7 @@ int main(int argc, char **argv) {
             // a real run amortises it over the whole topic, a 2e7-record measurement would be dominated by it
             KTA(kta_push(h, 0, 0, 0, nullptr, -1, 0));
             KTA(kta_sync(h));
-            KTA(kta_reset(h));
+            KTA(kta_reset(h));   // (keeps the timeline's configuration)
         }
         std::vector<int32_t> part(CH), kl(CH), vl(CH);
         std::vector<int64_t> off(CH), ts(CH);
@@ -445,13 +595,13 @@ int main(int argc, char **argv) {
 
     std::vector<int> all_partitions(P);
     for (int p = 0; p < P; p++) all_partitions[p] = p;
-    const int rc = print_report(h, topic, all_partitions, start_offsets, end_offsets, cfg.count_alive_keys == 1, hll, duration_secs);
+    const int rc = print_report(h, topic, all_partitions, start_offsets, end_offsets, cfg.count_alive_keys == 1, hll, duration_secs, tl);
     kta_destroy(h);
     return rc;
 }
 
 static int print_report(kta_handle *h, const std::string &topic, const std::vector<int> &partitions, const std::vector<int64_t> &start_offsets,
-                        const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs) {
+                        const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs, const TimelineOpt &tl) {
     kta_report::Summary s{};
     s.topic = topic;
     s.duration_secs = duration_secs;
@@ -480,5 +630,6 @@ static int print_report(kta_handle *h, const std::string &topic, const std::vect
     }
     fputs(kta_report::render(s, rows).c_str(), stdout);
     if (hll) { double e = 0; KTA(kta_alive_keys_hll(h, &e)); printf("| extension: HyperLogLog(p=%d) alive-key estimate: %.0f\n", hll, e); }
+    if (tl.on) print_timeline(h, partitions, tl);
     return 0;
 }

@@ -23,6 +23,7 @@
 #include "kta_kernels.cuh"
 #include "kta_logscan.cuh"
 #include "kta_synth.h"
+#include "kta_timeline.cuh"
 
 using namespace kta;
 
@@ -90,6 +91,17 @@ struct AliveKeys {
     std::vector<AlivePending> pending;
 };
 
+// The timeline extension (kta_set_timeline): its configuration and its three [P][B + 2] u64 arrays
+struct Timeline {
+    int32_t buckets = 0;                     // B; 0 = off
+    int64_t origin = 0, width = 1;           // O, W (seconds)
+    bool smem = false;                       // bins in shared memory (P * (B + 2) of them fit the opt-in shared memory)
+    int blocks_per_sm = 0;                   // CTAs of timeline_kernel per SM (occupancy of the chosen instance)
+    DevBuf<unsigned long long> d_bins;       // [3][P][B + 2]: records | tombstones | bytes
+    std::vector<uint64_t> h_bins;            // host mirror, valid after finalize
+    size_t words() const { return d_bins.cap > 0 ? (size_t)d_bins.cap : 0; }
+};
+
 struct kta_handle {
     kta_config cfg{};
     int device = 0;
@@ -106,6 +118,7 @@ struct kta_handle {
     uint32_t *d_hash_out = nullptr;          // test hook (the caller's buffer)
     DevBuf<uint64_t> d_tb_scratch;           // key_tile_base scratch for device batches and decoded segments
     LogScan log;
+    Timeline tl;
     size_t nsums = 0, nhll = 0;
     // landing ring
     Chunk chunks[NCHUNK];
@@ -646,6 +659,49 @@ static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, 
     return KTA_OK;
 }
 
+// Launch shape of the timeline pass over n records: one CTA of TL_THREADS per resident slot (at most one warp per tile),
+// and enough CTAs that none takes more than TL_MAX_CTA_TILES tiles
+static void timeline_shape(const kta_handle *h, int64_t n, int &grid, int &threads, size_t &smem) {
+    const Timeline &t = h->tl;
+    const int64_t ntiles = (n + TILE - 1) / TILE;
+    threads = TL_THREADS;
+    smem = t.smem ? (size_t)h->cfg.num_partitions * (size_t)(t.buckets + 2) * 16 : 0;
+    const int64_t warps = TL_THREADS / 32;
+    int64_t g = std::min<int64_t>((ntiles + warps - 1) / warps, (int64_t)h->sm_count * t.blocks_per_sm);
+    g = std::max<int64_t>(g, (ntiles + TL_MAX_CTA_TILES - 1) / TL_MAX_CTA_TILES);
+    grid = (int)std::max<int64_t>(g, 1);
+}
+
+// the timeline pass over the columns a counted scan has just read (same stream, so a ring chunk's free_ev, recorded
+// after launch_scan, covers it)
+static int launch_timeline(kta_handle *h, const ScanParams &prm) {
+    const Timeline &t = h->tl;
+    TimelineParams tp{};
+    tp.n = prm.n;
+    tp.ntiles = (prm.n + TILE - 1) / TILE;
+    tp.partition = prm.partition;
+    tp.ts_ms = prm.ts_ms;
+    tp.key_len = prm.key_len;
+    tp.value_len = prm.value_len;
+    tp.P = h->cfg.num_partitions;
+    tp.shard_world = h->shard_world;
+    tp.shard_rank = h->shard_rank;
+    tp.B = t.buckets;
+    tp.origin = t.origin;
+    tp.width = (uint64_t)t.width;
+    tp.span = (uint64_t)t.buckets * (uint64_t)t.width;
+    tp.inv_width = 1.0 / (double)t.width;
+    tp.out = t.d_bins;
+    int grid = 0, threads = 0;
+    size_t smem = 0;
+    timeline_shape(h, prm.n, grid, threads, smem);
+    if (t.smem) timeline_kernel<true><<<grid, threads, smem, h->stream>>>(tp);
+    else timeline_kernel<false><<<grid, threads, 0, h->stream>>>(tp);
+    CU(cudaGetLastError());
+    h->launches++;
+    return KTA_OK;
+}
+
 // one scan of a batch whose columns lie in ring chunk `chunk` (-1: elsewhere); `seq_ends`: see alive_prepare
 static int launch_scan(kta_handle *h, ScanParams prm, int64_t key_readable, int64_t key_bytes, int chunk = -1,
                        const uint64_t *seq_ends = nullptr) {
@@ -654,6 +710,7 @@ static int launch_scan(kta_handle *h, ScanParams prm, int64_t key_readable, int6
     int rc;
     if (exact && (rc = alive_prepare(h, prm, seq_ends))) return rc;
     if ((rc = launch_scan_raw(h, prm, key_readable, key_bytes))) return rc;
+    if (h->tl.buckets && (rc = launch_timeline(h, prm))) return rc;
     if (exact && (rc = alive_scanned(h, prm, key_readable, key_bytes, chunk))) return rc;
     h->records += (uint64_t)prm.n;
     h->finalized = false;
@@ -1162,6 +1219,7 @@ extern "C" int kta_reset(kta_handle *h) {
     o.set = 0;
     o.dirty = !o.win.empty();
     for (uint64_t &v : o.totals) v = 0;
+    if (h->tl.buckets) CU(cudaMemsetAsync(h->tl.d_bins, 0, h->tl.words() * 8, h->stream));   // (its configuration stays)
     return state_reset_device(h);
 }
 
@@ -1185,6 +1243,10 @@ extern "C" int kta_finalize(kta_handle *h) {
     CU(cudaMemcpyAsync(h->h_sums.data(), h->d_sums, h->nsums * 8, cudaMemcpyDeviceToHost, s));
     CU(cudaMemcpyAsync(h->h_minmax, h->d_minmax, 32, cudaMemcpyDeviceToHost, s));
     if (h->nhll) CU(cudaMemcpyAsync(h->h_hll.data(), h->d_hll, h->nhll * 4, cudaMemcpyDeviceToHost, s));
+    if (h->tl.buckets) {
+        h->tl.h_bins.resize(h->tl.words());
+        CU(cudaMemcpyAsync(h->tl.h_bins.data(), h->tl.d_bins, h->tl.words() * 8, cudaMemcpyDeviceToHost, s));
+    }
     CU(cudaStreamSynchronize(s));
     if ((rc = collect_timing(h))) return rc;
     h->h_alive = h->alive.now;   // counted over the table by alive_settle above (sum_all_alive, src/metric.rs:282-284)
@@ -1353,6 +1415,76 @@ extern "C" int kta_hist(const kta_handle *h, int which, int32_t partition, uint6
     return KTA_OK;
 }
 
+extern "C" int kta_set_timeline(kta_handle *h, int64_t origin_s, int64_t width_s, int32_t buckets) {
+    if (!h) return fail(KTA_ERR_INVALID, "null handle");
+    if (h->records || h->pc.n)
+        return fail(KTA_ERR_INVALID, "the timeline is configured before the first record: records were pushed or scanned "
+                    "since create or the last kta_reset");
+    if (width_s < 1) return fail(KTA_ERR_INVALID, "timeline width %lld s: must be at least 1", (long long)width_s);
+    if (buckets < 0 || buckets > TL_MAX_BUCKETS)
+        return fail(KTA_ERR_INVALID, "timeline buckets %d outside [0, %d]", buckets, TL_MAX_BUCKETS);
+    __int128 end = (__int128)origin_s + (__int128)buckets * (__int128)width_s;
+    if (end > (__int128)INT64_MAX)
+        return fail(KTA_ERR_INVALID, "timeline origin %lld + %d buckets x %lld s overflows int64", (long long)origin_s, buckets,
+                    (long long)width_s);
+    const int64_t P = h->cfg.num_partitions;
+    const int64_t bins = P * ((int64_t)buckets + 2);
+    if (buckets && bins > TL_MAX_BINS)
+        return fail(KTA_ERR_INVALID, "timeline of %lld partitions x %d indices exceeds 2^24 bins", (long long)P, buckets + 2);
+    int rc;
+    if ((rc = set_device(h))) return rc;
+    // the new configuration is built aside and swapped in only when complete: a failure keeps the old one
+    Timeline t;
+    if (buckets) {
+        if ((rc = t.d_bins.alloc(3 * bins))) return rc;
+        t.buckets = buckets;
+        t.origin = origin_s;
+        t.width = width_s;
+        t.smem = (size_t)bins * 16 <= h->smem_optin;
+        if (t.smem) {
+            CU(cudaFuncSetAttribute(timeline_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&t.blocks_per_sm, timeline_kernel<true>, TL_THREADS, (size_t)bins * 16));
+        } else {
+            CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&t.blocks_per_sm, timeline_kernel<false>, TL_THREADS, 0));
+        }
+        if (t.blocks_per_sm < 1) return fail(KTA_ERR_CUDA, "timeline kernel does not fit an SM");
+        CU(cudaMemsetAsync(t.d_bins, 0, (size_t)t.d_bins.cap * 8, h->stream));
+        t.h_bins.assign((size_t)t.d_bins.cap, 0);   // nothing scanned yet: a finalized handle reads zeros
+    }
+    CU(cudaStreamSynchronize(h->stream));   // the zeroing has landed, and no queued pass still uses the old arrays
+    h->tl = std::move(t);
+    return KTA_OK;
+}
+
+extern "C" int kta_timeline(const kta_handle *h, int which, int32_t partition, uint64_t *out, int64_t cap) {
+    if (!h || which < KTA_TIMELINE_RECORDS || which > KTA_TIMELINE_BYTES || cap < 0 || (cap && !out))
+        return fail(KTA_ERR_INVALID, "bad argument");
+    if (!h->tl.buckets) return fail(KTA_ERR_NOT_ENABLED, "the timeline is off (kta_set_timeline)");
+    const int rc = check_read(h, partition, true);
+    if (rc > 0) return rc;
+    const int64_t row = (int64_t)h->tl.buckets + 2, n = std::min<int64_t>(cap, row);
+    if (rc < 0) {
+        std::fill(out, out + n, (uint64_t)0);
+        return KTA_OK;
+    }
+    const size_t at = ((size_t)which * (size_t)h->cfg.num_partitions + (size_t)partition) * (size_t)row;
+    std::copy(h->tl.h_bins.begin() + (long)at, h->tl.h_bins.begin() + (long)(at + (size_t)n), out);
+    return KTA_OK;
+}
+
+// test hook: the timeline pass's launch shape for a scan of n records (grid, threads, 1 = bins in shared memory)
+extern "C" int kta_timeline_shape(const kta_handle *h, int64_t n, int32_t *grid, int32_t *threads, int32_t *smem_bins) {
+    if (!h || n < 0 || !grid || !threads || !smem_bins) return fail(KTA_ERR_INVALID, "bad argument");
+    if (!h->tl.buckets) return fail(KTA_ERR_NOT_ENABLED, "the timeline is off (kta_set_timeline)");
+    int g = 0, th = 0;
+    size_t sm = 0;
+    timeline_shape(h, n, g, th, sm);
+    *grid = g;
+    *threads = th;
+    *smem_bins = h->tl.smem ? 1 : 0;
+    return KTA_OK;
+}
+
 // Ertl 2017, "New cardinality estimation algorithms for HyperLogLog sketches": improved raw estimator
 static double hll_sigma(double x) {
     if (x == 1.0) return INFINITY;
@@ -1438,9 +1570,12 @@ extern "C" int kta_set_hash_capture(kta_handle *h, uint32_t *dev_out) {
 // ------------------------------------------------------------------------------------------------
 // multi-GPU merge
 // ------------------------------------------------------------------------------------------------
+// words of the merge buffer in front of the timeline segment
+static size_t merge_base_words(const kta_handle *h, int32_t world) { return h->nsums + (size_t)world * 4 + (size_t)world * (h->nhll / 8); }
+
 extern "C" int64_t kta_merge_words(const kta_handle *h, int32_t world) {
     if (!h || world < 1) return -1;
-    return (int64_t)(h->nsums + (size_t)world * 4 + (size_t)world * (h->nhll / 8));
+    return (int64_t)(merge_base_words(h, world) + h->tl.words());
 }
 
 extern "C" int kta_merge_export_device(kta_handle *h, int32_t rank, int32_t world, uint64_t *dev_buf) {
@@ -1453,6 +1588,9 @@ extern "C" int kta_merge_export_device(kta_handle *h, int32_t rank, int32_t worl
                                                            world, reinterpret_cast<unsigned long long *>(dev_buf));
     h->launches++;
     CU(cudaGetLastError());
+    // the timeline arrays go at the end as they are: the SUM all-reduce adds every rank's rows (foreign rows are zero)
+    if (h->tl.buckets)
+        CU(cudaMemcpyAsync(dev_buf + merge_base_words(h, world), h->tl.d_bins, h->tl.words() * 8, cudaMemcpyDeviceToDevice, h->stream));
     // With its own stream the handle must finish before the caller's collective may read the buffer.  On an
     // adopted stream (kta_set_stream) the caller's collective is ordered behind this kernel by the stream itself.
     if (h->own_stream) {
@@ -1471,6 +1609,8 @@ extern "C" int kta_merge_import_device(kta_handle *h, int32_t world, const uint6
                                                            reinterpret_cast<const unsigned long long *>(dev_buf));
     h->launches++;
     CU(cudaGetLastError());
+    if (h->tl.buckets)
+        CU(cudaMemcpyAsync(h->tl.d_bins, dev_buf + merge_base_words(h, world), h->tl.words() * 8, cudaMemcpyDeviceToDevice, h->stream));
     h->finalized = false;
     if (h->own_stream) CU(cudaStreamSynchronize(h->stream));
     return KTA_OK;

@@ -54,18 +54,22 @@ def allreduce_merge(engine: KtaEngine, group=None, counters_only: bool = False) 
 # ---------------------------------------------------------------------------------------------------
 # Host-side statement of the merge-buffer layout (what merge_export_kernel / merge_import_kernel do on the
 # device, csrc/kta_kernels.cuh).  Used by the gloo CPU tests of the N>1 logic and usable for host-side merges.
-#   [ sums (nsums u64) | world × 4 extrema slots | world × (nhll/8) words, eight one-byte registers per word ]
-# Every rank fills only its own slots, so ONE SUM all-reduce hands every rank's values to every rank.
+#   [ sums (nsums u64) | world × 4 extrema slots | world × (nhll/8) words, eight one-byte registers per word
+#     | timeline (3 × P × (B + 2) u64, only when the timeline is on) ]
+# Every rank fills only its own slots, so ONE SUM all-reduce hands every rank's values to every rank.  The timeline
+# segment is summed as it is (a sharded rank's foreign rows are zero); every rank must use the same timeline.
 # ---------------------------------------------------------------------------------------------------
-def merge_words(nsums: int, nhll: int, world: int) -> int:
-    return nsums + world * 4 + world * (nhll // 8)
+def merge_words(nsums: int, nhll: int, world: int, timeline_words: int = 0) -> int:
+    return nsums + world * 4 + world * (nhll // 8) + timeline_words
 
 
-def pack_merge_buffer(sums, minmax, hll, rank: int, world: int):
-    """sums u64[nsums]; minmax = (min_ts i64, max_ts i64, min_size u64, max_size u64); hll u32[nhll]."""
+def pack_merge_buffer(sums, minmax, hll, rank: int, world: int, timeline=None):
+    """sums u64[nsums]; minmax = (min_ts i64, max_ts i64, min_size u64, max_size u64); hll u32[nhll];
+    timeline: None, or the u64 [3][P][B + 2] arrays (any shape; taken flat)."""
     import numpy as np
     nsums, nhll = len(sums), len(hll)
-    buf = np.zeros(merge_words(nsums, nhll, world), dtype=np.uint64)
+    tl = None if timeline is None else np.asarray(timeline, dtype=np.uint64).ravel()
+    buf = np.zeros(merge_words(nsums, nhll, world, 0 if tl is None else tl.size), dtype=np.uint64)
     buf[:nsums] = np.asarray(sums, dtype=np.uint64)
     mm = np.array([minmax[0], minmax[1]], dtype=np.int64).view(np.uint64)
     buf[nsums + 4 * rank: nsums + 4 * rank + 2] = mm
@@ -76,11 +80,14 @@ def pack_merge_buffer(sums, minmax, hll, rank: int, world: int):
         regs = np.asarray(hll, dtype=np.uint8)
         o = nsums + 4 * world + rank * hw
         buf[o:o + hw] = regs.view(np.uint64) if regs.flags["C_CONTIGUOUS"] else np.ascontiguousarray(regs).view(np.uint64)
+    if tl is not None:
+        buf[merge_words(nsums, nhll, world):] = tl
     return buf
 
 
-def fold_merge_buffer(buf, nsums: int, nhll: int, world: int):
-    """inverse of pack after the SUM all-reduce: returns (sums, (min_ts, max_ts, min_size, max_size), hll)."""
+def fold_merge_buffer(buf, nsums: int, nhll: int, world: int, timeline_words: int = 0):
+    """inverse of pack after the SUM all-reduce: returns (sums, (min_ts, max_ts, min_size, max_size), hll), and the
+    flat timeline segment as a fourth element when timeline_words > 0."""
     import numpy as np
     sums = buf[:nsums].copy()
     mm = buf[nsums:nsums + 4 * world].reshape(world, 4)
@@ -92,4 +99,7 @@ def fold_merge_buffer(buf, nsums: int, nhll: int, world: int):
         hw = nhll // 8
         w = np.ascontiguousarray(buf[nsums + 4 * world:nsums + 4 * world + world * hw]).view(np.uint8).reshape(world, nhll)
         hll[:] = w.max(axis=0)
+    if timeline_words:
+        base = merge_words(nsums, nhll, world)
+        return sums, (tmin, tmax, smin, smax), hll, np.asarray(buf[base:base + timeline_words], dtype=np.uint64).copy()
     return sums, (tmin, tmax, smin, smax), hll

@@ -87,6 +87,7 @@ class KtaEngine:
         self.count_alive_keys = bool(count_alive_keys)
         self.hll_precision = hll_precision
         self.shares_caller_stream = False   # True after set_stream(): work is ordered by the caller's stream
+        self.timeline_buckets = 0           # set_timeline
         self.message_metrics = MessageMetrics(self)
         self.log_compaction_metrics = LogCompactionInMemoryMetrics(self) if count_alive_keys else None
 
@@ -230,6 +231,28 @@ class KtaEngine:
         v = [C.c_uint64() for _ in range(2)]
         check(lib().kta_log_offset_stats(self._h, *[C.byref(x) for x in v]))
         return tuple(x.value for x in v)
+
+    def set_timeline(self, origin_s: int, width_s: int, buckets: int) -> None:
+        """Count each partition's records, tombstones and bytes per time bucket: index 0 before origin_s, index
+        1 + (t - origin_s) // width_s for the `buckets` buckets of width_s seconds, index buckets + 1 after them
+        (include/kta.h).  Only before the first record (after create or reset); buckets = 0 turns it off; reset()
+        keeps the setting."""
+        check(lib().kta_set_timeline(self._h, origin_s, width_s, buckets))
+        self.timeline_buckets = buckets
+
+    def timeline(self, which: int, p: int) -> np.ndarray:
+        """One partition's row of a timeline counter (N.TIMELINE_RECORDS / _TOMBSTONES / _BYTES): buckets + 2 u64,
+        after finalize()."""
+        n = self.timeline_buckets + 2
+        out = np.zeros(n, dtype=np.uint64)
+        check(lib().kta_timeline(self._h, which, p, out.ctypes.data_as(C.POINTER(C.c_uint64)), n))
+        return out
+
+    def timeline_shape(self, n: int):
+        """(grid, threads, bins in shared memory) of the timeline pass over a scan of n records (test hook)."""
+        g, t, s = C.c_int32(), C.c_int32(), C.c_int32()
+        check(lib().kta_timeline_shape(self._h, n, C.byref(g), C.byref(t), C.byref(s)))
+        return g.value, t.value, bool(s.value)
 
     def sync(self) -> None:
         check(lib().kta_sync(self._h))
