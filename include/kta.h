@@ -77,7 +77,11 @@ typedef struct kta_config {
     int32_t shard_world;       /* partition-sharded job (one handle per GPU, gpu = partition mod G, SURVEY.md §8 e): this */
     int32_t shard_rank;        /*   handle scans only partitions p with p % shard_world == shard_rank; records of other
                                     partitions are left out like out-of-range ones.  0 or 1 = not sharded.  The handle
-                                    still holds (and, after kta_merge_import_device, reports) all num_partitions. */
+                                    still holds (and, after kta_merge_import_device, reports) all num_partitions.
+                                    Shapes are limited by the scan's division p / G = mulhi(p, ceil(2^32 / G)): with
+                                    e = ceil(2^32 / G) * G - 2^32, kta_create refuses (KTA_ERR_INVALID) unless
+                                    (num_partitions - 1) * e < 2^32.  Every num_partitions <= 65536 and every
+                                    shard_world <= 4096 is accepted. */
 } kta_config;
 
 /* kta_batch.seq_base value that means "continue this handle's running count" (what kta_push does: the consumer's

@@ -548,6 +548,14 @@ static int create_impl(const kta_config *cfg, kta_handle *h) {
     if (cfg->shard_world > 1) {
         if (cfg->shard_rank < 0 || cfg->shard_rank >= cfg->shard_world || cfg->shard_world > P)
             return fail(KTA_ERR_INVALID, "shard_rank %d / shard_world %d invalid for %d partitions", cfg->shard_rank, cfg->shard_world, P);
+        // the scan finds a partition's column p / G as mulhi(p, m), m = ceil(2^32 / G) (ScanParams::shard_magic).  With
+        // e = m G - 2^32 that is exact whenever p e < 2^32, so the shape is taken only if the largest id, P - 1, meets it:
+        // every P <= 65536 and every G <= 4096 does (e < G)
+        const uint64_t G = (uint64_t)cfg->shard_world, e = (((uint64_t)1 << 32) + G - 1) / G * G - ((uint64_t)1 << 32);
+        if ((uint64_t)(P - 1) * e >= (uint64_t)1 << 32)
+            return fail(KTA_ERR_INVALID, "shard_world %d with %d partitions: the scan's partition division is exact only when "
+                        "(P - 1) * (ceil(2^32 / G) * G - 2^32) < 2^32 (every P <= 65536 and every G <= 4096 qualify)",
+                        cfg->shard_world, P);
         h->shard_world = cfg->shard_world;
         h->shard_rank = cfg->shard_rank;
     }

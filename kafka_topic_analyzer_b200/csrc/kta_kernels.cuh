@@ -78,7 +78,7 @@ struct ScanParams {
     int32_t P;                       // partitions of the topic (ids 0..P-1)
     int32_t shard_world, shard_rank; // this handle scans only partitions p with p % shard_world == shard_rank (1, 0 = all)
     int32_t Pc;                      // counter columns = owned partitions; column c holds partition c * shard_world + shard_rank
-    uint32_t shard_magic;            // ceil(2^32 / shard_world): p / shard_world = mulhi(p, magic) for p < 2^20
+    uint32_t shard_magic;            // m = ceil(2^32 / G), G = shard_world: p / G = mulhi(p, m) when p (m G - 2^32) < 2^32 (kta_create: every p < P)
     int32_t hll_p;                   // HLL index bits (MODE_HLL)
     uint64_t stage_limit;            // bytes readable from key_bytes by 16-byte bulk copies, rounded DOWN to 16; 0 = staging not allowed
     int32_t hdr_stage;               // 1: stages hold header slices too; full tiles stage them by bulk copies (columns 16-byte aligned)

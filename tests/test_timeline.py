@@ -1,10 +1,13 @@
 """The timeline extension (include/kta.h, kta_set_timeline / kta_timeline): per partition and time bucket, the records,
 tombstones and bytes the counters count.
 
-CPU: the numpy restatement against the record-at-a-time one over the edge seconds (hypothesis), and the merge buffer's
-timeline segment (distributed.py).  GPU: every entry point against the numpy restatement fed the delivered records, with
-the invariants against kta_counter; the edge seconds and shapes; warp aggregation; both bin paths; the byte carry; the
-depth of a launch; the multi-GPU merge; the handle's lifecycle; and that nothing else changes."""
+CPU: the numpy restatement against the record-at-a-time one over the edge seconds (hypothesis), the kernel's bucket
+quotient and correction step against exact division (hypothesis), the shard rule against brute force, and the merge
+buffer's timeline segment (distributed.py).  GPU: every entry point against the numpy restatement fed the delivered
+records, with the invariants against kta_counter; the edge seconds and shapes; the bucket edges that need the correction
+step; warp aggregation; sharded handles at their limit shapes; both bin paths; the byte carry and a row's high word;
+full tiles read row by row; the depth of a launch; the multi-GPU merge; the handle's lifecycle; and that nothing else
+changes."""
 import ctypes as C
 import datetime
 import os
@@ -48,6 +51,18 @@ def edge_ms(rng, n, origin, width, buckets):
             v = (origin + int(rng.integers(0, max(buckets * width, 1)))) * 1000 + int(rng.integers(0, 1000))
         out.append(min(max(v, I64_MIN), I64_MAX))
     return np.array(out, dtype=np.int64)
+
+
+# Ranges whose bucket edges need timeline_index's correction step, as (O, W, B, needs q--, needs q++).  The quotient
+# (double)d * (1/W) lands one too low at some edges of 30-day buckets (the first edge among them: d = W gives 0.99999...)
+# and of W = 999 999 937; it lands one too high only where d passes 2^53, which takes an origin near the most negative
+# second an int64 millisecond value reaches.  B = 2048 fits shared memory up to P = 7, B = 65536 does not fit it at all.
+CORRECTION_RANGES = {
+    "30d": (1_498_176_000, 2_592_000, 1000, False, True),
+    "w999999937": (T0, 999_999_937, 65536, False, True),
+    "w2^43-1": (-TR.SMAX, (1 << 43) - 1, 2048, True, True),
+    "w2^38-1": (-TR.SMAX, (1 << 38) - 1, 65536, True, True),
+}
 
 
 # ---- CPU ------------------------------------------------------------------------------------------------------------
@@ -95,6 +110,89 @@ def test_edge_seconds_by_hand():
     got = [TR.record_index(s * 1000, O, W, B) for s in (O - 1, O, O + W - 1, O + W, O + B * W - 1, O + B * W)]
     assert got == [0, 1, 1, 2, B, B + 1]
     assert list(TR.index_np(np.array([s * 1000 for s in (O - 1, O, O + W - 1, O + W, O + B * W - 1, O + B * W)]), O, W, B)) == got
+
+
+@settings(max_examples=1000, deadline=None)
+@given(st.data())
+def test_kernel_index_matches_exact_division(data):
+    """the kernel's bucket index (its double-precision quotient and one correction step) equals the exact one, for W up
+    to (2^63 - 1) / B, seconds at and beside multiples of W, and origins at the reachable extremes; and the quotient
+    before the correction is never off by more than one, for every d below B W (reachable or not)"""
+    B = data.draw(st.one_of(st.just(1), st.just(65536), st.integers(1, 65536)), label="B")
+    wmax = I64_MAX // B
+    W = data.draw(st.one_of(st.integers(1, wmax), st.integers(max(1, wmax - 4096), wmax),
+                            st.sampled_from([1, 3, 3600, 2_592_000, 999_999_937, (1 << 38) - 1, 1 << 40, (1 << 43) - 1])),
+                  label="W")
+    top = I64_MAX - B * W                                   # the largest origin kta_set_timeline accepts
+    O = data.draw(st.one_of(st.just(-TR.SMAX), st.integers(-TR.SMAX - 4096, -TR.SMAX + 4096), st.just(I64_MIN),
+                            st.just(top), st.just(TR.SMAX - B * W), st.just(0), st.integers(I64_MIN, top)), label="O")
+    q = data.draw(st.one_of(st.integers(0, B), st.sampled_from([0, 1, B - 1, B])), label="q")
+    delta = data.draw(st.one_of(st.integers(-2, 2), st.integers(-W, W)), label="delta")
+    s = min(max(O + q * W + delta, -TR.SMAX), TR.SMAX)
+    ms = data.draw(st.sampled_from([0, 1, 999]), label="ms")
+    ts = min(max(s * 1000 + (ms if s >= 0 else -ms), I64_MIN), I64_MAX)
+    assert TR.second(ts) == s
+    assert TR.kernel_index(ts, O, W, B)[0] == TR.record_index(ts, O, W, B)
+    d = min(max(q * W + delta, 0), B * W - 1)
+    assert abs(TR.kernel_quotient(d, W, B) - d // W) <= 1
+
+
+def test_boundary_ms_by_hand():
+    O, W, B = -3, 5, 2
+    want_s = [O - 1, O, O + 1, O + W - 1, O + W, O + W + 1, O + 2 * W - 1, O + 2 * W, O + 2 * W + 1]
+    got = TR.boundary_ms(O, W, B)
+    assert [TR.second(int(v)) for v in got] == [s for s in want_s for _ in (0, 999)]
+    assert list(got[:4]) == [-4000, -4999, -3000, -3999] and list(got[-2:]) == [8000, 8999]
+    # the ends of the int64 range keep their second, seconds past them are left out
+    low = TR.boundary_ms(-TR.SMAX, 1, 1)
+    assert [TR.second(int(v)) for v in low[::2]] == [-TR.SMAX, 1 - TR.SMAX, -TR.SMAX, 1 - TR.SMAX, 2 - TR.SMAX]
+    assert low[1] == I64_MIN and TR.boundary_ms(TR.SMAX - 1, 1, 1)[-1] == I64_MAX
+    # a large B: every q within `ends` of both ends, `sample` between
+    qs = {(TR.second(int(v)) - T0 + 1) // 7 for v in TR.boundary_ms(T0, 7, 65536)}
+    assert len(qs) == 2 * 1024 + 4096 and set(range(1024)) <= qs and set(range(65537 - 1024, 65537)) <= qs
+
+
+@pytest.mark.parametrize("name", list(CORRECTION_RANGES))
+def test_correction_ranges_need_their_corrections(name):
+    """each range test_bucket_boundaries runs on the GPU has records that need the correction step it is there for"""
+    O, W, B, down, up = CORRECTION_RANGES[name]
+    steps = {-1: 0, 0: 0, 1: 0}
+    for v in TR.boundary_ms(O, W, B).tolist():
+        i, step = TR.kernel_index(v, O, W, B)
+        assert i == TR.record_index(v, O, W, B)
+        steps[step] += 1
+    assert (steps[-1] > 0, steps[1] > 0) == (down, up), "%s: %d records need q--, %d need q++" % (name, steps[-1], steps[1])
+
+
+def shard_division_exact(P, G):
+    """the scan's column mulhi(p, ceil(2^32 / G)) is p / G for every p < P: checked at p = kG - 1 (the largest remainder
+    of each quotient, where the rounded-up multiplier errs first) and at P - 1"""
+    p = np.append(np.arange(G - 1, P, G), P - 1).astype(np.uint64)
+    return bool(np.array_equal(TR.shard_column_mulhi(p, G), p // np.uint64(G)))
+
+
+def test_shard_rule_against_brute_force():
+    """kta_create's shard rule accepts only shapes whose every partition the scan divides exactly: all G <= 4096 at
+    P = 2^20, every G at P <= 65536, and a seeded sample of larger G; the shapes it refuses include ones the division
+    gets wrong"""
+    P = 1 << 20
+    for G in range(2, 4097):
+        assert TR.shard_accepted(P, G) and shard_division_exact(P, G), G
+    assert all(TR.shard_accepted(65536, G) for G in range(2, 65537))
+    rng = np.random.default_rng(20)
+    refused = 0
+    for G in rng.integers(4097, P + 1, size=3000).tolist():
+        for PP in (G, min(G, 65536), int(rng.integers(G, P + 1)), P):
+            PP = max(PP, G)
+            if TR.shard_accepted(PP, G):
+                assert shard_division_exact(PP, G), (PP, G)
+            else:
+                refused += 1
+    assert refused > 0
+    # where the division is wrong: column 1 for partition 65 536 of 65 537 shards; partition 1 031 965 of rank 4177
+    for P_, G, p in ((65537, 65537, 65536), (1_031_966, 4178, 1_031_965)):
+        assert not TR.shard_accepted(P_, G) and not shard_division_exact(P_, G)
+        assert int(TR.shard_column_mulhi([p], G)[0]) == p // G + 1
 
 
 @pytest.mark.parametrize("world", [1, 4])
@@ -246,6 +344,31 @@ def test_edge_seconds(origin, width, buckets):
         assert_timeline(e, P, origin, width, buckets, part, ts, kl, vl)
 
 
+BOUNDARY_CASES = [("30d", True), ("30d", False), ("w999999937", False), ("w2^43-1", True), ("w2^43-1", False),
+                  ("w2^38-1", False)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,smem", BOUNDARY_CASES,
+                         ids=["%s-%s" % (n, "smem" if s else "global") for n, s in BOUNDARY_CASES])
+def test_bucket_boundaries(name, smem):
+    """every bucket edge (sampled between the ends for B = 65536) of a range whose quotients need the correction step,
+    three seconds at each, at ms 0 and 999, on the given bin path"""
+    O, W, B = CORRECTION_RANGES[name][:3]
+    P = 3 if smem else max(3, smem_max_bins() // (B + 2) + 1)
+    ts = TR.boundary_ms(O, W, B)
+    n = ts.size
+    rng = np.random.default_rng(B)
+    part = rng.integers(0, P, size=n).astype(np.int32)
+    kl = rng.integers(-1, 24, size=n).astype(np.int32)
+    vl = rng.choice(np.array([-1, 0, 7, 65536], dtype=np.int32), size=n)
+    with engine_tl(P, O, W, B) as e:
+        assert e.timeline_shape(n)[2] == smem
+        scan_cols(e, part, ts, kl, vl)
+        e.finalize()
+        assert_timeline(e, P, O, W, B, part, ts, kl, vl)
+
+
 @pytest.mark.gpu
 def test_setter_refusals_and_the_largest_range():
     with KtaEngine(2, now=feed.NOW) as e:
@@ -301,6 +424,61 @@ def test_bad_and_foreign_partitions(rank):
         assert_timeline(e, P, O, W, B, part, ts, kl, vl, shard=(rank, 3))
 
 
+@pytest.mark.gpu
+@pytest.mark.parametrize("P,G,rank", [(65537, 65537, 65536), (1_031_966, 4178, 4177)])
+def test_shard_shapes_the_scan_cannot_divide_are_refused(P, G, rank):
+    """the scan would put partition P - 1 (65 536) in column 1 instead of 0, or partition 1 031 965 of rank 4177 in the
+    wrong column, leaving the handle's own records out as foreign: kta_create refuses both shapes"""
+    assert not TR.shard_accepted(P, G)
+    with pytest.raises(KtaError) as ex:
+        KtaEngine(P, now=feed.NOW, shard=(rank, G)).close()
+    assert ex.value.code == N.ERR_INVALID
+
+
+# accepted shard shapes at the limits: P = 2^20 with G = 4096 (rank 4095 owns partition 2^20 - 1) and G = 4095 (rank
+# 4094's largest partition is one below a multiple of G, where (P - 1) e is closest to 2^32); 65 536 partitions over
+# 65 536 and 65 535 shards
+SHARD_LIMITS = [(1 << 20, 4096, 4095), (1 << 20, 4095, 4094), (65536, 65536, 65535), (65536, 65535, 65534)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("mode", ["counters", "hll", "exact"])
+@pytest.mark.parametrize("P,G,rank", SHARD_LIMITS, ids=["P%d-G%d-r%d" % s for s in SHARD_LIMITS])
+def test_shard_limit_shapes_count_their_own_partitions(P, G, rank, mode):
+    """a handle fed only its own partitions, up to the largest, counts every record: no record is reported out of range,
+    and each own partition's counters and timeline row (P (B + 2) <= 2^24) agree with the restatement"""
+    assert TR.shard_accepted(P, G)
+    O, W, B = T0, 600, 14
+    assert P * (B + 2) <= 1 << 24
+    own = np.arange(rank, P, G)
+    rng = np.random.default_rng(G)
+    n = 30_000
+    part = rng.choice(own, size=n).astype(np.int32)
+    part[: own.size] = own[::-1]                         # every own partition, the largest first
+    ts = edge_ms(rng, n, O, W, B)
+    kl = rng.integers(-1, 24, size=n).astype(np.int32)
+    vl = rng.choice(np.array([-1, 0, 1, 300, 65536], dtype=np.int32), size=n)
+    kb = rng.integers(0, 256, size=int(np.maximum(kl, 0).sum()), dtype=np.uint8)
+    t = feed.HostTopic(part, np.arange(n, dtype=np.int64), ts, kl, vl, np.arange(n, dtype=np.uint64), kb,
+                       feed.tile_base_from_key_len(kl))
+    kw = {"counters": {}, "hll": dict(hll_precision=10), "exact": dict(count_alive_keys=True)}[mode]
+    with engine_tl(P, O, W, B, shard=(rank, G), **kw) as e:
+        feed.scan(e, t)
+        assert e.finalize(strict=False) == 0 and e.bad_partition_records() == 0
+        # the own partitions renumbered 0 .. len(own) - 1 for the restatement (a whole [3][P][B + 2] would be 400 MB)
+        want = TR.timeline_np(own.size, O, W, B, (part - rank) // G, ts, kl, vl)
+        got = np.stack([np.stack([e.timeline(w, int(p)) for p in own]) for w in range(3)])
+        assert np.array_equal(got, want)
+        for j, p in enumerate(own.tolist()):
+            mine = part == p
+            assert e.counter(M.TOTAL, p) == int(mine.sum()) == int(got[0, j].sum())
+            assert e.counter(M.TOMBSTONES, p) == int((vl[mine] < 0).sum()) == int(got[1, j].sum())
+            assert (e.counter(M.KEY_SIZE_SUM, p) + e.counter(M.VALUE_SIZE_SUM, p) == int(got[2, j].sum())
+                    == int(np.maximum(kl[mine], 0).sum() + np.maximum(vl[mine], 0).sum()))
+        for p in (0, rank - 1, P - 1 if (P - 1) % G != rank else P - 2):   # foreign partitions read as zeros
+            assert p % G != rank and not e.timeline(0, p).any() and e.counter(M.TOTAL, p) == 0
+
+
 # ---- GPU: both bin paths, byte carry, depth -------------------------------------------------------------------------
 def smem_max_bins():
     return torch.cuda.get_device_properties(0).shared_memory_per_block_optin // 16
@@ -345,17 +523,26 @@ def test_exact_smem_edge_and_many_partitions():
         assert_invariants(e, P, got)
 
 
+BYTE_ROWS = [(True, "mixed"), (False, "mixed"), (True, "one_bin"), (False, "one_bin"), (True, "alternating"),
+             (False, "alternating")]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("smem", [True, False])
-def test_bytes_past_2_32_in_one_cta(smem):
-    """two bins take 64 x (2^31 - 1 + 20) bytes each from a single CTA, their records alternating between lanes so that
-    every row is mixed: in shared memory each record's add carries from the low word into the high word; in global memory the group
-    sums are 64-bit"""
+@pytest.mark.parametrize("smem,rows", BYTE_ROWS, ids=["%s%s" % (s, "" if r == "mixed" else "-" + r) for s, r in BYTE_ROWS])
+def test_bytes_past_2_32_in_one_cta(smem, rows):
+    """bins take more than 2^32 bytes from a single CTA (32 full tiles), records of 2^31 - 1 + 20 bytes; lane l reads
+    records 4 l .. 4 l + 3.  "mixed": two bins, neighbouring lanes differ, so every row is mixed and in shared memory each
+    record's add carries from the low word into the high word (in global memory the group sums are 64-bit).
+    "one_bin": every row lies in one bin, so the warp's sum of a row passes 2^36 and its own high word is nonzero.
+    "alternating": the first two rows of a tile lie in one bin and the last two alternate between two, so the rows' high
+    words and the per-record carries meet in the same bin"""
     P = 64
     B = 4 if smem else smem_max_bins() // P
-    n = 128
-    part = (np.arange(n) // 4 % 2).astype(np.int32)   # lane l reads records 4 l .. 4 l + 3: neighbouring lanes differ
-    ts = np.full(n, (T0 + 5) * 1000, np.int64)
+    n = 128 * 32
+    i = np.arange(n)
+    part = {"mixed": i // 4 % 2, "one_bin": np.zeros(n, np.int64), "alternating": np.where(i % 4 < 2, 0, i // 4 % 2)}[rows]
+    part = part.astype(np.int32)
+    ts = np.full(n, (T0 + 5) * 1000, np.int64) + i % 1000
     kl = np.full(n, 20, np.int32)
     vl = np.full(n, (1 << 31) - 1, np.int32)
     with engine_tl(P, T0, 10, B) as e:
@@ -363,14 +550,48 @@ def test_bytes_past_2_32_in_one_cta(smem):
         scan_cols(e, part, ts, kl, vl)
         e.finalize()
         for p in (0, 1):
-            assert int(e.timeline(N.TIMELINE_BYTES, p)[1]) == n // 2 * ((1 << 31) - 1 + 20) > 1 << 32
+            assert int(e.timeline(N.TIMELINE_BYTES, p)[1]) == int((part == p).sum()) * ((1 << 31) - 1 + 20)
+        assert int(e.timeline(N.TIMELINE_BYTES, 0)[1]) > 1 << 32
         assert_timeline(e, P, T0, 10, B, part, ts, kl, vl)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("buckets", [197, 20_000])
-def test_depth(buckets):
-    """every warp of the launch takes at least 64 tiles, and the last tile is partial"""
+@pytest.mark.parametrize("smem", [True, False])
+@pytest.mark.parametrize("column", ["partition", "ts_ms", "key_len", "value_len", "all"])
+def test_full_tiles_row_by_row(column, smem):
+    """a column that starts one element past a 16-byte boundary sends every tile, the full ones too, down the row-by-row
+    path: each column on its own, then all four.  Half the records are edge timestamps over random partitions (mixed
+    rows), half time-ordered runs of one partition (rows in one bin)"""
+    P = 64
+    B = 40 if smem else smem_max_bins() // P
+    rng = np.random.default_rng(17)
+    n = 128 * 400
+    part, ts, kl, vl, _ = cols_topic(rng, n, P, T0, 60, B)
+    i = np.arange(n // 2)
+    part[n // 2:] = i // 200 % P
+    ts[n // 2:] = T0 * 1000 + i * 71
+    names = ("partition", "ts_ms", "key_len", "value_len")
+    d = [feed.device(a, shift=1 if column in (name, "all") else 0) for name, a in zip(names, (part, ts, kl, vl))]
+    assert sum(c.data_ptr() % 16 != 0 for c in d) == (4 if column == "all" else 1)
+    with engine_tl(P, T0, 60, B) as e:
+        assert e.timeline_shape(n)[2] == smem
+        feed.settle()
+        e.scan_batch_device(*d)
+        e.finalize()
+        assert_timeline(e, P, T0, 60, B, part, ts, kl, vl)
+
+
+DEPTH_CASES = [(197, "spread"), (20_000, "spread"), (197, "one_bin"), (20_000, "one_bin"), (197, "offset"),
+               (20_000, "offset")]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("buckets,layout", DEPTH_CASES,
+                         ids=["%d%s" % (b, "" if l == "spread" else "-" + l) for b, l in DEPTH_CASES])
+def test_depth(buckets, layout):
+    """every warp of the launch takes at least 64 tiles, and the last tile is partial; "one_bin": every record in one
+    bin, so every CTA adds to and flushes into the same bins; "offset": every column one element past a 16-byte
+    boundary, so every tile is read row by row"""
     P, O, W = 64, T0, 3600
     with engine_tl(P, O, W, buckets) as e:
         grid, threads, _ = e.timeline_shape(1 << 33)     # the full grid
@@ -380,10 +601,17 @@ def test_depth(buckets):
         assert ntiles // grid // (threads // 32) >= 64
         # built and restated on the device (timeline_torch): the host holds no column of the 3.5e7 records
         i = torch.arange(n, dtype=torch.int64, device="cuda")
-        part = ((i // 512) % P).to(torch.int32)
-        ts = T0 * 1000 + i * 7 + (i * 2654435761 % 5)
+        if layout == "one_bin":
+            part = torch.full((n,), 5, dtype=torch.int32, device="cuda")
+            ts = (T0 + 100) * 1000 + i % 1000
+        else:
+            part = ((i // 512) % P).to(torch.int32)
+            ts = T0 * 1000 + i * 7 + (i * 2654435761 % 5)
         kl = torch.full((n,), 16, dtype=torch.int32, device="cuda")
         vl = torch.where(i % 20 == 0, -1, 100 + i % 300).to(torch.int32)
+        del i
+        if layout == "offset":
+            part, ts, kl, vl = (feed.device(c, shift=1) for c in (part, ts, kl, vl))
         feed.settle()
         e.scan_batch_device(part, ts, kl, vl)
         e.finalize()
@@ -391,6 +619,8 @@ def test_depth(buckets):
         got = got_arrays(e, P)
         assert np.array_equal(got, want)
         assert_invariants(e, P, got)
+        if layout == "one_bin":
+            assert int(got[0, 5, 1]) == n and int(got[2, 5, 1]) > 1 << 32
 
 
 # ---- GPU: merge -----------------------------------------------------------------------------------------------------

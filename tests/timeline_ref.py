@@ -39,6 +39,67 @@ def record_counts(P, origin, width, buckets, records, shard=None):
     return out
 
 
+SMAX = 9_223_372_036_854_775   # |second(ts_ms)| of every int64 ts_ms: the reachable seconds are [-SMAX, SMAX]
+
+
+def kernel_quotient(d: int, width: int, buckets: int) -> int:
+    """timeline_index's quotient before its correction step: (uint64)((double)d * inv_width) clamped to B - 1, with
+    inv_width = 1.0 / (double)W as the host computes it.  Python floats are IEEE doubles: float() of an int rounds to
+    nearest like the kernel's u64 → f64 conversion, the product rounds to nearest like DMUL, and int() truncates
+    toward zero like cvt.rzi."""
+    return min(int(float(d) * (1.0 / float(width))), buckets - 1)
+
+
+def kernel_index(ts_ms: int, origin: int, width: int, buckets: int):
+    """timeline_index (csrc/kta_timeline.cuh) restated statement by statement.  Returns (index, step): step is -1 where
+    the correction ran q--, +1 where it ran q++, 0 where the quotient stood"""
+    s = second(ts_ms)
+    if s < origin:
+        return 0, 0
+    d = s - origin                        # (uint64)s - (uint64)O: in [0, 2^64) since s >= O
+    if d >= buckets * width:              # span = B W < 2^64
+        return buckets + 1, 0
+    q = kernel_quotient(d, width, buckets)
+    lo = q * width                        # <= (B - 1) W: no wrap
+    if lo > d:
+        return q, -1                      # 1 + (q - 1)
+    if d - lo >= width:
+        return q + 2, 1                   # 1 + (q + 1)
+    return q + 1, 0
+
+
+def boundary_ms(origin: int, width: int, buckets: int, ends: int = 1024, sample: int = 4096, seed: int = 0):
+    """int64 timestamps at q W - 1, q W and q W + 1 seconds past O for q = 0 .. B, each at millisecond 0 and 999 of its
+    second (truncating toward zero: second -5 at 999 ms is -5999 ms), clipped to int64 (which keeps the second);
+    seconds outside [-SMAX, SMAX] cannot occur and are left out.  When B + 1 > 2 ends + sample: the q within `ends` of
+    either end and a seeded sample of `sample` between them."""
+    if buckets + 1 <= 2 * ends + sample:
+        qs = list(range(buckets + 1))
+    else:
+        mid = np.random.default_rng(seed).choice(np.arange(ends, buckets + 1 - ends), sample, replace=False)
+        qs = list(range(ends)) + sorted(mid.tolist()) + list(range(buckets + 1 - ends, buckets + 1))
+    out = []
+    for q in qs:
+        for s in (origin + q * width - 1, origin + q * width, origin + q * width + 1):
+            if -SMAX <= s <= SMAX:
+                out += [min(max(s * 1000 + (ms if s >= 0 else -ms), -(1 << 63)), (1 << 63) - 1) for ms in (0, 999)]
+    return np.array(out, dtype=np.int64)
+
+
+def shard_accepted(P: int, G: int) -> bool:
+    """kta_create's rule for a sharded handle (G = shard_world > 1, G <= P): the scan's column p / G is
+    mulhi(p, m) with m = ceil(2^32 / G), exact when p e < 2^32 for e = m G - 2^32; the shape is accepted when the
+    largest partition id, P - 1, meets that"""
+    m = -(-(1 << 32) // G)
+    return (P - 1) * (m * G - (1 << 32)) < 1 << 32
+
+
+def shard_column_mulhi(p, G: int):
+    """the scan's column of partition ids p (numpy, < 2^32): __umulhi(p, ceil(2^32 / G))"""
+    m = np.uint64(-(-(1 << 32) // G))
+    return (np.asarray(p, dtype=np.uint64) * m) >> np.uint64(32)
+
+
 def seconds_np(ts_ms):
     t = np.where(ts_ms == -1, 0, ts_ms).astype(np.int64)
     q = t // 1000
