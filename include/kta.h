@@ -367,6 +367,9 @@ int kta_set_stream(kta_handle *h, void *stream);
  * VALUES_GEOMETRIC: the uniform value length is multiplied by 2^g, P(g = k) = 2^-(k+1), g <= 6 — a geometric tail. */
 #define KTA_SYNTH_KEYS_LOGUNIFORM 0x100
 #define KTA_SYNTH_VALUES_GEOMETRIC 0x200
+/* The largest value_mean a spec may ask for: the largest uniform value length, floor(mean/2) + mean, is then exactly
+ * INT32_MAX.  Every entry point refuses a larger mean as an invalid spec (kta_synth_shard_records returns -1). */
+#define KTA_SYNTH_MAX_VALUE_MEAN 1431655765
 
 typedef struct kta_synth_spec {
     uint64_t seed;               /* default 0x4B544131 ("KTA1") */
@@ -377,7 +380,7 @@ typedef struct kta_synth_spec {
     int32_t key_mode;            /* low byte: 0 = 16-byte binary (id, id*phi64) LE; 1 = ASCII "key-<id>";
                                     2 = variable-length binary, 0..40 bytes.  Optional flags (stress cases):
                                     KTA_SYNTH_KEYS_LOGUNIFORM, KTA_SYNTH_VALUES_GEOMETRIC */
-    int32_t value_mean;          /* value_len uniform in [mean/2, 3*mean/2] */
+    int32_t value_mean;          /* value_len uniform in [mean/2, 3*mean/2]; at most KTA_SYNTH_MAX_VALUE_MEAN */
     int32_t null_key_per_10k;
     int32_t tombstone_per_10k;
     int32_t ts_missing_per_10k;
@@ -393,7 +396,9 @@ int kta_synth_fill_host(const kta_synth_spec *s, int32_t rank, int32_t world, in
                         int32_t *key_len, int32_t *value_len, uint64_t *seq, uint8_t *key_bytes,
                         int64_t key_bytes_cap, int64_t *key_bytes_len);
 /* Same on the device (pointers are device memory; key_tile_base must hold
- * ceil(count/KTA_KEY_TILE)+1 words).  Synchronous. */
+ * ceil(count/KTA_KEY_TILE)+1 words).  Synchronous.  The key bytes are placed by the tile bases, so a call
+ * that asks for key_bytes or key_bytes_len without key_tile_base is refused with KTA_ERR_INVALID before
+ * anything is written.  key_bytes_cap smaller than the slice's key bytes: KTA_ERR_NOMEM, no key byte written. */
 int kta_synth_fill_device(const kta_synth_spec *s, int32_t device, int32_t rank, int32_t world,
                           int64_t start, int64_t count, int32_t *partition, int64_t *offset,
                           int64_t *ts_ms, int32_t *key_len, int32_t *value_len, uint64_t *seq,

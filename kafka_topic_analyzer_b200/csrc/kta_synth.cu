@@ -82,6 +82,8 @@ extern "C" int kta_synth_fill_device(const kta_synth_spec *s, int32_t device, in
                                      int64_t key_bytes_cap, uint64_t *key_tile_base, int64_t *key_bytes_len) {
     if (synth_check(s, rank, world) || start < 0 || count < 0 || start + count > s->n_total / world) return KTA_ERR_INVALID;
     if (!key_len && (key_bytes || key_tile_base)) return KTA_ERR_INVALID;
+    // the key bytes are placed by the tile bases: without them no key could be written (refused before any launch)
+    if (!key_tile_base && (key_bytes || key_bytes_len)) return KTA_ERR_INVALID;
     if (device >= 0 && cudaSetDevice(device) != cudaSuccess) return KTA_ERR_CUDA;
     if (count == 0) {
         if (key_bytes_len) *key_bytes_len = 0;

@@ -14,6 +14,8 @@ static int synth_check(const kta_synth_spec *s, int32_t rank, int32_t world) {
     if (!s || s->num_partitions < 1 || s->run_len < 1 || s->n_total < 0 || world < 1 || rank < 0 || rank >= world)
         return KTA_ERR_INVALID;
     if (s->key_mode < 0 || (s->key_mode & 0xff) > 2 || (s->key_mode & ~0x3ff) || s->value_mean < 0) return KTA_ERR_INVALID;
+    // the largest uniform value length, mean/2 + mean, must fit value_len's int32 (KTA_SYNTH_MAX_VALUE_MEAN)
+    if (s->value_mean > KTA_SYNTH_MAX_VALUE_MEAN) return KTA_ERR_INVALID;
     if (s->n_total % ((int64_t)s->num_partitions * s->run_len) != 0) return KTA_ERR_INVALID;
     if (world > 1 && s->num_partitions % world != 0) return KTA_ERR_INVALID;
     return KTA_OK;

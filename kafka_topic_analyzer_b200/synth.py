@@ -14,6 +14,7 @@ from ._native import SynthSpec, KtaError, lib, synth_lib
 DEFAULT_SEED = 0x4B544131  # "KTA1"
 KEYS_LOGUNIFORM = 0x100     # include/kta.h KTA_SYNTH_KEYS_LOGUNIFORM
 VALUES_GEOMETRIC = 0x200    # include/kta.h KTA_SYNTH_VALUES_GEOMETRIC
+MAX_VALUE_MEAN = 1431655765  # include/kta.h KTA_SYNTH_MAX_VALUE_MEAN: floor(mean/2) + mean == INT32_MAX
 
 
 @dataclass
@@ -57,7 +58,8 @@ def shard_records(spec: SynthSpec, rank: int = 0, world: int = 1) -> int:
     n = synth_lib().kta_synth_shard_records(C.byref(spec), rank, world)
     if n < 0:
         raise KtaError(N.ERR_INVALID, "invalid synthetic topic spec (n_total must be a multiple of "
-                       "num_partitions*run_len; num_partitions a multiple of world)")
+                       "num_partitions*run_len; num_partitions a multiple of world; value_mean at most "
+                       "%d)" % MAX_VALUE_MEAN)
     return n
 
 
