@@ -219,13 +219,49 @@ enum { KTA_TIMELINE_RECORDS = 0, KTA_TIMELINE_TOMBSTONES = 1, KTA_TIMELINE_BYTES
 int kta_set_timeline(kta_handle *h, int64_t origin_s, int64_t width_s, int32_t buckets);
 int kta_timeline(const kta_handle *h, int which, int32_t partition, uint64_t *out, int64_t cap);
 
+/* Partitioner check: per partition, how many keyed records sit where the common producers' partitioners would put them,
+ * so that a key written to two partitions (the partition count was raised, or producers with different partitioners
+ * wrote the topic) shows up: log compaction works per partition, and such a key keeps a live value in each.  Off by
+ * default.
+ *   Records checked: exactly the records the counters count (as the timeline's), and only those with a non-null key
+ *   (key_len >= 0; an empty key is hashed like any other).  Stamps-only re-runs of the alive-key table are not counted
+ *   again.
+ *   For a record with key bytes k in partition p and each j < C:
+ *     murmur2 at N_j: (murmur2(k) & 0x7fffffff) % N_j == p, with Kafka's Utils.murmur2 (seed 0x9747b28c, m 0x5bd1e995,
+ *       r 24, little-endian 4-byte words, tail bytes folded high to low before one multiply): the Java producer's
+ *       partitioner for keyed records, and librdkafka's murmur2 / murmur2_random;
+ *     CRC-32 at N_j: crc32(k) % N_j == p, unsigned, with zlib's CRC-32 (reflected 0xEDB88320, init and xorout
+ *       0xFFFFFFFF): librdkafka's consistent / consistent_random (its default) for non-empty keys;
+ *     neither: the record matched no (function, count) pair.
+ *   Not claimed: librdkafka's *_random variants may send an EMPTY key to a random partition (it is counted as hashed
+ *   here); fnv1a (librdkafka, Sarama) and custom partitioners are not modelled.
+ * kta_set_partitioner_check: ncounts = C in [0, KTA_PARTITIONER_MAX_COUNTS]; 0 turns the check off.  Every count lies in
+ * [1, 2^31 - 1] and the counts are distinct.  KTA_ERR_INVALID, with nothing changed, on any violation and when a record
+ * has been pushed or scanned since create or the last kta_reset (records still in the landing ring included).  The
+ * counters take (2C + 1) * num_partitions u64 of device memory; kta_reset zeroes them and keeps the configuration.  Every
+ * counted scan is followed by one more kernel (kta_stats counts it) that reads partition, key_len and the key bytes.
+ * With the check on, key bytes reach the device on every handle, a counters-only one included: a batch with keyed
+ * records must then carry key_bytes (KTA_ERR_INVALID otherwise), and kta_push copies each key.
+ * kta_partitioner_check: valid after kta_finalize; copies min(cap, 2C + 1) words of one partition: murmur2 matches for
+ * counts[0..C), CRC-32 matches for counts[0..C), neither.  KTA_ERR_NOT_ENABLED when the check is off,
+ * KTA_ERR_NOT_FINALIZED before kta_finalize; a partition outside [0, P) reads as zeros.  A sharded handle keeps all P
+ * rows; foreign rows stay zero.
+ * kta_partitioner_hash_host: the check's own device hash functions over n packed keys given in HOST memory (test hook,
+ * like kta_fnv32_host); key_len[i] < 0 yields 0 for both. */
+#define KTA_PARTITIONER_MAX_COUNTS 8
+int kta_set_partitioner_check(kta_handle *h, const int32_t *counts, int32_t ncounts);
+int kta_partitioner_check(const kta_handle *h, int32_t partition, uint64_t *out, int64_t cap);
+int kta_partitioner_hash_host(kta_handle *h, int64_t n, const int32_t *key_len, const uint8_t *key_bytes,
+                              int64_t key_bytes_len, uint32_t *murmur2, uint32_t *crc32);
+
 /* ---- multi-GPU merge (one process per GPU; the collective itself is the caller's: NCCL via
  * torch.distributed, or ncclAllReduce directly) ----
  * The mergeable state is exported as ONE array of u64 laid out so that a single SUM all-reduce
  * merges everything: sums as they are; min/max scalars and HLL registers in per-rank slots
  * (zero elsewhere) that the import folds with min/max.  words = kta_merge_words(h, world).
- * With the timeline on, its 3 * P * (B + 2) words follow at the end, summed as they are: every rank must use the same
- * timeline configuration (origin, width, buckets). */
+ * With the timeline on, its 3 * P * (B + 2) words follow, summed as they are: every rank must use the same
+ * timeline configuration (origin, width, buckets).  With the partitioner check on, its (2C + 1) * P words follow at
+ * the end (after the timeline's), summed as they are: every rank must check the same counts. */
 int64_t kta_merge_words(const kta_handle *h, int32_t world);
 int kta_merge_export_device(kta_handle *h, int32_t rank, int32_t world, uint64_t *dev_buf);
 int kta_merge_import_device(kta_handle *h, int32_t world, const uint64_t *dev_buf);

@@ -24,6 +24,7 @@ SEQ_AUTO = (1 << 64) - 1   # include/kta.h KTA_SEQ_AUTO
 READ_UNCOMMITTED, READ_COMMITTED = 0, 1   # include/kta.h KTA_READ_UNCOMMITTED / KTA_READ_COMMITTED
 TIMELINE_RECORDS, TIMELINE_TOMBSTONES, TIMELINE_BYTES = 0, 1, 2   # include/kta.h KTA_TIMELINE_*
 TIMELINE_MAX_BUCKETS = 65536
+PARTITIONER_MAX_COUNTS = 8   # include/kta.h KTA_PARTITIONER_MAX_COUNTS
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -141,6 +142,9 @@ SYMBOLS = {
     "kta_fnv32_host": (C.c_int, [_P, C.c_int64, _P, _P, C.c_int64, _P]),
     "kta_set_timeline": (C.c_int, [_P, C.c_int64, C.c_int64, C.c_int32]),
     "kta_timeline": (C.c_int, [_P, C.c_int, C.c_int32, C.POINTER(C.c_uint64), C.c_int64]),
+    "kta_set_partitioner_check": (C.c_int, [_P, C.POINTER(C.c_int32), C.c_int32]),
+    "kta_partitioner_check": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_uint64), C.c_int64]),
+    "kta_partitioner_hash_host": (C.c_int, [_P, C.c_int64, _P, _P, C.c_int64, _P, _P]),
     "kta_merge_words": (C.c_int64, [_P, C.c_int32]),
     "kta_merge_export_device": (C.c_int, [_P, C.c_int32, C.c_int32, _P]),
     "kta_merge_import_device": (C.c_int, [_P, C.c_int32, _P]),
@@ -173,6 +177,9 @@ SYMBOLS = {
     # test hook, not part of kta.h's stable surface
     "kta_set_hash_capture": (C.c_int, [_P, _P]),
     "kta_timeline_shape": (C.c_int, [_P, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "kta_partitioner_limit_grid": (C.c_int, [_P, C.c_int32]),
+    "kta_partitioner_shape": (C.c_int, [_P, C.c_int64, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                        C.POINTER(C.c_int32)]),
 }
 
 _lib = None

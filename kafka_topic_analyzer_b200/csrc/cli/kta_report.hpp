@@ -130,4 +130,40 @@ inline std::string render_timeline(int64_t origin, int64_t width, int64_t bucket
     return o + render_table(t);
 }
 
+// extension (--partitioner-check): per partition, its keyed records and where the partitioners would put them
+// (include/kta.h kta_partitioner_check), then the total over the rows
+struct PartitionerRow {
+    int32_t partition;
+    uint64_t keyed;                  // KTA_KEY_NON_NULL
+    std::vector<uint64_t> counts;    // murmur2 per count | CRC-32 per count | neither
+};
+
+inline std::string render_partitioner_check(const std::vector<int32_t> &counts, const std::vector<PartitionerRow> &rows) {
+    std::string o = "| extension: partitioner check, keyed records placed as murmur2 (Java) or CRC-32 (librdkafka) would place "
+                    "them at";
+    for (size_t j = 0; j < counts.size(); j++) o += (j ? ", " : " ") + std::to_string(counts[j]);
+    o += " partitions\n";
+    std::vector<std::vector<std::string>> t;
+    std::vector<std::string> head = {"P", "Keyed"};
+    for (int32_t n : counts) head.push_back("murmur2@" + std::to_string(n));
+    for (int32_t n : counts) head.push_back("crc32@" + std::to_string(n));
+    head.push_back("Neither");
+    t.push_back(head);
+    PartitionerRow total{};
+    total.counts.assign(2 * counts.size() + 1, 0);
+    for (const auto &r : rows) {
+        std::vector<std::string> cells = {std::to_string(r.partition), std::to_string(r.keyed)};
+        for (size_t b = 0; b < total.counts.size(); b++) {
+            cells.push_back(std::to_string(r.counts[b]));
+            total.counts[b] += r.counts[b];
+        }
+        total.keyed += r.keyed;
+        t.push_back(cells);
+    }
+    std::vector<std::string> cells = {"total", std::to_string(total.keyed)};
+    for (uint64_t v : total.counts) cells.push_back(std::to_string(v));
+    t.push_back(cells);
+    return o + render_table(t);
+}
+
 }  // namespace kta_report

@@ -31,6 +31,10 @@
 //                              before the first record: under --log-dir every batch's baseTimestamp and maxTimestamp (a
 //                              header-only walk of the segments), under --synthetic the timestamps of the first and last
 //                              record; the origin is rounded down to a multiple of W.  More than 10 000 buckets are refused.
+//   --partitioner-check N[,N...]  extension: after the report (and the timeline), one row per partition: its keyed records,
+//                              how many of them sit where Kafka's murmur2 partitioner would put them at each N, where
+//                              librdkafka's CRC-32 partitioner would, and where neither would; then a total row.  At most 8
+//                              distinct counts, each in [1, 2^31 - 1].
 //
 // There is no librdkafka and no broker in this build (SURVEY.md D9): without --synthetic the program explains
 // that and exits, like the reference does when it cannot fetch metadata.  Everything numeric comes from the
@@ -171,8 +175,50 @@ static void print_timeline(kta_handle *h, const std::vector<int> &partitions, co
     fputs(kta_report::render_timeline(t.origin, t.width, t.buckets, rows).c_str(), stdout);
 }
 
+// "N[,N...]": at most KTA_PARTITIONER_MAX_COUNTS distinct counts in [1, 2^31 - 1]; false (with a message) otherwise
+static bool parse_partitioner_check(const std::string &arg, std::vector<int32_t> &counts) {
+    counts.clear();
+    for (size_t p = 0;;) {
+        const size_t e = arg.find(',', p);
+        const std::string f = arg.substr(p, e == std::string::npos ? std::string::npos : e - p);
+        int64_t v = 0;
+        if (!parse_i64(f, v) || v < 1 || v > INT32_MAX) {
+            fprintf(stderr, "error: --partitioner-check takes N[,N...]: partition counts in [1, 2147483647], not '%s'\n", arg.c_str());
+            return false;
+        }
+        if (std::find(counts.begin(), counts.end(), (int32_t)v) != counts.end()) {
+            fprintf(stderr, "error: --partitioner-check: the count %lld is given twice\n", (long long)v);
+            return false;
+        }
+        counts.push_back((int32_t)v);
+        if (e == std::string::npos) break;
+        p = e + 1;
+    }
+    if (counts.size() > KTA_PARTITIONER_MAX_COUNTS) {
+        fprintf(stderr, "error: --partitioner-check: %zu counts is more than %d\n", counts.size(), KTA_PARTITIONER_MAX_COUNTS);
+        return false;
+    }
+    return true;
+}
+
+// one row per report partition: keyed records (KTA_KEY_NON_NULL) and the check's 2C + 1 counters, then their total
+static void print_partitioner_check(kta_handle *h, const std::vector<int> &partitions, const std::vector<int32_t> &counts) {
+    const size_t nv = 2 * counts.size() + 1;
+    std::vector<kta_report::PartitionerRow> rows;
+    for (int p : partitions) {
+        kta_report::PartitionerRow r{};
+        r.partition = p;
+        KTA(kta_counter(h, KTA_KEY_NON_NULL, p, &r.keyed));
+        r.counts.resize(nv);
+        KTA(kta_partitioner_check(h, p, r.counts.data(), (int64_t)nv));
+        rows.push_back(r);
+    }
+    fputs(kta_report::render_partitioner_check(counts, rows).c_str(), stdout);
+}
+
 static int print_report(kta_handle *h, const std::string &topic, const std::vector<int> &partitions, const std::vector<int64_t> &start_offsets,
-                        const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs, const TimelineOpt &tl);
+                        const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs, const TimelineOpt &tl,
+                        const std::vector<int32_t> &pcounts);
 
 // check.crcs: every kept failure as librdkafka words the consumer error it raises (RD_KAFKA_RESP_ERR__BAD_MSG), logged as
 // the reference logs a failed poll; the failures beyond those kept in one line
@@ -251,7 +297,7 @@ static bool log_dir_seconds(const std::map<int, std::vector<std::string>> &segs,
 }
 
 static int analyze_log_dir(const std::string &topic, const std::string &dir, bool alive, int hll, bool read_committed, bool check_crcs,
-                           std::chrono::steady_clock::time_point start_time, TimelineOpt tl) {
+                           std::chrono::steady_clock::time_point start_time, TimelineOpt tl, const std::vector<int32_t> &pcounts) {
     // get_topic_offsets (src/kafka.rs:60-72) from the files: partitions = <topic>-<n> directories, low watermark =
     // first batch's baseOffset, high watermark = last batch's baseOffset + lastOffsetDelta + 1; for the partitions the
     // broker's checkpoint files list, its log start offset and high watermark instead (and only what lies between is read)
@@ -301,6 +347,7 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
     KTA(kta_create(&cfg, &h));
     if (check_crcs) KTA(kta_log_set_check_crcs(h, 1));
     if (tl.on) KTA(kta_set_timeline(h, tl.origin, tl.width, (int32_t)tl.buckets));
+    if (!pcounts.empty()) KTA(kta_set_partitioner_check(h, pcounts.data(), (int32_t)pcounts.size()));
     // the window of every partition the checkpoints list: the log start offset raised to the first segment's base offset
     // (its 20-digit file name, as the broker loads a log), the high watermark no lower than that (it is clamped to the log
     // end offset once the files are read: no batch lies beyond it, so the window reads the same either way)
@@ -395,7 +442,7 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
     // the report has one row per partition of the topic's metadata (main.rs:103-106): the <topic>-<n> directories found
     std::vector<int> present;
     for (auto &kv : segs) present.push_back(kv.first);
-    const int rc = print_report(h, topic, present, start_offsets, end_offsets, alive, hll, secs, tl);
+    const int rc = print_report(h, topic, present, start_offsets, end_offsets, alive, hll, secs, tl, pcounts);
     kta_destroy(h);
     return rc;
 }
@@ -404,6 +451,7 @@ int main(int argc, char **argv) {
     std::string topic, bootstrap, librdkafka, synthetic, log_dir, feed = "batch";
     int count_alive_occurrences = 0, hll = 0;
     TimelineOpt tl;
+    std::vector<int32_t> pcounts;
     for (int i = 1; i < argc; i++) {
         const std::string a = argv[i];
         auto val = [&]() -> std::string { if (i + 1 >= argc) { fprintf(stderr, "error: %s needs a value\n", a.c_str()); exit(2); } return argv[++i]; };
@@ -417,6 +465,7 @@ int main(int argc, char **argv) {
         else if (a == "--feed") feed = val();
         else if (a == "--hll") hll = atoi(val().c_str());
         else if (a == "--timeline") { if (!parse_timeline(val(), tl)) return 2; }
+        else if (a == "--partitioner-check") { if (!parse_partitioner_check(val(), pcounts)) return 2; }
         else if (a == "-V" || a == "--version") { puts("Kafka Topic Analyzer 0.4.1"); return 0; }  // main.rs:35
         else if (a == "-h" || a == "--help") {
             puts("Kafka Topic Analyzer 0.4.1\n\nUSAGE:\n    kafka-topic-analyzer [FLAGS] [OPTIONS] --bootstrap-server <BOOTSTRAP_SERVER> --topic <TOPIC>\n\n"
@@ -440,7 +489,10 @@ int main(int argc, char **argv) {
                  "        --timeline <W[,ORIGIN,BUCKETS]>          extension: records, tombstones and bytes per W-second bucket\n"
                  "                                                 (UTC), printed after the report; without ORIGIN and BUCKETS\n"
                  "                                                 the range covers the records' timestamps (at most 10000\n"
-                 "                                                 buckets)");
+                 "                                                 buckets)\n"
+                 "        --partitioner-check <N[,N...]>           extension: per partition, the keyed records that murmur2\n"
+                 "                                                 (Java) and CRC-32 (librdkafka) would place there at each\n"
+                 "                                                 partition count N, printed after the report");
             return 0;
         } else { fprintf(stderr, "error: Found argument '%s' which wasn't expected\n", a.c_str()); return 2; }
     }
@@ -479,7 +531,7 @@ int main(int argc, char **argv) {
     }
     const auto start_time = std::chrono::steady_clock::now();  // main.rs:69
     if (!log_dir.empty())
-        return analyze_log_dir(topic, log_dir, count_alive_occurrences == 1, hll, read_committed, check_crcs, start_time, tl);
+        return analyze_log_dir(topic, log_dir, count_alive_occurrences == 1, hll, read_committed, check_crcs, start_time, tl, pcounts);
 
     std::map<std::string, std::string> kv;
     for (size_t p = 0; p < synthetic.size();) {
@@ -531,6 +583,7 @@ int main(int argc, char **argv) {
     kta_handle *h = nullptr;
     KTA(kta_create(&cfg, &h));
     if (tl.on) KTA(kta_set_timeline(h, tl.origin, tl.width, (int32_t)tl.buckets));
+    if (!pcounts.empty()) KTA(kta_set_partitioner_check(h, pcounts.data(), (int32_t)pcounts.size()));
 
     printf("Subscribing to %s\n", topic.c_str());          // src/kafka.rs:88
     printf("Starting message consumption...\n");            // src/kafka.rs:91
@@ -595,13 +648,15 @@ int main(int argc, char **argv) {
 
     std::vector<int> all_partitions(P);
     for (int p = 0; p < P; p++) all_partitions[p] = p;
-    const int rc = print_report(h, topic, all_partitions, start_offsets, end_offsets, cfg.count_alive_keys == 1, hll, duration_secs, tl);
+    const int rc = print_report(h, topic, all_partitions, start_offsets, end_offsets, cfg.count_alive_keys == 1, hll, duration_secs, tl,
+                                pcounts);
     kta_destroy(h);
     return rc;
 }
 
 static int print_report(kta_handle *h, const std::string &topic, const std::vector<int> &partitions, const std::vector<int64_t> &start_offsets,
-                        const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs, const TimelineOpt &tl) {
+                        const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs, const TimelineOpt &tl,
+                        const std::vector<int32_t> &pcounts) {
     kta_report::Summary s{};
     s.topic = topic;
     s.duration_secs = duration_secs;
@@ -631,5 +686,6 @@ static int print_report(kta_handle *h, const std::string &topic, const std::vect
     fputs(kta_report::render(s, rows).c_str(), stdout);
     if (hll) { double e = 0; KTA(kta_alive_keys_hll(h, &e)); printf("| extension: HyperLogLog(p=%d) alive-key estimate: %.0f\n", hll, e); }
     if (tl.on) print_timeline(h, partitions, tl);
+    if (!pcounts.empty()) print_partitioner_check(h, partitions, pcounts);
     return 0;
 }

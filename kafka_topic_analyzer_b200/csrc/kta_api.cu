@@ -22,6 +22,7 @@
 #include "kta_host.cuh"
 #include "kta_kernels.cuh"
 #include "kta_logscan.cuh"
+#include "kta_partitioner.cuh"
 #include "kta_synth.h"
 #include "kta_timeline.cuh"
 
@@ -102,6 +103,17 @@ struct Timeline {
     size_t words() const { return d_bins.cap > 0 ? (size_t)d_bins.cap : 0; }
 };
 
+// The partitioner check (kta_set_partitioner_check): its counts and its [2C + 1][P] u64 counters
+struct Partitioner {
+    int32_t ncounts = 0;                     // C; 0 = off
+    int32_t counts[KTA_PARTITIONER_MAX_COUNTS] = {};
+    bool smem = false;                       // counters in shared memory ((2C + 1) P of them fit beside the table and stages)
+    int32_t max_grid = 0;                    // test hook (kta_partitioner_limit_grid): at most this many CTAs; 0 = no limit
+    DevBuf<unsigned long long> d_counts;     // [2C + 1][P]: murmur2 per count | CRC-32 per count | neither
+    std::vector<uint64_t> h_counts;          // host mirror, valid after finalize
+    size_t words() const { return d_counts.cap > 0 ? (size_t)d_counts.cap : 0; }
+};
+
 struct kta_handle {
     kta_config cfg{};
     int device = 0;
@@ -119,6 +131,8 @@ struct kta_handle {
     DevBuf<uint64_t> d_tb_scratch;           // key_tile_base scratch for device batches and decoded segments
     LogScan log;
     Timeline tl;
+    Partitioner pt;
+    DevBuf<uint32_t> d_crc32_tables;         // zlib CRC-32 slicing tables of the partitioner check (made on first use)
     size_t nsums = 0, nhll = 0;
     // landing ring
     Chunk chunks[NCHUNK];
@@ -161,8 +175,9 @@ static int set_device(const kta_handle *h) {
     return KTA_OK;
 }
 
-// key bytes travel to the device only when they are hashed (kta_push reads the copy in pc.hash)
-static bool keys_travel(const kta_handle *h) { return h->need_hash || h->d_hash_out; }
+// key bytes travel to the device only when they are hashed, by the scan or by the partitioner check (kta_push reads the
+// copy in pc.hash)
+static bool keys_travel(const kta_handle *h) { return h->need_hash || h->d_hash_out || h->pt.ncounts; }
 
 static size_t scan_smem_bytes(bool hash, bool smem, int P, int threads, int keybuf, int stages, bool hdr) {
     return (smem ? smem_counter_bytes(P) : CTA_SCRATCH) + (size_t)(threads / 32) * warp_smem_bytes(hash, keybuf, stages, hdr);
@@ -710,15 +725,76 @@ static int launch_timeline(kta_handle *h, const ScanParams &prm) {
     return KTA_OK;
 }
 
+// Launch shape of the partitioner pass over n records with key_bytes key bytes: PC_THREADS per CTA, a stage per warp
+// sized from the mean key span of a tile (12.5 % headroom, as the scan sizes its key stage) within what the shared memory
+// leaves beside the table and the counters, as many CTAs as are resident (at most one warp per tile), and enough that none
+// takes more than PC_MAX_CTA_TILES tiles
+static int partitioner_shape(const kta_handle *h, int64_t n, int64_t key_bytes, int &grid, int &stage, size_t &smem) {
+    const Partitioner &t = h->pt;
+    const int64_t ntiles = (n + TILE - 1) / TILE;
+    const size_t fixed = (size_t)PC_TABLE_WORDS * 4 + (t.smem ? ((size_t)(2 * t.ncounts + 1) * h->cfg.num_partitions + 3) / 4 * 16 : 0);
+    const int64_t room = ((int64_t)h->smem_optin - (int64_t)fixed) / PC_WARPS - PC_STAGE_PAD;
+    const int64_t per_tile = n > 0 ? (std::max<int64_t>(key_bytes, 0) * TILE + n - 1) / n : 0;
+    int64_t want = (per_tile + per_tile / 8 + 64 + 15) / 16 * 16;
+    want = std::min<int64_t>(std::max<int64_t>(want, PC_STAGE_MIN), PC_STAGE_MAX);
+    stage = (int)std::min<int64_t>(want, room / 16 * 16);
+    smem = fixed + (size_t)PC_WARPS * (size_t)(stage + PC_STAGE_PAD);
+    int per_sm = 0;
+    if (t.smem) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, partitioner_kernel<true>, PC_THREADS, smem));
+    else CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, partitioner_kernel<false>, PC_THREADS, smem));
+    if (per_sm < 1) return fail(KTA_ERR_CUDA, "partitioner kernel does not fit an SM (%zu B shared memory)", smem);
+    int64_t g = std::min<int64_t>((ntiles + PC_WARPS - 1) / PC_WARPS, (int64_t)h->sm_count * per_sm);
+    if (t.max_grid) g = std::min<int64_t>(g, t.max_grid);
+    g = std::max<int64_t>(g, (ntiles + PC_MAX_CTA_TILES - 1) / PC_MAX_CTA_TILES);
+    grid = (int)std::max<int64_t>(g, 1);
+    return KTA_OK;
+}
+
+// the partitioner pass over the columns and key bytes a counted scan has just read (same stream, so a ring chunk's
+// free_ev, recorded after launch_scan, covers it)
+static int launch_partitioner(kta_handle *h, const ScanParams &prm, int64_t key_bytes) {
+    const Partitioner &t = h->pt;
+    PartitionerParams pp{};
+    pp.n = prm.n;
+    pp.ntiles = (prm.n + TILE - 1) / TILE;
+    pp.partition = prm.partition;
+    pp.key_len = prm.key_len;
+    pp.key_bytes = prm.key_bytes;
+    pp.key_tile_base = prm.key_tile_base;
+    pp.P = h->cfg.num_partitions;
+    pp.shard_world = h->shard_world;
+    pp.shard_rank = h->shard_rank;
+    pp.C = t.ncounts;
+    for (int j = 0; j < t.ncounts; j++) {
+        pp.count[j] = (uint32_t)t.counts[j];
+        pp.recip[j] = ~0ull / (uint64_t)t.counts[j] + 1ull;   // ceil(2^64 / N) mod 2^64
+    }
+    pp.tables = h->d_crc32_tables;
+    pp.out = t.d_counts;
+    int grid = 0, rc;
+    size_t smem = 0;
+    if ((rc = partitioner_shape(h, prm.n, key_bytes, grid, pp.stage, smem))) return rc;
+    if (t.smem) partitioner_kernel<true><<<grid, PC_THREADS, smem, h->stream>>>(pp);
+    else partitioner_kernel<false><<<grid, PC_THREADS, smem, h->stream>>>(pp);
+    CU(cudaGetLastError());
+    h->launches++;
+    return KTA_OK;
+}
+
 // one scan of a batch whose columns lie in ring chunk `chunk` (-1: elsewhere); `seq_ends`: see alive_prepare
 static int launch_scan(kta_handle *h, ScanParams prm, int64_t key_readable, int64_t key_bytes, int chunk = -1,
                        const uint64_t *seq_ends = nullptr) {
     if (prm.n <= 0) return KTA_OK;
     const bool exact = h->alive.d_table != nullptr;
     int rc;
+    if (h->pt.ncounts) {   // (checked before anything is launched: a refused batch leaves the handle as it was)
+        if (!prm.key_tile_base) return fail(KTA_ERR_INVALID, "internal: key_tile_base missing");
+        if (!prm.key_bytes && key_readable > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL but the partitioner check needs the keys");
+    }
     if (exact && (rc = alive_prepare(h, prm, seq_ends))) return rc;
     if ((rc = launch_scan_raw(h, prm, key_readable, key_bytes))) return rc;
     if (h->tl.buckets && (rc = launch_timeline(h, prm))) return rc;
+    if (h->pt.ncounts && (rc = launch_partitioner(h, prm, key_bytes))) return rc;
     if (exact && (rc = alive_scanned(h, prm, key_readable, key_bytes, chunk))) return rc;
     h->records += (uint64_t)prm.n;
     h->finalized = false;
@@ -784,6 +860,17 @@ static int scan_device_batch(kta_handle *h, const kta_batch *b) {
     if (keys_travel(h) && !prm.key_tile_base) {
         if ((rc = derive_tile_base(h, b->key_len, b->n))) return rc;
         prm.key_tile_base = h->d_tb_scratch;
+    }
+    if (h->pt.ncounts && !b->key_bytes) {
+        // The partitioner check hashes every key: without key bytes the batch may only have null and empty keys.  A
+        // declared byte count is refused at once; otherwise the tile base's total is read back, one host round trip.  Only a
+        // caller's batch without key bytes pays it: the log path hands over its gather buffer, which is never NULL.
+        if (b->key_bytes_len > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL but key_bytes_len is %lld", (long long)b->key_bytes_len);
+        uint64_t total = 0;
+        CU(cudaMemcpyAsync(&total, prm.key_tile_base + (b->n + TILE - 1) / TILE, 8, cudaMemcpyDeviceToHost, h->stream));
+        CU(cudaStreamSynchronize(h->stream));
+        if (total) return fail(KTA_ERR_INVALID, "key_bytes is NULL but the batch has %llu key bytes (the partitioner check hashes them)",
+                               (unsigned long long)total);
     }
     if ((rc = launch_scan(h, prm, b->key_bytes_len, b->key_bytes_len))) return rc;
     h->next_seq = std::max<uint64_t>(h->next_seq, seq_base + (uint64_t)b->n);
@@ -1118,6 +1205,10 @@ extern "C" int kta_push_batch_host(kta_handle *h, const kta_batch *b) {
     if ((rc = check_batch(h, b)) || b->n == 0) return rc;
     const bool hash = keys_travel(h);
     if (hash && !b->key_bytes && b->key_bytes_len > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL");
+    if (h->pt.ncounts && !b->key_bytes)
+        for (int64_t i = 0; i < b->n; i++)
+            if (b->key_len[i] > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL but record %lld has a %d-byte key (the partitioner "
+                                               "check hashes it)", (long long)i, b->key_len[i]);
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;  // keep seq order with earlier kta_push records
     if ((rc = ring_dev_init(h))) return rc;
@@ -1228,6 +1319,7 @@ extern "C" int kta_reset(kta_handle *h) {
     o.dirty = !o.win.empty();
     for (uint64_t &v : o.totals) v = 0;
     if (h->tl.buckets) CU(cudaMemsetAsync(h->tl.d_bins, 0, h->tl.words() * 8, h->stream));   // (its configuration stays)
+    if (h->pt.ncounts) CU(cudaMemsetAsync(h->pt.d_counts, 0, h->pt.words() * 8, h->stream));   // (so does the check's)
     return state_reset_device(h);
 }
 
@@ -1254,6 +1346,10 @@ extern "C" int kta_finalize(kta_handle *h) {
     if (h->tl.buckets) {
         h->tl.h_bins.resize(h->tl.words());
         CU(cudaMemcpyAsync(h->tl.h_bins.data(), h->tl.d_bins, h->tl.words() * 8, cudaMemcpyDeviceToHost, s));
+    }
+    if (h->pt.ncounts) {
+        h->pt.h_counts.resize(h->pt.words());
+        CU(cudaMemcpyAsync(h->pt.h_counts.data(), h->pt.d_counts, h->pt.words() * 8, cudaMemcpyDeviceToHost, s));
     }
     CU(cudaStreamSynchronize(s));
     if ((rc = collect_timing(h))) return rc;
@@ -1493,6 +1589,86 @@ extern "C" int kta_timeline_shape(const kta_handle *h, int64_t n, int32_t *grid,
     return KTA_OK;
 }
 
+extern "C" int kta_set_partitioner_check(kta_handle *h, const int32_t *counts, int32_t ncounts) {
+    if (!h) return fail(KTA_ERR_INVALID, "null handle");
+    if (h->records || h->pc.n)
+        return fail(KTA_ERR_INVALID, "the partitioner check is configured before the first record: records were pushed or "
+                    "scanned since create or the last kta_reset");
+    if (ncounts < 0 || ncounts > KTA_PARTITIONER_MAX_COUNTS)
+        return fail(KTA_ERR_INVALID, "partitioner check of %d counts: outside [0, %d]", ncounts, KTA_PARTITIONER_MAX_COUNTS);
+    if (ncounts && !counts) return fail(KTA_ERR_INVALID, "counts is NULL");
+    for (int j = 0; j < ncounts; j++) {
+        if (counts[j] < 1) return fail(KTA_ERR_INVALID, "partition count %d: outside [1, 2^31 - 1]", counts[j]);
+        for (int i = 0; i < j; i++)
+            if (counts[i] == counts[j]) return fail(KTA_ERR_INVALID, "partition count %d given twice", counts[j]);
+    }
+    int rc;
+    if ((rc = set_device(h))) return rc;
+    if (ncounts && !h->d_crc32_tables) {
+        uint32_t tables[4][256];
+        crc_slicing_tables_host(tables, ZLIB_CRC32_POLY);
+        DevBuf<uint32_t> d;
+        if ((rc = d.alloc(PC_TABLE_WORDS))) return rc;
+        CU(cudaMemcpy(d, &tables[0][0], sizeof tables, cudaMemcpyHostToDevice));
+        h->d_crc32_tables = std::move(d);
+    }
+    // the new configuration is built aside and swapped in only when complete: a failure keeps the old one
+    Partitioner t;
+    if (ncounts) {
+        const int64_t words = (int64_t)(2 * ncounts + 1) * h->cfg.num_partitions;
+        if ((rc = t.d_counts.alloc(words))) return rc;
+        t.ncounts = ncounts;
+        std::copy(counts, counts + ncounts, t.counts);
+        // counters in shared memory when they fit beside the table and a smallest stage per warp
+        t.smem = (size_t)PC_TABLE_WORDS * 4 + (size_t)(words + 3) / 4 * 16 + (size_t)PC_WARPS * (PC_STAGE_MIN + PC_STAGE_PAD) <= h->smem_optin;
+        CU(cudaFuncSetAttribute(partitioner_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+        CU(cudaFuncSetAttribute(partitioner_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+        CU(cudaMemsetAsync(t.d_counts, 0, (size_t)words * 8, h->stream));
+        t.h_counts.assign((size_t)words, 0);   // nothing scanned yet: a finalized handle reads zeros
+    }
+    CU(cudaStreamSynchronize(h->stream));   // the zeroing has landed, and no queued pass still uses the old counters
+    h->pt = std::move(t);
+    h->pc.hash = keys_travel(h);   // from now on kta_push copies the keys (nothing is in the landing ring)
+    return KTA_OK;
+}
+
+extern "C" int kta_partitioner_check(const kta_handle *h, int32_t partition, uint64_t *out, int64_t cap) {
+    if (!h || cap < 0 || (cap && !out)) return fail(KTA_ERR_INVALID, "bad argument");
+    if (!h->pt.ncounts) return fail(KTA_ERR_NOT_ENABLED, "the partitioner check is off (kta_set_partitioner_check)");
+    const int rc = check_read(h, partition, true);
+    if (rc > 0) return rc;
+    const int64_t nv = 2 * (int64_t)h->pt.ncounts + 1, n = std::min<int64_t>(cap, nv);
+    for (int64_t b = 0; b < n; b++)
+        out[b] = rc < 0 ? 0 : h->pt.h_counts[(size_t)b * (size_t)h->cfg.num_partitions + (size_t)partition];
+    return KTA_OK;
+}
+
+// test hook: the partitioner pass's launch shape for a scan of n records with key_bytes key bytes (grid, stage bytes per
+// warp, 1 = counters in shared memory)
+extern "C" int kta_partitioner_shape(const kta_handle *h, int64_t n, int64_t key_bytes, int32_t *grid, int32_t *stage,
+                                     int32_t *smem_counters) {
+    if (!h || n < 0 || !grid || !stage || !smem_counters) return fail(KTA_ERR_INVALID, "bad argument");
+    if (!h->pt.ncounts) return fail(KTA_ERR_NOT_ENABLED, "the partitioner check is off (kta_set_partitioner_check)");
+    int rc;
+    if ((rc = set_device(h))) return rc;
+    int g = 0, st = 0;
+    size_t sm = 0;
+    if ((rc = partitioner_shape(h, n, key_bytes, g, st, sm))) return rc;
+    *grid = g;
+    *stage = st;
+    *smem_counters = h->pt.smem ? 1 : 0;
+    return KTA_OK;
+}
+
+// test hook: at most max_ctas CTAs per partitioner pass (0: as many as are resident), so that one CTA can be given its full
+// PC_MAX_CTA_TILES tiles; the tile cap still raises the grid above the limit
+extern "C" int kta_partitioner_limit_grid(kta_handle *h, int32_t max_ctas) {
+    if (!h || max_ctas < 0) return fail(KTA_ERR_INVALID, "bad argument");
+    if (!h->pt.ncounts) return fail(KTA_ERR_NOT_ENABLED, "the partitioner check is off (kta_set_partitioner_check)");
+    h->pt.max_grid = max_ctas;
+    return KTA_OK;
+}
+
 // Ertl 2017, "New cardinality estimation algorithms for HyperLogLog sketches": improved raw estimator
 static double hll_sigma(double x) {
     if (x == 1.0) return INFINITY;
@@ -1564,6 +1740,45 @@ extern "C" int kta_fnv32_host(kta_handle *h, int64_t n, const int32_t *key_len, 
     return KTA_OK;
 }
 
+extern "C" int kta_partitioner_hash_host(kta_handle *h, int64_t n, const int32_t *key_len, const uint8_t *key_bytes,
+                                         int64_t key_bytes_len, uint32_t *murmur2, uint32_t *crc32) {
+    if (!h || n < 0 || (n && (!key_len || !murmur2 || !crc32))) return fail(KTA_ERR_INVALID, "bad argument");
+    if (n == 0) return KTA_OK;
+    int rc;
+    if ((rc = set_device(h))) return rc;
+    std::vector<uint64_t> off((size_t)n);
+    uint64_t acc = 0;
+    for (int64_t i = 0; i < n; i++) {
+        off[(size_t)i] = acc;
+        acc += key_len[i] > 0 ? (uint64_t)key_len[i] : 0;
+    }
+    if ((int64_t)acc > key_bytes_len) return fail(KTA_ERR_INVALID, "key_bytes_len %lld < sum of key_len %llu",
+                                                  (long long)key_bytes_len, (unsigned long long)acc);
+    if (acc && !key_bytes) return fail(KTA_ERR_INVALID, "key_bytes is NULL");
+    uint32_t tables[4][256];
+    crc_slicing_tables_host(tables, ZLIB_CRC32_POLY);
+    DevBuf<int32_t> d_len;
+    DevBuf<uint64_t> d_off;
+    DevBuf<uint8_t> d_keys;
+    DevBuf<uint32_t> d_out, d_tables;
+    cudaStream_t s = h->stream;
+    if ((rc = d_len.alloc(n)) || (rc = d_off.alloc(n)) || (rc = d_keys.alloc((int64_t)acc + 16)) || (rc = d_out.alloc(2 * n)) ||
+        (rc = d_tables.alloc(PC_TABLE_WORDS)))
+        return rc;
+    CU(cudaMemcpyAsync(d_len, key_len, n * 4, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(d_off, off.data(), n * 8, cudaMemcpyHostToDevice, s));
+    CU(cudaMemcpyAsync(d_tables, &tables[0][0], sizeof tables, cudaMemcpyHostToDevice, s));
+    if (acc) CU(cudaMemcpyAsync(d_keys, key_bytes, acc, cudaMemcpyHostToDevice, s));
+    partitioner_hash_kernel<<<(int)std::min<int64_t>((n + 255) / 256, 1024), 256, 0, s>>>(n, d_len, d_off, d_keys, d_tables, d_out,
+                                                                                         d_out + n);
+    h->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(murmur2, d_out, n * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(crc32, d_out + n, n * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    return KTA_OK;
+}
+
 // test hook: capture the per-record hash computed inside the fused scan (device buffer of n u32, or NULL)
 extern "C" int kta_set_hash_capture(kta_handle *h, uint32_t *dev_out) {
     if (!h) return fail(KTA_ERR_INVALID, "null handle");
@@ -1578,12 +1793,12 @@ extern "C" int kta_set_hash_capture(kta_handle *h, uint32_t *dev_out) {
 // ------------------------------------------------------------------------------------------------
 // multi-GPU merge
 // ------------------------------------------------------------------------------------------------
-// words of the merge buffer in front of the timeline segment
+// words of the merge buffer in front of the timeline segment (the partitioner check's segment follows the timeline's)
 static size_t merge_base_words(const kta_handle *h, int32_t world) { return h->nsums + (size_t)world * 4 + (size_t)world * (h->nhll / 8); }
 
 extern "C" int64_t kta_merge_words(const kta_handle *h, int32_t world) {
     if (!h || world < 1) return -1;
-    return (int64_t)(merge_base_words(h, world) + h->tl.words());
+    return (int64_t)(merge_base_words(h, world) + h->tl.words() + h->pt.words());
 }
 
 extern "C" int kta_merge_export_device(kta_handle *h, int32_t rank, int32_t world, uint64_t *dev_buf) {
@@ -1599,6 +1814,10 @@ extern "C" int kta_merge_export_device(kta_handle *h, int32_t rank, int32_t worl
     // the timeline arrays go at the end as they are: the SUM all-reduce adds every rank's rows (foreign rows are zero)
     if (h->tl.buckets)
         CU(cudaMemcpyAsync(dev_buf + merge_base_words(h, world), h->tl.d_bins, h->tl.words() * 8, cudaMemcpyDeviceToDevice, h->stream));
+    // so do the partitioner check's counters, behind the timeline's
+    if (h->pt.ncounts)
+        CU(cudaMemcpyAsync(dev_buf + merge_base_words(h, world) + h->tl.words(), h->pt.d_counts, h->pt.words() * 8,
+                           cudaMemcpyDeviceToDevice, h->stream));
     // With its own stream the handle must finish before the caller's collective may read the buffer.  On an
     // adopted stream (kta_set_stream) the caller's collective is ordered behind this kernel by the stream itself.
     if (h->own_stream) {
@@ -1619,6 +1838,9 @@ extern "C" int kta_merge_import_device(kta_handle *h, int32_t world, const uint6
     CU(cudaGetLastError());
     if (h->tl.buckets)
         CU(cudaMemcpyAsync(h->tl.d_bins, dev_buf + merge_base_words(h, world), h->tl.words() * 8, cudaMemcpyDeviceToDevice, h->stream));
+    if (h->pt.ncounts)
+        CU(cudaMemcpyAsync(h->pt.d_counts, dev_buf + merge_base_words(h, world) + h->tl.words(), h->pt.words() * 8,
+                           cudaMemcpyDeviceToDevice, h->stream));
     h->finalized = false;
     if (h->own_stream) CU(cudaStreamSynchronize(h->stream));
     return KTA_OK;

@@ -66,14 +66,20 @@ __host__ __device__ __forceinline__ uint32_t crc32c_mulmod(uint32_t a, uint32_t 
     return p;
 }
 
-inline void log_crc_tables_host(LogCrcTables &t) {
+// the four slicing-by-4 tables of a reflected CRC-32 with polynomial `poly` (0x82F63B78 CRC-32C, 0xEDB88320 zlib's CRC-32):
+// t[0] the byte table, t[k][i] = t[0] applied to t[k-1][i] once more
+inline void crc_slicing_tables_host(uint32_t (&t)[4][256], uint32_t poly) {
     for (uint32_t i = 0; i < 256; i++) {
         uint32_t c = i;
-        for (int k = 0; k < 8; k++) c = (c >> 1) ^ ((0u - (c & 1u)) & CRC32C_POLY);
-        t.t[0][i] = c;
+        for (int k = 0; k < 8; k++) c = (c >> 1) ^ ((0u - (c & 1u)) & poly);
+        t[0][i] = c;
     }
     for (int k = 1; k < 4; k++)
-        for (int i = 0; i < 256; i++) t.t[k][i] = (t.t[k - 1][i] >> 8) ^ t.t[0][t.t[k - 1][i] & 0xffu];
+        for (int i = 0; i < 256; i++) t[k][i] = (t[k - 1][i] >> 8) ^ t[0][t[k - 1][i] & 0xffu];
+}
+
+inline void log_crc_tables_host(LogCrcTables &t) {
+    crc_slicing_tables_host(t.t, CRC32C_POLY);
     uint32_t xs = CRC32C_ONE;   // x^(8 S)
     for (uint32_t i = 0; i < 8 * LOG_CRC_SPAN; i++) xs = (xs >> 1) ^ ((0u - (xs & 1u)) & CRC32C_POLY);
     t.pow_lo[0] = CRC32C_ONE;
@@ -111,12 +117,16 @@ __device__ __forceinline__ void log_crc_count_pass(const uint8_t *bytes, int64_t
     if (blockIdx.x == 0 && threadIdx.x == 0) spans[0] = 0;
 }
 
-// table k, entry i, in the lane's replica (tl = table base + lane): word (k * 256 + i) * 32 sits in the lane's own bank
-#define LOG_CRC_T(k, i) tl[((k) * 256 + (i)) * 32]
+// The slicing steps of any reflected CRC-32: the polynomial lives in the tables (crc_slicing_tables_host).  Table k, entry
+// i, sits at word (k * 256 + i) * R of the table base tl.  R = 32: one replica per lane (tl = table base + lane), so the
+// word lies in the lane's own bank; R = 1: one shared copy.
+#define LOG_CRC_T(k, i) tl[((k) * 256 + (i)) * R]
 
+template <int R = 32>
 __device__ __forceinline__ uint32_t crc_byte(uint32_t crc, uint32_t byte, const uint32_t *tl) {
     return LOG_CRC_T(0, (crc ^ byte) & 0xffu) ^ (crc >> 8);
 }
+template <int R = 32>
 __device__ __forceinline__ uint32_t crc_word(uint32_t crc, uint32_t w, const uint32_t *tl) {
     crc ^= w;
     return LOG_CRC_T(3, crc & 0xffu) ^ LOG_CRC_T(2, (crc >> 8) & 0xffu) ^ LOG_CRC_T(1, (crc >> 16) & 0xffu) ^ LOG_CRC_T(0, crc >> 24);

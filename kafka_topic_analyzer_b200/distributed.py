@@ -55,21 +55,26 @@ def allreduce_merge(engine: KtaEngine, group=None, counters_only: bool = False) 
 # Host-side statement of the merge-buffer layout (what merge_export_kernel / merge_import_kernel do on the
 # device, csrc/kta_kernels.cuh).  Used by the gloo CPU tests of the N>1 logic and usable for host-side merges.
 #   [ sums (nsums u64) | world × 4 extrema slots | world × (nhll/8) words, eight one-byte registers per word
-#     | timeline (3 × P × (B + 2) u64, only when the timeline is on) ]
-# Every rank fills only its own slots, so ONE SUM all-reduce hands every rank's values to every rank.  The timeline
-# segment is summed as it is (a sharded rank's foreign rows are zero); every rank must use the same timeline.
+#     | timeline (3 × P × (B + 2) u64, only when the timeline is on)
+#     | partitioner check ((2C + 1) × P u64, only when the check is on) ]
+# Every rank fills only its own slots, so ONE SUM all-reduce hands every rank's values to every rank.  The timeline and
+# partitioner segments are summed as they are (a sharded rank's foreign rows are zero); every rank must use the same
+# timeline and check the same partition counts.
 # ---------------------------------------------------------------------------------------------------
-def merge_words(nsums: int, nhll: int, world: int, timeline_words: int = 0) -> int:
-    return nsums + world * 4 + world * (nhll // 8) + timeline_words
+def merge_words(nsums: int, nhll: int, world: int, timeline_words: int = 0, partitioner_words: int = 0) -> int:
+    return nsums + world * 4 + world * (nhll // 8) + timeline_words + partitioner_words
 
 
-def pack_merge_buffer(sums, minmax, hll, rank: int, world: int, timeline=None):
+def pack_merge_buffer(sums, minmax, hll, rank: int, world: int, timeline=None, partitioner=None):
     """sums u64[nsums]; minmax = (min_ts i64, max_ts i64, min_size u64, max_size u64); hll u32[nhll];
-    timeline: None, or the u64 [3][P][B + 2] arrays (any shape; taken flat)."""
+    timeline: None, or the u64 [3][P][B + 2] arrays (any shape; taken flat); partitioner: None, or the u64 [2C + 1][P]
+    partitioner-check counters (any shape; taken flat)."""
     import numpy as np
     nsums, nhll = len(sums), len(hll)
     tl = None if timeline is None else np.asarray(timeline, dtype=np.uint64).ravel()
-    buf = np.zeros(merge_words(nsums, nhll, world, 0 if tl is None else tl.size), dtype=np.uint64)
+    pt = None if partitioner is None else np.asarray(partitioner, dtype=np.uint64).ravel()
+    tw = 0 if tl is None else tl.size
+    buf = np.zeros(merge_words(nsums, nhll, world, tw, 0 if pt is None else pt.size), dtype=np.uint64)
     buf[:nsums] = np.asarray(sums, dtype=np.uint64)
     mm = np.array([minmax[0], minmax[1]], dtype=np.int64).view(np.uint64)
     buf[nsums + 4 * rank: nsums + 4 * rank + 2] = mm
@@ -81,13 +86,16 @@ def pack_merge_buffer(sums, minmax, hll, rank: int, world: int, timeline=None):
         o = nsums + 4 * world + rank * hw
         buf[o:o + hw] = regs.view(np.uint64) if regs.flags["C_CONTIGUOUS"] else np.ascontiguousarray(regs).view(np.uint64)
     if tl is not None:
-        buf[merge_words(nsums, nhll, world):] = tl
+        buf[merge_words(nsums, nhll, world):merge_words(nsums, nhll, world, tw)] = tl
+    if pt is not None:
+        buf[merge_words(nsums, nhll, world, tw):] = pt
     return buf
 
 
-def fold_merge_buffer(buf, nsums: int, nhll: int, world: int, timeline_words: int = 0):
+def fold_merge_buffer(buf, nsums: int, nhll: int, world: int, timeline_words: int = 0, partitioner_words: int = 0):
     """inverse of pack after the SUM all-reduce: returns (sums, (min_ts, max_ts, min_size, max_size), hll), and the
-    flat timeline segment as a fourth element when timeline_words > 0."""
+    flat timeline segment as a fourth element when timeline_words > 0.  With partitioner_words > 0 the result has five
+    elements: the timeline segment (empty without a timeline), then the flat partitioner-check segment."""
     import numpy as np
     sums = buf[:nsums].copy()
     mm = buf[nsums:nsums + 4 * world].reshape(world, 4)
@@ -99,7 +107,11 @@ def fold_merge_buffer(buf, nsums: int, nhll: int, world: int, timeline_words: in
         hw = nhll // 8
         w = np.ascontiguousarray(buf[nsums + 4 * world:nsums + 4 * world + world * hw]).view(np.uint8).reshape(world, nhll)
         hll[:] = w.max(axis=0)
+    base = merge_words(nsums, nhll, world)
+    tl = np.asarray(buf[base:base + timeline_words], dtype=np.uint64).copy()
+    if partitioner_words:
+        pt = np.asarray(buf[base + timeline_words:base + timeline_words + partitioner_words], dtype=np.uint64).copy()
+        return sums, (tmin, tmax, smin, smax), hll, tl, pt
     if timeline_words:
-        base = merge_words(nsums, nhll, world)
-        return sums, (tmin, tmax, smin, smax), hll, np.asarray(buf[base:base + timeline_words], dtype=np.uint64).copy()
+        return sums, (tmin, tmax, smin, smax), hll, tl
     return sums, (tmin, tmax, smin, smax), hll

@@ -88,6 +88,7 @@ class KtaEngine:
         self.hll_precision = hll_precision
         self.shares_caller_stream = False   # True after set_stream(): work is ordered by the caller's stream
         self.timeline_buckets = 0           # set_timeline
+        self.partitioner_counts = ()        # set_partitioner_check
         self.message_metrics = MessageMetrics(self)
         self.log_compaction_metrics = LogCompactionInMemoryMetrics(self) if count_alive_keys else None
 
@@ -253,6 +254,46 @@ class KtaEngine:
         g, t, s = C.c_int32(), C.c_int32(), C.c_int32()
         check(lib().kta_timeline_shape(self._h, n, C.byref(g), C.byref(t), C.byref(s)))
         return g.value, t.value, bool(s.value)
+
+    def set_partitioner_check(self, counts) -> None:
+        """Per partition, count the keyed records that Kafka's murmur2 partitioner and librdkafka's CRC-32 partitioner
+        would place there at each partition count in `counts` (at most 8, distinct, each in [1, 2^31 - 1];
+        include/kta.h).  Only before the first record (after create or reset); an empty list turns it off; reset() keeps
+        the setting."""
+        counts = [int(c) for c in counts]
+        bad = [c for c in counts if not 1 <= c < 1 << 31]
+        if bad:   # (ctypes would wrap them into int32 silently)
+            raise KtaError(N.ERR_INVALID, "partition count %d outside [1, 2^31 - 1]" % bad[0])
+        arr = (C.c_int32 * max(len(counts), 1))(*counts)
+        check(lib().kta_set_partitioner_check(self._h, arr, len(counts)))
+        self.partitioner_counts = tuple(counts)
+
+    def partitioner_check(self, p: int) -> np.ndarray:
+        """One partition's 2C + 1 u64 after finalize(): murmur2 matches per count, CRC-32 matches per count, neither."""
+        n = 2 * len(self.partitioner_counts) + 1
+        out = np.zeros(n, dtype=np.uint64)
+        check(lib().kta_partitioner_check(self._h, p, out.ctypes.data_as(C.POINTER(C.c_uint64)), n))
+        return out
+
+    def partitioner_limit_grid(self, max_ctas: int) -> None:
+        """at most max_ctas CTAs per partitioner pass, 0 = no limit (test hook)."""
+        check(lib().kta_partitioner_limit_grid(self._h, max_ctas))
+
+    def partitioner_shape(self, n: int, key_bytes: int):
+        """(grid, stage bytes per warp, counters in shared memory) of the partitioner pass over a scan of n records with
+        key_bytes key bytes (test hook)."""
+        g, s, m = C.c_int32(), C.c_int32(), C.c_int32()
+        check(lib().kta_partitioner_shape(self._h, n, key_bytes, C.byref(g), C.byref(s), C.byref(m)))
+        return g.value, s.value, bool(m.value)
+
+    def partitioner_hashes(self, key_len, key_bytes):
+        """(murmur2, crc32) u32 arrays of the check's device hash functions over packed host keys (test hook)."""
+        kl = np.ascontiguousarray(key_len, dtype=np.int32)
+        kb = np.ascontiguousarray(key_bytes, dtype=np.uint8)
+        mm, cc = np.zeros(kl.size, np.uint32), np.zeros(kl.size, np.uint32)
+        check(lib().kta_partitioner_hash_host(self._h, kl.size, kl.ctypes.data, kb.ctypes.data if kb.size else None, kb.size,
+                                              mm.ctypes.data, cc.ctypes.data))
+        return mm, cc
 
     def sync(self) -> None:
         check(lib().kta_sync(self._h))
