@@ -254,6 +254,73 @@ int kta_partitioner_check(const kta_handle *h, int32_t partition, uint64_t *out,
 int kta_partitioner_hash_host(kta_handle *h, int64_t n, const int32_t *key_len, const uint8_t *key_bytes,
                               int64_t key_bytes_len, uint32_t *murmur2, uint32_t *crc32);
 
+/* Hot keys: an exact, topic-wide table of per-key counters, filled on the GPU, and the top_k keys with the most records
+ * (which keys a compacted topic is made of: a high dirty ratio or a hot partition usually comes from a few keys rewritten
+ * constantly).  Off by default.
+ *   Records counted: exactly the records the counters count (as the timeline's), and only those with a non-null key
+ *   (key_len >= 0; an empty key is a key).  Stamps-only re-runs of the alive-key table are not counted again.
+ *   Key identity: a key is its 64-bit id, (uint64_t)crc32(key) << 32 | murmur2(key) with the partitioner check's two
+ *   hashes (zlib's CRC-32 and Kafka's murmur2, unmasked).  Two distinct keys with equal ids are merged into one entry; with
+ *   D distinct keys about D^2 / 2^65 pairs collide (3e-6 expected pairs at 1e7 keys).  The prefix and key_len of a merged
+ *   entry then come from whichever key claimed its slot.
+ *   Per key: records; tombstones (value_len < 0); bytes, the sum of key_len + max(value_len, 0); latest_s, the largest
+ *   (ts_ms == -1 ? 0 : ts_ms) / 1000 over its records (truncating, the timeline's second); the smallest and largest
+ *   partition it was written to; key_len and the first min(key_len, 32) bytes of the key, zeros after.
+ * kta_set_hot_keys: top_k = 0 turns the table off; otherwise top_k lies in [1, KTA_HOT_KEYS_MAX].  table_slots = 0 means
+ * 2^20; otherwise it is a power of two in [16, 2^31].  KTA_ERR_INVALID, with nothing changed, on any violation and when a
+ * record has been pushed or scanned since create or the last kta_reset (records still in the landing ring included).  The
+ * table takes 96 bytes per slot (plus one) of device memory and is grown by rehash, doubling, so that it stays at most half
+ * full: before a launch the library keeps an upper bound on the occupancy; when a batch could take it past half the slots it
+ * reads the occupancy back (one copy to the host and a stream synchronisation), grows the table while it is more than a
+ * quarter full, and scans the batch in slices that cannot overfill it, reading the occupancy back between slices.  With the
+ * table on, a device batch may therefore wait for the device.  kta_reset zeroes the table and keeps its configuration and
+ * its allocation.  Every counted scan is followed by at least one more kernel (kta_stats counts them) that reads partition,
+ * key_len, value_len, ts_ms and the key bytes.  With the table on, key bytes reach the device on every handle: a batch with
+ * keyed records must carry key_bytes (KTA_ERR_INVALID otherwise), and kta_push copies each key.
+ * Out of memory: when the table cannot grow (cudaMalloc fails, or the kta_hot_keys_limit_slots cap), the call that scanned
+ * returns KTA_ERR_NOMEM and kta_last_error names the hot-key table.  Every other metric has counted the batch; the table
+ * stops counting, and kta_hot_keys, kta_hot_key_stats and the export return KTA_ERR_NOMEM until kta_reset.  The status is
+ * returned once, by the call whose scan hit it; a kta_push that returns it HAS taken its record (do not push it again).
+ * kta_finalize returns it only when it has no other status to return (KTA_ERR_INVALID for sequence numbers outside the
+ * window, KTA_ERR_PARTITION); the getters return it regardless.
+ * kta_hot_keys: valid after kta_finalize; copies min(cap, top_k, distinct) entries ordered by records descending, then id
+ * ascending; *count (may be NULL) = min(top_k, distinct).  KTA_ERR_NOT_ENABLED when the table is off, KTA_ERR_NOT_FINALIZED
+ * before kta_finalize.
+ * kta_hot_key_stats: valid after kta_finalize (any pointer may be NULL): the distinct keys (the table's occupancy), the keyed
+ * records (the sum of the entries' records, equal to the sum over partitions of KTA_KEY_NON_NULL), the slots, how often the
+ * table grew, and how many pass launches covered only part of a batch (slices) since create.
+ * Multi-GPU merge: the table does not travel in the merge buffer (kta_merge_words is unchanged).  kta_hot_keys_export_count
+ * gives the number of entries; kta_hot_keys_export_device writes every entry, in no particular order, to a device buffer
+ * of cap entries (KTA_ERR_INVALID if cap is smaller; *count gets the number either way).  kta_hot_keys_import_device adds
+ * count entries from device memory into the table: records, tombstones and bytes are summed, the partition range and
+ * latest_s are folded, the prefix and key_len come from the entry that claims the slot.  The table grows first, so an
+ * import never runs out of room.  The whole list is refused (KTA_ERR_INVALID, nothing applied) when an entry has
+ * records == 0, tombstones > records, key_len < 0, reserved != 0, or a partition outside [0, num_partitions) or
+ * min_partition > max_partition.  On a sharded handle the table holds the handle's own partitions' records; exporting every
+ * rank's entries and importing the others' on each rank makes it topic-wide.
+ * kta_hot_keys_limit_slots: test hook; the table may not grow beyond max_slots slots (0 = no cap). */
+#define KTA_HOT_KEYS_MAX 65536
+#define KTA_HOT_KEY_PREFIX 32
+typedef struct kta_hot_key {
+    uint64_t id;                 /* (uint64_t)crc32(key) << 32 | murmur2(key) */
+    uint64_t records;            /* delivered records with this key (key_len >= 0) */
+    uint64_t tombstones;         /* of which value_len < 0 */
+    uint64_t bytes;              /* sum of key_len + max(value_len, 0) */
+    int64_t latest_s;            /* max over its records of (ts_ms == -1 ? 0 : ts_ms) / 1000, truncating */
+    int32_t min_partition, max_partition;
+    int32_t key_len;
+    uint32_t reserved;           /* 0; keeps the struct at 88 bytes with no implicit padding */
+    uint8_t key_prefix[KTA_HOT_KEY_PREFIX];   /* first min(key_len, 32) bytes, zeros after */
+} kta_hot_key;                   /* 88 bytes */
+int kta_set_hot_keys(kta_handle *h, int32_t top_k, int64_t table_slots);
+int kta_hot_keys(const kta_handle *h, kta_hot_key *out, int64_t cap, int64_t *count);
+int kta_hot_key_stats(const kta_handle *h, uint64_t *distinct_keys, uint64_t *keyed_records, uint64_t *slots, uint64_t *grows,
+                      uint64_t *slices);
+int kta_hot_keys_export_count(kta_handle *h, int64_t *count);
+int kta_hot_keys_export_device(kta_handle *h, kta_hot_key *dev_out, int64_t cap, int64_t *count);
+int kta_hot_keys_import_device(kta_handle *h, const kta_hot_key *dev_in, int64_t count);
+int kta_hot_keys_limit_slots(kta_handle *h, int64_t max_slots);
+
 /* ---- multi-GPU merge (one process per GPU; the collective itself is the caller's: NCCL via
  * torch.distributed, or ncclAllReduce directly) ----
  * The mergeable state is exported as ONE array of u64 laid out so that a single SUM all-reduce

@@ -11,6 +11,8 @@ import os
 import subprocess
 import sys
 
+import numpy as np
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libkta_gpu.so")
@@ -25,6 +27,7 @@ READ_UNCOMMITTED, READ_COMMITTED = 0, 1   # include/kta.h KTA_READ_UNCOMMITTED /
 TIMELINE_RECORDS, TIMELINE_TOMBSTONES, TIMELINE_BYTES = 0, 1, 2   # include/kta.h KTA_TIMELINE_*
 TIMELINE_MAX_BUCKETS = 65536
 PARTITIONER_MAX_COUNTS = 8   # include/kta.h KTA_PARTITIONER_MAX_COUNTS
+HOT_KEYS_MAX, HOT_KEY_PREFIX = 65536, 32   # include/kta.h KTA_HOT_KEYS_MAX / KTA_HOT_KEY_PREFIX
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
@@ -113,6 +116,21 @@ class CrcFailure(C.Structure):
 LOG_CRC_KEEP = 4096   # include/kta.h KTA_LOG_CRC_KEEP
 
 
+class HotKey(C.Structure):
+    _fields_ = [
+        ("id", C.c_uint64), ("records", C.c_uint64), ("tombstones", C.c_uint64), ("bytes", C.c_uint64),
+        ("latest_s", C.c_int64), ("min_partition", C.c_int32), ("max_partition", C.c_int32), ("key_len", C.c_int32),
+        ("reserved", C.c_uint32), ("key_prefix", C.c_uint8 * HOT_KEY_PREFIX),
+    ]
+
+
+# include/kta.h kta_hot_key as a numpy record (88 bytes, the same offsets)
+HOT_KEY_DTYPE = np.dtype([
+    ("id", "<u8"), ("records", "<u8"), ("tombstones", "<u8"), ("bytes", "<u8"), ("latest_s", "<i8"),
+    ("min_partition", "<i4"), ("max_partition", "<i4"), ("key_len", "<i4"), ("reserved", "<u4"),
+    ("key_prefix", "u1", (HOT_KEY_PREFIX,))])
+
+
 # every symbol include/kta.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -145,6 +163,14 @@ SYMBOLS = {
     "kta_set_partitioner_check": (C.c_int, [_P, C.POINTER(C.c_int32), C.c_int32]),
     "kta_partitioner_check": (C.c_int, [_P, C.c_int32, C.POINTER(C.c_uint64), C.c_int64]),
     "kta_partitioner_hash_host": (C.c_int, [_P, C.c_int64, _P, _P, C.c_int64, _P, _P]),
+    "kta_set_hot_keys": (C.c_int, [_P, C.c_int32, C.c_int64]),
+    "kta_hot_keys": (C.c_int, [_P, _P, C.c_int64, C.POINTER(C.c_int64)]),
+    "kta_hot_key_stats": (C.c_int, [_P, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_uint64),
+                                    C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "kta_hot_keys_export_count": (C.c_int, [_P, C.POINTER(C.c_int64)]),
+    "kta_hot_keys_export_device": (C.c_int, [_P, _P, C.c_int64, C.POINTER(C.c_int64)]),
+    "kta_hot_keys_import_device": (C.c_int, [_P, _P, C.c_int64]),
+    "kta_hot_keys_limit_slots": (C.c_int, [_P, C.c_int64]),
     "kta_merge_words": (C.c_int64, [_P, C.c_int32]),
     "kta_merge_export_device": (C.c_int, [_P, C.c_int32, C.c_int32, _P]),
     "kta_merge_import_device": (C.c_int, [_P, C.c_int32, _P]),

@@ -55,11 +55,18 @@ inline std::string format_utc(int64_t secs, int32_t nanos) {
     return buf;
 }
 
+// columns a UTF-8 cell takes: its bytes that do not continue a character (ASCII cells: their size)
+inline size_t cell_width(const std::string &s) {
+    size_t n = 0;
+    for (unsigned char c : s) n += (c & 0xc0) != 0x80;
+    return n;
+}
+
 inline std::string render_table(const std::vector<std::vector<std::string>> &rows) {
     std::vector<size_t> w;
     for (const auto &r : rows) {
         if (w.size() < r.size()) w.resize(r.size(), 0);
-        for (size_t c = 0; c < r.size(); c++) w[c] = std::max(w[c], r[c].size());
+        for (size_t c = 0; c < r.size(); c++) w[c] = std::max(w[c], cell_width(r[c]));
     }
     std::string sep = "+";
     for (size_t c = 0; c < w.size(); c++) sep += std::string(w[c] + 2, '-') + "+";
@@ -69,7 +76,7 @@ inline std::string render_table(const std::vector<std::vector<std::string>> &row
         out += "|";
         for (size_t c = 0; c < w.size(); c++) {
             const std::string &cell = c < r.size() ? r[c] : std::string();
-            out += " " + cell + std::string(w[c] - cell.size(), ' ') + " |";
+            out += " " + cell + std::string(w[c] - cell_width(cell), ' ') + " |";
         }
         out += "\n" + sep;
     }
@@ -163,6 +170,47 @@ inline std::string render_partitioner_check(const std::vector<int32_t> &counts, 
     std::vector<std::string> cells = {"total", std::to_string(total.keyed)};
     for (uint64_t v : total.counts) cells.push_back(std::to_string(v));
     t.push_back(cells);
+    return o + render_table(t);
+}
+
+// extension (--hot-keys): the keys with the most records (include/kta.h kta_hot_keys), ranked
+struct HotKeyRow {
+    uint64_t records, tombstones, bytes;
+    int64_t latest_s;
+    int32_t min_partition, max_partition, key_len;
+    std::string prefix;              // the first min(key_len, 32) bytes
+};
+
+// a key as text when every byte of its prefix is printable ASCII, else as 0x-prefixed hex; "…" when the key is longer
+// than its prefix; an empty key as (empty)
+inline std::string render_key(const std::string &prefix, int32_t key_len) {
+    if (key_len == 0) return "(empty)";
+    bool text = true;
+    for (unsigned char c : prefix) text = text && c >= 0x20 && c < 0x7f;
+    std::string o;
+    if (text) {
+        o = prefix;
+    } else {
+        static const char *hex = "0123456789abcdef";
+        o = "0x";
+        for (unsigned char c : prefix) { o += hex[c >> 4]; o += hex[c & 15]; }
+    }
+    if ((size_t)key_len > prefix.size()) o += "\u2026";
+    return o;
+}
+
+inline std::string render_hot_keys(uint64_t distinct, const std::vector<HotKeyRow> &rows) {
+    std::string o = "| extension: hot keys, the keys with the most records\nDistinct keys: " + std::to_string(distinct) +
+                    " (by 64-bit id)\n";
+    std::vector<std::vector<std::string>> t = {{"#", "Records", "Tombstones", "Bytes", "Partitions", "Latest write", "Key"}};
+    for (size_t i = 0; i < rows.size(); i++) {
+        const HotKeyRow &r = rows[i];
+        const std::string parts = r.min_partition == r.max_partition
+                                      ? std::to_string(r.min_partition)
+                                      : std::to_string(r.min_partition) + "\u2013" + std::to_string(r.max_partition);
+        t.push_back({std::to_string(i + 1), std::to_string(r.records), std::to_string(r.tombstones), std::to_string(r.bytes), parts,
+                     format_utc(r.latest_s, 0), render_key(r.prefix, r.key_len)});
+    }
     return o + render_table(t);
 }
 

@@ -35,6 +35,10 @@
 //                              how many of them sit where Kafka's murmur2 partitioner would put them at each N, where
 //                              librdkafka's CRC-32 partitioner would, and where neither would; then a total row.  At most 8
 //                              distinct counts, each in [1, 2^31 - 1].
+//   --hot-keys K               extension: after the report (and the partitioner check), the number of distinct keys (by
+//                              their 64-bit id) and the K keys with the most records, ranked: records, tombstones, bytes,
+//                              the partition or partition range, the latest write (UTC) and the key (as text when its
+//                              first 32 bytes are printable, else as hex; "…" when it is longer).  K in [1, 65536].
 //
 // There is no librdkafka and no broker in this build (SURVEY.md D9): without --synthetic the program explains
 // that and exits, like the reference does when it cannot fetch metadata.  Everything numeric comes from the
@@ -216,6 +220,35 @@ static void print_partitioner_check(kta_handle *h, const std::vector<int> &parti
     fputs(kta_report::render_partitioner_check(counts, rows).c_str(), stdout);
 }
 
+// --hot-keys K: 0 = off.  Read by both analysis paths (the table is switched on right after kta_create) and by print_report.
+static int32_t g_hot_keys = 0;
+
+static bool parse_hot_keys(const std::string &arg) {
+    int64_t v = 0;
+    if (!parse_i64(arg, v) || v < 1 || v > KTA_HOT_KEYS_MAX) {
+        fprintf(stderr, "error: --hot-keys takes K: a number of keys in [1, %d], not '%s'\n", KTA_HOT_KEYS_MAX, arg.c_str());
+        return false;
+    }
+    g_hot_keys = (int32_t)v;
+    return true;
+}
+
+// the distinct keys, then the g_hot_keys keys with the most records
+static void print_hot_keys(kta_handle *h) {
+    std::vector<kta_hot_key> top((size_t)g_hot_keys);
+    int64_t n = 0;
+    uint64_t distinct = 0;
+    KTA(kta_hot_keys(h, top.data(), g_hot_keys, &n));
+    KTA(kta_hot_key_stats(h, &distinct, nullptr, nullptr, nullptr, nullptr));
+    std::vector<kta_report::HotKeyRow> rows;
+    for (int64_t i = 0; i < n; i++) {
+        const kta_hot_key &k = top[(size_t)i];
+        rows.push_back({k.records, k.tombstones, k.bytes, k.latest_s, k.min_partition, k.max_partition, k.key_len,
+                        std::string((const char *)k.key_prefix, (size_t)std::min(k.key_len, KTA_HOT_KEY_PREFIX))});
+    }
+    fputs(kta_report::render_hot_keys(distinct, rows).c_str(), stdout);
+}
+
 static int print_report(kta_handle *h, const std::string &topic, const std::vector<int> &partitions, const std::vector<int64_t> &start_offsets,
                         const std::vector<int64_t> &end_offsets, bool alive, int hll, uint64_t duration_secs, const TimelineOpt &tl,
                         const std::vector<int32_t> &pcounts);
@@ -348,6 +381,7 @@ static int analyze_log_dir(const std::string &topic, const std::string &dir, boo
     if (check_crcs) KTA(kta_log_set_check_crcs(h, 1));
     if (tl.on) KTA(kta_set_timeline(h, tl.origin, tl.width, (int32_t)tl.buckets));
     if (!pcounts.empty()) KTA(kta_set_partitioner_check(h, pcounts.data(), (int32_t)pcounts.size()));
+    if (g_hot_keys) KTA(kta_set_hot_keys(h, g_hot_keys, 0));
     // the window of every partition the checkpoints list: the log start offset raised to the first segment's base offset
     // (its 20-digit file name, as the broker loads a log), the high watermark no lower than that (it is clamped to the log
     // end offset once the files are read: no batch lies beyond it, so the window reads the same either way)
@@ -466,6 +500,7 @@ int main(int argc, char **argv) {
         else if (a == "--hll") hll = atoi(val().c_str());
         else if (a == "--timeline") { if (!parse_timeline(val(), tl)) return 2; }
         else if (a == "--partitioner-check") { if (!parse_partitioner_check(val(), pcounts)) return 2; }
+        else if (a == "--hot-keys") { if (!parse_hot_keys(val())) return 2; }
         else if (a == "-V" || a == "--version") { puts("Kafka Topic Analyzer 0.4.1"); return 0; }  // main.rs:35
         else if (a == "-h" || a == "--help") {
             puts("Kafka Topic Analyzer 0.4.1\n\nUSAGE:\n    kafka-topic-analyzer [FLAGS] [OPTIONS] --bootstrap-server <BOOTSTRAP_SERVER> --topic <TOPIC>\n\n"
@@ -492,7 +527,9 @@ int main(int argc, char **argv) {
                  "                                                 buckets)\n"
                  "        --partitioner-check <N[,N...]>           extension: per partition, the keyed records that murmur2\n"
                  "                                                 (Java) and CRC-32 (librdkafka) would place there at each\n"
-                 "                                                 partition count N, printed after the report");
+                 "                                                 partition count N, printed after the report\n"
+                 "        --hot-keys <K>                           extension: the number of distinct keys and the K keys with\n"
+                 "                                                 the most records, printed after the report");
             return 0;
         } else { fprintf(stderr, "error: Found argument '%s' which wasn't expected\n", a.c_str()); return 2; }
     }
@@ -584,6 +621,7 @@ int main(int argc, char **argv) {
     KTA(kta_create(&cfg, &h));
     if (tl.on) KTA(kta_set_timeline(h, tl.origin, tl.width, (int32_t)tl.buckets));
     if (!pcounts.empty()) KTA(kta_set_partitioner_check(h, pcounts.data(), (int32_t)pcounts.size()));
+    if (g_hot_keys) KTA(kta_set_hot_keys(h, g_hot_keys, 0));
 
     printf("Subscribing to %s\n", topic.c_str());          // src/kafka.rs:88
     printf("Starting message consumption...\n");            // src/kafka.rs:91
@@ -687,5 +725,6 @@ static int print_report(kta_handle *h, const std::string &topic, const std::vect
     if (hll) { double e = 0; KTA(kta_alive_keys_hll(h, &e)); printf("| extension: HyperLogLog(p=%d) alive-key estimate: %.0f\n", hll, e); }
     if (tl.on) print_timeline(h, partitions, tl);
     if (!pcounts.empty()) print_partitioner_check(h, partitions, pcounts);
+    if (g_hot_keys) print_hot_keys(h);
     return 0;
 }

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "kta_host.cuh"
+#include "kta_hotkeys.cuh"
 #include "kta_kernels.cuh"
 #include "kta_logscan.cuh"
 #include "kta_partitioner.cuh"
@@ -114,6 +115,29 @@ struct Partitioner {
     size_t words() const { return d_counts.cap > 0 ? (size_t)d_counts.cap : 0; }
 };
 
+// The hot-key table (kta_set_hot_keys): its configuration, the table, the occupancy bound and the host mirror; only the
+// hk_* functions and the hot-key entry points touch them
+struct HotKeys {
+    int32_t top_k = 0;                       // 0 = off
+    uint64_t slots = 0;                      // power of two; the side slot (id 0) follows them
+    uint64_t max_slots = 0;                  // test hook (kta_hot_keys_limit_slots): 0 = no cap
+    DevBuf<HkSlot> d_table;                  // [slots + 1]
+    DevBuf<unsigned long long> d_word;       // [0] occupancy, [1] probe failure (u32), [2] export cursor, [3] records, [4] refusal
+    uint64_t bound = 0;                      // U: the occupancy is at most this
+    uint64_t grows = 0, slices = 0;
+    bool nomem = false;                      // growth failed: nothing is counted until kta_reset
+    bool unreported = false;                 // ... and the entry point that scanned has not returned KTA_ERR_NOMEM yet
+    char nomem_msg[256] = "";
+    // finalize's scratch and the host mirror (valid after finalize)
+    DevBuf<kta_hot_key> d_entries, d_top;
+    DevBuf<HkSortKey> d_keys;                // [2][distinct]
+    DevBuf<uint32_t> d_idx;                  // [2][distinct]
+    DevBuf<uint8_t> d_sort_tmp;
+    std::vector<kta_hot_key> h_top;
+    uint64_t h_distinct = 0, h_keyed = 0;
+    HkTable table() { return HkTable{d_table, slots, d_word, reinterpret_cast<unsigned int *>(d_word.get() + 1)}; }
+};
+
 struct kta_handle {
     kta_config cfg{};
     int device = 0;
@@ -132,7 +156,8 @@ struct kta_handle {
     LogScan log;
     Timeline tl;
     Partitioner pt;
-    DevBuf<uint32_t> d_crc32_tables;         // zlib CRC-32 slicing tables of the partitioner check (made on first use)
+    HotKeys hk;
+    DevBuf<uint32_t> d_crc32_tables;         // zlib CRC-32 slicing tables of the partitioner check and the hot-key table (made on first use)
     size_t nsums = 0, nhll = 0;
     // landing ring
     Chunk chunks[NCHUNK];
@@ -175,9 +200,9 @@ static int set_device(const kta_handle *h) {
     return KTA_OK;
 }
 
-// key bytes travel to the device only when they are hashed, by the scan or by the partitioner check (kta_push reads the
-// copy in pc.hash)
-static bool keys_travel(const kta_handle *h) { return h->need_hash || h->d_hash_out || h->pt.ncounts; }
+// key bytes travel to the device only when they are hashed, by the scan, the partitioner check or the hot-key table
+// (kta_push reads the copy in pc.hash)
+static bool keys_travel(const kta_handle *h) { return h->need_hash || h->d_hash_out || h->pt.ncounts || h->hk.top_k; }
 
 static size_t scan_smem_bytes(bool hash, bool smem, int P, int threads, int keybuf, int stages, bool hdr) {
     return (smem ? smem_counter_bytes(P) : CTA_SCRATCH) + (size_t)(threads / 32) * warp_smem_bytes(hash, keybuf, stages, hdr);
@@ -247,6 +272,7 @@ static const ScanFn SCAN_KERNELS[2][2][3][2] = {
 // ------------------------------------------------------------------------------------------------
 static int launch_scan_raw(kta_handle *h, ScanParams prm, int64_t key_readable, int64_t key_bytes);
 static int ring_flush(kta_handle *h);
+static int hk_finalize(kta_handle *h);
 
 static int alive_create(kta_handle *h) {
     // open-addressed last-writer table keyed by the 32-bit hash, sized by the number of DISTINCT hashes and grown
@@ -729,15 +755,21 @@ static int launch_timeline(kta_handle *h, const ScanParams &prm) {
 // sized from the mean key span of a tile (12.5 % headroom, as the scan sizes its key stage) within what the shared memory
 // leaves beside the table and the counters, as many CTAs as are resident (at most one warp per tile), and enough that none
 // takes more than PC_MAX_CTA_TILES tiles
+// a warp's key stage for a pass over n records with key_bytes key bytes: the mean key span of a tile with 12.5 % headroom,
+// within [PC_STAGE_MIN, PC_STAGE_MAX] and the `room` bytes a warp has
+static int pass_stage_bytes(int64_t n, int64_t key_bytes, int64_t room) {
+    const int64_t per_tile = n > 0 ? (std::max<int64_t>(key_bytes, 0) * TILE + n - 1) / n : 0;
+    int64_t want = (per_tile + per_tile / 8 + 64 + 15) / 16 * 16;
+    want = std::min<int64_t>(std::max<int64_t>(want, PC_STAGE_MIN), PC_STAGE_MAX);
+    return (int)std::min<int64_t>(want, room / 16 * 16);
+}
+
 static int partitioner_shape(const kta_handle *h, int64_t n, int64_t key_bytes, int &grid, int &stage, size_t &smem) {
     const Partitioner &t = h->pt;
     const int64_t ntiles = (n + TILE - 1) / TILE;
     const size_t fixed = (size_t)PC_TABLE_WORDS * 4 + (t.smem ? ((size_t)(2 * t.ncounts + 1) * h->cfg.num_partitions + 3) / 4 * 16 : 0);
     const int64_t room = ((int64_t)h->smem_optin - (int64_t)fixed) / PC_WARPS - PC_STAGE_PAD;
-    const int64_t per_tile = n > 0 ? (std::max<int64_t>(key_bytes, 0) * TILE + n - 1) / n : 0;
-    int64_t want = (per_tile + per_tile / 8 + 64 + 15) / 16 * 16;
-    want = std::min<int64_t>(std::max<int64_t>(want, PC_STAGE_MIN), PC_STAGE_MAX);
-    stage = (int)std::min<int64_t>(want, room / 16 * 16);
+    stage = pass_stage_bytes(n, key_bytes, room);
     smem = fixed + (size_t)PC_WARPS * (size_t)(stage + PC_STAGE_PAD);
     int per_sm = 0;
     if (t.smem) CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, partitioner_kernel<true>, PC_THREADS, smem));
@@ -781,6 +813,126 @@ static int launch_partitioner(kta_handle *h, const ScanParams &prm, int64_t key_
     return KTA_OK;
 }
 
+// ------------------------------------------------------------------------------------------------
+// hot-key table: growth by rehash, the pass in slices that cannot overfill the table, export / import, finalize
+// ------------------------------------------------------------------------------------------------
+static constexpr uint64_t HK_DEFAULT_SLOTS = 1ull << 20, HK_MIN_SLOTS = 16, HK_MAX_SLOTS = 1ull << 31;
+
+// the table cannot grow: it stops counting until kta_reset, and the entry point that scanned reports it (hk_reported)
+static int hk_nomem(kta_handle *h, uint64_t want, const char *why) {
+    HotKeys &k = h->hk;
+    cudaGetLastError();   // a failed cudaMalloc must not be reported by the next launch check
+    snprintf(k.nomem_msg, sizeof k.nomem_msg, "hot-key table: cannot grow from %llu to %llu slots (%s); it has stopped counting "
+             "until kta_reset", (unsigned long long)k.slots, (unsigned long long)want, why);
+    k.nomem = k.unreported = true;
+    return fail(KTA_ERR_NOMEM, "%s", k.nomem_msg);
+}
+
+// KTA_ERR_NOMEM once for a table that ran out of memory during this call (every other metric has counted the batch)
+static int hk_reported(kta_handle *h) {
+    if (!h->hk.unreported) return KTA_OK;
+    h->hk.unreported = false;
+    return fail(KTA_ERR_NOMEM, "%s", h->hk.nomem_msg);
+}
+
+// the exact occupancy (one copy to the host and a stream synchronisation); a probe that found no slot is reported here
+static int hk_occupancy(kta_handle *h, uint64_t &occ) {
+    unsigned long long w[2] = {0, 0};
+    CU(cudaMemcpyAsync(w, h->hk.d_word, 16, cudaMemcpyDeviceToHost, h->stream));
+    CU(cudaStreamSynchronize(h->stream));
+    if ((uint32_t)w[1]) return fail(KTA_ERR_INVALID, "internal: a hot-key probe ran over the whole table");
+    occ = w[0];
+    return KTA_OK;
+}
+
+static int hk_grid(const kta_handle *h, int64_t items) {
+    return (int)std::max<int64_t>(std::min<int64_t>((items + 255) / 256, (int64_t)h->sm_count * 8), 1);
+}
+
+// doubles the table until it has at least `want` slots, by rehash; KTA_ERR_NOMEM (hk_nomem) when it cannot
+static int hk_grow(kta_handle *h, uint64_t want) {
+    HotKeys &k = h->hk;
+    uint64_t slots = k.slots;
+    while (slots < want) slots *= 2;
+    if (slots > HK_MAX_SLOTS) return hk_nomem(h, slots, "more than 2^31 slots");
+    if (k.max_slots && slots > k.max_slots) return hk_nomem(h, slots, "kta_hot_keys_limit_slots");
+    DevBuf<HkSlot> nt;
+    if (nt.alloc((int64_t)slots + 1)) return hk_nomem(h, slots, "cudaMalloc");
+    cudaStream_t s = h->stream;
+    CU(cudaMemsetAsync(nt, 0, (size_t)(slots + 1) * sizeof(HkSlot), s));
+    // the rehash counts its claims again, in word [2]: the table's occupancy word is replaced only once it has run
+    CU(cudaMemsetAsync(k.d_word + 2, 0, 8, s));
+    const HkTable to{nt, slots, k.d_word + 2, reinterpret_cast<unsigned int *>(k.d_word.get() + 1)};
+    hot_keys_rehash_kernel<<<hk_grid(h, (int64_t)k.slots + 1), 256, 0, s>>>(k.d_table, k.slots, to);
+    h->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(k.d_word, k.d_word + 2, 8, cudaMemcpyDeviceToDevice, s));
+    CU(cudaStreamSynchronize(s));
+    k.d_table = std::move(nt);   // nt frees the old table
+    k.slots = slots;
+    k.grows++;
+    return KTA_OK;
+}
+
+// the hot-key pass over tiles [t0, t1) of a counted scan's columns
+static int launch_hot_keys_tiles(kta_handle *h, const ScanParams &prm, int64_t key_bytes, int64_t t0, int64_t t1) {
+    HotKeysParams hp{};
+    hp.n = prm.n;
+    hp.tile_lo = t0;
+    hp.tile_hi = t1;
+    hp.partition = prm.partition;
+    hp.key_len = prm.key_len;
+    hp.value_len = prm.value_len;
+    hp.ts_ms = prm.ts_ms;
+    hp.key_bytes = prm.key_bytes;
+    hp.key_tile_base = prm.key_tile_base;
+    hp.P = h->cfg.num_partitions;
+    hp.shard_world = h->shard_world;
+    hp.shard_rank = h->shard_rank;
+    hp.tables = h->d_crc32_tables;
+    hp.table = h->hk.table();
+    const int64_t room = ((int64_t)h->smem_optin - (int64_t)PC_TABLE_WORDS * 4) / HK_WARPS - PC_STAGE_PAD;
+    hp.stage = pass_stage_bytes(prm.n, key_bytes, room);
+    const size_t smem = (size_t)PC_TABLE_WORDS * 4 + (size_t)HK_WARPS * (size_t)(hp.stage + PC_STAGE_PAD);
+    int per_sm = 0;
+    CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, hot_keys_kernel, HK_THREADS, smem));
+    if (per_sm < 1) return fail(KTA_ERR_CUDA, "hot-key kernel does not fit an SM (%zu B shared memory)", smem);
+    const int grid = (int)std::max<int64_t>(std::min<int64_t>((t1 - t0 + HK_WARPS - 1) / HK_WARPS, (int64_t)h->sm_count * per_sm), 1);
+    hot_keys_kernel<<<grid, HK_THREADS, smem, h->stream>>>(hp);
+    CU(cudaGetLastError());
+    h->launches++;
+    return KTA_OK;
+}
+
+// The hot-key pass over a counted scan's columns (same stream, so a ring chunk's free_ev, recorded after launch_scan, covers
+// it).  Counting is not idempotent, so no insert may fail: the table is kept at most half full.  U (bound) is an upper bound
+// on the occupancy, raised by every launch's records; a launch goes ahead without a read-back while U + n <= slots / 2.
+// Otherwise the exact occupancy is read back, the table grows while it is more than a quarter full or has less than a tile
+// of room, and the batch is cut into tile-aligned slices of at most slots / 2 - U records, reading back between slices.
+// A table that cannot grow stops counting (hk_nomem): the scan goes on, so every other metric counts the batch.
+static int launch_hot_keys(kta_handle *h, const ScanParams &prm, int64_t key_bytes) {
+    HotKeys &k = h->hk;
+    if (k.nomem) return KTA_OK;
+    const int64_t ntiles = (prm.n + TILE - 1) / TILE;
+    int rc;
+    for (int64_t t = 0; t < ntiles;) {
+        int64_t t1 = ntiles;
+        if (k.bound + (uint64_t)(prm.n - t * TILE) > k.slots / 2) {
+            uint64_t occ = 0;
+            if ((rc = hk_occupancy(h, occ))) return rc;
+            k.bound = occ;
+            while (k.bound * 4 > k.slots || k.slots / 2 - k.bound < (uint64_t)TILE)
+                if ((rc = hk_grow(h, k.slots * 2))) return k.nomem ? KTA_OK : rc;   // (hk_nomem has recorded an out-of-memory)
+            t1 = std::min<int64_t>(ntiles, t + (int64_t)((k.slots / 2 - k.bound) / TILE));
+        }
+        if (t1 - t < ntiles) k.slices++;
+        if ((rc = launch_hot_keys_tiles(h, prm, key_bytes, t, t1))) return rc;
+        k.bound += (uint64_t)(std::min<int64_t>(prm.n, t1 * TILE) - t * TILE);
+        t = t1;
+    }
+    return KTA_OK;
+}
+
 // one scan of a batch whose columns lie in ring chunk `chunk` (-1: elsewhere); `seq_ends`: see alive_prepare
 static int launch_scan(kta_handle *h, ScanParams prm, int64_t key_readable, int64_t key_bytes, int chunk = -1,
                        const uint64_t *seq_ends = nullptr) {
@@ -791,10 +943,15 @@ static int launch_scan(kta_handle *h, ScanParams prm, int64_t key_readable, int6
         if (!prm.key_tile_base) return fail(KTA_ERR_INVALID, "internal: key_tile_base missing");
         if (!prm.key_bytes && key_readable > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL but the partitioner check needs the keys");
     }
+    if (h->hk.top_k) {
+        if (!prm.key_tile_base) return fail(KTA_ERR_INVALID, "internal: key_tile_base missing");
+        if (!prm.key_bytes && key_readable > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL but the hot-key table needs the keys");
+    }
     if (exact && (rc = alive_prepare(h, prm, seq_ends))) return rc;
     if ((rc = launch_scan_raw(h, prm, key_readable, key_bytes))) return rc;
     if (h->tl.buckets && (rc = launch_timeline(h, prm))) return rc;
     if (h->pt.ncounts && (rc = launch_partitioner(h, prm, key_bytes))) return rc;
+    if (h->hk.top_k && (rc = launch_hot_keys(h, prm, key_bytes))) return rc;
     if (exact && (rc = alive_scanned(h, prm, key_readable, key_bytes, chunk))) return rc;
     h->records += (uint64_t)prm.n;
     h->finalized = false;
@@ -861,16 +1018,16 @@ static int scan_device_batch(kta_handle *h, const kta_batch *b) {
         if ((rc = derive_tile_base(h, b->key_len, b->n))) return rc;
         prm.key_tile_base = h->d_tb_scratch;
     }
-    if (h->pt.ncounts && !b->key_bytes) {
-        // The partitioner check hashes every key: without key bytes the batch may only have null and empty keys.  A
+    if ((h->pt.ncounts || h->hk.top_k) && !b->key_bytes) {
+        // The partitioner check and the hot-key table hash every key: without key bytes the batch may only have null and empty keys.  A
         // declared byte count is refused at once; otherwise the tile base's total is read back, one host round trip.  Only a
         // caller's batch without key bytes pays it: the log path hands over its gather buffer, which is never NULL.
         if (b->key_bytes_len > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL but key_bytes_len is %lld", (long long)b->key_bytes_len);
         uint64_t total = 0;
         CU(cudaMemcpyAsync(&total, prm.key_tile_base + (b->n + TILE - 1) / TILE, 8, cudaMemcpyDeviceToHost, h->stream));
         CU(cudaStreamSynchronize(h->stream));
-        if (total) return fail(KTA_ERR_INVALID, "key_bytes is NULL but the batch has %llu key bytes (the partitioner check hashes them)",
-                               (unsigned long long)total);
+        if (total) return fail(KTA_ERR_INVALID, "key_bytes is NULL but the batch has %llu key bytes (the partitioner check or the "
+                               "hot-key table hashes them)", (unsigned long long)total);
     }
     if ((rc = launch_scan(h, prm, b->key_bytes_len, b->key_bytes_len))) return rc;
     h->next_seq = std::max<uint64_t>(h->next_seq, seq_base + (uint64_t)b->n);
@@ -881,8 +1038,8 @@ extern "C" int kta_scan_batch_device(kta_handle *h, const kta_batch *b) {
     int rc;
     if ((rc = check_batch(h, b)) || b->n == 0) return rc;
     if ((rc = set_device(h))) return rc;
-    if ((rc = ring_flush(h))) return rc;   // records pushed earlier come first in seq order
-    return scan_device_batch(h, b);
+    if ((rc = ring_flush(h)) || (rc = scan_device_batch(h, b))) return rc;   // records pushed earlier come first in seq order
+    return hk_reported(h);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -941,13 +1098,15 @@ static int scan_log_batches(kta_handle *h, int32_t partition, const int32_t *dev
 
 extern "C" int kta_scan_log_segment_device(kta_handle *h, int32_t partition, const uint8_t *dev_bytes, int64_t len,
                                            const uint64_t *dev_batch_off, int64_t nbatches, int64_t *records_out) {
-    return scan_log_batches(h, partition, nullptr, dev_bytes, len, len, dev_batch_off, nbatches, records_out);
+    const int rc = scan_log_batches(h, partition, nullptr, dev_bytes, len, len, dev_batch_off, nbatches, records_out);
+    return rc ? rc : hk_reported(h);
 }
 
 extern "C" int kta_scan_log_batches_device(kta_handle *h, const uint8_t *dev_bytes, int64_t len, const uint64_t *dev_batch_off,
                                            const int32_t *dev_batch_partition, int64_t nbatches, int64_t *records_out) {
     if (nbatches && !dev_batch_partition) return fail(KTA_ERR_INVALID, "dev_batch_partition is NULL");
-    return scan_log_batches(h, 0, dev_batch_partition, dev_bytes, len, len, dev_batch_off, nbatches, records_out);
+    const int rc = scan_log_batches(h, 0, dev_batch_partition, dev_bytes, len, len, dev_batch_off, nbatches, records_out);
+    return rc ? rc : hk_reported(h);
 }
 
 extern "C" int kta_push_log_segments_host(kta_handle *h, int32_t nsegs, const int32_t *partitions, const uint8_t *const *bytes,
@@ -983,7 +1142,8 @@ extern "C" int kta_push_log_segments_host(kta_handle *h, int32_t nsegs, const in
     // the staging buffer has 64 bytes of slack behind `total`: 16-byte-granular bulk copies may run into it
     if ((rc = scan_log_batches(h, 0, L.part, L.bytes, total, total + 48, L.off, nb, records_out))) return rc;
     CU(cudaStreamSynchronize(s));   // the caller may reuse its buffers, and the scratch may be reused by the next call
-    return collect_timing(h);
+    if ((rc = collect_timing(h))) return rc;
+    return hk_reported(h);
 }
 
 extern "C" int kta_push_log_segment_host(kta_handle *h, int32_t partition, const uint8_t *bytes, int64_t len,
@@ -1171,9 +1331,11 @@ extern "C" int kta_push(kta_handle *h, int32_t partition, int64_t offset, int64_
     if (__builtin_expect(!h, 0)) return fail(KTA_ERR_INVALID, "null handle");
     auto &pc = h->pc;
     const int64_t kl = (pc.hash && key_len > 0) ? key_len : 0;  // key bytes only travel when they are hashed
+    int late = KTA_OK;   // a hot-key table that ran out of memory in the flush (the record still lands)
     if (__builtin_expect(pc.n == pc.cap || pc.kb + kl > pc.kcap, 0)) {
         const int rc = push_slow(h, kl);
         if (rc) return rc;
+        late = hk_reported(h);
     }
     const int64_t i = pc.n;
     if ((i & (TILE - 1)) == 0) pc.tile_base[i / TILE] = (uint64_t)pc.kb;
@@ -1197,7 +1359,7 @@ extern "C" int kta_push(kta_handle *h, int32_t partition, int64_t offset, int64_
     }
     pc.n = i + 1;
     h->finalized = false;
-    return KTA_OK;
+    return late;
 }
 
 extern "C" int kta_push_batch_host(kta_handle *h, const kta_batch *b) {
@@ -1205,10 +1367,10 @@ extern "C" int kta_push_batch_host(kta_handle *h, const kta_batch *b) {
     if ((rc = check_batch(h, b)) || b->n == 0) return rc;
     const bool hash = keys_travel(h);
     if (hash && !b->key_bytes && b->key_bytes_len > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL");
-    if (h->pt.ncounts && !b->key_bytes)
+    if ((h->pt.ncounts || h->hk.top_k) && !b->key_bytes)
         for (int64_t i = 0; i < b->n; i++)
             if (b->key_len[i] > 0) return fail(KTA_ERR_INVALID, "key_bytes is NULL but record %lld has a %d-byte key (the partitioner "
-                                               "check hashes it)", (long long)i, b->key_len[i]);
+                                               "check or the hot-key table hashes it)", (long long)i, b->key_len[i]);
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;  // keep seq order with earlier kta_push records
     if ((rc = ring_dev_init(h))) return rc;
@@ -1286,7 +1448,7 @@ extern "C" int kta_push_batch_host(kta_handle *h, const kta_batch *b) {
     CU(cudaStreamSynchronize(s));
     if ((rc = collect_timing(h))) return rc;
     h->next_seq = std::max<uint64_t>(h->next_seq, seq_base + (uint64_t)b->n);
-    return KTA_OK;
+    return hk_reported(h);
 }
 
 extern "C" int kta_sync(kta_handle *h) {
@@ -1295,8 +1457,8 @@ extern "C" int kta_sync(kta_handle *h) {
     if ((rc = set_device(h))) return rc;
     if ((rc = ring_flush(h))) return rc;
     CU(cudaStreamSynchronize(h->stream));
-    if ((rc = alive_settle(h))) return rc;
-    return collect_timing(h);
+    if ((rc = alive_settle(h)) || (rc = collect_timing(h))) return rc;
+    return hk_reported(h);
 }
 
 extern "C" int kta_reset(kta_handle *h) {
@@ -1320,6 +1482,15 @@ extern "C" int kta_reset(kta_handle *h) {
     for (uint64_t &v : o.totals) v = 0;
     if (h->tl.buckets) CU(cudaMemsetAsync(h->tl.d_bins, 0, h->tl.words() * 8, h->stream));   // (its configuration stays)
     if (h->pt.ncounts) CU(cudaMemsetAsync(h->pt.d_counts, 0, h->pt.words() * 8, h->stream));   // (so does the check's)
+    if (h->hk.top_k) {   // (the hot-key table keeps its configuration and its allocation)
+        HotKeys &k = h->hk;
+        CU(cudaMemsetAsync(k.d_table, 0, (size_t)(k.slots + 1) * sizeof(HkSlot), h->stream));
+        CU(cudaMemsetAsync(k.d_word, 0, 5 * 8, h->stream));
+        k.bound = 0;
+        k.nomem = k.unreported = false;
+        k.h_top.clear();
+        k.h_distinct = k.h_keyed = 0;
+    }
     return state_reset_device(h);
 }
 
@@ -1351,6 +1522,7 @@ extern "C" int kta_finalize(kta_handle *h) {
         h->pt.h_counts.resize(h->pt.words());
         CU(cudaMemcpyAsync(h->pt.h_counts.data(), h->pt.d_counts, h->pt.words() * 8, cudaMemcpyDeviceToHost, s));
     }
+    if (h->hk.top_k && !h->hk.nomem && (rc = hk_finalize(h))) return rc;
     CU(cudaStreamSynchronize(s));
     if ((rc = collect_timing(h))) return rc;
     h->h_alive = h->alive.now;   // counted over the table by alive_settle above (sum_all_alive, src/metric.rs:282-284)
@@ -1365,7 +1537,7 @@ extern "C" int kta_finalize(kta_handle *h) {
     if (bad)
         return fail(KTA_ERR_PARTITION, "%llu record(s) had a partition outside [0, %d) and were left out of every metric",
                     (unsigned long long)bad, h->cfg.num_partitions);
-    return KTA_OK;
+    return hk_reported(h);   // (after the statuses above: the hot-key getters keep returning KTA_ERR_NOMEM either way)
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1589,6 +1761,19 @@ extern "C" int kta_timeline_shape(const kta_handle *h, int64_t n, int32_t *grid,
     return KTA_OK;
 }
 
+// the zlib CRC-32 slicing tables of the partitioner check and the hot-key table, made on first use
+static int crc32_tables(kta_handle *h) {
+    if (h->d_crc32_tables) return KTA_OK;
+    uint32_t tables[4][256];
+    crc_slicing_tables_host(tables, ZLIB_CRC32_POLY);
+    DevBuf<uint32_t> d;
+    int rc;
+    if ((rc = d.alloc(PC_TABLE_WORDS))) return rc;
+    CU(cudaMemcpy(d, &tables[0][0], sizeof tables, cudaMemcpyHostToDevice));
+    h->d_crc32_tables = std::move(d);
+    return KTA_OK;
+}
+
 extern "C" int kta_set_partitioner_check(kta_handle *h, const int32_t *counts, int32_t ncounts) {
     if (!h) return fail(KTA_ERR_INVALID, "null handle");
     if (h->records || h->pc.n)
@@ -1604,14 +1789,7 @@ extern "C" int kta_set_partitioner_check(kta_handle *h, const int32_t *counts, i
     }
     int rc;
     if ((rc = set_device(h))) return rc;
-    if (ncounts && !h->d_crc32_tables) {
-        uint32_t tables[4][256];
-        crc_slicing_tables_host(tables, ZLIB_CRC32_POLY);
-        DevBuf<uint32_t> d;
-        if ((rc = d.alloc(PC_TABLE_WORDS))) return rc;
-        CU(cudaMemcpy(d, &tables[0][0], sizeof tables, cudaMemcpyHostToDevice));
-        h->d_crc32_tables = std::move(d);
-    }
+    if (ncounts && (rc = crc32_tables(h))) return rc;
     // the new configuration is built aside and swapped in only when complete: a failure keeps the old one
     Partitioner t;
     if (ncounts) {
@@ -1666,6 +1844,175 @@ extern "C" int kta_partitioner_limit_grid(kta_handle *h, int32_t max_ctas) {
     if (!h || max_ctas < 0) return fail(KTA_ERR_INVALID, "bad argument");
     if (!h->pt.ncounts) return fail(KTA_ERR_NOT_ENABLED, "the partitioner check is off (kta_set_partitioner_check)");
     h->pt.max_grid = max_ctas;
+    return KTA_OK;
+}
+
+extern "C" int kta_set_hot_keys(kta_handle *h, int32_t top_k, int64_t table_slots) {
+    if (!h) return fail(KTA_ERR_INVALID, "null handle");
+    if (h->records || h->pc.n)
+        return fail(KTA_ERR_INVALID, "the hot-key table is configured before the first record: records were pushed or scanned "
+                    "since create or the last kta_reset");
+    if (top_k < 0 || top_k > KTA_HOT_KEYS_MAX) return fail(KTA_ERR_INVALID, "top_k %d outside [0, %d]", top_k, KTA_HOT_KEYS_MAX);
+    if (table_slots != 0 && (table_slots < (int64_t)HK_MIN_SLOTS || table_slots > (int64_t)HK_MAX_SLOTS || (table_slots & (table_slots - 1))))
+        return fail(KTA_ERR_INVALID, "table_slots %lld: 0 or a power of two in [16, 2^31]", (long long)table_slots);
+    int rc;
+    if ((rc = set_device(h))) return rc;
+    // the new configuration is built aside and swapped in only when complete: a failure keeps the old one
+    HotKeys k;
+    if (top_k) {
+        if ((rc = crc32_tables(h))) return rc;
+        k.slots = table_slots ? (uint64_t)table_slots : HK_DEFAULT_SLOTS;
+        if ((rc = k.d_table.alloc((int64_t)k.slots + 1)) || (rc = k.d_word.alloc(5))) return rc;
+        CU(cudaFuncSetAttribute(hot_keys_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->smem_optin));
+        CU(cudaMemsetAsync(k.d_table, 0, (size_t)(k.slots + 1) * sizeof(HkSlot), h->stream));
+        CU(cudaMemsetAsync(k.d_word, 0, 5 * 8, h->stream));
+        k.top_k = top_k;
+    }
+    CU(cudaStreamSynchronize(h->stream));   // the zeroing has landed, and no queued pass still uses the old table
+    h->hk = std::move(k);
+    h->pc.hash = keys_travel(h);   // from now on kta_push copies the keys (nothing is in the landing ring)
+    return KTA_OK;
+}
+
+static int hk_check(const kta_handle *h) {
+    if (!h) return fail(KTA_ERR_INVALID, "null handle");
+    if (!h->hk.top_k) return fail(KTA_ERR_NOT_ENABLED, "the hot-key table is off (kta_set_hot_keys)");
+    if (h->hk.nomem) return fail(KTA_ERR_NOMEM, "%s", h->hk.nomem_msg);
+    return KTA_OK;
+}
+
+extern "C" int kta_hot_keys(const kta_handle *h, kta_hot_key *out, int64_t cap, int64_t *count) {
+    if (!h || cap < 0 || (cap && !out)) return fail(KTA_ERR_INVALID, "bad argument");
+    int rc;
+    if ((rc = hk_check(h)) || (rc = check_read(h, 0, false))) return rc;
+    const std::vector<kta_hot_key> &top = h->hk.h_top;
+    const size_t n = std::min<size_t>((size_t)cap, top.size());
+    if (n) memcpy(out, top.data(), n * sizeof(kta_hot_key));
+    if (count) *count = (int64_t)top.size();
+    return KTA_OK;
+}
+
+extern "C" int kta_hot_key_stats(const kta_handle *h, uint64_t *distinct_keys, uint64_t *keyed_records, uint64_t *slots,
+                                 uint64_t *grows, uint64_t *slices) {
+    int rc;
+    if ((rc = hk_check(h)) || (rc = check_read(h, 0, false))) return rc;
+    const HotKeys &k = h->hk;
+    if (distinct_keys) *distinct_keys = k.h_distinct;
+    if (keyed_records) *keyed_records = k.h_keyed;
+    if (slots) *slots = k.slots;
+    if (grows) *grows = k.grows;
+    if (slices) *slices = k.slices;
+    return KTA_OK;
+}
+
+// every entry into out[0, cap) (cap 0: none); `records` (may be NULL) gets their records' sum; count = the occupancy
+static int hk_export(kta_handle *h, kta_hot_key *out, int64_t cap, unsigned long long *records, uint64_t &count) {
+    HotKeys &k = h->hk;
+    int rc;
+    if ((rc = hk_occupancy(h, count))) return rc;
+    cudaStream_t s = h->stream;
+    CU(cudaMemsetAsync(k.d_word + 2, 0, 16, s));
+    hot_keys_export_kernel<<<hk_grid(h, (int64_t)k.slots + 1), 256, 0, s>>>(k.d_table, k.slots, k.d_word + 2, k.d_word + 3, out,
+                                                                            (unsigned long long)cap);
+    h->launches++;
+    CU(cudaGetLastError());
+    if (records) CU(cudaMemcpyAsync(records, k.d_word + 3, 8, cudaMemcpyDeviceToHost, s));
+    return KTA_OK;
+}
+
+// finalize: the occupied slots compacted, sorted by (records descending, id ascending), the first top_k to the host
+static int hk_finalize(kta_handle *h) {
+    HotKeys &k = h->hk;
+    cudaStream_t s = h->stream;
+    uint64_t n = 0;
+    unsigned long long keyed = 0;
+    int rc;
+    if ((rc = hk_occupancy(h, n)) || (rc = k.d_entries.grow(s, (int64_t)std::max<uint64_t>(n, 1))) ||
+        (rc = hk_export(h, k.d_entries, k.d_entries.cap, &keyed, n)))
+        return rc;
+    k.bound = n;
+    const int64_t top = (int64_t)std::min<uint64_t>(n, (uint64_t)k.top_k);
+    k.h_top.resize((size_t)top);
+    if (n) {
+        size_t tmp = 0;
+        CU(hot_keys_sort(nullptr, tmp, nullptr, nullptr, nullptr, nullptr, (int64_t)n, s));
+        if ((rc = k.d_keys.grow(s, 2 * (int64_t)n)) || (rc = k.d_idx.grow(s, 2 * (int64_t)n)) || (rc = k.d_sort_tmp.grow(s, (int64_t)tmp)) ||
+            (rc = k.d_top.grow(s, top)))
+            return rc;
+        tmp = (size_t)k.d_sort_tmp.cap;
+        hot_keys_sort_keys_kernel<<<hk_grid(h, (int64_t)n), 256, 0, s>>>(k.d_entries, (int64_t)n, k.d_keys, k.d_idx);
+        CU(hot_keys_sort(k.d_sort_tmp, tmp, k.d_keys, k.d_keys + n, k.d_idx, k.d_idx + n, (int64_t)n, s));
+        hot_keys_gather_kernel<<<hk_grid(h, top), 256, 0, s>>>(k.d_entries, k.d_idx + n, top, k.d_top);
+        h->launches += 3;
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(k.h_top.data(), k.d_top, (size_t)top * sizeof(kta_hot_key), cudaMemcpyDeviceToHost, s));
+    }
+    CU(cudaStreamSynchronize(s));
+    k.h_distinct = n;
+    k.h_keyed = keyed;
+    return KTA_OK;
+}
+
+extern "C" int kta_hot_keys_export_count(kta_handle *h, int64_t *count) {
+    if (!count) return fail(KTA_ERR_INVALID, "bad argument");
+    int rc;
+    if ((rc = hk_check(h)) || (rc = set_device(h)) || (rc = ring_flush(h))) return rc;
+    if (h->hk.nomem) return hk_check(h);   // (the flush may have run the table out of memory)
+    uint64_t n = 0;
+    if ((rc = hk_occupancy(h, n))) return rc;
+    *count = (int64_t)n;
+    return KTA_OK;
+}
+
+extern "C" int kta_hot_keys_export_device(kta_handle *h, kta_hot_key *dev_out, int64_t cap, int64_t *count) {
+    if (!count || cap < 0 || (cap && !dev_out)) return fail(KTA_ERR_INVALID, "bad argument");
+    int rc;
+    if ((rc = hk_check(h)) || (rc = set_device(h)) || (rc = ring_flush(h))) return rc;
+    if (h->hk.nomem) return hk_check(h);
+    uint64_t n = 0;
+    if ((rc = hk_export(h, dev_out, cap, nullptr, n))) return rc;
+    CU(cudaStreamSynchronize(h->stream));
+    *count = (int64_t)n;
+    if ((int64_t)n > cap) return fail(KTA_ERR_INVALID, "export buffer too small: %llu > %lld", (unsigned long long)n, (long long)cap);
+    return KTA_OK;
+}
+
+// the list is checked on the device (one read-back) before anything is applied; the table grows first, so that every entry
+// finds a slot and the table stays at most half full
+extern "C" int kta_hot_keys_import_device(kta_handle *h, const kta_hot_key *dev_in, int64_t count) {
+    if (count < 0 || (count && !dev_in)) return fail(KTA_ERR_INVALID, "bad argument");
+    int rc;
+    if ((rc = hk_check(h))) return rc;
+    if (count == 0) return KTA_OK;
+    if ((rc = set_device(h))) return rc;
+    HotKeys &k = h->hk;
+    cudaStream_t s = h->stream;
+    unsigned int bad = 0;
+    CU(cudaMemsetAsync(k.d_word + 4, 0, 8, s));
+    hot_keys_validate_kernel<<<hk_grid(h, count), 256, 0, s>>>(dev_in, count, h->cfg.num_partitions,
+                                                               reinterpret_cast<unsigned int *>(k.d_word.get() + 4));
+    h->launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(&bad, k.d_word + 4, 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    if (bad)
+        return fail(KTA_ERR_INVALID, "hot-key import refused: an entry has records == 0, tombstones > records, key_len < 0, a "
+                    "nonzero reserved word, or a partition range outside [0, %d)", h->cfg.num_partitions);
+    uint64_t occ = 0;
+    if ((rc = hk_occupancy(h, occ))) return rc;
+    k.bound = occ + (uint64_t)count;
+    if (k.bound > k.slots / 2 && (rc = hk_grow(h, k.bound * 2))) return k.nomem ? hk_reported(h) : rc;
+    hot_keys_import_kernel<<<hk_grid(h, count), 256, 0, s>>>(dev_in, count, k.table());
+    h->launches++;
+    CU(cudaGetLastError());
+    h->finalized = false;
+    return hk_occupancy(h, occ);   // (the caller may free its list when this returns)
+}
+
+extern "C" int kta_hot_keys_limit_slots(kta_handle *h, int64_t max_slots) {
+    if (!h || max_slots < 0) return fail(KTA_ERR_INVALID, "bad argument");
+    if (!h->hk.top_k) return fail(KTA_ERR_NOT_ENABLED, "the hot-key table is off (kta_set_hot_keys)");
+    h->hk.max_slots = (uint64_t)max_slots;
     return KTA_OK;
 }
 

@@ -29,6 +29,8 @@ def allreduce_merge(engine: KtaEngine, group=None, counters_only: bool = False) 
     if not engine.shares_caller_stream:
         torch.cuda.current_stream().synchronize()
     engine.merge_import(world, buf)
+    if engine.hot_keys_top_k and not counters_only:
+        allgather_hot_keys(engine, group)
     if engine.count_alive_keys and not counters_only:
         n_local = engine.alive_export_count()
         counts = torch.zeros(world, dtype=torch.int64, device=dev)
@@ -49,6 +51,36 @@ def allreduce_merge(engine: KtaEngine, group=None, counters_only: bool = False) 
         for r in range(world):
             if r != rank and cl[r]:
                 engine.alive_import(h_all[r * cap:], s_all[r * cap:], int(cl[r]))
+
+
+def allgather_hot_keys(engine: KtaEngine, group=None) -> None:
+    """Makes every rank's hot-key table topic-wide: each rank exports its entries (88 bytes each, include/kta.h
+    kta_hot_key), the counts and then the entries are all-gathered, and each rank imports the other ranks' entries.  The
+    table cannot travel in the SUM buffer: its entries are keyed by id, in no fixed order."""
+    import torch
+    import torch.distributed as dist
+    from ._native import HOT_KEY_DTYPE
+
+    world, rank = dist.get_world_size(group), dist.get_rank(group)
+    if world == 1:
+        return
+    dev = torch.device("cuda", torch.cuda.current_device())
+    counts = torch.zeros(world, dtype=torch.int64, device=dev)
+    counts[rank] = engine.hot_keys_export_count()
+    dist.all_reduce(counts, op=dist.ReduceOp.SUM, group=group)
+    cl = counts.tolist()
+    cap = max(cl)
+    if cap == 0:
+        return
+    size = HOT_KEY_DTYPE.itemsize
+    loc = torch.zeros(cap * size, dtype=torch.uint8, device=dev)
+    engine.hot_keys_export(loc, cap)
+    every = torch.empty(world * cap * size, dtype=torch.uint8, device=dev)
+    dist.all_gather_into_tensor(every, loc, group=group)
+    torch.cuda.current_stream().synchronize()
+    for r in range(world):
+        if r != rank and cl[r]:
+            engine.hot_keys_import(every[r * cap * size:], int(cl[r]))
 
 
 # ---------------------------------------------------------------------------------------------------

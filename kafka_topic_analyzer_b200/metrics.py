@@ -89,6 +89,7 @@ class KtaEngine:
         self.shares_caller_stream = False   # True after set_stream(): work is ordered by the caller's stream
         self.timeline_buckets = 0           # set_timeline
         self.partitioner_counts = ()        # set_partitioner_check
+        self.hot_keys_top_k = 0             # set_hot_keys
         self.message_metrics = MessageMetrics(self)
         self.log_compaction_metrics = LogCompactionInMemoryMetrics(self) if count_alive_keys else None
 
@@ -294,6 +295,52 @@ class KtaEngine:
         check(lib().kta_partitioner_hash_host(self._h, kl.size, kl.ctypes.data, kb.ctypes.data if kb.size else None, kb.size,
                                               mm.ctypes.data, cc.ctypes.data))
         return mm, cc
+
+    def set_hot_keys(self, top_k: int, table_slots: int = 0) -> None:
+        """Count every key's records, tombstones and bytes in an exact table on the GPU and keep the top_k keys with the
+        most records (include/kta.h).  top_k in [1, 65536], 0 turns it off; table_slots 0 (2^20) or a power of two in
+        [16, 2^31].  Only before the first record (after create or reset); reset() keeps the setting."""
+        top_k, table_slots = int(top_k), int(table_slots)
+        if not 0 <= top_k < 1 << 31 or not 0 <= table_slots < 1 << 63:   # (ctypes would wrap them silently)
+            raise KtaError(N.ERR_INVALID, "top_k %d / table_slots %d out of range" % (top_k, table_slots))
+        check(lib().kta_set_hot_keys(self._h, top_k, table_slots))
+        self.hot_keys_top_k = top_k
+
+    def hot_keys(self, as_dicts: bool = False):
+        """The top keys after finalize(), by records descending then id ascending: a numpy structured array of
+        _native.HOT_KEY_DTYPE, or (as_dicts) a list of dicts whose key_prefix is the key's first min(key_len, 32) bytes."""
+        out = np.zeros(max(self.hot_keys_top_k, 1), dtype=N.HOT_KEY_DTYPE)
+        n = C.c_int64()
+        check(lib().kta_hot_keys(self._h, out.ctypes.data, out.size, C.byref(n)))
+        out = out[:n.value]
+        if not as_dicts:
+            return out
+        return [dict({f: int(r[f]) for f in N.HOT_KEY_DTYPE.names if f != "key_prefix"},
+                     key_prefix=bytes(r["key_prefix"][:min(int(r["key_len"]), N.HOT_KEY_PREFIX)])) for r in out]
+
+    def hot_key_stats(self):
+        """(distinct keys, keyed records, slots, grows, slices) after finalize()."""
+        v = [C.c_uint64() for _ in range(5)]
+        check(lib().kta_hot_key_stats(self._h, *[C.byref(x) for x in v]))
+        return tuple(x.value for x in v)
+
+    def hot_keys_export_count(self) -> int:
+        n = C.c_int64()
+        check(lib().kta_hot_keys_export_count(self._h, C.byref(n)))
+        return n.value
+
+    def hot_keys_export(self, dev_out, cap: int) -> int:
+        """every entry into a device buffer of cap 88-byte entries; returns how many"""
+        n = C.c_int64()
+        check(lib().kta_hot_keys_export_device(self._h, _ptr(dev_out), cap, C.byref(n)))
+        return n.value
+
+    def hot_keys_import(self, dev_in, count: int) -> None:
+        check(lib().kta_hot_keys_import_device(self._h, _ptr(dev_in), count))
+
+    def hot_keys_limit_slots(self, max_slots: int) -> None:
+        """the table may not grow beyond max_slots slots, 0 = no cap (test hook)."""
+        check(lib().kta_hot_keys_limit_slots(self._h, max_slots))
 
     def sync(self) -> None:
         check(lib().kta_sync(self._h))
